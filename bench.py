@@ -1,16 +1,21 @@
 #!/usr/bin/env python
-"""bench.py -- headline benchmark of the LIBXSMM hot path on B200 (contract: one JSON line on stdout).
+"""bench.py -- headline benchmark of the LIBXSMM hot path on an H100 (one JSON line on stdout).
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload brgemm|fsspmdm|bcsc|sweep]
+                  [--dump-outputs DIR]
 
 Workload (BASELINE.json configs[1]): batched BRGEMM bf16 x bf16 -> f32, m=n=k=64, br=8 (stride mode),
 batch = 65536 independent tiles PER GPU with all operands unique ("mode S" of SURVEY.md 8d). One step is
-one pass over the batch = ONE launch of the tcgen05 tile kernel through the C ABI
+one pass over the batch = ONE launch of the wgmma tile kernel through the C ABI
 (libxsmm_b200_gemm_batch_strided). Inputs (8.6 GB) are far larger than L2, so no flush is needed.
+Inputs are seeded: with the same arguments every run computes on the same data. --steps is the number of timed steps of the
+selected workload (the secondary `also` legs of the default run keep their own counts: max(5, K), max(3, K // 4) or
+max(5, K // 2) steps, so that each secondary number rests on several steps); --dump-outputs DIR writes what the last timed step computed (a fixed sample of it) as DIR/<name>.npy.
 
   value  whole-job GFLOP/s, operands resident in HBM, CUDA events on the launching stream, max over ranks
   e2e    same metric through the same C-ABI call with HOST (pinned) buffers: H2D + kernel + D2H per step
-  roofline      achieved algorithmic GB/s of the dominant kernel vs the measured HBM peak
+  roofline      achieved algorithmic GB/s of the dominant kernel vs the HBM peak (MEASURED_PEAKS.json if present, else the
+                H100 SXM data sheet)
   cpu_baseline  the reference's own JIT kernel (oracle/_ref, all host cores) on a bounded sample
   also          fsspmdm (config 3) and BCSC (config 4) with their own roofline numbers
 
@@ -38,21 +43,11 @@ FLAG_BETA_0 = 4
 METRIC = "batched BRGEMM GFLOP/s (bf16, m=n=k=64, br=8, batch=65536/GPU, unique operands)"
 WORKLOAD = ("configs[1]: batched BRGEMM bf16->f32 m=n=k=64 brcount=8 batch=65536 per GPU, stride-BR, beta=0, "
             "mode S (all operands unique)")
-# dram__bytes_read.sum + dram__bytes_write.sum of ONE launch from the committed `ncu --set full` captures (bytes)
-NCU_TRAFFIC = {"gemm_tc_kernel<64>": (9673.1e6, "profiles/r02_ncu_gemm_tc.txt"),
-               "sreg_kernel<float>": (622.1e6, "profiles/r02_ncu_sreg.txt"),
-               "bcsc_ts_kernel<32,2>": (491.3e6, "profiles/r02_ncu_bcsc_ts.txt"),       # below the 537 MB of algorithmic bytes: part of C is still in L2 when the capture ends
-               "gemm_pool_kernel": (495.2e6, "profiles/r02_ncu_gemm_pool.txt"),           # C writes (537 MB algorithmic); the operand pools stay in L2
-               "gemm_ts_kernel": (745.9e6, "profiles/r02_ncu_gemm_ts_i8.txt")}
-
-
-def traffic(kernel):
-    t = NCU_TRAFFIC.get(kernel, (None, None))
-    return t[0]
+DUMP_BYTES = 64 << 20     # --dump-outputs: at most this many bytes in all
 
 
 def peaks():
-    p = {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "src": "fallback"}
+    p = {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "src": "H100 SXM data sheet (dense)"}
     try:
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             j = json.load(f)
@@ -63,7 +58,7 @@ def peaks():
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks/throttle reasons sampled DURING the timed region (read-only queries)."""
 
     def __init__(self, index):
         self.rows, self.stop_flag, self.index = [], False, index
@@ -135,6 +130,31 @@ def time_steps(torch, fn, steps, warmup, dist=None):
     return total_ms, per
 
 
+def dump_outputs(dirname, arrays):
+    """write {name: torch tensor or numpy array} as DIR/<name>.npy in float32 (float64 stays float64)"""
+    import numpy as np
+    if not dirname:
+        return
+    os.makedirs(dirname, exist_ok=True)
+    total = 0
+    for name, a in arrays.items():
+        if not isinstance(a, np.ndarray):
+            a = a.detach().float().cpu().numpy()
+        if a.dtype != np.float64:
+            a = a.astype(np.float32)
+        total += a.nbytes
+        assert total <= DUMP_BYTES, "dumped outputs exceed %d bytes" % DUMP_BYTES
+        np.save(os.path.join(dirname, name + ".npy"), a)
+
+
+def sample_rows(n, k, seed=1234):
+    """a fixed, seeded, sorted choice of k of n row indices (all of them when k >= n)"""
+    import numpy as np
+    if k >= n:
+        return np.arange(n)
+    return np.sort(np.random.default_rng(seed).choice(n, size=k, replace=False))
+
+
 # ------------------------------------------------------------------------------------------------ BRGEMM
 def brgemm_setup(X, torch, batch, out_f32=True):
     tc = F32 if out_f32 else BF16
@@ -142,7 +162,7 @@ def brgemm_setup(X, torch, batch, out_f32=True):
     cfg = X.libxsmm_create_gemm_batch_reduce_config(X.GEMM_BATCH_REDUCE_STRIDE, M * K * 2, K * N * 2, 0)
     kernel = X.libxsmm_dispatch_brgemm(shape, FLAG_BETA_0, 0, cfg)
     assert kernel, "dispatch failed"
-    assert X.libxsmm_b200_kernel_backend(kernel) == X.BACKEND_TCGEN05, "tcgen05 kernel not selected"
+    assert X.libxsmm_b200_kernel_backend(kernel) == X.BACKEND_TCGEN05, "tensor-core kernel not selected"
     a = torch.empty(batch * BR * M * K, dtype=torch.bfloat16, device="cuda")
     b = torch.empty(batch * BR * K * N, dtype=torch.bfloat16, device="cuda")
     c = torch.empty(batch * M * N, dtype=torch.float32 if out_f32 else torch.bfloat16, device="cuda")
@@ -181,6 +201,7 @@ def run_ours(args):
     X.libxsmm_b200_set_device(local)
     X.libxsmm_b200_set_stream(torch.cuda.current_stream().cuda_stream)
     X.libxsmm_b200_set_blocking(0)
+    torch.manual_seed(555)          # every input below is drawn from seeded generators: identical from run to run
     pk = peaks()
     out = {}
     if args.workload == "brgemm":
@@ -196,6 +217,9 @@ def run_ours(args):
             total_ms, per = time_steps(torch, step, args.steps, args.warmup, dist)
         launches = X.libxsmm_b200_launch_count() - launches0 - args.warmup
         X.check()
+        if rank == 0 and args.dump_outputs:     # C of the last timed step: a fixed sample of 1024 of the tiles
+            tiles = torch.from_numpy(sample_rows(BATCH, 1024)).cuda()
+            dump_outputs(args.dump_outputs, {"brgemm_c_tiles": c.view(BATCH, N, M)[tiles], "brgemm_tile_index": tiles.double()})
         from libxsmm_b200.shard import weak_batch
         per_gpu, job_tiles = weak_batch(BATCH, world)      # batch is the only shard axis: every rank owns BATCH tiles, no collective
         flops = 2.0 * M * N * K * BR * per_gpu
@@ -209,9 +233,8 @@ def run_ours(args):
                "vs_baseline": None, "dtype": "bf16", "data": "synthetic",
                "config": {"workload": WORKLOAD,
                           "batch_per_gpu": BATCH, "parallelism": "batch sharded, no collective", "l2_policy": "inputs (8.6 GB) larger than L2, no flush"},
-               "roofline": {"bound": "hbm", "achieved": ach, "peak": pk["hbm_gbs"], "unit": "GB/s", "frac": ach / pk["hbm_gbs"], "traffic": traffic("gemm_tc_kernel<64>"),
-                            "traffic_src": NCU_TRAFFIC["gemm_tc_kernel<64>"][1], "algorithmic_bytes": bytes_alg,
-                            "peak_src": pk["src"], "kernel": "gemm_tc_kernel<64>", "kernel_ms": kern_ms,
+               "roofline": {"bound": "hbm", "achieved": ach, "peak": pk["hbm_gbs"], "unit": "GB/s", "frac": ach / pk["hbm_gbs"], "algorithmic_bytes": bytes_alg,
+                            "peak_src": pk["src"], "kernel": "gemm_wg_kernel", "kernel_ms": kern_ms,
                             "tensor_frac_of_measured_bf16_peak": (flops / (kern_ms * 1e-3) / 1e12) / pk["bf16_tflops"]},
                "gpu_launches": int(launches), "clocks": clocks.summary()}
         if not args.no_e2e:
@@ -242,7 +265,7 @@ def run_ours(args):
     elif args.workload == "brgemm_r":
         out = also_brgemm_r(X, torch, pk, args, full=True)
     elif args.workload == "sweep":
-        out = sweep(X, torch, pk, args)
+        out = sweep(X, torch, pk, args, full=True)
     if dist is not None:
         dist.barrier()
         dist.destroy_process_group()
@@ -325,15 +348,17 @@ def also_fsspmdm(X, torch, pk, args, full=False, n_cols=1000000, dist=None):
     h = X.libxsmm_fsspmdm_create(F32, Mf, Nf, Kf, Kf, Nf, Nf, one.ctypes.data, zero.ctypes.data, a.ctypes.data, 0, None)
     assert h
     b = torch.randn(Kf * Nf, device="cuda"); c = torch.empty(Mf * Nf, device="cuda")
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
 
     def step():
         X.libxsmm_fsspmdm_execute(h, b.data_ptr(), c.data_ptr())
     step(); X.check()
     checked = fsspmdm_check(torch, a, b, c, Mf, Kf, Nf)
-    steps = max(5, args.steps)
-    total_ms, per = time_steps(torch, step, steps, 3, dist)
+    steps = args.steps if full else max(5, args.steps)
+    total_ms, per = time_steps(torch, step, steps, 3 if not full else args.warmup, dist)
     X.check()
+    if full and args.dump_outputs:          # C (M x N, row-major) of the last timed step: a fixed sample of 4096 columns
+        cols = torch.from_numpy(sample_rows(Nf, 4096)).cuda()
+        dump_outputs(args.dump_outputs, {"fsspmdm_c_cols": c.view(Mf, Nf)[:, cols], "fsspmdm_col_index": cols.double()})
     ms = sorted(per)[len(per) // 2] if dist is None else total_ms / steps
     bytes_alg = 4.0 * (Kf * Nf + Mf * Nf)
     ach = bytes_alg / (ms * 1e-3) / 1e9
@@ -343,7 +368,7 @@ def also_fsspmdm(X, torch, pk, args, full=False, n_cols=1000000, dist=None):
         cpu = cpu_baseline_fsspmdm(a, Mf, Kf, nnz)
     return {"cpu_baseline": cpu, "metric": "fsspmdm GFLOP/s (f32 M=32 K=128 N=1e6, 15% nnz)", "value": 2.0 * nnz * Nf / (ms * 1e-3) / 1e9, "unit": "GFLOP/s (sparse)",
             "dense_equiv_gflops": 2.0 * Mf * Kf * Nf / (ms * 1e-3) / 1e9, "ms_per_step": ms, "nnz": nnz, "oracle_check": checked,
-            "roofline": {"bound": "hbm", "achieved": ach, "peak": pk["hbm_gbs"], "unit": "GB/s", "frac": ach / pk["hbm_gbs"], "traffic": traffic("sreg_kernel<float>"), "algorithmic_bytes": bytes_alg, "kernel": "sreg_kernel<float>"},
+            "roofline": {"bound": "hbm", "achieved": ach, "peak": pk["hbm_gbs"], "unit": "GB/s", "frac": ach / pk["hbm_gbs"], "algorithmic_bytes": bytes_alg, "kernel": "sreg_kernel<float>"},
             "config": {"workload": "configs[2]: fsspmdm f32 M=32 K=128 N=1e6 15% nnz beta=0; B+C = 640 MB per step (> L2)"}}
 
 
@@ -412,11 +437,13 @@ def also_bcsc(X, torch, pk, args, full=False, mblocks=8192, dist=None):
     step(); X.check()
     checked = bcsc_check(torch, a, bv, c, colptr, rowidx, (Mb, Kb, Nb, bk, bn), mblocks)
     variant = int(X.libxsmm_b200_bcsc_variant(kernel, nbc))
-    assert variant in (1, 2), "BCSC bench did not take a tcgen05 kernel (variant %d)" % variant
-    kname = "bcsc_ts_kernel<32,2>" if variant == 2 else "bcsc_tc_kernel<32>"
-    steps = max(3, args.steps // 4)
-    total_ms, per = time_steps(torch, step, steps, 3, dist)
+    assert variant == 1, "BCSC bench did not take the tensor-core kernel (variant %d)" % variant
+    steps = args.steps if full else max(3, args.steps // 4)
+    total_ms, per = time_steps(torch, step, steps, 3 if not full else args.warmup, dist)
     X.check()
+    if full and args.dump_outputs:          # C of the last timed step: a fixed sample of 256 m_blocks (N x M each)
+        blocks = torch.from_numpy(sample_rows(mblocks, 256)).cuda()
+        dump_outputs(args.dump_outputs, {"bcsc_c_mblocks": c.view(mblocks, Nb * Mb)[blocks], "bcsc_mblock_index": blocks.double()})
     ms = sorted(per)[len(per) // 2] if dist is None else total_ms / steps
     bytes_alg = 2.0 * (mblocks * Kb * Mb + mblocks * Nb * Mb) + 2.0 * nnzb * bk * bn
     ach = bytes_alg / (ms * 1e-3) / 1e9
@@ -427,8 +454,8 @@ def also_bcsc(X, torch, pk, args, full=False, mblocks=8192, dist=None):
     return {"cpu_baseline": cpu, "metric": "BCSC spmm GFLOP/s dense-equivalent (bf16, M=32 N=K=512, 32x32 blocks, 50%, m_blocks=8192)",
             "value": 2.0 * Mb * mblocks * Nb * Kb / (ms * 1e-3) / 1e9, "unit": "GFLOP/s (dense-equivalent)",
             "effective_gflops": 2.0 * Mb * mblocks * nnzb * bk * bn / (ms * 1e-3) / 1e9, "ms_per_step": ms, "oracle_check": checked,
-            "roofline": {"bound": "hbm", "achieved": ach, "peak": pk["hbm_gbs"], "unit": "GB/s", "frac": ach / pk["hbm_gbs"], "traffic": traffic(kname), "algorithmic_bytes": bytes_alg,
-                         "kernel": kname + " (+ bcsc_prep_kernel, bcsc_pack_b_kernel: the timed call is all three launches)"},
+            "roofline": {"bound": "hbm", "achieved": ach, "peak": pk["hbm_gbs"], "unit": "GB/s", "frac": ach / pk["hbm_gbs"], "algorithmic_bytes": bytes_alg,
+                         "kernel": "bcsc_wg_kernel"},
             "config": {"workload": "configs[3] on one GPU: BCSC bf16 M=32 N=K=512 bk=bn=32 50% m_blocks=8192; A+C = 537 MB per step (> L2)"}}
 
 
@@ -453,7 +480,7 @@ def sweep_check(torch, a, b, c, m, types, flags, esz, csz, batch):
     return {"tiles": 3, "max_normf_rel": worst, "bit_exact": esz == 1}
 
 
-def sweep(X, torch, pk, args, batch=32768):
+def sweep(X, torch, pk, args, batch=32768, full=False):
     """configs[4]: int8 x int8 -> int32 (U8 x I8, VNNI4 A) and F16 x F16 -> F32, m=n=k in {8..128}, br=1, unique operands"""
     I8, U8, I32, F16 = 12, 13, 8, 3
     pts = []
@@ -476,8 +503,13 @@ def sweep(X, torch, pk, args, batch=32768):
                 assert rc == 0, X.libxsmm_b200_last_error_string()
             step(); X.check()
             chk = sweep_check(torch, a, b, c, m, (ta, tb, tcomp, tcc), flags, esz, csz, batch)
-            total_ms, per = time_steps(torch, step, max(5, args.steps // 2), 3)
+            total_ms, per = time_steps(torch, step, args.steps if full else max(5, args.steps // 2), args.warmup if full else 3)
             X.check()
+            if full and args.dump_outputs:      # C of the last timed step of this point: a fixed sample of 64 tiles
+                tiles = torch.from_numpy(sample_rows(batch, 64)).cuda()
+                cc = c.view(batch, m * m * csz)[tiles]
+                cc = cc.view(torch.int32).double() if esz == 1 else cc.view(torch.float32)
+                dump_outputs(args.dump_outputs, {"sweep_%s_m%d_c_tiles" % ("i8" if esz == 1 else "f16", m): cc})
             ms = sorted(per)[len(per) // 2]
             bytes_alg = float(batch) * (sa + sb + sc)
             ach = bytes_alg / (ms * 1e-3) / 1e9
@@ -487,7 +519,7 @@ def sweep(X, torch, pk, args, batch=32768):
     return {"metric": "mixed-precision sweep GFLOP/s (configs[4], diagonal m=n=k)", "value": best["gflops"], "unit": "GFLOP/s", "n_gpus": 1, "steps": args.steps,
             "warmup": 3, "higher_is_better": True, "dtype": "u8/i8->i32, f16->f32", "data": "synthetic",
             "config": {"workload": "configs[4]: int8 and f16 GEMM m=n=k in {8,16,32,64,128}, batch=32768, br=1, beta=0, unique operands"},
-            "points": pts, "roofline": {"bound": "hbm", "achieved": best["gbs"], "peak": pk["hbm_gbs"], "unit": "GB/s", "frac": best["hbm_frac"], "traffic": None}}
+            "points": pts, "roofline": {"bound": "hbm", "achieved": best["gbs"], "peak": pk["hbm_gbs"], "unit": "GB/s", "frac": best["hbm_frac"]}}
 
 
 def also_brgemm_r(X, torch, pk, args, full=False, pool_sets=64, batch=BATCH):
@@ -495,7 +527,7 @@ def also_brgemm_r(X, torch, pk, args, full=False, pool_sets=64, batch=BATCH):
     from a pool of 64 sets each (8 MB, L2-resident), C unique bf16 -- the tensor-core-bound variant of configs[1]. One step = one
     libxsmm_b200_gemm_plan_run over 65536 per-tile argument structs (the plan sorts tiles by set pair; equal neighbours share their
     operands in shared memory; pairs of tiles with the same B set share one M=128 instruction). Roofline: dense bf16 tensor throughput
-    (MEASURED_PEAKS bf16_tflops, burst: the kernel is timed alone)."""
+    (MEASURED_PEAKS bf16_tflops if present, else the data sheet)."""
     import numpy as np
     from oracle_ffi import oracle, run_gemm
     import gen
@@ -536,18 +568,19 @@ def also_brgemm_r(X, torch, pk, args, full=False, pool_sets=64, batch=BATCH):
         err = gen.normf_rel(gen.to_f64(want, BF16), gen.to_f64(got, BF16))
         assert err <= 5e-3, "mode R output differs from the oracle (tile %d, err %g)" % (t, err)
         worst = max(worst, err)
-    total_ms, per = time_steps(torch, step, max(5, args.steps), 3)
+    total_ms, per = time_steps(torch, step, args.steps if full else max(5, args.steps), args.warmup if full else 3)
     X.check()
+    if full and args.dump_outputs:          # C of the last timed step: a fixed sample of 1024 tiles
+        tiles = torch.from_numpy(sample_rows(batch, 1024)).cuda()
+        dump_outputs(args.dump_outputs, {"brgemm_r_c_tiles": c.view(batch, N, M)[tiles], "brgemm_r_tile_index": tiles.double()})
     ms = sorted(per)[len(per) // 2]
     X.libxsmm_b200_gemm_plan_destroy(plan)
     flops = 2.0 * M * N * K * BR * batch
     tf = flops / (ms * 1e-3) / 1e12
     return {"metric": "batched BRGEMM GFLOP/s, mode R (bf16 64^3 br=8, address batch-reduce, operand pool of %d block-sets, C bf16 unique)" % pool_sets,
             "value": flops / (ms * 1e-3) / 1e9, "unit": "GFLOP/s", "ms_per_step": ms, "oracle_check": {"tiles": 4, "max_normf_rel": worst},
-            "roofline": {"bound": "tensor", "achieved": tf, "peak": pk["bf16_tflops"], "unit": "TFLOP/s", "frac": tf / pk["bf16_tflops"], "traffic": traffic("gemm_pool_kernel"),
-                         "kernel": "gemm_pool_kernel (resident operand sets, two tiles per M=128 instruction)",
-                         "note": "a 128x64x16 tcgen05.mma costs 48 cycles (profiles/r01_umma_cost.txt: max(N/2, 32+N/4)), i.e. 67 % of the nominal "
-                                 "2.38 PFLOP/s at 1965 MHz = 95 % of the measured cuBLAS peak: the bound of this tile shape"},
+            "roofline": {"bound": "tensor", "achieved": tf, "peak": pk["bf16_tflops"], "unit": "TFLOP/s", "frac": tf / pk["bf16_tflops"],
+                         "kernel": "gemm_wg_kernel (two tiles that share B per item, one warpgroup each)"},
             "config": {"workload": "configs[1] mode R: tiles draw their A and B block-sets from pools of %d (L2-resident); C %.0f MB per step" % (pool_sets, batch * M * N * 2 / 1e6)}}
 
 
@@ -786,13 +819,14 @@ def run_reference(args):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=20)
+    ap.add_argument("--steps", type=int, default=20, help="timed steps of the selected workload (the `also` legs time at least 3-5 steps each)")
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--workload", default="brgemm", choices=["brgemm", "brgemm_r", "fsspmdm", "bcsc", "sweep"])
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-also", action="store_true")
     ap.add_argument("--no-cpu", action="store_true")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write what the last timed step computed as DIR/<name>.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
     if args.impl == "reference":

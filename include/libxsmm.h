@@ -2,7 +2,7 @@
  *
  * Every entry point below keeps the name, argument meaning and error behaviour (NULL on
  * unsupported/failed, library is mute unless libxsmm_verbosity != 0) of the reference API, but the
- * handle that dispatch returns launches a hand-written sm_100a CUDA kernel instead of JIT'ed x86.
+ * handle that dispatch returns launches a hand-written sm_90a CUDA kernel instead of JIT'ed x86.
  * Each declaration cites the reference interface it replaces (file:line in /root/reference).
  * Additive, GPU-only entry points (batch launch, streams, device memory) live in libxsmm_b200.h.
  */
@@ -33,7 +33,7 @@ LIBXSMM_API void libxsmm_init(void);
 LIBXSMM_API void libxsmm_finalize(void);
 LIBXSMM_API int libxsmm_get_target_archid(void);
 LIBXSMM_API void libxsmm_set_target_archid(int id);
-LIBXSMM_API const char* libxsmm_get_target_arch(void);          /* returns "sm_100a" */
+LIBXSMM_API const char* libxsmm_get_target_arch(void);          /* returns "sm_90a" */
 LIBXSMM_API void libxsmm_set_target_arch(const char* arch);     /* accepted and ignored */
 LIBXSMM_API const char* libxsmm_get_typename(libxsmm_datatype datatype);
 LIBXSMM_API int libxsmm_get_verbosity(void);

@@ -23,7 +23,7 @@ extern "C" {
 typedef enum libxsmm_b200_backend {
   LIBXSMM_B200_BACKEND_NONE = 0,
   LIBXSMM_B200_BACKEND_SIMT = 1,        /* exact-order CUDA-core kernel (all dtypes/layouts) */
-  LIBXSMM_B200_BACKEND_TCGEN05 = 2,     /* TMA -> SMEM -> tcgen05.mma -> TMEM tile kernel */
+  LIBXSMM_B200_BACKEND_TCGEN05 = 2,     /* tensor-core tile kernel: TMA -> SMEM -> wgmma.mma_async -> registers (sm_90a) */
   LIBXSMM_B200_BACKEND_STREAM = 3,      /* HBM-streaming kernels (fsspmdm, packed sparse, meltw) */
   LIBXSMM_B200_BACKEND_NOOP = 4         /* tile-config handles */
 } libxsmm_b200_backend;
@@ -41,7 +41,7 @@ LIBXSMM_API const char* libxsmm_b200_last_error_string(void);
 LIBXSMM_API unsigned long long libxsmm_b200_launch_count(void); /* kernels launched by this library */
 LIBXSMM_API int libxsmm_b200_kernel_backend(const void* kernel);
 /* BCSC handles (libxsmm_create_packed_spgemm_bcsc): the kernel a call with `n_block_columns` (= *b.quaternary) takes:
- * 0 exact-order CUDA-core kernel, 1 tcgen05 with A converted in shared memory, 2 tcgen05 with A in tensor memory; -1: not BCSC */
+ * 0 exact-order CUDA-core kernel, 1 wgmma tensor-core kernel; -1: not BCSC */
 LIBXSMM_API int libxsmm_b200_bcsc_variant(const void* kernel, unsigned long long n_block_columns);
 /* force the SIMT kernel for dense GEMM handles dispatched afterwards (debug / parity checking) */
 LIBXSMM_API void libxsmm_b200_set_force_simt(int on);

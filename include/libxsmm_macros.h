@@ -63,7 +63,7 @@
 #define LIBXSMM_RV64_MVL256_LMUL      3004
 #define LIBXSMM_RV64_ALLFEAT          3999
 /* this backend's single target; ordered above every CPU id so that "at least <target>" feature tests hold */
-#define LIBXSMM_B200_SM100A           100000
+#define LIBXSMM_B200_SM90A           100000
 
 /* ---- token helpers ----------------------------------------------------------------------------------------------- */
 #define LIBXSMM_CONCATENATE2(A, B) A##B

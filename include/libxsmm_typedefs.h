@@ -1,4 +1,4 @@
-/* libxsmm_b200 -- type/enum surface of the LIBXSMM 2.x C API, re-stated for the B200 backend.
+/* libxsmm_b200 -- type/enum surface of the LIBXSMM 2.x C API, re-stated for the H100 (sm_90a) backend.
  *
  * This header is written from scratch; it mirrors names, enumerator VALUES and struct layouts of
  * the reference's include/libxsmm_typedefs.h so that callers compiled against either header are

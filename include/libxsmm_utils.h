@@ -130,7 +130,7 @@ LIBXSMM_API void libxsmm_rne_convert_fp32_hf8(const float* in, libxsmm_hfloat8* 
 LIBXSMM_API void libxsmm_convert_hf8_f32(const libxsmm_hfloat8* in, float* out, size_t length);
 
 /* ---- target queries (reference include/libxsmm_cpuid.h:80-120) ----------------------------------------------------
- * libxsmm_cpuid: this backend's single target, ordered above every x86 id (see LIBXSMM_B200_SM100A above).
+ * libxsmm_cpuid: this backend's single target, ordered above every x86 id (see LIBXSMM_B200_SM90A above).
  * libxsmm_cpuid_dot_pack_factor: elements of a k-group in the "VNNI" operand layouts the kernels consume:
  * 2 for 16-bit types, 4 for 8-bit types, else 1 -- the x86 convention (src/libxsmm_cpuid_x86.c), which IS the ABI. */
 typedef struct libxsmm_cpuid_info { char model[1024]; int constant_tsc; int has_context; } libxsmm_cpuid_info;

@@ -1,965 +1,156 @@
-// libxsmm_b200 -- packed block-sparse (BCSC) B x dense A on the tcgen05 tensor cores (sm_100a), bf16.
+// libxsmm_b200 -- packed block-sparse (BCSC) B x dense A on the Hopper tensor cores (sm_90a, wgmma.mma_async), bf16.
 //
 // For every m_block mb:  C_mb[N][M] = beta * C_mb + A_mb(M x K) * B(K x N),  B given as BCSC blocks [bn][bk].
 // Replaces src/generator_packed_spgemm_bcsc_bsparse_avx_avx2_avx512_amx.c (AMX/AVX-512 per block);
 // semantics are those of the driver's dense gold (samples/xgemm_sparse/spmm_kernel.c:74-217) with f32
-// accumulation in tensor memory (tolerance 5e-3 for bf16 like spmm_kernel.c:1019-1029).
+// accumulation in registers (tolerance 5e-3 for bf16 like spmm_kernel.c:1019-1029).
 //
-// Mapping. B is shared by all m_blocks, so 128/M consecutive m_blocks are stacked into ONE M=128 MMA operand
-// ("group"). Every non-zero block (kb, j) contributes bk/16 instructions
-//   D[:, j*bn : (j+1)*bn] += A_grp[:, kb*bk : (kb+1)*bk] * B_blk^T;
-// adjacent blocks of a block-row are merged into one wider instruction. Two tiny kernels run in front on every call
-// (pattern and values arrive with the call):
-//   bcsc_prep_kernel   re-sorts the CSC block pattern into per (column part, k-step) lists of ready-to-issue MMA
-//                      operations; it first compares the pattern with the copy cached for the calling stream and
-//                      returns at once when nothing changed
-//   bcsc_pack_b_kernel copies the B blocks into visiting order, pre-swizzled to the shared-memory image the MMA
-//                      descriptor expects, so that one k-range of a part is ONE contiguous bulk copy
-//
-// Main kernel `bcsc_ts_kernel` (K <= 512): THE A OPERAND LIVES IN TENSOR MEMORY. For kind::f16 a 32-bit TMEM cell of
-// the A operand holds two consecutive k of one row -- exactly one VNNI2 word of the caller's A[K/2][M][2] layout. So the
-// packed layout needs no conversion at all, only a transposing copy: thread = row m reads its 32 words of a 64-wide k-step
-// from the raw TMA stage and writes them with one tcgen05.st.32x32b.x32. The whole K range of a group (K/2 <= 256
-// columns) stays resident while the column parts (<= 128 accumulator columns each, two slots) are swept, so A is
-// fetched from HBM exactly once and never touched by the MMAs' shared-memory port (TS-form MMA: N/2 cycles per
-// M=128 x N x 16 instruction instead of 32 + N/4 with A in shared memory, profiles/r01_umma_cost.txt).
-//   warp 0        A producer: TMA 3-D box of the raw VNNI words of one k-step (128 rows x 64 k = 16 KB)
-//   warp 1        B producer: one cp.async.bulk per (part, k-chunk) list of packed blocks
-//   warp 2        MMA issuer: tcgen05.mma.cta_group::1.kind::f16 [D], [A in TMEM], B descriptor; also owns TMEM
-//   warps 4-7     copy     : raw stage -> TMEM A slot of the k-step (one warp per TMEM lane quadrant)
-//   warps 8-15    epilogue : tcgen05.ld -> bf16 (RNE) -> packed stores, 128 contiguous bytes per warp instruction
-// TMEM plan: columns 0-255 two accumulator slots, columns 256-511 A (eight k-step slots of 32 columns).
-// Hand-overs per group: 8 A k-steps (copy -> MMA, MMA -> copy), nparts x k-chunks B stages, nparts accumulators.
-//
-// `bcsc_tc_kernel` (A converted to the canonical shared-memory operand by 8 converter warps, SS-form MMA) is the
-// round-1 kernel, kept for K > 512 and for A/B comparison (LIBXSMM_B200_BCSC_V1=1).
+// Mapping. The m_blocks are M rows each and stacked, so 64 consecutive rows of the stacked A form one wgmma M=64 operand
+// ("group"). A work item is (group, block-column j); one warpgroup per CTA walks the items round-robin. For every non-zero
+// block (kb, j) of the column:
+//   D[:, 0 : bn] += A_grp[:, kb*bk : (kb+1)*bk] * B_blk^T          (bk/16 instructions m64 x bn x k16)
+// A is VNNI2-packed (A[K/2][M][2]): a 32-bit word holds two consecutive k of one row, which is exactly one register of the
+// wgmma A fragment, so A goes from global memory (L2-resident across the columns of a group) straight into registers.
+// B blocks ([bn][bk], k contiguous: the K-major operand) are copied into the canonical no-swizzle shared-memory layout
+// (8 x 16-byte core matrices), two buffers so that the copy of the next block overlaps the MMAs of the current one.
+// The pattern (colptr, rowidx) and the values arrive with the call and are read directly: no preparation kernel.
 #include <cuda.h>
-#include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdlib.h>
 #include <string.h>
-#include <mutex>
-#include <vector>
 #include "xb_internal.h"
 #include "xb_device.cuh"
-#include "xb_tma.cuh"
+#include "xb_wgmma.cuh"
+#include "xb_epilogue.cuh"
 
 namespace {
 
-struct BcscTcParams {
-  int bn, bk, nbc, nks, ksteps;             // nks: 64-wide k-steps, ksteps = bk / 16
-  long long m_blocks, ngroups;
-  int ncols, slot_cols, nslot;              // N = nbc*bn, TMEM columns per work item, slots
-  int nparts, part_cols;                    // column parts per group (each <= 256 columns so that TMEM holds >= 2 items)
-  int raw_stages, can_stages, b_stages, b_stage_bytes;
-  const unsigned int* list_ptr;             // [nparts*nks + 1] first block of every (part, k-step) list
-  const unsigned int* wranges;              // [4 * lists] {first op | count << 16} per MMA warp
-  const uint4* ops;                         // {d col | A row offset/16 << 16, B offset/16, idesc N bits, accumulate}
-  const unsigned int* col_any;              // [nbc] column has at least one block
-  const char* b_packed;                     // B blocks in visiting order, pre-swizzled (bcsc_pack_b_kernel)
-  int mma_warps, ops_cap;                   // ops_cap: operations that fit the shared-memory copy (variant 2)
-  char* c; int beta0;
-  uint32_t idesc, b_layout, b_sbo16;        // UMMA descriptor pieces
-};
-
-// layout of the per-handle index buffer (words); shared by host and prep kernel
-struct BcscIdxLayout {
-  unsigned int hdr, cache_cp, cache_ri, list_ptr, entries, col_any, wranges, ops, total;
-  __host__ __device__ BcscIdxLayout(unsigned int nbc, unsigned int nl, unsigned int cap) {
-    hdr = 0; cache_cp = 16; cache_ri = cache_cp + nbc + 1; list_ptr = cache_ri + cap; entries = list_ptr + nl + 1;
-    col_any = entries + cap; wranges = col_any + nbc; ops = (wranges + 4 * nl + 3) & ~3u; total = ops + 4 * cap + 4;
-  }
+struct BcscParams {
+  int M, K, bk, bn, nbc;                  // packed width, depth, block shape, block-columns
+  long long m_blocks, ngroups, items;     // items = ngroups * nbc
+  const uint32_t* a;                      // VNNI2 words, m_block mb at a + mb * (K/2) * M
+  const uint4* b_vals;                    // [nnzb][bn][bk] bf16
+  const unsigned int* colptr; const unsigned int* rowidx;
+  unsigned short* c; int beta0;
 };
 
 
-// programmatic dependent launch: the three kernels of a call are chained without host-visible gaps -- a kernel lets its
-// successor start launching at once and the successor waits (for completion and visibility of its predecessors) right
-// before it first reads what they wrote
-__device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" :: "r"(bar), "r"(count) : "memory"); }
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) { asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(bar), "r"(bytes) : "memory"); }
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" :: "r"(bar) : "memory"); }
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  uint32_t done;
-  do {
-    asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                 : "=r"(done) : "r"(bar), "r"(parity) : "memory");
-  } while (!done);
-}
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-               :: "r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate));
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) { asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" :: "r"(bar) : "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-               "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-               "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-                 "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-                 "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-                 "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-               : "r"(taddr) : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-// high word of an SMEM matrix descriptor (stride offset, version 1, layout); the low word carries address and LBO
-__device__ __forceinline__ uint32_t desc_hi(uint32_t sbo16, uint32_t layout) { return (sbo16 & 0x3FFFu) | (1u << 14) | (layout << 29); }
-__device__ __forceinline__ uint32_t desc_lo(uint32_t smem_addr, uint32_t lbo16) { return ((smem_addr & 0x3FFFFu) >> 4) | ((lbo16 & 0x3FFFu) << 16); }
-__device__ __forceinline__ uint64_t desc64(uint32_t hi, uint32_t lo) { return ((uint64_t)hi << 32) | lo; }
-
-// ---- prep: CSC block pattern -> per (part, k-step) lists of MMA operations ---------------------------------------------
-// Every MMA warp OWNS cpw adjacent block-columns of a part (merged runs never cross owners): all instructions on one
-// accumulator column are issued by one thread in k order, so 'overwrite' always precedes 'accumulate' and the summation
-// order is fixed without any cross-warp synchronisation. Lists are stored owner-major: (warp, block-row, column).
-__global__ void __launch_bounds__(256) bcsc_prep_kernel(const unsigned int* __restrict__ colptr, const unsigned int* __restrict__ rowidx,
-                                                        int nbc, int nkb, int bn, int bk, int nparts, int bpp, int cpw, unsigned int cap,
-                                                        unsigned int resident_cap_blocks, unsigned int* buf) {
-  pdl_launch_dependents();
-  const int KBS = 64 / bk, nks = (nkb + KBS - 1) / KBS, nl = nparts * nks;
-  const BcscIdxLayout L((unsigned int)nbc, (unsigned int)nl, cap);
-  __shared__ unsigned int s_cp[257];
-  __shared__ unsigned int s_ri[2048];
-  __shared__ unsigned short s_map[2048];          // dense (block-row, column) -> block index + 1
-  __shared__ unsigned int cnt[513];
-  __shared__ unsigned int s_kmin[256];
-  for (int j = threadIdx.x; j <= nbc; j += blockDim.x) s_cp[j] = colptr[j];
-  __syncthreads();
-  unsigned int nnzb = s_cp[nbc]; if (nnzb > cap) nnzb = cap;
-  for (unsigned int z = threadIdx.x; z < nnzb; z += blockDim.x) s_ri[z] = rowidx[z];
-  // unchanged pattern (the usual case: weights are re-used across calls)? compare in full with the cached copy
-  // (the buffer capacity is part of the key: every offset of BcscIdxLayout depends on it)
-  const unsigned int key[11] = {0xb200c5c5u, (unsigned int)nbc, (unsigned int)nkb, (unsigned int)bn, (unsigned int)bk, (unsigned int)nparts,
-                                (unsigned int)bpp, (unsigned int)cpw, nnzb, cap, resident_cap_blocks};
-  int same = 1;
-  if (threadIdx.x < 11) same = (buf[L.hdr + threadIdx.x] == key[threadIdx.x]);
-  for (int j = threadIdx.x; j <= nbc; j += blockDim.x) same &= (buf[L.cache_cp + j] == s_cp[j]);
-  for (unsigned int z = threadIdx.x; z < nnzb; z += blockDim.x) same &= (buf[L.cache_ri + z] == s_ri[z]);
-  if (__syncthreads_and(same)) return;
-
-  for (int i = threadIdx.x; i <= nl; i += blockDim.x) cnt[i] = 0;
-  for (int i = threadIdx.x; i < nbc * nkb; i += blockDim.x) s_map[i] = 0;
-  __syncthreads();
-  for (int j = threadIdx.x; j < nbc; j += blockDim.x) {
-    unsigned int kmin = 0xffffffffu;
-    for (unsigned int z = s_cp[j]; z < s_cp[j + 1] && z < nnzb; ++z) {
-      const unsigned int kb = s_ri[z];
-      if (kb < (unsigned int)nkb) {
-        s_map[kb * nbc + j] = (unsigned short)(z + 1);
-        atomicAdd(&cnt[(j / bpp) * nks + kb / KBS + 1], 1u);
-        kmin = (kb < kmin) ? kb : kmin;
-      }
-    }
-    s_kmin[j] = kmin; buf[L.col_any + j] = (kmin != 0xffffffffu) ? 1u : 0u;
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) { for (int i = 0; i < nl; ++i) cnt[i + 1] += cnt[i]; }
-  __syncthreads();
-  for (int i = threadIdx.x; i <= nl; i += blockDim.x) buf[L.list_ptr + i] = cnt[i];
-  uint4* ops = reinterpret_cast<uint4*>(buf + L.ops);
-  const int maxrun = 256 / bn;
-  const unsigned int blk16 = (unsigned int)(bn * bk * 2) >> 4;
-  for (int l = threadIdx.x; l < nl; l += blockDim.x) {
-    const int part = l / nks, ks = l % nks, j0 = part * bpp, j1 = (j0 + bpp < nbc) ? j0 + bpp : nbc;
-    unsigned int e = cnt[l], o = cnt[l], pos = 0;
-    for (int w = 0; w < 4; ++w) {
-      const int c0 = j0 + w * cpw, c1 = (c0 + cpw < j1) ? c0 + cpw : j1;
-      const unsigned int ostart = o;
-      for (int kbi = 0; kbi < KBS && ks * KBS + kbi < nkb; ++kbi) {
-        const int kb = ks * KBS + kbi;
-        const unsigned int a_off16 = (unsigned int)(kbi * bk * 128) >> 4;
-        int run_j = 0, run_len = 0; unsigned int run_first = 0, run_pos = 0;
-        for (int j = c0; j < c1; ++j) {
-          const unsigned int zz = s_map[kb * nbc + j];
-          if (zz == 0) continue;
-          const unsigned int first = ((unsigned int)kb == s_kmin[j]) ? 1u : 0u;
-          buf[L.entries + e++] = zz - 1;
-          if (run_len > 0 && j == run_j + run_len && first == run_first && run_len < maxrun) ++run_len;
-          else {
-            if (run_len > 0) ops[o++] = make_uint4((unsigned int)((run_j - j0) * bn) | (a_off16 << 16), run_pos * blk16, ((unsigned int)(run_len * bn) >> 3) << 17, run_first ^ 1u);
-            run_j = j; run_len = 1; run_first = first; run_pos = pos;
-          }
-          ++pos;
-        }
-        if (run_len > 0) ops[o++] = make_uint4((unsigned int)((run_j - j0) * bn) | (a_off16 << 16), run_pos * blk16, ((unsigned int)(run_len * bn) >> 3) << 17, run_first ^ 1u);
-      }
-      buf[L.wranges + 4 * l + w] = ostart | ((o - ostart) << 16);
-    }
-  }
-  for (int j = threadIdx.x; j <= nbc; j += blockDim.x) buf[L.cache_cp + j] = s_cp[j];
-  for (unsigned int z = threadIdx.x; z < nnzb; z += blockDim.x) buf[L.cache_ri + z] = s_ri[z];
-  if (threadIdx.x < 11) buf[L.hdr + threadIdx.x] = key[threadIdx.x];
-  // plan for the TS-form kernel (header words 12, 13): the column parts are cut into S contiguous sets such that the B blocks
-  // of a set fit the shared memory left beside the A ring; S CTAs then share a group (each re-reads its A, from L2) and keep
-  // their set of B RESIDENT for the whole launch. S = 0: no such split with S <= 4, B is streamed per (part, k-chunk).
-  if (threadIdx.x == 0) {
-    unsigned int plan_s = 0, plan_pps = 0;
-    for (unsigned int s = 1; s <= 4u && s <= (unsigned int)nparts && plan_s == 0; ++s) {
-      const unsigned int pps = ((unsigned int)nparts + s - 1) / s;
-      unsigned int worst = 0;
-      for (unsigned int p = 0; p < (unsigned int)nparts; p += pps) {
-        const unsigned int pe = (p + pps < (unsigned int)nparts) ? p + pps : (unsigned int)nparts;
-        const unsigned int blocks = cnt[pe * nks] - cnt[p * nks];
-        worst = (blocks > worst) ? blocks : worst;
-      }
-      if (worst <= resident_cap_blocks && (pps * s - (unsigned int)nparts) < pps) { plan_s = s; plan_pps = pps; }
-    }
-    buf[L.hdr + 12] = plan_s; buf[L.hdr + 13] = plan_pps;
+// element (n, k) of a block in shared memory: core matrix (n / 8, k / 8) at (n / 8) * sbo + (k / 8) * 128, row n % 8 at 16 bytes
+__device__ __forceinline__ void stage_block(uint8_t* dst, const uint4* src, int bn, int bk) {
+  const int kc = bk / 8, sbo = kc * 128, chunks = bn * kc;
+  for (int i = threadIdx.x; i < chunks; i += blockDim.x) {
+    const int n = i / kc, k8 = i - n * kc;
+    *reinterpret_cast<uint4*>(dst + (n >> 3) * sbo + k8 * 128 + (n & 7) * 16) = src[i];
   }
 }
 
-// ---- B repack: blocks in visiting order, each already in the shared-memory image the MMA descriptor expects ------------
-// (K-major, rows of S = 2*bk bytes, 16-byte chunks XOR-swizzled exactly like the hardware SWIZZLE_<S>B mode). One k-step
-// of a column part is then ONE contiguous run and is fetched with a single bulk copy. (Fetching the caller's blocks with a
-// 2D tensor map costs the TMA unit ~5 cycles per 64-byte row: measured 287K of 357K cycles per CTA.)
-__global__ void __launch_bounds__(256) bcsc_pack_b_kernel(const uint4* __restrict__ b_vals, const unsigned int* __restrict__ entries,
-                                                          const unsigned int* __restrict__ list_ptr, int nl, uint4* __restrict__ out, int bn, int bk) {
-  pdl_launch_dependents();
-  pdl_wait();                                                        // the visiting order comes from the prep kernel
-  const unsigned int nnzb = list_ptr[nl];
-  const unsigned int cpr = (unsigned int)bk >> 3;                    // 16-byte chunks per row (2, 4 or 8)
-  const unsigned int cpb = (unsigned int)bn * cpr;                   // chunks per block
-  const unsigned long long total = (unsigned long long)nnzb * cpb;
-  for (unsigned long long t = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (unsigned long long)gridDim.x * blockDim.x) {
-    const unsigned int e = (unsigned int)(t / cpb), ci = (unsigned int)(t % cpb);
-    const unsigned int n = ci / cpr, c = ci % cpr;
-    const unsigned int z = entries[e];
-    const unsigned int sw = ((n * cpr * 16u) >> 7) & (cpr - 1u);     // Swizzle<log2(cpr),4,3>: address bits [7,..) folded onto the chunk bits
-    out[(size_t)e * cpb + n * cpr + (c ^ sw)] = b_vals[(size_t)z * cpb + ci];
-  }
+template <int NC>
+__device__ __forceinline__ void mma_rs(float (&d)[NC / 2], const uint32_t (&a)[4], uint64_t b, int scale_d) {
+  if (NC == 16) xb_wgmma_rs_bf16_n16(*reinterpret_cast<float(*)[8]>(&d), a, b, scale_d);
+  if (NC == 32) xb_wgmma_rs_bf16_n32(*reinterpret_cast<float(*)[16]>(&d), a, b, scale_d);
+  if (NC == 64) xb_wgmma_rs_bf16_n64(*reinterpret_cast<float(*)[32]>(&d), a, b, scale_d);
 }
 
-// ---- shared epilogue: one 32-column chunk of a 128-row group from registers to C -------------------------------------------
-// v[j] is the f32 accumulator of (row of this lane, column c0+j). C_mb is [N][M] (m contiguous): lanes 2i/2i+1 hold rows
-// m/m+1, so after one exchange per column PAIR the even lane owns (m, m+1) of column c and the odd lane (m, m+1) of column
-// c+1 -- one 4-byte store per lane, and the 32 lanes of the instruction cover 2 x 64 contiguous bytes (all lanes shuffle).
-template <int M>
-__device__ __forceinline__ void bcsc_store_chunk(const uint32_t (&v)[32], __nv_bfloat16* dst, int ncol, bool any0, bool any1,
-                                                 bool valid, int beta0, int lane) {
-  if (beta0 && (M % 2) == 0) {
-    const bool odd = lane & 1;
-    unsigned int* dst32 = reinterpret_cast<unsigned int*>(dst - (odd ? 1 : 0));
+// NC: columns per instruction, NCH: instructions side by side (NC * NCH >= bn)
+template <int NC, int NCH>
+__global__ void __launch_bounds__(128, (NCH >= 4) ? 2 : 4)
+bcsc_wg_kernel(const BcscParams P) {
+  extern __shared__ __align__(128) uint8_t smem_raw[];
+  const int buf_bytes = NC * NCH * P.bk * 2;                 // the instructions read NC * NCH rows of a block
+  uint8_t* sbuf[2] = {smem_raw, smem_raw + buf_bytes};
+  const int lane = threadIdx.x & 31, wq = threadIdx.x >> 5, q = lane & 3;
+  const int sbo = (P.bk / 8) * 128, ksteps = P.bk / 16;
+  const long long KW = P.K / 2;
+  float acc[NCH][NC / 2];
+  int buf = 0;
+  for (long long item = blockIdx.x; item < P.items; item += gridDim.x) {
+    const long long grp = item / P.nbc;
+    const int j = (int)(item - grp * P.nbc);
+    // fragment rows r0, r0 + 8 of the group: stacked row R = 64 grp + r is row R % M of m_block R / M
+    const uint32_t* arow[2]; bool avalid[2];
 #pragma unroll
-    for (int jj = 0; jj < 32; jj += 2) {
-      const bool anyc = (jj < 16) ? any0 : any1;
-      const float mine_c0 = anyc ? __uint_as_float(v[jj]) : 0.0f, mine_c1 = anyc ? __uint_as_float(v[jj + 1]) : 0.0f;
-      const float send = odd ? mine_c0 : mine_c1;                 // even lanes give away column c+1, odd lanes column c
-      const float got = __shfl_xor_sync(0xffffffffu, send, 1);
-      const __nv_bfloat162 pk = odd ? __floats2bfloat162_rn(got, mine_c1) : __floats2bfloat162_rn(mine_c0, got);
-      if (valid && (jj < 16 || ncol == 32)) dst32[((jj + (odd ? 1 : 0)) * M) >> 1] = *reinterpret_cast<const unsigned int*>(&pk);
+    for (int h = 0; h < 2; ++h) {
+      const long long R = grp * 64 + 16 * wq + (lane >> 2) + 8 * h, mb = R / P.M;
+      avalid[h] = mb < P.m_blocks;
+      arow[h] = P.a + (avalid[h] ? mb * KW * P.M + (R - mb * P.M) : 0);
     }
-  } else if (valid) {
+    const unsigned int z0 = P.colptr[j], z1 = P.colptr[j + 1];
+    bool started = false;
+    for (unsigned int z = z0; z < z1; ++z) {
+      const unsigned int kb = P.rowidx[z];
+      if (kb >= (unsigned int)(P.K / P.bk)) continue;     // block-row outside A: ignored (uniform over the CTA)
+      // every warp has passed its wait_group after the MMAs that read this buffer two blocks ago (or the previous item's
+      // wait_group 0): only then may any warp overwrite it
+      __syncthreads();
+      stage_block(sbuf[buf], P.b_vals + (size_t)z * (P.bn * P.bk / 8), P.bn, P.bk);
+      xb_fence_proxy_async();
+      __syncthreads();
+      const long long kw0 = (long long)kb * (P.bk / 2);
+      const uint32_t sb = xb_smem_u32(sbuf[buf]);
+      xb_wgmma_fence();
+      for (int ks = 0; ks < ksteps; ++ks) {
+        uint32_t a[4];
 #pragma unroll
-    for (int jj = 0; jj < 32; ++jj) {
-      if (jj < 16 || ncol == 32) {
-        float acc = ((jj < 16) ? any0 : any1) ? __uint_as_float(v[jj]) : 0.0f;
-        if (!beta0) acc += __bfloat162float(dst[jj * M]);
-        dst[jj * M] = __float2bfloat16_rn(acc);
-      }
-    }
-  }
-}
-
-// all 32 columns present, whole warp valid, beta = 0: one conversion and one 2-byte store per value. The 32 lanes of a
-// store cover 64 contiguous bytes (two full sectors) of C_mb[n][0..31]; nothing depends on anything else, so the stores
-// stream out without the shuffle/select chains of the packed variant (which kept 8 epilogue warps busy 80 % of the time)
-template <int M>
-__device__ __forceinline__ void bcsc_store_chunk_fast(const uint32_t (&v)[32], __nv_bfloat16* dst) {
+        for (int r = 0; r < 4; ++r) a[r] = avalid[r & 1] ? __ldg(arow[r & 1] + (kw0 + 8 * ks + q + 4 * (r >> 1)) * P.M) : 0u;
+        const int scale_d = (started || ks > 0) ? 1 : 0;
 #pragma unroll
-  for (int jj = 0; jj < 32; ++jj) dst[jj * M] = __float2bfloat16_rn(__uint_as_float(v[jj]));
-}
-__device__ __forceinline__ void tmem_ld32_nowait(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-               "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-               "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-                 "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-                 "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-                 "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-               : "r"(taddr) : "memory");
-}
-
-// ---- round-1 kernel: A converted to the canonical shared-memory operand (SS-form MMA) ---------------------------------------
-// Pipeline per CTA (persistent, one per SM, 22 warps): warp 0 A producer (TMA 3-D box of raw VNNI words), warp 2 B producer,
-// warps 12-19 converters (VNNI2 words -> two k-rows of the canonical MN-major SWIZZLE_128B operand, fence.proxy.async),
-// warps 1,3,20,21 MMA issuers (each OWNS a range of block-columns), warps 4-11 epilogue. A work item is (group, <=256-column
-// part); A is re-read (from L2) for the second part. Measured 0.39 of the HBM roofline on BASELINE configs[3].
-constexpr int kThreads = 704, kConvWarps = 8;      // 22 warps: A prod, B prod, 4 MMA, 8 epilogue, 8 converters
-constexpr int kMaxStages = 16, kMaxSlots = 4, kMaxEntries = 2048, kMaxLists = 512;
-constexpr int A_STAGE = 128 * 64 * 2;               // bytes of one k-step of A (raw or canonical): 128 rows x 64 k
-
-template <int M>
-__global__ void __launch_bounds__(kThreads, 1)
-bcsc_tc_kernel(const __grid_constant__ CUtensorMap map_a, const BcscTcParams P) {
-  pdl_wait();
-  constexpr int G = 128 / M;                       // m_blocks per group
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-  // carve: canonical A ring | raw A ring | B ring | operations | list pointers | per-warp ranges | col flags | barriers | tmem word
-  uint8_t* s_can = smem;
-  uint8_t* s_raw = s_can + (size_t)P.can_stages * A_STAGE;
-  uint8_t* s_b = s_raw + (size_t)P.raw_stages * A_STAGE;
-  uint4* s_ops = (uint4*)(s_b + (size_t)P.b_stages * P.b_stage_bytes);
-  unsigned int* s_lp = (unsigned int*)(s_ops + kMaxEntries + 1);       // +1: the MMA loop reads one operation ahead
-  unsigned int* s_wr = s_lp + kMaxLists + 8;
-  unsigned char* s_any = (unsigned char*)(s_wr + 4 * kMaxLists);
-  uint64_t* bars = (uint64_t*)(s_any + 1024);
-  const uint32_t bar0 = smem_u32(bars);
-  const int RS = P.raw_stages, CS = P.can_stages, BS = P.b_stages, NS = P.nslot;
-  const uint32_t raw_full = bar0, raw_empty = raw_full + 8 * kMaxStages, can_full = raw_empty + 8 * kMaxStages, can_empty = can_full + 8 * kMaxStages;
-  const uint32_t b_full = can_empty + 8 * kMaxStages, b_empty = b_full + 8 * kMaxStages;
-  const uint32_t t_full = b_empty + 8 * kMaxStages, t_empty = t_full + 8 * kMaxSlots;
-  uint32_t* tmem_word = (uint32_t*)(bars + 6 * kMaxStages + 2 * kMaxSlots);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const long long Gd = gridDim.x, bid = blockIdx.x;
-  const int NP = P.nparts, NKS = P.nks, NL = P.nparts * P.nks;
-  // work items of this CTA: its groups, each as NP consecutive column parts (the second read of A hits L2)
-  const long long n_local = ((bid < P.ngroups) ? (P.ngroups - bid + Gd - 1) / Gd : 0) * NP;
-  const uint32_t blk_bytes = (uint32_t)P.bn * P.bk * 2;
-
-  {
-    const unsigned int nnzb = P.list_ptr[NL];
-    for (unsigned int i = threadIdx.x; i < nnzb; i += blockDim.x) s_ops[i] = P.ops[i];      // #operations <= #blocks
-    for (int i = threadIdx.x; i < 4 * NL; i += blockDim.x) s_wr[i] = P.wranges[i];
-    for (int i = threadIdx.x; i <= NL; i += blockDim.x) s_lp[i] = P.list_ptr[i];
-    for (int i = threadIdx.x; i < P.nbc; i += blockDim.x) s_any[i] = (unsigned char)P.col_any[i];
-  }
-  if (threadIdx.x == 0) {
-    asm volatile("prefetch.tensormap [%0];" :: "l"(&map_a) : "memory");
-    for (int i = 0; i < RS; ++i) { mbar_init(raw_full + 8 * i, 1); mbar_init(raw_empty + 8 * i, kConvWarps); }
-    for (int i = 0; i < CS; ++i) { mbar_init(can_full + 8 * i, kConvWarps); mbar_init(can_empty + 8 * i, (uint32_t)P.mma_warps); }
-    for (int i = 0; i < BS; ++i) { mbar_init(b_full + 8 * i, 1u); mbar_init(b_empty + 8 * i, (uint32_t)P.mma_warps); }
-    for (int i = 0; i < NS; ++i) { mbar_init(t_full + 8 * i, (uint32_t)P.mma_warps); mbar_init(t_empty + 8 * i, 8); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" :: "r"(smem_u32(tmem_word)), "r"(512u) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_word;
-
-  if (warp == 0) {
-    // ========================================= A producer =======================================
-    if (lane == 0) {
-      int rs = 0; uint32_t rph = 0;
-      for (long long i = 0; i < n_local; ++i) {
-        const long long grp = bid + (i / NP) * Gd;
-        for (int ks = 0; ks < NKS; ++ks) {
-          mbar_wait(raw_empty + 8 * rs, rph ^ 1);
-          mbar_expect_tx(raw_full + 8 * rs, (uint32_t)A_STAGE);     // rows beyond K are zero-filled by the TMA unit
-          asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];"
-                       :: "r"(smem_u32(s_raw + (size_t)rs * A_STAGE)), "l"(&map_a), "r"(0), "r"(ks * 32), "r"((int)(grp * G)),
-                          "r"(raw_full + 8 * rs) : "memory");
-          if (++rs == RS) { rs = 0; rph ^= 1; }
-        }
+        for (int c = 0; c < NCH; ++c)
+          mma_rs<NC>(acc[c], a, xb_wg_desc(sb + (uint32_t)((c * NC / 8) * sbo + ks * 256), 128, (uint32_t)sbo, 0), scale_d);
       }
+      xb_wgmma_commit();
+      xb_wgmma_wait<1>();             // this thread's previous group (the other buffer) retired
+      started = true;
+      buf ^= 1;
     }
-  } else if (warp == 2) {
-    // ========================================= B producer =======================================
-    if (lane == 0) {
-      int bs = 0; uint32_t bph = 0;
-      for (long long i = 0; i < n_local; ++i) {
-        const int l0 = (int)(i % NP) * NKS;
-        for (int ks = 0; ks < NKS; ++ks) {
-          const unsigned int e0 = s_lp[l0 + ks], e1 = s_lp[l0 + ks + 1];
-          mbar_wait(b_empty + 8 * bs, bph ^ 1);
-          mbar_expect_tx(b_full + 8 * bs, (e1 - e0) * blk_bytes);     // zero blocks: the barrier completes at once
-          if (e1 > e0) {
-            asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                         :: "r"(smem_u32(s_b + (size_t)bs * P.b_stage_bytes)), "l"(P.b_packed + (size_t)e0 * blk_bytes), "r"((e1 - e0) * blk_bytes),
-                            "r"(b_full + 8 * bs) : "memory");
-          }
-          if (++bs == BS) { bs = 0; bph ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1 || (warp == 3 && P.mma_warps >= 2) || (warp >= 20 && warp - 18 < P.mma_warps)) {
-    // ========================================= MMA issuers ======================================
-    // The whole warp runs the loop (warp-uniform control flow keeps descriptor arithmetic on the uniform datapath);
-    // one elected lane issues the tcgen05 instructions.
-    uint32_t leader;
-    asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(leader));
-    const int mw = (warp == 1) ? 0 : ((warp == 3) ? 1 : warp - 18);
-    int cs = 0, bs = 0; uint32_t cph = 0, bph = 0;
-    const uint32_t a_hi = desc_hi(1024 >> 4, 2), b_hi = desc_hi(P.b_sbo16, P.b_layout);
-    const uint32_t a_lo0 = desc_lo(smem_u32(s_can), (uint32_t)(64 * 128) >> 4);   // MN-major SW128: LBO = distance of the two 64-row atoms
-    const uint32_t b_lo0 = desc_lo(smem_u32(s_b), 1);
-    const int ksteps = P.ksteps;
-    for (long long i = 0; i < n_local; ++i) {
-      const int slot = (int)(i % NS);
-      mbar_wait(t_empty + 8 * slot, (uint32_t)(((i / NS) & 1) ^ 1));
-      tc_fence_after();
-      const uint32_t d_base = tmem_base + (uint32_t)(slot * P.slot_cols);
-      const int l0 = (int)(i % NP) * NKS;
-      for (int ks = 0; ks < NKS; ++ks) {
-        const unsigned int rng = s_wr[4 * (l0 + ks) + mw], ob = rng & 0xFFFFu, on = rng >> 16;   // this warp's operations of the k-step
-        uint4 op = s_ops[ob];                                          // fetched ahead of the waits (a stale/unused slot is harmless)
-        mbar_wait(can_full + 8 * cs, cph);
-        mbar_wait(b_full + 8 * bs, bph);
-        tc_fence_after();
-        const uint32_t a_lo = a_lo0 + (uint32_t)cs * (A_STAGE >> 4);
-        const uint32_t b_stage_lo = b_lo0 + (uint32_t)bs * ((uint32_t)P.b_stage_bytes >> 4);
-        for (unsigned int o = 0; o < on; ++o) {
-          const uint4 nxt = s_ops[ob + o + 1];
-          const uint32_t d = d_base + (op.x & 0xFFFFu), a_op = a_lo + (op.x >> 16), b_lo = b_stage_lo + op.y, idesc = P.idesc | op.z;
-          uint32_t accumulate = op.w;
-          for (int kk = 0; kk < ksteps; ++kk) {
-            if (leader) umma_f16(d, desc64(a_hi, a_op + kk * (2048 >> 4)), desc64(b_hi, b_lo + kk * (32 >> 4)), idesc, accumulate);
-            accumulate = 1;
-          }
-          op = nxt;
-        }
-        if (leader) { umma_commit(can_empty + 8 * cs); umma_commit(b_empty + 8 * bs); }
-        __syncwarp();
-        if (++cs == CS) { cs = 0; cph ^= 1; }
-        if (++bs == BS) { bs = 0; bph ^= 1; }
-      }
-      if (leader) umma_commit(t_full + 8 * slot);
-      __syncwarp();
-    }
-  } else if (warp >= 4 && warp < 12) {
-    // ========================================= epilogue (8 warps: two per TMEM quadrant, half the columns each) =====
-    const int q = warp & 3, half = (warp - 4) >> 2;
-    const int row = 32 * q + lane;                       // row of the 128-row group
-    const int mbl = row / M, m = row % M;
-    const bool bn32 = (P.bn % 32) == 0;
-    for (long long i = 0; i < n_local; ++i) {
-      const int slot = (int)(i % NS);
-      const long long grp = bid + (i / NP) * Gd;
-      const long long mb = grp * G + mbl;
-      const bool valid = mb < P.m_blocks;
-      const int part = (int)(i % NP), pc0 = part * P.part_cols;                      // first column of this part
-      const int pcols = (P.ncols - pc0 < P.part_cols) ? (P.ncols - pc0) : P.part_cols;
-      const int nchunks = (pcols + 31) / 32, cbeg = half ? (nchunks + 1) / 2 : 0, cend = half ? nchunks : (nchunks + 1) / 2;
-      __nv_bfloat16* cblk = reinterpret_cast<__nv_bfloat16*>(P.c) + ((size_t)mb * P.ncols + pc0) * M + m;
-      mbar_wait(t_full + 8 * slot, (uint32_t)((i / NS) & 1));
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + (uint32_t)(slot * P.slot_cols) + ((uint32_t)(q * 32) << 16);
-      if (cbeg == cend) { tc_fence_before(); __syncwarp(); if (lane == 0) mbar_arrive(t_empty + 8 * slot); }
-      for (int ch = cbeg; ch < cend; ++ch) {
-        const int c0 = ch * 32;
-        uint32_t v[32];
-        tmem_ld32(taddr + (uint32_t)c0, v);
-        if (ch + 1 == cend) { tc_fence_before(); __syncwarp(); if (lane == 0) mbar_arrive(t_empty + 8 * slot); }
-        const int ncol = (pcols - c0 < 32) ? (pcols - c0) : 32;              // 16 or 32 (bn is a multiple of 16)
-        const int jb = (pc0 + c0) / P.bn;
-        const bool any0 = s_any[jb] != 0, any1 = bn32 ? any0 : (s_any[(pc0 + c0 + 16) / P.bn < P.nbc ? (pc0 + c0 + 16) / P.bn : jb] != 0);
-        bcsc_store_chunk<M>(v, cblk + (size_t)c0 * M, ncol, any0, any1, valid, P.beta0, lane);
-      }
-    }
-  } else if (warp >= 12 && warp < 12 + kConvWarps) {
-    // ========================================= converters =======================================
-    // One work unit = 4 consecutive rows (m) of one k-pair: a 16-byte read of VNNI words, two 8-byte writes (rows k, k+1 of
-    // the canonical operand). Lanes 0-15 of a half-warp take the 16 units of ONE (k-pair, 64-row atom).
-    const int cw = warp - 12, q = lane & 15, kp_lo = lane >> 4;
-    int rs = 0, cs = 0; uint32_t rph = 0, cph = 0;
-    for (long long i = 0; i < n_local; ++i) {
-      for (int ks = 0; ks < NKS; ++ks) {
-        mbar_wait(raw_full + 8 * rs, rph);
-        mbar_wait(can_empty + 8 * cs, cph ^ 1);
-        const uint8_t* src = s_raw + (size_t)rs * A_STAGE;
-        uint8_t* dst = s_can + (size_t)cs * A_STAGE;
+    xb_wgmma_wait<0>();
+    if (!started) {
 #pragma unroll
-        for (int it = 0; it < 32 / kConvWarps; ++it) {
-          const int idx = cw * (32 / kConvWarps) + it;          // 0..31: (atom, pair of k-pairs)
-          const int atom = idx & 1, kp = (idx >> 1) * 2 + kp_lo;
-          const int mrow = atom * 64 + 4 * q, g = mrow / M, mm = mrow % M;
-          const uint4 w = *reinterpret_cast<const uint4*>(src + ((size_t)(g * 32 + kp) * M + mm) * 4);
-          uint2 ev, od;
-          ev.x = __byte_perm(w.x, w.y, 0x5410); ev.y = __byte_perm(w.z, w.w, 0x5410);
-          od.x = __byte_perm(w.x, w.y, 0x7632); od.y = __byte_perm(w.z, w.w, 0x7632);
-          uint8_t* base = dst + (size_t)atom * (64 * 128);
-          const int k0 = 2 * kp, k1 = 2 * kp + 1, ch = q >> 1, sub = (q & 1) << 3;
-          *reinterpret_cast<uint2*>(base + k0 * 128 + ((ch ^ (k0 & 7)) << 4) + sub) = ev;
-          *reinterpret_cast<uint2*>(base + k1 * 128 + ((ch ^ (k1 & 7)) << 4) + sub) = od;
-        }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy stores -> visible to the tensor core (async proxy)
-        __syncwarp();
-        if (lane == 0) { mbar_arrive(can_full + 8 * cs); mbar_arrive(raw_empty + 8 * rs); }
-        if (++rs == RS) { rs = 0; rph ^= 1; }
-        if (++cs == CS) { cs = 0; cph ^= 1; }
-      }
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" :: "r"(tmem_base), "r"(512u) : "memory");
-  }
-}
-
-// ---- main kernel: the A operand lives in tensor memory (TS-form MMA) ---------------------------------------------------------
-constexpr int kTsThreads = 960;      // 30 warps: A producer, B producer, 4 MMA issuers, 4 copy, 16 epilogue (one 32-column chunk each), 4 more MMA issuers (k-major sweep)
-constexpr int kTsDCols = 128;        // accumulator columns per column part (two slots: TMEM columns 0..255)
-constexpr int kTsACol0 = 256;        // A operand: TMEM columns 256..511, 32 per k-step of 64
-constexpr int kTsMaxKS = 8;          // => K <= 512
-
-struct BcscTsParams {
-  int bn, bk, nbc, nks, ksteps;             // nks: 64-wide k-steps, ksteps = bk / 16
-  long long m_blocks, ngroups;
-  int ncols, nparts, part_cols;             // N = nbc*bn; column parts of part_cols (<= 128) columns
-  int kpc, nchunks;                         // k-steps per B stage, B stages per part = ceil(nks / kpc)
-  int raw_stages, b_stages, b_stage_bytes;
-  const unsigned int* list_ptr;             // [nparts*nks + 1] first block of every (part, k-step) list
-  const unsigned int* wranges;              // [4 * lists] {first op | count << 16} per MMA warp (owner of a range of block-columns)
-  int mma_warps;
-  const uint4* ops;                         // {d col | A byte offset/16 inside the k-step << 16, B offset/16 inside the list, idesc N bits, accumulate}
-  const unsigned int* col_any;              // [nbc] column has at least one block
-  const char* b_packed;
-  int ops_cap;
-  const unsigned int* plan;                 // {S, parts per set} from the prep kernel (S = 0: stream B)
-  int ring_bytes;                           // shared memory available for the A ring + B (resident set or ring)
-  int raw_cap;                              // upper bound on A stages (tuning)
-  int kmajor;                               // resident sets of <= 2 parts: sweep k-major (tuning switch, same result)
-  char* c; int beta0;
-  uint32_t idesc, b_layout, b_sbo16;
-};
-
-__device__ __forceinline__ void umma_f16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-               :: "r"(d_tmem), "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(accumulate));
-}
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&v)[32]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-               "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-               "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-               :: "r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]),
-                  "r"(v[8]), "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]),
-                  "r"(v[16]), "r"(v[17]), "r"(v[18]), "r"(v[19]), "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]),
-                  "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]), "r"(v[28]), "r"(v[29]), "r"(v[30]), "r"(v[31]) : "memory");
-  asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-}
-
-__device__ __forceinline__ uint4 lds128(uint32_t addr) {
-  uint4 v;
-  asm("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr));
-  return v;
-}
-__device__ __forceinline__ uint32_t lds32(uint32_t addr) { uint32_t v; asm("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(addr)); return v; }
-
-// KSTEPS = bk / 16: tcgen05.mma instructions per block (compile-time so that the issue loop is straight-line code)
-//
-// Two ways of feeding B, chosen ON THE DEVICE from the plan the prep kernel left in the header (the host cannot know the
-// per-part block counts of a device-resident pattern):
-//   resident (plan S >= 1): the column parts are cut into S sets; CTA c serves set c % S of the groups c / S, c / S + grid / S, ...
-//             and loads the packed B blocks of its set ONCE. S CTAs read the same A (the second read hits L2). No B ring,
-//             no per-chunk hand-over: per group only the 8 A k-steps and the accumulator slots are handed over.
-//   streamed (plan S == 0): every CTA sweeps all parts of its groups and streams B per (part, k-chunk) through a ring.
-template <int M, int KSTEPS>
-__global__ void __launch_bounds__(kTsThreads, 1)
-bcsc_ts_kernel(const __grid_constant__ CUtensorMap map_a, const BcscTsParams P) {
-  constexpr int G = 128 / M;                       // m_blocks per group
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-  const int NP = P.nparts, NKS = P.nks, NL = NP * NKS;
-  const uint32_t blk_bytes = (uint32_t)P.bn * P.bk * 2;
-  const long long Gd = gridDim.x, bid = blockIdx.x;
-
-  if (threadIdx.x == 0) asm volatile("prefetch.tensormap [%0];" :: "l"(&map_a) : "memory");
-  pdl_wait();                                          // plan, operation lists and packed B come from the two kernels in front
-  // ---- mode and work assignment (uniform per CTA) ----
-  const int S = (int)P.plan[0];
-  const bool resident = S > 0;
-  const int pps = resident ? (int)P.plan[1] : NP;
-  const int set = resident ? (int)(bid % S) : 0;
-  const int p0 = set * pps, p1 = (p0 + pps < NP) ? p0 + pps : NP;          // parts of this CTA
-  const long long lanes = resident ? Gd / S : Gd;                            // CTAs sharing the group axis
-  const long long lane_id = resident ? bid / S : bid;
-  const long long n_groups = (lane_id < lanes && lane_id < P.ngroups) ? (P.ngroups - lane_id + lanes - 1) / lanes : 0;
-  const uint32_t e_set0 = P.list_ptr[p0 * NKS], e_set1 = P.list_ptr[p1 * NKS];
-  const uint32_t b_region = resident ? (((e_set1 - e_set0) * blk_bytes + 1023u) & ~1023u) : (uint32_t)(P.b_stages * P.b_stage_bytes);
-  int RS = resident ? (int)(((uint32_t)P.ring_bytes - b_region) / (uint32_t)A_STAGE) : P.raw_stages;
-  RS = (RS > P.raw_cap) ? P.raw_cap : RS; RS = (RS > 8) ? 8 : RS;
-  const int BS = resident ? 1 : P.b_stages, KPC = resident ? NKS : P.kpc, NCH = resident ? 1 : P.nchunks;
-
-  // carve: B (resident set or ring) | raw A ring | operations | list pointers | op ranges | col flags | barriers | tmem word
-  uint8_t* s_b = smem;
-  uint8_t* s_raw = s_b + b_region;
-  uint4* s_ops = (uint4*)(smem + P.ring_bytes);
-  unsigned int* s_lp = (unsigned int*)(s_ops + P.ops_cap + 1);
-  unsigned int* s_wr = s_lp + NL + 1;
-  unsigned char* s_any = (unsigned char*)(s_wr + 4 * NL);
-  uint64_t* bars = (uint64_t*)(((uintptr_t)(s_any + P.nbc) + 15) & ~(uintptr_t)15);
-  const uint32_t bar0 = smem_u32(bars);
-  const uint32_t raw_full = bar0, raw_empty = raw_full + 8 * 8, a_full = raw_empty + 8 * 8, a_empty = a_full + 8 * kTsMaxKS;
-  const uint32_t b_full = a_empty + 8 * kTsMaxKS, b_empty = b_full + 8 * 8, t_full = b_empty + 8 * 8, t_empty = t_full + 8 * 2;
-  uint32_t* tmem_word = (uint32_t*)(bars + 4 * 8 + 2 * kTsMaxKS + 4);
-  uint32_t* s_fcnt = tmem_word + 1;                                        // [8] records per MMA warp (flat lists)
-  uint4* s_flat = (uint4*)(((uintptr_t)(s_fcnt + 8) + 15) & ~(uintptr_t)15);   // [ops_cap + 8*NKS + 8] flat records
-  const bool flat = resident && P.kmajor && (p1 - p0) == 2;     // one part per CTA: the part-major loop is already k-major
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-
-  {
-    const unsigned int nops = P.list_ptr[NL];            // #operations <= #blocks
-    for (unsigned int i = threadIdx.x; i < nops && i < (unsigned int)P.ops_cap; i += blockDim.x) s_ops[i] = P.ops[i];
-    for (int i = threadIdx.x; i < 4 * NL; i += blockDim.x) s_wr[i] = P.wranges[i];
-    for (int i = threadIdx.x; i <= NL; i += blockDim.x) s_lp[i] = P.list_ptr[i];
-    for (int i = threadIdx.x; i < P.nbc; i += blockDim.x) s_any[i] = (unsigned char)P.col_any[i];
-  }
-  if (threadIdx.x == 0) {
-    asm volatile("prefetch.tensormap [%0];" :: "l"(&map_a) : "memory");
-    for (int i = 0; i < RS; ++i) { mbar_init(raw_full + 8 * i, 1); mbar_init(raw_empty + 8 * i, 4); }
-    for (int i = 0; i < NKS; ++i) { mbar_init(a_full + 8 * i, 4); mbar_init(a_empty + 8 * i, (uint32_t)(flat ? 2 * P.mma_warps : P.mma_warps)); }
-    for (int i = 0; i < BS; ++i) { mbar_init(b_full + 8 * i, 1); mbar_init(b_empty + 8 * i, (uint32_t)P.mma_warps); }
-    for (int i = 0; i < 2; ++i) { mbar_init(t_full + 8 * i, (uint32_t)P.mma_warps); mbar_init(t_empty + 8 * i, 16); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" :: "r"(smem_u32(tmem_word)), "r"(512u) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_word;
-  const uint32_t tmem_a = tmem_base + (uint32_t)kTsACol0;
-
-  // ---- flat per-warp operation lists (resident B, k-major sweep) ----------------------------------------------------------
-  // Everything an instruction needs is known once the CTA knows its set: accumulator column (part q lives in slot q),
-  // A columns of the k-step, descriptor of the resident B block. So each MMA warp gets ONE list for a whole group, in issue
-  // order, with absolute operands {D address, A address | accumulate << 31, B descriptor low word, instruction descriptor};
-  // a record with w == 0 ends a k-step (commit a_empty). The issue loop is then one 16-byte shared load per operation.
-  // In this mode EIGHT warps issue: warps 2..5 own part p0 (slot 0), warps 26..29 part p0+1 (slot 1), each one block-column
-  // range of its part -- the issue loop of one thread (~30 instructions per operation), not the tensor pipe, bounds the
-  // sweep (measured: tensor pipe 25 % active with four issuers), and accumulator columns stay owned by one thread.
-  const int MW = P.mma_warps;
-  const bool issuer = (warp >= 2 && warp < 2 + MW) || (flat && warp >= 26 && warp < 26 + MW);
-  const int mw = (warp >= 26) ? MW + (warp - 26) : warp - 2;            // issuer index; flat: part = mw / MW, column range = mw % MW
-  if (flat) {
-    const uint32_t blk16f = blk_bytes >> 4, b_lo_base = desc_lo(smem_u32(s_b), 1);
-    const int q = mw / MW, ww = mw % MW;
-    if (issuer && lane == 0) {
-      uint32_t n = 0;
-      for (int ks = 0; ks < NKS; ++ks) n += s_wr[4 * ((p0 + q) * NKS + ks) + ww] >> 16;
-      s_fcnt[mw] = n + (uint32_t)NKS;
-    }
-    __syncthreads();
-    if (issuer && lane == 0) {
-      uint32_t off = 0;
-      for (int w = 0; w < mw; ++w) off += s_fcnt[w];
-      uint4* out = s_flat + off;
-      for (int ks = 0; ks < NKS; ++ks) {
-        const uint32_t l = (uint32_t)((p0 + q) * NKS + ks);
-        const uint32_t rng = s_wr[4 * l + ww], ob = rng & 0xFFFFu, on = rng >> 16;
-        const uint32_t b_list_lo = b_lo_base + (s_lp[l] - e_set0) * blk16f;
-        for (uint32_t o = 0; o < on; ++o) {
-          const uint4 op = s_ops[ob + o];
-          *out++ = make_uint4(tmem_base + (uint32_t)(q * kTsDCols) + (op.x & 0xFFFFu),
-                              (tmem_a + (uint32_t)ks * 32u + (op.x >> 20)) | (op.w << 31), b_list_lo + op.y, P.idesc | op.z);
-        }
-        *out++ = make_uint4(0u, 0u, 0u, 0u);
-      }
-    }
-    __syncthreads();
-  }
-
-  if (warp == 0) {
-    // ========================================= A producer =======================================
-    if (lane == 0) {
-      int rs = 0; uint32_t rph = 0;
-      for (long long i = 0; i < n_groups; ++i) {
-        const long long grp = lane_id + i * lanes;
-        for (int ks = 0; ks < NKS; ++ks) {
-          mbar_wait(raw_empty + 8 * rs, rph ^ 1);
-          mbar_expect_tx(raw_full + 8 * rs, (uint32_t)A_STAGE);     // k-pairs beyond K and m_blocks beyond the end are zero-filled
-          asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];"
-                       :: "r"(smem_u32(s_raw + (size_t)rs * A_STAGE)), "l"(&map_a), "r"(0), "r"(ks * 32), "r"((int)(grp * G)),
-                          "r"(raw_full + 8 * rs) : "memory");
-          if (++rs == RS) { rs = 0; rph ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ========================================= B producer =======================================
-    if (lane == 0 && n_groups > 0) {
-      if (resident) {
-        // the whole set once: bulk copies of <= 32 KB on one barrier
-        const uint32_t total = (e_set1 - e_set0) * blk_bytes;
-        mbar_expect_tx(b_full, total);
-        for (uint32_t off = 0; off < total; off += 32768u) {
-          const uint32_t n = (total - off < 32768u) ? (total - off) : 32768u;
-          asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                       :: "r"(smem_u32(s_b) + off), "l"(P.b_packed + (size_t)e_set0 * blk_bytes + off), "r"(n), "r"(b_full) : "memory");
-        }
-      } else {
-        int bs = 0; uint32_t bph = 0;
-        for (long long i = 0; i < n_groups; ++i) {
-          for (int part = p0; part < p1; ++part) {
-            for (int ch = 0; ch < NCH; ++ch) {
-              const int l0 = part * NKS + ch * KPC, l1 = (ch * KPC + KPC < NKS) ? l0 + KPC : part * NKS + NKS;
-              const unsigned int e0 = s_lp[l0], e1 = s_lp[l1];
-              mbar_wait(b_empty + 8 * bs, bph ^ 1);
-              mbar_expect_tx(b_full + 8 * bs, (e1 - e0) * blk_bytes);     // zero blocks: the barrier completes at once
-              if (e1 > e0) {
-                asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                             :: "r"(smem_u32(s_b + (size_t)bs * P.b_stage_bytes)), "l"(P.b_packed + (size_t)e0 * blk_bytes), "r"((e1 - e0) * blk_bytes),
-                                "r"(b_full + 8 * bs) : "memory");
-              }
-              if (++bs == BS) { bs = 0; bph ^= 1; }
-            }
-          }
-        }
-      }
-    }
-  } else if (issuer) {
-    // ========================================= MMA issuers ======================================
-    // Each warp OWNS a range of block-columns of every part (lists are stored owner-major by the prep kernel), so every
-    // accumulator column is written by one thread in k order. The whole warp runs the loop (warp-uniform control flow);
-    // one elected lane issues. Operations are fetched one ahead with explicit shared-memory loads: the issue loop of a
-    // single thread, not the tensor pipe, bounds this kernel when it carries avoidable latency (256 instructions of 16
-    // cycles per group against ~100 cycles per operation in the first version).
-    uint32_t leader;
-    asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(leader));
-    int bs = 0; uint32_t bph = 0;
-    const uint32_t b_hi = desc_hi(P.b_sbo16, P.b_layout);
-    const uint32_t b_lo0 = desc_lo(smem_u32(s_b), 1);
-    const uint32_t blk16 = blk_bytes >> 4;
-    const uint32_t ops_sa = smem_u32(s_ops), lp_sa = smem_u32(s_lp), wr_sa = smem_u32(s_wr) + 4u * (uint32_t)mw;
-    long long item = 0;
-    if (resident && n_groups > 0) mbar_wait(b_full, 0);                    // the set's B blocks have landed (once per launch)
-    // all operations of one (part, k-step) list owned by this warp
-    auto issue_list = [&](uint32_t l, uint32_t d_base, uint32_t b_stage_lo, uint32_t e0, int ks) {
-      const uint32_t rng = lds32(wr_sa + 16u * l), ob = rng & 0xFFFFu, on = rng >> 16;
-      const uint32_t b_list_lo = b_stage_lo + (lds32(lp_sa + 4u * l) - e0) * blk16;
-      const uint32_t a_ks = tmem_a + (uint32_t)ks * 32u;
-      uint32_t op_sa = ops_sa + 16u * ob;
-      uint4 op = lds128(op_sa);
-      for (uint32_t o = 0; o < on; ++o) {
-        op_sa += 16u;
-        const uint4 nxt = lds128(op_sa);                          // one past the last operation is allocated
-        const uint32_t d = d_base + (op.x & 0xFFFFu), a_col = a_ks + (op.x >> 20), b_lo = b_list_lo + op.y, idesc = P.idesc | op.z;
-        if (leader) {
-          umma_f16_ts(d, a_col, desc64(b_hi, b_lo), idesc, op.w);
+      for (int c = 0; c < NCH; ++c)
 #pragma unroll
-          for (int kk = 1; kk < KSTEPS; ++kk) umma_f16_ts(d, a_col + (uint32_t)kk * 8u, desc64(b_hi, b_lo + (uint32_t)kk * (32u >> 4)), idesc, 1u);
-        }
-        op = nxt;
-      }
-    };
-    if (flat) {
-      // k-major sweep: both parts of the set accumulate side by side in the two slots, so the A columns of a k-step are
-      // released as soon as that k-step is consumed and the copy warps refill them for the NEXT group while this group's
-      // later k-steps are still being multiplied.
-      const int q = mw / MW;                                                    // this warp's part lives in slot q
-      uint32_t foff = 0;
-      for (int w = 0; w < mw; ++w) foff += s_fcnt[w];
-      const uint32_t flat_sa = smem_u32(s_flat) + 16u * foff;
-      for (long long i = 0; i < n_groups; ++i) {
-        const uint32_t gpar = (uint32_t)(i & 1);
-        uint32_t rec = flat_sa;
-        uint4 op = lds128(rec);
-        mbar_wait(t_empty + 8 * q, gpar ^ 1);
-        tc_fence_after();
-        for (int ks = 0; ks < NKS; ++ks) {
-          mbar_wait(a_full + 8 * ks, gpar);
-          tc_fence_after();
-          while (op.w != 0u) {
-            rec += 16u;
-            const uint4 nxt = lds128(rec);
-            if (leader) {
-              const uint32_t a_col = op.y & 0x7FFFFFFFu;
-              umma_f16_ts(op.x, a_col, desc64(b_hi, op.z), op.w, op.y >> 31);
+        for (int i = 0; i < NC / 2; ++i) acc[c][i] = 0.0f;
+    }
+    // C_mb[n][m]: the group's rows are not one column-major tile when M < 64, so every fragment row is resolved to its m_block
+    const long long ncols = (long long)P.nbc * P.bn;
+    const int r0 = 16 * wq + (lane >> 2), c0 = 2 * q;
 #pragma unroll
-              for (int kk = 1; kk < KSTEPS; ++kk) umma_f16_ts(op.x, a_col + (uint32_t)kk * 8u, desc64(b_hi, op.z + (uint32_t)kk * (32u >> 4)), op.w, 1u);
-            }
-            op = nxt;
-          }
-          rec += 16u;
-          op = lds128(rec);                                                      // first record of the next k-step (spare records are allocated)
-          if (leader) umma_commit(a_empty + 8 * ks);
-          __syncwarp();
-        }
-        if (leader) umma_commit(t_full + 8 * q);
-        __syncwarp();
-      }
-    } else {
-    for (long long i = 0; i < n_groups; ++i) {
-      const uint32_t gpar = (uint32_t)(i & 1);
-      for (int part = p0; part < p1; ++part, ++item) {
-        const int slot = (int)(item & 1);
-        mbar_wait(t_empty + 8 * slot, (uint32_t)(((item >> 1) & 1) ^ 1));
-        tc_fence_after();
-        const uint32_t d_base = tmem_base + (uint32_t)(slot * kTsDCols);
-        for (int ch = 0; ch < NCH; ++ch) {
-          const int ks0 = ch * KPC, ks1 = (ks0 + KPC < NKS) ? ks0 + KPC : NKS;
-          const uint32_t e0 = resident ? e_set0 : lds32(lp_sa + 4u * (uint32_t)(part * NKS + ks0));
-          if (part == p0) { for (int ks = ks0; ks < ks1; ++ks) mbar_wait(a_full + 8 * ks, gpar); }   // this group's A k-steps are in TMEM
-          if (!resident) mbar_wait(b_full + 8 * bs, bph);
-          tc_fence_after();
-          const uint32_t b_stage_lo = b_lo0 + (uint32_t)bs * ((uint32_t)P.b_stage_bytes >> 4);
-          for (int ks = ks0; ks < ks1; ++ks) issue_list((uint32_t)(part * NKS + ks), d_base, b_stage_lo, e0, ks);
-          if (leader) {
-            if (!resident) umma_commit(b_empty + 8 * bs);
-            if (part == p1 - 1) { for (int ks = ks0; ks < ks1; ++ks) umma_commit(a_empty + 8 * ks); }   // last reader of these A columns
-          }
-          __syncwarp();
-          if (!resident && ++bs == BS) { bs = 0; bph ^= 1; }
-        }
-        if (leader) umma_commit(t_full + 8 * slot);
-        __syncwarp();
-      }
-    }
-    }
-  } else if (warp >= 6 && warp < 10) {
-    // ========================================= copy: raw VNNI words -> TMEM A ===================
-    // this warp owns rows 32q .. 32q+31 (its TMEM lane quadrant); lanes read consecutive words: conflict-free
-    const int q = warp & 3, mrow = 32 * q + lane, g = mrow / M, mm = mrow % M;
-    int rs = 0; uint32_t rph = 0;
-    for (long long i = 0; i < n_groups; ++i) {
-      const uint32_t gpar = (uint32_t)(i & 1);
-      for (int ks = 0; ks < NKS; ++ks) {
-        mbar_wait(raw_full + 8 * rs, rph);
-        mbar_wait(a_empty + 8 * ks, gpar ^ 1);            // the previous group's MMAs have consumed these columns
-        tc_fence_after();
-        const unsigned int* src = reinterpret_cast<const unsigned int*>(s_raw + (size_t)rs * A_STAGE) + (size_t)g * 32 * M + mm;
-        uint32_t w[32];
+    for (int c = 0; c < NCH; ++c) {
 #pragma unroll
-        for (int kp = 0; kp < 32; ++kp) w[kp] = src[(size_t)kp * M];
-        tmem_st32(tmem_a + (uint32_t)ks * 32u + ((uint32_t)(q * 32) << 16), w);
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) { mbar_arrive(a_full + 8 * ks); mbar_arrive(raw_empty + 8 * rs); }
-        if (++rs == RS) { rs = 0; rph ^= 1; }
+      for (int i = 0; i < NC / 2; ++i) {
+        const int col = c * NC + c0 + 8 * (i >> 2) + (i & 1), h = (i >> 1) & 1;
+        if (col >= P.bn || !avalid[h]) continue;
+        const long long R = grp * 64 + r0 + 8 * h, mb = R / P.M;
+        char* p = reinterpret_cast<char*>(P.c + (mb * ncols + (long long)j * P.bn + col) * P.M + (R - mb * P.M));
+        if (P.beta0) xb_ep_store_one<XB_EP_BF16, true>(__float_as_uint(acc[c][i]), p, 0.0f);
+        else xb_ep_store_one<XB_EP_BF16, false>(__float_as_uint(acc[c][i]), p, 0.0f);
       }
     }
-  } else if (warp >= 10 && warp < 26) {
-    // ========================================= epilogue (16 warps: four per TMEM quadrant, one 32-column chunk each) =====
-    const int q = warp & 3, cw = (warp - 10) >> 2;
-    const int row = 32 * q + lane;                       // row of the 128-row group
-    const int mbl = row / M, m = row % M;
-    const bool bn32 = (P.bn % 32) == 0;
-    long long item = 0;
-    for (long long i = 0; i < n_groups; ++i) {
-      const long long mb = (lane_id + i * lanes) * G + mbl;
-      const bool valid = mb < P.m_blocks;
-      for (int part = p0; part < p1; ++part, ++item) {
-        const int slot = (int)(item & 1);
-        const int pc0 = part * P.part_cols;                                        // first column of this part
-        const int pcols = (P.ncols - pc0 < P.part_cols) ? (P.ncols - pc0) : P.part_cols;
-        const int nchunks = (pcols + 31) / 32;                                     // <= 4 (part_cols <= 128)
-        const bool mine = cw < nchunks;
-        __nv_bfloat16* cblk = reinterpret_cast<__nv_bfloat16*>(P.c) + ((size_t)mb * P.ncols + pc0) * M + m;
-        mbar_wait(t_full + 8 * slot, (uint32_t)((item >> 1) & 1));
-        tc_fence_after();
-        const uint32_t taddr = tmem_base + (uint32_t)(slot * kTsDCols) + ((uint32_t)(q * 32) << 16);
-        // fetch the chunk, hand the accumulator slot back to the MMA warps at once, then convert and store from registers
-        uint32_t v[32];
-        if (mine) tmem_ld32_nowait(taddr + (uint32_t)(cw * 32), v);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        tc_fence_before(); __syncwarp();
-        if (lane == 0) mbar_arrive(t_empty + 8 * slot);
-        if (mine) {
-          const int c0 = cw * 32;
-          const int ncol = (pcols - c0 < 32) ? (pcols - c0) : 32;              // 16 or 32 (bn is a multiple of 16)
-          const int jb = (pc0 + c0) / P.bn;
-          const bool any0 = s_any[jb] != 0, any1 = bn32 ? any0 : (s_any[(pc0 + c0 + 16) / P.bn < P.nbc ? (pc0 + c0 + 16) / P.bn : jb] != 0);
-          const bool whole = __all_sync(0xffffffffu, valid) && P.beta0 != 0;
-          if (whole && any0 && any1 && ncol == 32) bcsc_store_chunk_fast<M>(v, cblk + (size_t)c0 * M);
-          else bcsc_store_chunk<M>(v, cblk + (size_t)c0 * M, ncol, any0, any1, valid, P.beta0, lane);
-        }
-      }
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" :: "r"(tmem_base), "r"(512u) : "memory");
   }
 }
-
-// ---- host side -------------------------------------------------------------------------------------------------------------------
-// Per-handle state. A call needs two scratch buffers that outlive the call on the device (the cached pattern / operation lists
-// and the re-packed B values). They are kept PER (device, stream): launches on one stream are ordered, so re-use is safe there,
-// while concurrent callers on different streams get different buffers. The three launches of a call are enqueued under the
-// handle's mutex, so two host threads sharing a stream cannot interleave them. Nothing in the handle's descriptor is mutated
-// by a call (the reference's handles are re-entrant, SURVEY.md 8b).
-int env_int(const char* name, int lo, int hi, int dflt);
-struct BcscBuffers { int device; cudaStream_t stream; unsigned int* idx; size_t idx_bytes; void* val; size_t val_bytes; };
-struct BcscState { std::mutex mu; std::vector<BcscBuffers> sets; };
-std::mutex g_state_mu;
 
 int device_sms() {
   static int sms[64] = {0};
   int dev = 0; cudaGetDevice(&dev);
-  if (dev < 0 || dev >= 64) return 148;
-  if (sms[dev] == 0) { int n = 0; cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev); sms[dev] = (n > 0) ? n : 148; }
+  if (dev < 0 || dev >= 64) return 132;
+  if (sms[dev] == 0) { int n = 0; cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev); sms[dev] = (n > 0) ? n : 132; }
   return sms[dev];
 }
 
-// MaxDynamicSharedMemorySize is a per-device function attribute: set it once per (kernel, device)
-template <typename K>
-void ensure_smem_attr(K kernel, int bytes, unsigned long long* done_mask) {
-  int dev = 0; cudaGetDevice(&dev);
-  if (dev < 0 || dev >= 64) { cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes); return; }
-  if (!((*done_mask >> dev) & 1ull)) { cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes); *done_mask |= (1ull << dev); }
-}
-
-template <int M>
-cudaError_t launch_v1(long long grid, size_t smem, cudaStream_t stream, const CUtensorMap& ma, const BcscTcParams& P) {
-  static unsigned long long done = 0;
-  ensure_smem_attr(bcsc_tc_kernel<M>, 227 * 1024, &done);
-  cudaLaunchConfig_t cfg; cudaLaunchAttribute attr[1];
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3((unsigned int)grid); cfg.blockDim = dim3(kThreads); cfg.dynamicSmemBytes = smem; cfg.stream = stream;
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization; attr[0].val.programmaticStreamSerializationAllowed = env_int("LIBXSMM_B200_BCSC_PDL", 0, 1, 0);
-  cfg.attrs = attr; cfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&cfg, bcsc_tc_kernel<M>, ma, P);
-}
-
-template <int M, int KSTEPS>
-cudaError_t launch_ts2(long long grid, size_t smem, cudaStream_t stream, const CUtensorMap& ma, const BcscTsParams& P) {
-  static unsigned long long done = 0;
-  ensure_smem_attr(bcsc_ts_kernel<M, KSTEPS>, 227 * 1024, &done);
-  cudaLaunchConfig_t cfg; cudaLaunchAttribute attr[1];
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3((unsigned int)grid); cfg.blockDim = dim3(kTsThreads); cfg.dynamicSmemBytes = smem; cfg.stream = stream;
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization; attr[0].val.programmaticStreamSerializationAllowed = env_int("LIBXSMM_B200_BCSC_PDL", 0, 1, 0);
-  cfg.attrs = attr; cfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&cfg, bcsc_ts_kernel<M, KSTEPS>, ma, P);
-}
-template <int M>
-cudaError_t launch_ts(long long grid, size_t smem, cudaStream_t stream, const CUtensorMap& ma, const BcscTsParams& P) {
-  return (P.ksteps == 1) ? launch_ts2<M, 1>(grid, smem, stream, ma, P) : ((P.ksteps == 2) ? launch_ts2<M, 2>(grid, smem, stream, ma, P)
-                                                                                           : launch_ts2<M, 4>(grid, smem, stream, ma, P));
-}
-
-int env_int(const char* name, int lo, int hi, int dflt) {
-  const char* e = getenv(name);
-  if (e == nullptr || *e == 0) return dflt;
-  const int v = atoi(e);
-  return (v < lo || v > hi) ? dflt : v;
+// MaxDynamicSharedMemorySize is a per-device function attribute: set it once per (instantiation, device)
+template <int NC, int NCH>
+cudaError_t launch(long long grid, size_t smem, cudaStream_t stream, const BcscParams& P) {
+  static unsigned long long done = 0ull;
+  if (xb_rt_first_use_on_device(&done)) cudaFuncSetAttribute(bcsc_wg_kernel<NC, NCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * NC * NCH * 64 * 2);
+  bcsc_wg_kernel<NC, NCH><<<(unsigned int)grid, 128, smem, stream>>>(P);
+  return cudaGetLastError();
 }
 
 }  // namespace
 
-extern "C" void xb_bcsc_state_free(void* work) {
-  BcscState* st = (BcscState*)work;
-  if (st == nullptr) return;
-  for (BcscBuffers& b : st->sets) {
-    int cur = 0; cudaGetDevice(&cur);
-    if (cur != b.device) cudaSetDevice(b.device);
-    cudaStreamSynchronize(b.stream);
-    cudaFree(b.idx); cudaFree(b.val);
-    if (cur != b.device) cudaSetDevice(cur);
-  }
-  (void)cudaGetLastError();
-  delete st;
-}
+// the kernel keeps no per-handle state: pattern and values are read as they arrive with every call
+extern "C" void xb_bcsc_state_free(void* work) { (void)work; }
 
-// which kernel a call with this geometry takes: 0 none (caller falls back to the exact-order kernel), 1 round-1 SS-form, 2 TS-form
+// which kernel a call with this geometry takes: 0 none (caller falls back to the exact-order kernel), 1 the wgmma kernel
 extern "C" int xb_bcsc_tc_variant(const xb_sparse_desc* d, unsigned long long n_blocks) {
   const unsigned int bad = LIBXSMM_GEMM_FLAG_TRANS_A | LIBXSMM_GEMM_FLAG_TRANS_B | LIBXSMM_GEMM_FLAG_VNNI_B;
   const int M = d->packed_width, K = d->k, bk = d->bk, bn = d->bn;
@@ -968,168 +159,33 @@ extern "C" int xb_bcsc_tc_variant(const xb_sparse_desc* d, unsigned long long n_
   if ((d->flags & bad) != 0 || (d->flags & LIBXSMM_GEMM_FLAG_VNNI_A) == 0) return 0;
   if (!(M == 16 || M == 32 || M == 64 || M == 128)) return 0;
   if (!(bk == 16 || bk == 32 || bk == 64) || (bn % 16) != 0 || bn > 256 || bn < 16 || K < 64 || (K % bk) != 0) return 0;
-  const int nkb = K / bk, nks = (K + 63) / 64;
-  if (n_blocks == 0 || nkb > 255 || n_blocks > 255 || n_blocks * (unsigned long long)nkb > 2047ull) return 0;
-  const bool ts_ok = nks <= kTsMaxKS && bn <= kTsDCols && (int)((n_blocks + (kTsDCols / bn) - 1) / (kTsDCols / bn)) * nks <= kMaxLists - 1;
-  if (ts_ok && env_int("LIBXSMM_B200_BCSC_V1", 0, 1, 0) == 0) return 2;
-  if ((long long)n_blocks * bn > 512) return 0;
+  if (n_blocks == 0 || n_blocks > 0x7fffffffull) return 0;
   return 1;
 }
 
-// returns 0 if launched, <0 if this descriptor/problem is not served by a tensor-core kernel (caller falls back)
+// returns 0 if launched, <0 if this descriptor/problem is not served by the tensor-core kernel (caller falls back)
 extern "C" int xb_bcsc_tc_launch(const xb_sparse_desc* d, void** work, const void* a, const void* b_vals, const unsigned int* colptr,
                                  const unsigned int* rowidx, unsigned long long n_blocks, unsigned int nnzb, void* c)
 {
-  const int variant = xb_bcsc_tc_variant(d, n_blocks);
-  if (variant == 0) return -1;
-  const int M = d->packed_width, K = d->k, bk = d->bk, bn = d->bn;
-  const long long ncols = (long long)n_blocks * bn;
-  const int nkb = K / bk, nks = (K + 63) / 64;
-  // nnzb == 0: unknown on the host (pattern lives in device memory): bound it by the dense block count; the kernels
-  // read the true count from the prep output
-  if (nnzb == 0) nnzb = (unsigned int)((unsigned long long)n_blocks * nkb < 2047ull ? n_blocks * nkb : 2047ull);
-  if (nnzb > 2047) return -1;
+  (void)work; (void)nnzb;
+  if (xb_bcsc_tc_variant(d, n_blocks) == 0) return -1;
   if ((((uintptr_t)a | (uintptr_t)b_vals | (uintptr_t)c) & 15) != 0) return -1;
-  xb_encode_tiled_fn enc = xb_tma_encoder();
-  if (enc == nullptr) return -1;
-  const int sms = device_sms();
+  BcscParams P; memset(&P, 0, sizeof(P));
+  P.M = d->packed_width; P.K = d->k; P.bk = d->bk; P.bn = d->bn; P.nbc = (int)n_blocks;
+  P.m_blocks = d->m; P.ngroups = (d->m * (long long)P.M + 63) / 64; P.items = P.ngroups * P.nbc;
+  P.a = (const uint32_t*)a; P.b_vals = (const uint4*)b_vals; P.colptr = colptr; P.rowidx = rowidx;
+  P.c = (unsigned short*)c; P.beta0 = d->beta0;
+  const int nt = P.bn <= 16 ? 16 : (P.bn <= 32 ? 32 : (P.bn <= 64 ? 64 : (P.bn <= 128 ? 128 : 256)));
+  long long grid = P.items; const long long cap = (long long)device_sms() * 8; if (grid > cap) grid = cap; if (grid < 1) grid = 1;
+  const size_t smem = 2 * (size_t)nt * P.bk * 2;
   cudaStream_t stream = (cudaStream_t)xb_rt_stream();
-  const int G = 128 / M, blk_bytes = bn * bk * 2;
-  const long long ngroups = (d->m + G - 1) / G;
-
-  // column parts: TS-form: <= 128 accumulator columns, two TMEM slots; round-1 kernel: <= 256 columns, so that the epilogue
-  // of one work item overlaps the MMAs of the next
-  int bpp, nparts, mma_warps;
-  if (variant == 2) { bpp = kTsDCols / bn; mma_warps = env_int("LIBXSMM_B200_BCSC_MMAW", 1, 4, 4); if (mma_warps > bpp) mma_warps = bpp; }
-  else { bpp = (ncols > 256) ? 256 / bn : (int)n_blocks; mma_warps = env_int("LIBXSMM_B200_BCSC_MMAW", 1, 4, 4); }
-  if (bpp > (int)n_blocks) bpp = (int)n_blocks;
-  nparts = ((int)n_blocks + bpp - 1) / bpp;
-  const int nl = nparts * nks;
-  if (nl > kMaxLists - 1) return -1;
-  const int cpw = (bpp + mma_warps - 1) / mma_warps;
-
-  CUtensorMap map_a;
-  {
-    const cuuint64_t dims[3] = {(cuuint64_t)M, (cuuint64_t)(K / 2), (cuuint64_t)d->m};
-    const cuuint64_t strides[2] = {(cuuint64_t)M * 4, (cuuint64_t)K * M * 2};
-    const cuuint32_t box[3] = {(cuuint32_t)M, 32u, (cuuint32_t)G};
-    const cuuint32_t estr[3] = {1, 1, 1};
-    if (CUDA_SUCCESS != enc(&map_a, CU_TENSOR_MAP_DATA_TYPE_UINT32, 3, (void*)a, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                            CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE)) return -1;
-  }
-
-  // shared-memory plans (decided before anything is enqueued so that an unsupported geometry can still fall back)
-  BcscTcParams P1; memset(&P1, 0, sizeof(P1));
-  BcscTsParams P2; memset(&P2, 0, sizeof(P2));
-  size_t smem = 0;
-  unsigned int resident_cap_blocks = 0;
-  if (variant == 2) {
-    P2.bn = bn; P2.bk = bk; P2.nbc = (int)n_blocks; P2.nks = nks; P2.ksteps = bk / 16;
-    P2.m_blocks = d->m; P2.ngroups = ngroups; P2.ncols = (int)ncols; P2.nparts = nparts; P2.part_cols = bpp * bn;
-    const int ks_bytes = bpp * (64 / bk) * blk_bytes;                 // worst case of one (part, k-step) list: every block present
-    int kpc = 1; while (kpc * 2 <= nks && ks_bytes * kpc * 2 <= 32 * 1024) kpc *= 2;
-    kpc = env_int("LIBXSMM_B200_BCSC_KPC", 1, nks, kpc);
-    P2.kpc = kpc; P2.nchunks = (nks + kpc - 1) / kpc; P2.b_stage_bytes = ks_bytes * kpc;
-    P2.ops_cap = (int)nnzb; P2.mma_warps = mma_warps;
-    const size_t meta = ((size_t)P2.ops_cap + 1) * 16 + ((size_t)5 * nl + 2) * 4 + (size_t)n_blocks + 16 + (4 * 8 + 2 * kTsMaxKS + 4 + 1) * 8
-                      + 48 + ((size_t)P2.ops_cap + 8 * kTsMaxKS + 8) * 16;       // + flat per-warp lists of the k-major sweep
-    const size_t total = 226 * 1024;                       // dynamic shared memory requested: 1 KB alignment slack + rings + metadata
-    if (meta + 1024 + 5 * (size_t)A_STAGE > total) return -1;
-    P2.ring_bytes = (int)((total - 1024 - meta) & ~(size_t)1023);
-    P2.b_stages = env_int("LIBXSMM_B200_BCSC_BST", 2, 8, 3);
-    while (P2.b_stages > 2 && (size_t)P2.b_stages * P2.b_stage_bytes + 3 * (size_t)A_STAGE > (size_t)P2.ring_bytes) --P2.b_stages;
-    if ((size_t)P2.b_stages * P2.b_stage_bytes + 2 * (size_t)A_STAGE > (size_t)P2.ring_bytes) return -1;
-    int raw = (int)(((size_t)P2.ring_bytes - (size_t)P2.b_stages * P2.b_stage_bytes) / A_STAGE); if (raw > 8) raw = 8;
-    P2.raw_cap = env_int("LIBXSMM_B200_BCSC_RAW", 2, 8, 8);
-    P2.raw_stages = (raw < P2.raw_cap) ? raw : P2.raw_cap;
-    P2.kmajor = env_int("LIBXSMM_B200_BCSC_KMAJOR", 0, 1, 1);
-    // resident-B plan: a set of column parts may occupy the ring space minus three A stages (decided by the prep kernel)
-    resident_cap_blocks = (env_int("LIBXSMM_B200_BCSC_RESIDENT", 0, 1, 1) == 1) ? (unsigned int)(((size_t)P2.ring_bytes - 3 * (size_t)A_STAGE) / blk_bytes) : 0u;
-    smem = total;
-  } else {
-    P1.bn = bn; P1.bk = bk; P1.nbc = (int)n_blocks; P1.nks = nks; P1.ksteps = bk / 16;
-    P1.m_blocks = d->m; P1.ngroups = ngroups;
-    P1.ncols = (int)ncols; P1.nparts = nparts; P1.part_cols = (nparts == 1) ? (int)ncols : bpp * bn;
-    P1.slot_cols = (P1.part_cols + 31) & ~31; P1.nslot = 512 / P1.slot_cols; if (P1.nslot > 4) P1.nslot = 4;
-    P1.b_stage_bytes = bpp * (64 / bk) * blk_bytes;                   // a B stage holds one whole k-step of a part
-    const size_t meta = (size_t)(kMaxEntries + 1) * 16 + (5 * kMaxLists + 8) * 4 + 1024 + (6 * kMaxStages + 2 * kMaxSlots) * 8 + 64 + 1024;
-    const size_t budget = 224 * 1024 - meta;
-    P1.b_stages = env_int("LIBXSMM_B200_BCSC_BST", 2, 16, 3); P1.can_stages = env_int("LIBXSMM_B200_BCSC_CAN", 2, 8, 3);
-    while (P1.b_stages > 2 && (size_t)P1.b_stages * P1.b_stage_bytes + (size_t)(P1.can_stages + 2) * A_STAGE > budget) --P1.b_stages;
-    if ((size_t)P1.b_stages * P1.b_stage_bytes + (size_t)(P1.can_stages + 2) * A_STAGE > budget) return -1;
-    P1.raw_stages = (int)((budget - (size_t)P1.b_stages * P1.b_stage_bytes - (size_t)P1.can_stages * A_STAGE) / A_STAGE);
-    if (P1.raw_stages > 8) P1.raw_stages = 8;
-    P1.raw_stages = env_int("LIBXSMM_B200_BCSC_RAW", 2, P1.raw_stages, P1.raw_stages);
-    P1.mma_warps = mma_warps; P1.ops_cap = (int)nnzb;
-    smem = meta + (size_t)(P1.raw_stages + P1.can_stages) * A_STAGE + (size_t)P1.b_stages * P1.b_stage_bytes;
-  }
-
-  // per (handle, device, stream) scratch
-  BcscState* st;
-  {
-    std::lock_guard<std::mutex> lk(g_state_mu);
-    if (*work == nullptr) *work = new BcscState();
-    st = (BcscState*)*work;
-  }
-  std::lock_guard<std::mutex> lk(st->mu);
-  int dev = 0; cudaGetDevice(&dev);
-  BcscBuffers* bufs = nullptr;
-  for (BcscBuffers& s : st->sets) if (s.device == dev && s.stream == stream) { bufs = &s; break; }
-  if (bufs == nullptr) { st->sets.push_back(BcscBuffers{dev, stream, nullptr, 0, nullptr, 0}); bufs = &st->sets.back(); }
-  const BcscIdxLayout L((unsigned int)n_blocks, (unsigned int)nl, nnzb);
-  const size_t need = (size_t)L.total * sizeof(unsigned int);
-  if (bufs->idx == nullptr || bufs->idx_bytes < need) {
-    if (bufs->idx != nullptr) { cudaStreamSynchronize(stream); cudaFree(bufs->idx); bufs->idx = nullptr; bufs->idx_bytes = 0; }
-    if (cudaMalloc((void**)&bufs->idx, need) != cudaSuccess) { bufs->idx = nullptr; (void)cudaGetLastError(); return -1; }
-    bufs->idx_bytes = need;
-    cudaMemsetAsync(bufs->idx, 0, 64, stream);      // fresh buffer: no cached pattern yet (the header is the cache key)
-  }
-  const size_t bneed = (size_t)nnzb * blk_bytes;
-  if (bufs->val == nullptr || bufs->val_bytes < bneed) {
-    if (bufs->val != nullptr) { cudaStreamSynchronize(stream); cudaFree(bufs->val); bufs->val = nullptr; bufs->val_bytes = 0; }
-    if (cudaMalloc(&bufs->val, bneed) != cudaSuccess) { bufs->val = nullptr; (void)cudaGetLastError(); return -1; }
-    bufs->val_bytes = bneed;
-  }
-  unsigned int* buf = bufs->idx;
-  bcsc_prep_kernel<<<1, 256, 0, stream>>>(colptr, rowidx, (int)n_blocks, nkb, bn, bk, nparts, bpp, cpw, nnzb, resident_cap_blocks, buf);
-  xb_rt_count_launch();
-  {
-    const unsigned long long chunks = (unsigned long long)bneed / 16;
-    const unsigned int pgrid = (unsigned int)((chunks + 255) / 256 < 1024 ? (chunks + 255) / 256 : 1024);
-    cudaLaunchConfig_t cfg; cudaLaunchAttribute attr[1];
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(pgrid ? pgrid : 1); cfg.blockDim = dim3(256); cfg.dynamicSmemBytes = 0; cfg.stream = stream;
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization; attr[0].val.programmaticStreamSerializationAllowed = env_int("LIBXSMM_B200_BCSC_PDL", 0, 1, 0);
-    cfg.attrs = attr; cfg.numAttrs = 1;
-    cudaLaunchKernelEx(&cfg, bcsc_pack_b_kernel, (const uint4*)b_vals, (const unsigned int*)(buf + L.entries), (const unsigned int*)(buf + L.list_ptr), nl, (uint4*)bufs->val, bn, bk);
-    xb_rt_count_launch();
-  }
-  const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | (1u << 15) | (0u << 16) | ((uint32_t)(128 >> 4) << 24);   // N is filled in per (merged) operation
-  const uint32_t b_layout = (bk == 16) ? 6u : ((bk == 32) ? 4u : 2u);
-  const uint32_t b_sbo16 = (uint32_t)(8 * bk * 2) >> 4;
-  cudaError_t e = cudaErrorInvalidValue;
-  // TS-form: the device may split the column parts over up to 4 CTAs per group (resident-B plan), so offer up to 4 CTAs per group
-  const long long grid = (variant == 2) ? ((ngroups * 4 < sms) ? ngroups * 4 : sms) : (ngroups < sms ? ngroups : sms);
-  if (variant == 2) {
-    P2.b_packed = (const char*)bufs->val;
-    P2.list_ptr = buf + L.list_ptr; P2.wranges = buf + L.wranges; P2.ops = (const uint4*)(buf + L.ops); P2.col_any = buf + L.col_any;
-    P2.plan = buf + L.hdr + 12;
-    P2.c = (char*)c; P2.beta0 = d->beta0;
-    P2.idesc = idesc & ~(1u << 15);                 // A from TMEM: rows in lanes, k along the columns (K-major)
-    P2.b_layout = b_layout; P2.b_sbo16 = b_sbo16;
-    if (M == 16) e = launch_ts<16>(grid, smem, stream, map_a, P2);
-    else if (M == 32) e = launch_ts<32>(grid, smem, stream, map_a, P2);
-    else if (M == 64) e = launch_ts<64>(grid, smem, stream, map_a, P2);
-    else e = launch_ts<128>(grid, smem, stream, map_a, P2);
-  } else {
-    P1.b_packed = (const char*)bufs->val;
-    P1.list_ptr = buf + L.list_ptr; P1.wranges = buf + L.wranges; P1.ops = (const uint4*)(buf + L.ops); P1.col_any = buf + L.col_any;
-    P1.c = (char*)c; P1.beta0 = d->beta0;
-    P1.idesc = idesc; P1.b_layout = b_layout; P1.b_sbo16 = b_sbo16;
-    if (M == 16) e = launch_v1<16>(grid, smem, stream, map_a, P1);
-    else if (M == 32) e = launch_v1<32>(grid, smem, stream, map_a, P1);
-    else if (M == 64) e = launch_v1<64>(grid, smem, stream, map_a, P1);
-    else e = launch_v1<128>(grid, smem, stream, map_a, P1);
+  cudaError_t e;
+  switch (nt) {
+    case 16:  e = launch<16, 1>(grid, smem, stream, P); break;
+    case 32:  e = launch<32, 1>(grid, smem, stream, P); break;
+    case 64:  e = launch<64, 1>(grid, smem, stream, P); break;
+    case 128: e = launch<64, 2>(grid, smem, stream, P); break;
+    default:  e = launch<64, 4>(grid, smem, stream, P); break;
   }
   xb_rt_count_launch();
   if (e != cudaSuccess) { xb_rt_note_error((int)e, "bcsc_tc"); return (int)e; }

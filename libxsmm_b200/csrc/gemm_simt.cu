@@ -1,4 +1,4 @@
-// libxsmm_b200 -- exact-order dense GEMM/BRGEMM on CUDA cores (sm_100a).
+// libxsmm_b200 -- exact-order dense GEMM/BRGEMM on CUDA cores (sm_90a).
 //
 // This is the "every datatype, every layout flag" kernel: one CTA per tile, one thread per C element,
 // and for each element the SAME sequence of multiply/add operations the reference's C kernel performs
@@ -655,7 +655,7 @@ extern "C" int xb_gemm_simt_launch(const xb_gemm_launch* L) {
     const size_t smem = (size_t)words * 4 * groups;
     if (wpt <= I8_WARPS && smem <= 200 * 1024) {
       static int sms = 0;
-      if (sms == 0) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); if (sms <= 0) sms = 148; }
+      if (sms == 0) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); if (sms <= 0) sms = 132; }
       const long long ctas_needed = (L->count + groups - 1) / groups;
       long long per_sm = (long long)((220 * 1024) / (smem + 1024)); if (per_sm < 1) per_sm = 1; if (per_sm > 2) per_sm = 2;   // 64 registers x 512 threads: two CTAs per SM
       long long grid = (long long)sms * per_sm;

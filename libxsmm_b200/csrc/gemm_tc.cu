@@ -1,32 +1,30 @@
-// libxsmm_b200 -- batched small-tile GEMM/BRGEMM on the 5th-generation tensor cores (sm_100a).
+// libxsmm_b200 -- batched small-tile GEMM/BRGEMM on the Hopper tensor cores (sm_90a, wgmma.mma_async).
 //
 //   C_t(m x n) = beta * C_t + sum_{r < br} A_{t,r}(m x k) * B_{t,r}(k x n)      for t < count tiles
 //
 // Replaces the reference's per-ISA GEMM micro-kernels (src/generator_gemm_amx*.c,
-// src/generator_gemm_avx512_microkernel.c) for the 16-bit floating-point dense path; semantics are those
-// of libxsmm_ref_matmul (src/generator_gemm_reference_impl.c:2025-2170, 2367-2419) with f32
-// accumulation in tensor memory instead of a sequential scalar loop (tolerance, not bit-exact).
+// src/generator_gemm_avx512_microkernel.c) for the 16-bit floating-point and 8-bit integer dense paths; semantics are those
+// of libxsmm_ref_matmul (src/generator_gemm_reference_impl.c:2025-2170, 2367-2419, 1452-1683) with f32 accumulation in
+// registers instead of a sequential scalar loop (tolerance, not bit-exact); integer sums are exact in any order, so the
+// 8-bit path is bit-identical to the reference.
 //
-// Kernels in this file:
-//   gemm_tc_kernel<UM, WIDE, CT>  the general form below (stride / no batch-reduce, and the ring form of pooled ADDRESS/OFFSET mode);
-//                                 1..6 CTAs per SM, chosen by the launcher from the number of loads per tile
-//   gemm_pool_kernel              pooled mode with whole operand sets resident in shared memory (mode R of the benchmark)
-//
-// Data flow per CTA of gemm_tc_kernel (persistent, tiles assigned round-robin):
-//   warp 0   TMA producer : cp.async.bulk.tensor.4d of one A k-chunk and one B k-chunk per stage,
-//                           SWIZZLE_128B, ring of STAGES stages guarded by full/empty mbarriers
-//   warp 1   MMA issuer   : one lane issues tcgen05.mma.cta_group::1.kind::f16 (K=16 per instruction)
-//                           accumulating br * ceil(k/16) steps into a TMEM slot; tcgen05.commit frees
-//                           the SMEM stage and finally publishes the slot
-//   warps 2-5 epilogue    : tcgen05.ld 32x32b -> registers -> (convert) -> global stores; frees the slot
-//
-// Operand layouts (libxsmm column-major): A[k*lda+m] is M-contiguous => UMMA "MN-major" A operand,
-// B[n*ldb+k] is K-contiguous => UMMA "K-major" B operand; both land in SMEM in the canonical
-// SWIZZLE_128B layout directly from TMA (box inner extent 64 elements = 128 bytes).
-// For m <= 64 the M=64 instruction shape is used: its accumulator occupies lanes 0-15 of each 32-lane
-// TMEM quadrant, so two tiles share one slot (the second at lane offset 16) and one tcgen05.ld feeds
-// all 32 lanes of an epilogue warp. Flat tiles with m = 16 or 32 are packed 4 or 2 per instruction (block-diagonal product, the
-// narrower swizzle modes describe the stacked A blocks); see tc_launch_common.
+// One kernel, `gemm_wg_kernel<AMODE, NC, NCH, WG>`, persistent, tiles assigned round-robin over the CTAs:
+//   warps 0 .. 4*WG-1   WG consumer warpgroups; warpgroup g owns rows 64g .. 64g+63 of the tile (m <= 64: one warpgroup;
+//                       pooled pair mode: warpgroup g owns the item's tile g) and issues wgmma m64 x (NC*NCH) x k16/k32
+//   warp 4*WG           TMA producer: cp.async.bulk.tensor.4d of the A and B boxes of one (tile, r, k-chunk) per stage,
+//                       ring of `stages` stages guarded by full/empty mbarriers
+// A operand forms (AMODE):
+//   XB_WG_SS16  A[k*lda+m] is M-contiguous: the box lands in the SWIZZLE_128B MN-major layout and wgmma reads it through a
+//               descriptor with the transpose bit set (bf16 / f16)
+//   XB_WG_RS16, XB_WG_RS8  VNNI-packed A (the reference's canonical low-precision layouts, A[(k/v)*lda*v + m*v + k%v], v = 2
+//               for 16-bit, 4 for 8-bit): one 32-bit word holds v consecutive k of one row, which is exactly one register of
+//               a wgmma A fragment, so the words go from the raw TMA stage straight into registers
+// B[n*ldb+k] is K-contiguous: the K-major operand, SWIZZLE_128B boxes of 128 bytes of k x (NC*NCH) rows, rows beyond n and
+// k beyond the matrix are zero-filled by TMA. A stage is released (empty barrier) once the wgmma group that read it retired.
+// The code keeps one group in flight while the next stage is issued, but ptxas serializes the wgmma of every instantiation
+// (C7520: the run-time bf16/f16 and int8-signedness selection around each instruction), so in the binary a stage's MMAs finish
+// before the next are issued. Several CTAs share an SM, so one CTA's MMAs and epilogue (direct stores of the accumulator
+// fragments, xb_epilogue.cuh) overlap the others' loads; the HBM-bound shapes are limited by the loads, not by that.
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -35,540 +33,232 @@
 #include <string.h>
 #include "xb_internal.h"
 #include "xb_device.cuh"
+#include "xb_tma.cuh"
+#include "xb_wgmma.cuh"
 #include "xb_epilogue.cuh"
 
 namespace {
 
-struct TcParams {
+enum { XB_WG_SS16 = 0, XB_WG_RS16 = 1, XB_WG_RS8 = 2 };
+
+struct WgParams {
   int m, n, k;
-  int np;                 // N of the instruction: n rounded up to the MMA's granularity (grp > 1: grp tiles side by side)
-  int grp, npt;           // small tiles (m = 16 or 32, M = 64 instruction): grp = 64 / m tiles per item, block-diagonal; npt = columns per tile
-  long long tiles;        // number of tiles (count = items = ceil(tiles / grp))
-  int kchunks;            // ceil(k / 64)
-  int stages, stage_bytes, a_bytes;
-  int nslot, slot_cols, tmem_cols, evict_first;
+  int kchunks, kc_elems, kinst;       // k per stage (64 for 16-bit, 128 for 8-bit), k per instruction (16 or 32)
+  int stages, stage_bytes, a_bytes, tx_bytes;
+  int bf16;                           // 16-bit forms: bf16 (1) or f16 (0)
+  int sgn;                            // 8-bit form: bit 1 A signed, bit 0 B signed
   unsigned long long br;
-  long long count;
-  char* c; long long tile_stride_c; long long ldc;
-  int c_type, a_type, beta0;
-  int ep_mode, c_esz;                 // xb_epilogue.cuh
-  int sets_in_smem;                   // pooled: the CTA's slice of `sets` is copied behind the barriers at start
-  int pair;                           // pooled, m <= 64: an item is TWO tiles that share B -- tile 0 in rows 0..63, tile 1 in rows 64..127 of one M=128 instruction
-  uint32_t idesc;
-  uint32_t lbo_a, sbo_a, lbo_b, sbo_b;   // in 16-byte units
-  uint32_t a_layout, a_kstep;            // A descriptor: swizzle mode bits (<< 29 of the high word) and the advance per 16 k in 16-byte units
-  // pooled address mode (libxsmm_b200_gemm_plan over ADDRESS batch-reduce): item p reads block-set sets[p].x of A (and, in pair
-  // mode, sets[p].y for its second tile) and sets[p].z of B (4th tensor-map coordinate) and writes cptrs[p] (pair mode:
-  // cptrs[2p], cptrs[2p+1], the second may be null); items are sorted by set, a CTA owns a contiguous range and keeps the
-  // operands of a run of equal items resident in its stage ring
-  const int4* sets; char* const* cptrs;
+  long long count;                    // items the CTAs walk (tiles; pooled pair mode: pairs of tiles)
+  char* c; long long tile_stride_c, ldc;
+  int ep_mode, c_esz, beta0;
+  float scf;
+  // pooled address mode (libxsmm_b200_gemm_plan over ADDRESS/OFFSET batch-reduce): item p reads block-set sets[p].x of A (pair
+  // mode: sets[p].y for its second tile) and sets[p].z of B (4th tensor-map coordinate) and writes cptrs[p] (pair mode:
+  // cptrs[2p], cptrs[2p+1], the second may be null)
+  const int4* sets; char* const* cptrs; int pair;
 };
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+template <int NC>
+__device__ __forceinline__ void wg_mma16(int bf16, float (&d)[NC / 2], uint64_t a, uint64_t b, int scale_d) {
+  if (NC == 16) { if (bf16) xb_wgmma_ss_bf16_n16<1>(*reinterpret_cast<float(*)[8]>(&d), a, b, scale_d); else xb_wgmma_ss_f16_n16<1>(*reinterpret_cast<float(*)[8]>(&d), a, b, scale_d); }
+  if (NC == 32) { if (bf16) xb_wgmma_ss_bf16_n32<1>(*reinterpret_cast<float(*)[16]>(&d), a, b, scale_d); else xb_wgmma_ss_f16_n32<1>(*reinterpret_cast<float(*)[16]>(&d), a, b, scale_d); }
+  if (NC == 64) { if (bf16) xb_wgmma_ss_bf16_n64<1>(*reinterpret_cast<float(*)[32]>(&d), a, b, scale_d); else xb_wgmma_ss_f16_n64<1>(*reinterpret_cast<float(*)[32]>(&d), a, b, scale_d); }
+}
+template <int NC>
+__device__ __forceinline__ void wg_mma16_rs(int bf16, float (&d)[NC / 2], const uint32_t (&a)[4], uint64_t b, int scale_d) {
+  if (NC == 16) { if (bf16) xb_wgmma_rs_bf16_n16(*reinterpret_cast<float(*)[8]>(&d), a, b, scale_d); else xb_wgmma_rs_f16_n16(*reinterpret_cast<float(*)[8]>(&d), a, b, scale_d); }
+  if (NC == 32) { if (bf16) xb_wgmma_rs_bf16_n32(*reinterpret_cast<float(*)[16]>(&d), a, b, scale_d); else xb_wgmma_rs_f16_n32(*reinterpret_cast<float(*)[16]>(&d), a, b, scale_d); }
+  if (NC == 64) { if (bf16) xb_wgmma_rs_bf16_n64(*reinterpret_cast<float(*)[32]>(&d), a, b, scale_d); else xb_wgmma_rs_f16_n64(*reinterpret_cast<float(*)[32]>(&d), a, b, scale_d); }
+}
+#define XB_WG_I8(N) \
+  switch (sgn) { case 0: xb_wgmma_rs_u8u8_n##N(*reinterpret_cast<int(*)[N / 2]>(&d), a, b, scale_d); break; \
+                 case 1: xb_wgmma_rs_u8s8_n##N(*reinterpret_cast<int(*)[N / 2]>(&d), a, b, scale_d); break; \
+                 case 2: xb_wgmma_rs_s8u8_n##N(*reinterpret_cast<int(*)[N / 2]>(&d), a, b, scale_d); break; \
+                 default: xb_wgmma_rs_s8s8_n##N(*reinterpret_cast<int(*)[N / 2]>(&d), a, b, scale_d); break; }
+template <int NC>
+__device__ __forceinline__ void wg_mma8_rs(int sgn, float (&d)[NC / 2], const uint32_t (&a)[4], uint64_t b, int scale_d) {
+  if (NC == 16) { XB_WG_I8(16) }
+  if (NC == 32) { XB_WG_I8(32) }
+  if (NC == 64) { XB_WG_I8(64) }
+}
+#undef XB_WG_I8
 
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" :: "r"(bar), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" :: "r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  uint32_t done;
-  do {
-    asm volatile("{\n\t.reg .pred p;\n\t"
-                 "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-                 "selp.u32 %0, 1, 0, p;\n\t}"
-                 : "=r"(done) : "r"(bar), "r"(parity) : "memory");
-  } while (!done);
-}
-__device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2, int c3) {
-  asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5}], [%6];"
-               :: "r"(dst), "l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(bar) : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_hint(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2, int c3, uint64_t policy) {
-  asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%2, %3, %4, %5}], [%6], %7;"
-               :: "r"(dst), "l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(bar), "l"(policy) : "memory");
-}
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-               "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-               :: "r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" :: "r"(bar) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-               "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-               "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-                 "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-                 "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-                 "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-               : "r"(taddr) : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-__device__ __forceinline__ uint64_t desc64(uint32_t hi, uint32_t lo) { return ((uint64_t)hi << 32) | lo; }
-// 16 columns only: the last tile of a packed item must not read past its slot (TMEM beyond the CTA's allocation faults)
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-               "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-                 "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-               : "r"(taddr) : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-// SMEM matrix descriptor, SWIZZLE_128B, descriptor version 1 (Blackwell)
-__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr, uint32_t lbo16, uint32_t sbo16) {
-  return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo16 & 0x3FFFu) << 16) | ((uint64_t)(sbo16 & 0x3FFFu) << 32)
-       | (1ull << 46) | (2ull << 61);
-}
-
-// WIDE = false: 192 threads, registers capped so that six CTAs share an SM (the latency-bound small-load shapes need that);
-// WIDE = true: 320 threads (eight epilogue warps) for the one-CTA-per-SM configurations
-// CT = minimum co-resident CTAs the register budget must allow: 6 (56 registers, small spills) only for the shapes that really run
-// five or six CTAs per SM, 4 (80 registers, no spills) for the rest of the 192-thread configurations, 1 for the wide form
-template <int UM, bool WIDE, int CT>
-__global__ void __launch_bounds__(WIDE ? 320 : 192, CT)
-gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const TcParams P) {
+// NC: columns per instruction, NCH: instructions side by side (N = NC * NCH), WG: consumer warpgroups
+template <int AMODE, int NC, int NCH, int WG>
+__global__ void __launch_bounds__(WG * 128 + 32, (NCH == 1 && WG == 1) ? 3 : 1)
+gemm_wg_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const WgParams P) {
   extern __shared__ uint8_t smem_raw[];
-  constexpr int TPS = (UM == 64) ? 2 : 1;          // tiles per TMEM slot
-  constexpr int MAX_STAGES = 16, MAX_SLOTS = 8;
-
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-  const uint32_t smem_base = smem_u32(smem);
-  uint64_t* bars = (uint64_t*)(smem + (size_t)P.stages * P.stage_bytes);
-  // barrier map: [0,S) full, [S,2S) empty, [2S,2S+NS) tmem_full, [2S+NS,2S+2NS) tmem_empty, then the TMEM base word
-  const uint32_t bar_base = smem_u32(bars);
-  const int S = P.stages, NS = P.nslot;
-  uint32_t* tmem_word = (uint32_t*)(bars + 2 * MAX_STAGES + 2 * MAX_SLOTS);
-
+  const uint32_t smem_base = xb_smem_u32(smem);
+  const int S = P.stages;
+  const uint32_t full0 = xb_smem_u32(smem + (size_t)S * P.stage_bytes), empty0 = full0 + 8 * S;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const long long G = gridDim.x, b = blockIdx.x;
+  const long long n_local = (b < P.count) ? (P.count - b + G - 1) / G : 0;
   const bool pooled = P.sets != nullptr;
-  const long long chunk = (P.count + G - 1) / G;                       // pooled: contiguous range per CTA
-  const long long n_local = pooled ? ((b * chunk < P.count) ? ((P.count - b * chunk < chunk) ? P.count - b * chunk : chunk) : 0)
-                                   : ((b < P.count) ? (P.count - b + G - 1) / G : 0);
-  const int4* s_sets = reinterpret_cast<const int4*>(bars + 2 * MAX_STAGES + 2 * MAX_SLOTS + 2);     // pooled: this CTA's slice of the items
-  const int4* my_sets = P.sets_in_smem ? s_sets : (pooled ? P.sets + b * chunk : nullptr);
-  if (P.sets_in_smem) { int4* w = const_cast<int4*>(s_sets); for (long long i = threadIdx.x; i < n_local; i += blockDim.x) w[i] = P.sets[b * chunk + i]; }
-  const int loads_per_tile = (int)P.br * P.kchunks;
-  const bool can_hold = pooled && loads_per_tile <= P.stages;          // a tile's operands fit the ring: equal neighbours re-use them
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     asm volatile("prefetch.tensormap [%0];" :: "l"(&map_a) : "memory");
     asm volatile("prefetch.tensormap [%0];" :: "l"(&map_b) : "memory");
-    for (int i = 0; i < S; ++i) { mbar_init(bar_base + 8 * i, 1); mbar_init(bar_base + 8 * (S + i), 1); }
-    for (int i = 0; i < NS; ++i) { mbar_init(bar_base + 8 * (2 * S + i), 1); mbar_init(bar_base + 8 * (2 * S + NS + i), (blockDim.x >> 5) - 2); }
+    for (int i = 0; i < S; ++i) { xb_mbar_init(full0 + 8 * i, 1); xb_mbar_init(empty0 + 8 * i, 4 * WG); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {   // TMEM: whole 512 columns (one CTA per SM)
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" :: "r"(smem_u32(tmem_word)), "r"((uint32_t)P.tmem_cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_word;
 
-  // The producer and the MMA warp run their loops with ALL lanes (every lane computes the same, provably warp-uniform values) and
-  // only the instruction itself is predicated on one elected lane: operands then sit in uniform registers. Under `if (lane == 0)`
-  // the compiler cannot know that and wraps every tcgen05.mma / TMA issue into an R2UR.BROADCAST loop (33 instructions per MMA).
-  if (warp == 0) {
+  if (warp == 4 * WG) {
     // ===================================== TMA producer =====================================
-    {
-      uint32_t leader;
-      asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(leader));
+    if (lane == 0) {
       int stage = 0; uint32_t phase = 0;
-      uint64_t policy = 0;
-      if (P.evict_first) asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(policy));
-      int4 prev = make_int4(-1, -1, -1, -1);
       for (long long i = 0; i < n_local; ++i) {
-        const long long t = pooled ? b * chunk + i : b + i * G;
-        int ta = (int)t, ta1 = (int)t, tb = (int)t, m1 = 64;             // second 64-row box of an M=128 stage: rows 64.. of the same tile
+        const long long t = b + i * G;
+        int ta0 = (int)t, ta1 = (int)t, tb = (int)t, m1 = 64;            // warpgroup 1: rows 64.. of the same tile
         if (pooled) {
-          const int4 st = my_sets[i];
-          const bool same = can_hold && i > 0 && st.x == prev.x && st.y == prev.y && st.z == prev.z;
-          prev = st; ta = st.x; ta1 = st.x; tb = st.z;
-          if (P.pair) { ta1 = st.y; m1 = 0; }                             // pair mode: rows 0.. of the item's second tile
-          if (same) continue;                                          // operands of the previous tile are still in the ring
+          const int4 st = P.sets[t];
+          ta0 = st.x; ta1 = P.pair ? st.y : st.x; tb = st.z; m1 = P.pair ? 0 : 64;
         }
         for (unsigned long long r = 0; r < P.br; ++r) {
           for (int kc = 0; kc < P.kchunks; ++kc) {
-            if (leader) mbar_wait(bar_base + 8 * (S + stage), phase ^ 1);
-            __syncwarp();
-            const uint32_t full = bar_base + 8 * stage;
-            const uint32_t sa = smem_base + stage * P.stage_bytes, sb = sa + P.a_bytes;
-            if (leader) {
-            mbar_expect_tx(full, (uint32_t)P.stage_bytes);
-            if (P.evict_first) {
-              tma_load_4d_hint(sa, &map_a, full, 0, kc * 64, (int)r, ta, policy);
-              if (UM == 128) tma_load_4d_hint(sa + 8192, &map_a, full, m1, kc * 64, (int)r, ta1, policy);
-              tma_load_4d_hint(sb, &map_b, full, kc * 64, 0, (int)r, tb, policy);
+            xb_mbar_wait(empty0 + 8 * stage, phase ^ 1);
+            const uint32_t full = full0 + 8 * stage, sa = smem_base + stage * P.stage_bytes, sb = sa + P.a_bytes;
+            xb_mbar_expect_tx(full, (uint32_t)P.tx_bytes);
+            if (AMODE == XB_WG_SS16) {
+              xb_tma_load_4d(sa, &map_a, full, 0, kc * 64, (int)r, ta0);
+              if (WG == 2) xb_tma_load_4d(sa + 8192, &map_a, full, m1, kc * 64, (int)r, ta1);
             } else {
-              if (P.grp > 1) {      // packed small tiles: both boxes span grp tiles (4th dimension)
-                tma_load_4d(sa, &map_a, full, 0, kc * 64, (int)r, ta * P.grp);
-                tma_load_4d(sb, &map_b, full, kc * 64, 0, (int)r, tb * P.grp);
-              } else {
-              tma_load_4d(sa, &map_a, full, 0, kc * 64, (int)r, ta);
-              if (UM == 128) tma_load_4d(sa + 8192, &map_a, full, m1, kc * 64, (int)r, ta1);
-              tma_load_4d(sb, &map_b, full, kc * 64, 0, (int)r, tb);
-              }
+              xb_tma_load_4d(sa, &map_a, full, 0, kc * 32, (int)r, ta0);       // m words x 32 word-rows
             }
-            }
-            __syncwarp();
+            xb_tma_load_4d(sb, &map_b, full, kc * P.kc_elems, 0, (int)r, tb);
             if (++stage == S) { stage = 0; phase ^= 1; }
           }
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================================== MMA issuer =======================================
-    {
-      uint32_t leader;
-      asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(leader));
-      int stage = 0; uint32_t phase = 0;                  // cursor of the next freshly loaded stage
-      int run_stage = 0; uint32_t run_phase = 0;          // first stage of the run of equal set pairs this tile belongs to
-      const uint32_t hi_a = (P.sbo_a & 0x3FFFu) | (1u << 14) | (P.a_layout << 29), hi_b = (P.sbo_b & 0x3FFFu) | (1u << 14) | (2u << 29);
-      const uint32_t aks = P.a_kstep;                  // A advance per 16 k (16-byte units): 128 for the 128-byte-row layout
-      // per-stage descriptor low words: (address >> 4) | lbo << 16; the high words are constant. A k-step advances A by 16 rows of
-      // 128 bytes and B by 16 elements inside the swizzled row: one 32-bit add per operand and instruction.
-      const uint32_t stage_step = (uint32_t)P.stage_bytes >> 4;
-      const uint32_t a_lo0 = ((smem_base & 0x3FFFFu) >> 4) | ((P.lbo_a & 0x3FFFu) << 16);
-      const uint32_t b_lo0 = (((smem_base + (uint32_t)P.a_bytes) & 0x3FFFFu) >> 4) | ((P.lbo_b & 0x3FFFu) << 16);
-      const uint32_t full0 = bar_base, empty0 = bar_base + 8 * S, tfull0 = bar_base + 8 * (2 * S), tempty0 = bar_base + 8 * (2 * S + NS);
-      const int nload = loads_per_tile, kchunks = P.kchunks;
-      const int ks_last = (P.k - (kchunks - 1) * 64 + 15) / 16;           // k-steps of a tile's last k-chunk (4 when k % 64 == 0)
-      const uint32_t idesc = P.idesc;
-      int slot = 0; uint32_t slot_par = 1; int half = 0;                   // TMEM slot cursor (TPS tiles per slot)
-      for (long long i = 0; i < n_local; ++i) {
-        bool reuse = false, last_of_run = true;
-        if (can_hold) {
-          const int4 st = my_sets[i];
-          if (i > 0) { const int4 pv = my_sets[i - 1]; reuse = (pv.x == st.x && pv.y == st.y && pv.z == st.z); }
-          if (i + 1 < n_local) { const int4 nx = my_sets[i + 1]; last_of_run = !(nx.x == st.x && nx.y == st.y && nx.z == st.z); }
-        }
-        if (!reuse) { run_stage = stage; run_phase = phase; }
-        int cs = run_stage; uint32_t cph = run_phase;
-        if (half == 0) {
-          if (leader) mbar_wait(tempty0 + 8 * slot, slot_par);
-          __syncwarp();
-        }
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(slot * P.slot_cols) + (half ? (16u << 16) : 0u);
-        uint32_t accumulate = 0;
-        int kc = 0;
-        if (reuse && ks_last == 4) {
-          // the operands of this tile are already resident (same set pair as the previous tile): nothing to wait for, every k-chunk
-          // is full -- a straight run of 4 instructions per stage, descriptors advanced by adds
-          uint32_t a_lo = a_lo0 + (uint32_t)cs * stage_step, b_lo = b_lo0 + (uint32_t)cs * stage_step;
-          for (int l = 0; l < nload; ++l) {
-            if (leader) {
-              umma_f16(d_tmem, desc64(hi_a, a_lo), desc64(hi_b, b_lo), idesc, l == 0 ? 0u : 1u);
-              umma_f16(d_tmem, desc64(hi_a, a_lo + aks), desc64(hi_b, b_lo + 2), idesc, 1u);
-              umma_f16(d_tmem, desc64(hi_a, a_lo + 2 * aks), desc64(hi_b, b_lo + 4), idesc, 1u);
-              umma_f16(d_tmem, desc64(hi_a, a_lo + 3 * aks), desc64(hi_b, b_lo + 6), idesc, 1u);
-              if (last_of_run) umma_commit(empty0 + 8 * cs);
-            }
-            a_lo += stage_step; b_lo += stage_step;
-            if (++cs == S) { cs = 0; a_lo = a_lo0; b_lo = b_lo0; }
-          }
-        } else
-        for (int l = 0; l < nload; ++l) {
-          if (!reuse) { if (leader) mbar_wait(full0 + 8 * cs, cph); __syncwarp(); tc_fence_after(); }
-          const uint32_t a_lo = a_lo0 + (uint32_t)cs * stage_step, b_lo = b_lo0 + (uint32_t)cs * stage_step;
-          const int ksteps = (kc == kchunks - 1) ? ks_last : 4;
-          if (leader) {
-            if (ksteps == 4) {
-              umma_f16(d_tmem, desc64(hi_a, a_lo), desc64(hi_b, b_lo), idesc, accumulate);
-              umma_f16(d_tmem, desc64(hi_a, a_lo + aks), desc64(hi_b, b_lo + 2), idesc, 1u);
-              umma_f16(d_tmem, desc64(hi_a, a_lo + 2 * aks), desc64(hi_b, b_lo + 4), idesc, 1u);
-              umma_f16(d_tmem, desc64(hi_a, a_lo + 3 * aks), desc64(hi_b, b_lo + 6), idesc, 1u);
-            } else {
-              for (int ks = 0; ks < ksteps; ++ks) umma_f16(d_tmem, desc64(hi_a, a_lo + ks * aks), desc64(hi_b, b_lo + ks * 2), idesc, ks == 0 ? accumulate : 1u);
-            }
-            if (last_of_run) umma_commit(empty0 + 8 * cs);               // stage reusable once the MMAs of the whole run retired
-          }
-          accumulate = 1;
-          if (++kc == kchunks) kc = 0;
-          if (++cs == S) { cs = 0; cph ^= 1; }
-        }
-        if (!reuse) { stage = cs; phase = cph; }
-        if ((half == TPS - 1 || i == n_local - 1) && leader) umma_commit(tfull0 + 8 * slot);
-        __syncwarp();
-        if (++half == TPS) { half = 0; if (++slot == NS) { slot = 0; slot_par ^= 1; } }
-      }
-    }
-  } else {
-    // ===================================== epilogue =========================================
-    // 4 or 8 epilogue warps (192 or 320 threads per CTA): warp w reads TMEM lane quadrant w % 4; with 8 warps the two warps of a
-    // quadrant take alternate 32-column chunks
-    const int q = warp & 3;                         // TMEM lane quadrant this warp may read
-    const int cgrp = (warp - 2) >> 2, cstep = 32 * (((int)(blockDim.x >> 5) - 2) >> 2);
-    const long long n_slots = (n_local + TPS - 1) / TPS;
-    const int half = (UM == 64) ? (lane >> 4) : 0;
-    const int row = (UM == 64) ? (16 * q + (lane & 15)) : (P.pair ? ((32 * q + lane) & 63) : (32 * q + lane));
-    const int second = (UM == 128 && P.pair) ? (q >> 1) : 0;                 // pair mode: quadrants 2, 3 hold the item's second tile
-    for (long long slot_seq = 0; slot_seq < n_slots; ++slot_seq) {
-      const int slot = (int)(slot_seq % NS);
-      mbar_wait(bar_base + 8 * (2 * S + slot), (uint32_t)((slot_seq / NS) & 1));
-      tc_fence_after();
-      const long long i = slot_seq * TPS + half;
-      const long long t = pooled ? b * chunk + i : b + i * G;
-      // packed small tiles: row r of the M=64 instruction is row r % m of tile (item * grp + r / m), whose results sit in columns
-      // (r / m) * npt ...; m is 16 or 32, so the 16 rows of a warp all belong to one tile
-      const int tl = (P.grp > 1) ? row / P.m : 0, trow = row - tl * P.m;
-      const long long tile = t * P.grp + tl;
-      char* ctile = pooled ? ((i < n_local) ? (P.pair ? P.cptrs[2 * t + second] : P.cptrs[t]) : nullptr) : P.c + tile * P.tile_stride_c;
-      const bool valid = (i < n_local) && (trow < P.m) && tile < P.tiles && ctile != nullptr;
-      const uint32_t taddr = tmem_base + (uint32_t)(slot * P.slot_cols) + ((uint32_t)(q * 32) << 16) + (uint32_t)(tl * P.npt);
-      const long long ldcb = P.ldc * P.c_esz;
-      char* crow = valid ? ctile + (long long)trow * P.c_esz : nullptr;
-      if (32 * cgrp >= P.npt) { tc_fence_before(); __syncwarp(); if (lane == 0) mbar_arrive(bar_base + 8 * (2 * S + NS + slot)); }   // no chunk for this warp
-      for (int c0 = 32 * cgrp; c0 < P.npt; c0 += cstep) {
-        uint32_t v[32];
-        if (P.npt - c0 <= 16) tmem_ld16(taddr + (uint32_t)c0, v); else tmem_ld32(taddr + (uint32_t)c0, v);
-        if (c0 + cstep >= P.npt) {                  // this warp's last read of the slot: hand it back to the MMA warp
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(bar_base + 8 * (2 * S + NS + slot));
-        }
-        if (valid && c0 < P.n) xb_ep_store_chunk(P.ep_mode, P.beta0, v, crow + c0 * ldcb, ldcb, P.n - c0, 0.0f);
-      }
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" :: "r"(tmem_base), "r"((uint32_t)P.tmem_cols) : "memory");
+  // ===================================== consumer warpgroups =====================================
+  const int g = warp >> 2, wq = warp & 3;
+  const int row_a = 64 * g + 16 * wq + (lane >> 2), q = lane & 3;      // RS forms: fragment rows row_a, row_a + 8 of the tile
+  const int loads = (int)P.br * P.kchunks;
+  float acc[NCH][NC / 2];
+  int stage = 0; uint32_t phase = 0;
+  for (long long i = 0; i < n_local; ++i) {
+    const long long t = b + i * G;
+    int kc = 0, prev = -1;
+    for (int l = 0; l < loads; ++l) {
+      xb_mbar_wait(full0 + 8 * stage, phase);
+      const uint32_t sa = smem_base + stage * P.stage_bytes, sb = sa + P.a_bytes;
+      const int krem = P.k - kc * P.kc_elems;
+      const int ksteps = (krem >= P.kc_elems) ? P.kc_elems / P.kinst : (krem + P.kinst - 1) / P.kinst;
+      xb_wgmma_fence();
+      for (int ks = 0; ks < ksteps; ++ks) {
+        const int scale_d = (l > 0 || ks > 0) ? 1 : 0;
+        if (AMODE == XB_WG_SS16) {
+          // A: MN-major SWIZZLE_128B, 128-byte rows of 64 m per k, 8-row atoms 1024 bytes apart, 16 k = 2048 bytes per step
+          const uint64_t ad = xb_wg_desc(sa + 8192u * g + 2048u * ks, 8192, 1024, 1);
+#pragma unroll
+          for (int c = 0; c < NCH; ++c) wg_mma16<NC>(P.bf16, acc[c], ad, xb_wg_desc(sb + (uint32_t)(c * NC * 128) + 32u * ks, 16, 1024, 1), scale_d);
+        } else {
+          // raw stage: [32 word-rows][m words]; register j of the fragment is word-row 8*ks + q + 4*(j >> 1), row row_a + 8*(j & 1)
+          const uint32_t* w = reinterpret_cast<const uint32_t*>(smem + (size_t)stage * P.stage_bytes);
+          uint32_t a[4];
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            const int rr = row_a + 8 * (j & 1), kw = 8 * ks + q + 4 * (j >> 1);
+            a[j] = (rr < P.m) ? w[kw * P.m + rr] : 0u;
+          }
+#pragma unroll
+          for (int c = 0; c < NCH; ++c) {
+            const uint64_t bd = xb_wg_desc(sb + (uint32_t)(c * NC * 128) + 32u * ks, 16, 1024, 1);
+            if (AMODE == XB_WG_RS16) wg_mma16_rs<NC>(P.bf16, acc[c], a, bd, scale_d);
+            else wg_mma8_rs<NC>(P.sgn, acc[c], a, bd, scale_d);
+          }
+        }
+      }
+      xb_wgmma_commit();
+      xb_wgmma_wait<1>();                      // the previous stage's group retired: hand that stage back to the producer
+      if (prev >= 0) { __syncwarp(); if (lane == 0) xb_mbar_arrive(empty0 + 8 * prev); }
+      prev = stage;
+      if (++kc == P.kchunks) kc = 0;
+      if (++stage == S) { stage = 0; phase ^= 1; }
+    }
+    xb_wgmma_wait<0>();
+    if (prev >= 0) { __syncwarp(); if (lane == 0) xb_mbar_arrive(empty0 + 8 * prev); }
+    // epilogue
+    char* ctile; int row0 = 64 * g;
+    if (!pooled) ctile = P.c + t * P.tile_stride_c;
+    else if (P.pair) { ctile = P.cptrs[2 * t + g]; row0 = 0; }
+    else ctile = P.cptrs[t];
+    if (ctile == nullptr) continue;
+    // ctile - row0 rows: the fragment store adds 64g + 16*warp + ...; in pair mode warpgroup g's rows start at row 0 of its tile
+    char* cbase = ctile - (long long)(64 * g - row0) * P.c_esz;
+#pragma unroll
+    for (int c = 0; c < NCH; ++c) {
+      if (c * NC >= P.n) break;
+      xb_ep_store_frag<NC / 2>(P.ep_mode, P.beta0, *reinterpret_cast<const uint32_t(*)[NC / 2]>(&acc[c]), cbase, 64 * g, c * NC,
+                               P.m + (64 * g - row0), P.n, P.ldc * P.c_esz, P.c_esz, P.scf);
+    }
   }
 }
 
-
-// ---- pooled mode, second form: whole operand SETS resident ----------------------------------------------------------------------
-// Mode R of the benchmark (SURVEY.md 8d): every tile reads one of a few A block-sets and one of a few B block-sets. Items (pairs of
-// tiles that share the B set, see xb_plan_try_pool) arrive sorted by (B set, A set), so over a CTA's slice the B set changes a couple
-// of times and the A set walks upwards. This kernel keeps ONE B set and TWO A sets in shared memory (set = br x kchunks blocks):
-//   * the MMA of an item takes its rows 0..63 from one resident A set and rows 64..127 from another (or the same) one: the two
-//     64-row halves of an MN-major M=128 operand are `leading byte offset` apart, and that offset is just a descriptor field --
-//     the distance between the two buffers, or 0 when both tiles use the same set;
-//   * while the items of set s run, the producer loads the next set into the other buffer (sets are needed in first-use order,
-//     alternating buffers); a buffer is released by a tcgen05.commit after the last item that reads it;
-//   * no operand byte is fetched twice per run of equal sets and nothing is fetched per tile.
-// Roles (352 threads): warp 0 producer, warps 1 and 10 MMA issuers, warps 2..9 epilogue (two per TMEM lane quadrant, alternate column chunks).
-// Producer, issuer and epilogue each replay the same cheap scan over the item list to know which load a set corresponds to.
-struct PoolParams {
-  int m, n, np, k, kchunks, br, loads;      // loads = br * kchunks blocks per set
-  int b_blk;                                // bytes of one B block: np rows x 128 bytes
-  int nslot, slot_cols, tmem_cols;
-  long long count, ldc;                     // items
-  int ep_mode, c_esz, beta0;
-  uint32_t idesc, sbo_a, sbo_b, lbo_b;
-  const int4* items; char* const* cptrs;
-  int issuers;                              // 1 or 2 MMA-issuing warps (warp 1 and, if 2, warp 10); items alternate between them
-};
-
-__global__ void __launch_bounds__(352, 1)
-gemm_pool_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const PoolParams P) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-  const uint32_t smem_base = smem_u32(smem);
-  const uint32_t a_set_bytes = (uint32_t)P.loads * 8192u, b_set_bytes = (uint32_t)P.loads * (uint32_t)P.b_blk;
-  const uint32_t sA = smem_base, sB = smem_base + 2u * a_set_bytes;
-  uint64_t* bars = (uint64_t*)(smem + 2u * a_set_bytes + b_set_bytes);
-  const uint32_t bar0 = smem_u32(bars);
-  const int NS = P.nslot;
-  // barriers: a_full[2], a_empty[2], b_full, b_empty, t_full[NS<=4], t_empty[NS<=4]
-  const uint32_t a_full = bar0, a_empty = bar0 + 16, b_full = bar0 + 32, b_empty = bar0 + 40, t_full = bar0 + 48, t_empty = bar0 + 80;
-  uint32_t* tmem_word = (uint32_t*)(bars + 14);
-  int4* s_items = reinterpret_cast<int4*>(bars + 16);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const long long G = gridDim.x, b = blockIdx.x;
-  const long long chunk = (P.count + G - 1) / G;
-  const long long n_local = (b * chunk < P.count) ? ((P.count - b * chunk < chunk) ? P.count - b * chunk : chunk) : 0;
-  for (long long i = threadIdx.x; i < n_local; i += blockDim.x) s_items[i] = P.items[b * chunk + i];
-  if (threadIdx.x == 0) {
-    asm volatile("prefetch.tensormap [%0];" :: "l"(&map_a) : "memory");
-    asm volatile("prefetch.tensormap [%0];" :: "l"(&map_b) : "memory");
-    // a buffer is released when EVERY issuing warp has committed past its last reader (tcgen05.commit only tracks the issuing thread's MMAs)
-    mbar_init(a_full, 1); mbar_init(a_full + 8, 1); mbar_init(a_empty, P.issuers); mbar_init(a_empty + 8, P.issuers); mbar_init(b_full, 1); mbar_init(b_empty, P.issuers);
-    for (int i = 0; i < NS; ++i) { mbar_init(t_full + 8 * i, 1); mbar_init(t_empty + 8 * i, 8); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" :: "r"(smem_u32(tmem_word)), "r"((uint32_t)P.tmem_cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_word;
-
-  if (warp == 0) {
-    // ===================================== producer =====================================
-    uint32_t leader;
-    asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(leader));
-    int last = -1, j = -1, cur_sb = -1, jb = -1;
-    for (long long i = 0; i < n_local; ++i) {
-      const int4 it = s_items[i];
-      if (it.z != cur_sb) {                                        // new B set: the single buffer must have been released
-        cur_sb = it.z; ++jb;
-        if (leader) {
-          mbar_wait(b_empty, (uint32_t)((jb & 1) ^ 1));
-          mbar_expect_tx(b_full, b_set_bytes);
-          int l = 0;
-          for (int r = 0; r < P.br; ++r) for (int kc = 0; kc < P.kchunks; ++kc, ++l) tma_load_4d(sB + (uint32_t)l * (uint32_t)P.b_blk, &map_b, b_full, kc * 64, 0, r, it.z);
-        }
-        __syncwarp();
-      }
-      for (int h = 0; h < 2; ++h) {
-        const int s = h ? it.y : it.x;
-        if (s != last) {                                           // first use of this A set: load it into the other buffer
-          last = s; ++j;
-          const uint32_t buf = (uint32_t)(j & 1);
-          if (leader) {
-            mbar_wait(a_empty + 8 * buf, (uint32_t)(((j >> 1) & 1) ^ 1));
-            mbar_expect_tx(a_full + 8 * buf, a_set_bytes);
-            int l = 0;
-            for (int r = 0; r < P.br; ++r) for (int kc = 0; kc < P.kchunks; ++kc, ++l) tma_load_4d(sA + buf * a_set_bytes + (uint32_t)l * 8192u, &map_a, a_full + 8 * buf, 0, kc * 64, r, s);
-          }
-          __syncwarp();
-        }
-      }
-    }
-  } else if (warp == 1 || warp == 10) {
-    // ===================================== MMA issuer(s) =====================================
-    // One issuing thread needs ~80 cycles per tcgen05.mma here while the instruction occupies the tensor pipe for 48: with two
-    // issuing warps (items alternate, each item has its own TMEM slot) the pipe is the limit again. Both warps walk ALL items so that
-    // they observe every barrier phase and both commit every release; only the owner of an item issues its MMAs.
-    uint32_t leader;
-    asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(leader));
-    const uint32_t hi_a = (P.sbo_a & 0x3FFFu) | (1u << 14) | (2u << 29), hi_b = (P.sbo_b & 0x3FFFu) | (1u << 14) | (2u << 29);
-    const uint32_t b_lo0 = ((sB & 0x3FFFFu) >> 4) | ((P.lbo_b & 0x3FFFu) << 16);
-    const int ks_last = (P.k - (P.kchunks - 1) * 64 + 15) / 16;
-    const int me = (warp == 1) ? 0 : 1, nis = P.issuers;
-    int last = -1, j = -1, cur_sb = -1, jb = -1, slot = 0; uint32_t slot_par = 1;
-    for (long long i = 0; i < n_local; ++i) {
-      const int4 it = s_items[i];
-      const bool mine = ((int)(i % nis) == me);
-      if (it.z != cur_sb) { cur_sb = it.z; ++jb; if (leader) mbar_wait(b_full, (uint32_t)(jb & 1)); __syncwarp(); }
-      if (it.x != last) { last = it.x; ++j; if (leader) mbar_wait(a_full + 8 * (j & 1), (uint32_t)((j >> 1) & 1)); __syncwarp(); }
-      const int j0 = j;
-      if (it.y != last) { last = it.y; ++j; if (leader) mbar_wait(a_full + 8 * (j & 1), (uint32_t)((j >> 1) & 1)); __syncwarp(); }
-      const int j1 = j;
-      if (mine) { if (leader) mbar_wait(t_empty + 8 * slot, slot_par); __syncwarp(); }
-      tc_fence_after();
-      // rows 0..63 come from the lower of the two buffers, rows 64..127 from `lbo` bytes above it (0: the same set twice)
-      const uint32_t buf_lo = (uint32_t)(((j0 & 1) < (j1 & 1)) ? (j0 & 1) : (j1 & 1)), lbo = (uint32_t)(((j0 ^ j1) & 1) ? (a_set_bytes >> 4) : 0u);
-      const uint32_t a_lo0 = (((sA + buf_lo * a_set_bytes) & 0x3FFFFu) >> 4) | ((lbo & 0x3FFFu) << 16);
-      const uint32_t d_tmem = tmem_base + (uint32_t)(slot * P.slot_cols);
-      // measured: issuing from inside the elected lane's branch (operands in vector registers, one R2UR each) is faster here than the
-      // all-lanes form used in gemm_tc_kernel (0.283 vs 0.322 ms on mode R)
-      if (leader) {
-        if (mine) {
-        int kc = 0;
-        uint32_t a_lo = a_lo0, b_lo = b_lo0, acc = 0u;
-        for (int l = 0; l < P.loads; ++l) {
-          const int ksteps = (kc == P.kchunks - 1) ? ks_last : 4;
-          if (ksteps == 4) {
-            umma_f16(d_tmem, desc64(hi_a, a_lo), desc64(hi_b, b_lo), P.idesc, acc);
-            umma_f16(d_tmem, desc64(hi_a, a_lo + 128), desc64(hi_b, b_lo + 2), P.idesc, 1u);
-            umma_f16(d_tmem, desc64(hi_a, a_lo + 256), desc64(hi_b, b_lo + 4), P.idesc, 1u);
-            umma_f16(d_tmem, desc64(hi_a, a_lo + 384), desc64(hi_b, b_lo + 6), P.idesc, 1u);
-          } else {
-            for (int ks = 0; ks < ksteps; ++ks) umma_f16(d_tmem, desc64(hi_a, a_lo + ks * 128), desc64(hi_b, b_lo + ks * 2), P.idesc, ks == 0 ? acc : 1u);
-          }
-          acc = 1u;
-          a_lo += 8192u >> 4; b_lo += (uint32_t)P.b_blk >> 4;
-          if (++kc == P.kchunks) kc = 0;
-        }
-        umma_commit(t_full + 8 * slot);
-        }
-        // release what the next item no longer reads (every issuing warp arrives, whether or not this item was its own)
-        const bool more = (i + 1 < n_local);
-        const int4 nx = more ? s_items[i + 1] : make_int4(-2, -2, -2, 0);
-        if (more) {
-          if (nx.x != it.x && nx.y != it.x) umma_commit(a_empty + 8 * (j0 & 1));
-          if (j1 != j0 && nx.x != it.y && nx.y != it.y) umma_commit(a_empty + 8 * (j1 & 1));
-          if (nx.z != it.z) umma_commit(b_empty);
-        }
-      }
-      __syncwarp();
-      if (++slot == NS) { slot = 0; slot_par ^= 1; }
-    }
-  } else if (warp < 10) {
-    // ===================================== epilogue =====================================
-    const int q = warp & 3, cgrp = (warp - 2) >> 2;
-    const int row = (32 * q + lane) & 63, upper = q >> 1;              // rows 64..127 of the instruction: TMEM lane quadrants 2, 3
-    int last = -1, j = -1, slot = 0; uint32_t slot_par = 0;
-    for (long long i = 0; i < n_local; ++i) {
-      const int4 it = s_items[i];
-      if (it.x != last) { last = it.x; ++j; }
-      const int j0 = j;
-      if (it.y != last) { last = it.y; ++j; }
-      const int j1 = j;
-      const int swapped = ((j0 & 1) > (j1 & 1)) ? 1 : 0;                // the item's first tile sits in the upper buffer: rows 64..127
-      mbar_wait(t_full + 8 * slot, slot_par);
-      tc_fence_after();
-      char* ctile = P.cptrs[2 * (b * chunk + i) + (upper ^ swapped)];
-      const bool valid = (row < P.m) && ctile != nullptr;
-      const uint32_t taddr = tmem_base + (uint32_t)(slot * P.slot_cols) + ((uint32_t)(q * 32) << 16);
-      const long long ldcb = P.ldc * P.c_esz;
-      char* crow = valid ? ctile + (long long)row * P.c_esz : nullptr;
-      if (32 * cgrp >= P.np) { tc_fence_before(); __syncwarp(); if (lane == 0) mbar_arrive(t_empty + 8 * slot); }
-      for (int c0 = 32 * cgrp; c0 < P.np; c0 += 64) {
-        uint32_t v[32];
-        tmem_ld32(taddr + (uint32_t)c0, v);
-        if (c0 + 64 >= P.np) { tc_fence_before(); __syncwarp(); if (lane == 0) mbar_arrive(t_empty + 8 * slot); }
-        if (valid && c0 < P.n) xb_ep_store_chunk(P.ep_mode, P.beta0, v, crow + c0 * ldcb, ldcb, P.n - c0, 0.0f);
-      }
-      if (++slot == NS) { slot = 0; slot_par ^= 1; }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" :: "r"(tmem_base), "r"((uint32_t)P.tmem_cols) : "memory");
-  }
-}
-
-// ---- host side -------------------------------------------------------------------------------------
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeTiledFn g_encode = nullptr;
 int g_num_sms = 0;
-unsigned long long g_attr_set[6] = {0ull, 0ull, 0ull, 0ull, 0ull, 0ull};   // MaxDynamicSharedMemorySize is a per-device attribute: one bit per device
-
-int tc_init_once() {
-  if (g_encode == nullptr) {
-    void* fn = nullptr; cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres) != cudaSuccess || fn == nullptr) {
-      (void)cudaGetLastError(); return 1;
-    }
-    g_encode = (EncodeTiledFn)fn;
-  }
-  if (g_num_sms == 0) {
-    int dev = 0; cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
-    if (g_num_sms <= 0) g_num_sms = 148;
-  }
-  return 0;
-}
 
 int env_int(const char* name, int fallback) {
   const char* e = getenv(name);
   return (e != nullptr && *e != 0) ? atoi(e) : fallback;
+}
+
+int num_sms() {
+  if (g_num_sms == 0) {
+    int dev = 0; cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
+    if (g_num_sms <= 0) g_num_sms = 132;
+  }
+  return g_num_sms;
+}
+
+// MaxDynamicSharedMemorySize is a per-device function attribute: one bit per (instantiation, device)
+template <int AMODE, int NC, int NCH, int WG>
+cudaError_t launch_one(long long grid, size_t smem, cudaStream_t stream, const CUtensorMap& ma, const CUtensorMap& mb, const WgParams& P) {
+  static unsigned long long done = 0ull;
+  if (xb_rt_first_use_on_device(&done)) cudaFuncSetAttribute(gemm_wg_kernel<AMODE, NC, NCH, WG>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+  gemm_wg_kernel<AMODE, NC, NCH, WG><<<(unsigned int)grid, WG * 128 + 32, smem, stream>>>(ma, mb, P);
+  return cudaGetLastError();
+}
+
+template <int AMODE, int WG>
+cudaError_t launch_n(int nt, long long grid, size_t smem, cudaStream_t stream, const CUtensorMap& ma, const CUtensorMap& mb, const WgParams& P) {
+  switch (nt) {
+    case 16:  return launch_one<AMODE, 16, 1, WG>(grid, smem, stream, ma, mb, P);
+    case 32:  return launch_one<AMODE, 32, 1, WG>(grid, smem, stream, ma, mb, P);
+    case 64:  return launch_one<AMODE, 64, 1, WG>(grid, smem, stream, ma, mb, P);
+    case 128: return launch_one<AMODE, 64, 2, WG>(grid, smem, stream, ma, mb, P);
+    default:  return launch_one<AMODE, 64, 4, WG>(grid, smem, stream, ma, mb, P);
+  }
+}
+
+// columns of the instruction: n rounded up to 16, 32, 64, 128 or 256
+int n_tile(int n) { return n <= 16 ? 16 : (n <= 32 ? 32 : (n <= 64 ? 64 : (n <= 128 ? 128 : 256))); }
+
+// ring size and co-resident CTAs: several CTAs per SM hide each other's epilogues; the ring takes what shared memory is left
+void plan_stages(WgParams& P, int nt, int wg, int* ctas) {
+  int c = (nt == 64 && wg == 1) || nt < 64 ? 3 : 1;
+  while (c > 1 && 2 * P.stage_bytes + 2048 > (227 * 1024) / c) --c;
+  int st = ((227 * 1024) / c - 2048) / P.stage_bytes; if (st > 8) st = 8; if (st < 2) st = 2;
+  P.stages = st; *ctas = c;
+}
+
+int wg_launch(int amode, int wg, int nt, const WgParams& P, int ctas, const CUtensorMap& ma, const CUtensorMap& mb, const char* where) {
+  const size_t smem = (size_t)P.stages * P.stage_bytes + 1024 /*align slack*/ + 2 * 8 * P.stages;
+  long long grid = P.count; if (grid > (long long)num_sms() * ctas) grid = (long long)num_sms() * ctas; if (grid < 1) grid = 1;
+  cudaStream_t stream = (cudaStream_t)xb_rt_stream();
+  cudaError_t e;
+  if (amode == XB_WG_SS16) e = (wg == 2) ? launch_n<XB_WG_SS16, 2>(nt, grid, smem, stream, ma, mb, P) : launch_n<XB_WG_SS16, 1>(nt, grid, smem, stream, ma, mb, P);
+  else if (amode == XB_WG_RS16) e = (wg == 2) ? launch_n<XB_WG_RS16, 2>(nt, grid, smem, stream, ma, mb, P) : launch_n<XB_WG_RS16, 1>(nt, grid, smem, stream, ma, mb, P);
+  else e = (wg == 2) ? launch_n<XB_WG_RS8, 2>(nt, grid, smem, stream, ma, mb, P) : launch_n<XB_WG_RS8, 1>(nt, grid, smem, stream, ma, mb, P);
+  xb_rt_count_launch();
+  if (e != cudaSuccess) { xb_rt_note_error((int)e, where); return (int)e; }
+  return 0;
 }
 
 }  // namespace
@@ -596,59 +286,13 @@ extern "C" int xb_gemm_tc_supported(const xb_gemm_desc* d) {
 }
 
 static int tc_launch_common(const xb_gemm_launch* L, const xb_tc_pool* pool);
-static int pool_sets_launch(const xb_gemm_desc& d, const xb_tc_pool* pool, unsigned long long br, long long items);
 extern "C" int xb_gemm_tc_launch(const xb_gemm_launch* L) { return tc_launch_common(L, nullptr); }
 extern "C" int xb_gemm_tc_launch_pooled(const xb_gemm_desc* d, const xb_tc_pool* pool, unsigned long long br, long long count) {
   xb_gemm_launch L; memset(&L, 0, sizeof(L));
   L.d = *d; L.count = count; L.br = br;
   L.a = pool->base_a; L.b = pool->base_b; L.c = (void*)pool->cptrs;        // non-null markers; the pool carries the real addressing
   L.tile_stride_a = pool->set_a; L.tile_stride_b = pool->set_b; L.tile_stride_c = 16;
-  { const int rc = pool_sets_launch(*d, pool, br, count); if (rc >= 0) return rc; }
   return tc_launch_common(&L, pool);
-}
-// resident-set form of the pooled mode (gemm_pool_kernel): returns -1 when the geometry does not fit (the caller then uses the ring form)
-unsigned long long g_pool_attr = 0ull;
-static int pool_sets_launch(const xb_gemm_desc& d, const xb_tc_pool* pool, unsigned long long br, long long items) {
-  if (!pool->pair || env_int("LIBXSMM_B200_TC_POOLSETS", 1) == 0 || tc_init_once() != 0) return -1;
-  PoolParams P; memset(&P, 0, sizeof(P));
-  const int es = 2;
-  P.m = d.m; P.n = d.n; P.k = d.k; P.np = (d.n + 15) & ~15; P.kchunks = (d.k + 63) / 64; P.br = (int)br;
-  P.loads = P.br * P.kchunks; P.b_blk = P.np * 128;
-  const size_t a_set = (size_t)P.loads * 8192, b_set = (size_t)P.loads * P.b_blk;
-  long long grid = items < g_num_sms ? items : g_num_sms; if (grid < 1) grid = 1;
-  const size_t items_bytes = (size_t)((items + grid - 1) / grid) * sizeof(int4);
-  const size_t smem = 2 * a_set + b_set + 1024 + 128 + items_bytes + 64;
-  if (br > 64 || smem > (size_t)227 * 1024 || (a_set >> 4) > 0x3FFF || d.m > 64 || P.np > 256) return -1;
-  P.slot_cols = (P.np + 31) & ~31; P.nslot = 512 / P.slot_cols; if (P.nslot > 4) P.nslot = 4; P.tmem_cols = 512;
-  P.count = items; P.ldc = d.ldc; P.ep_mode = xb_ep_mode(d.ta, d.tc, &P.c_esz); P.beta0 = (d.flags & LIBXSMM_GEMM_FLAG_BETA_0) ? 1 : 0;
-  const uint32_t fmt = (d.ta == LIBXSMM_DATATYPE_BF16) ? 1u : 0u;
-  P.idesc = (1u << 4) | (fmt << 7) | (fmt << 10) | (1u << 15) | (0u << 16) | ((uint32_t)(P.np >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-  P.sbo_a = 1024 >> 4; P.sbo_b = 1024 >> 4; P.lbo_b = 1;
-  P.items = (const int4*)pool->sets; P.cptrs = (char* const*)pool->cptrs;
-  P.issuers = (env_int("LIBXSMM_B200_TC_POOL_ISSUERS", 2) == 1) ? 1 : 2;
-  const CUtensorMapDataType dt = (d.ta == LIBXSMM_DATATYPE_BF16) ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
-  const cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUtensorMap map_a, map_b;
-  {
-    const cuuint64_t dims[4] = {(cuuint64_t)d.m, (cuuint64_t)d.k, (cuuint64_t)br, (cuuint64_t)pool->nsets_a};
-    const cuuint64_t strides[3] = {(cuuint64_t)d.lda * es, (cuuint64_t)pool->blk_a, (cuuint64_t)pool->set_a};
-    const cuuint32_t box[4] = {64, 64, 1, 1};
-    if (CUDA_SUCCESS != g_encode(&map_a, dt, 4, (void*)pool->base_a, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                                 CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE)) return -1;
-  }
-  {
-    const cuuint64_t dims[4] = {(cuuint64_t)d.k, (cuuint64_t)d.n, (cuuint64_t)br, (cuuint64_t)pool->nsets_b};
-    const cuuint64_t strides[3] = {(cuuint64_t)d.ldb * es, (cuuint64_t)pool->blk_b, (cuuint64_t)pool->set_b};
-    const cuuint32_t box[4] = {64, (cuuint32_t)P.np, 1, 1};
-    if (CUDA_SUCCESS != g_encode(&map_b, dt, 4, (void*)pool->base_b, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                                 CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE)) return -1;
-  }
-  if (xb_rt_first_use_on_device(&g_pool_attr)) cudaFuncSetAttribute(gemm_pool_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-  gemm_pool_kernel<<<(unsigned int)grid, P.issuers == 2 ? 352 : 320, smem, (cudaStream_t)xb_rt_stream()>>>(map_a, map_b, P);
-  xb_rt_count_launch();
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) { xb_rt_note_error((int)e, "gemm_pool"); return (int)e; }
-  return 0;
 }
 
 static int tc_launch_common(const xb_gemm_launch* L, const xb_tc_pool* pool) {
@@ -663,63 +307,26 @@ static int tc_launch_common(const xb_gemm_launch* L, const xb_tc_pool* pool) {
   const int es = 2;
   const bool aligned = (((uintptr_t)a | (uintptr_t)b) & 15) == 0 && (sa % 16) == 0 && (sb % 16) == 0
                     && (L->count == 1 || (sa > 0 && sb > 0));
-  if (br == 0 || !aligned || L->count <= 0 || br > 0x7fffffffull || L->count > 0x7fffffffll || tc_init_once() != 0) {
+  xb_encode_tiled_fn enc = xb_tma_encoder();
+  if (br == 0 || !aligned || L->count <= 0 || br > 0x7fffffffull || L->count > 0x7fffffffll || enc == nullptr) {
     return (pool != nullptr) ? 1 : xb_gemm_simt_launch(L);
   }
 
-  const int UM = (d.m <= 64 && !(pool != nullptr && pool->pair)) ? 64 : 128;
-  TcParams P; memset(&P, 0, sizeof(P));
+  const int wg = (d.m <= 64 && !(pool != nullptr && pool->pair)) ? 1 : 2;
+  const int nt = n_tile(d.n);
+  WgParams P; memset(&P, 0, sizeof(P));
   P.m = d.m; P.n = d.n; P.k = d.k;
-  P.np = (UM == 64) ? ((d.n + 7) & ~7) : ((d.n + 15) & ~15);
-  // small tiles (m = 16 or 32): 64 / m tiles at constant stride share one M=64 instruction as a block-diagonal product. One TMA box
-  // fetches the A blocks of all of them (each its own [64 k][m] block, the narrower swizzle modes describe exactly that), B's tiles
-  // land side by side as N. One load, one barrier round trip and one instruction chain then serve 2 or 4 tiles.
-  P.grp = 1; P.npt = P.np; P.tiles = L->count;
-  long long items = L->count;
-  if (pool == nullptr && UM == 64 && (d.m == 16 || d.m == 32) && L->count >= 8 && (64 / d.m) * P.np <= 256 && (P.np == 16 || (P.np % 32) == 0)
-      && env_int("LIBXSMM_B200_TC_PACK", 1) != 0) {          // columns per tile: 16 or a multiple of 32, so that no TMEM read leaves the item's slot
-    P.grp = 64 / d.m; P.np = P.grp * P.npt; items = (L->count + P.grp - 1) / P.grp;
-  }
-  P.kchunks = (d.k + 63) / 64;
-  P.a_bytes = UM * 128; P.stage_bytes = P.a_bytes + P.np * 128;
-  // several independent (producer, MMA, epilogue) pipelines per SM hide each other's serial phases. Measured on B200:
-  // 64^3 x 8 bf16 streaming: 1 CTA/SM 77%, 2 CTAs/SM 105% of the copy-measured HBM peak (4 CTAs: 102%);
-  // f16 64^3 br=1: 2 CTAs 43%, 4 CTAs 83%; 128^3 br=1: 41% -> 60%. Tiles with few stage loads are latency-bound per
-  // tile, so they get more co-resident CTAs (registers cap this at 6 x 192 threads).
-  const long long loads_per_tile = (long long)P.kchunks * (long long)br;
-  P.slot_cols = (P.np + 31) & ~31;
-  // six CTAs leave 64 TMEM columns each: worth it only while that still holds two accumulator slots (f16 64^3: 4 CTAs 83%, 6 CTAs 77%)
-  int ctas = env_int("LIBXSMM_B200_TC_CTAS", loads_per_tile <= 2 ? ((2 * P.slot_cols <= 64) ? 6 : 4) : (loads_per_tile <= 4 ? 4 : 2));
-  if (pool != nullptr && loads_per_tile * (long long)P.stage_bytes + 2048 <= 224 * 1024) {   // pooled: the ring must hold a whole tile so that equal neighbours share it
-    ctas = 1; while (ctas < 4 && loads_per_tile * (long long)P.stage_bytes + 2048 <= (224 * 1024) / (ctas * 2)) ctas *= 2;
-  }
-  if (ctas < 1) ctas = 1; if (ctas > 6) ctas = 6;
-  auto tmem_for = [](int c) { return c == 1 ? 512 : (c == 2 ? 256 : (c <= 4 ? 128 : 64)); };   // power-of-two allocations that sum to <= 512
-  while (ctas > 1 && (2 * P.stage_bytes + 2048 > (224 * 1024) / ctas || P.slot_cols > tmem_for(ctas))) --ctas;
-  P.stages = ((224 * 1024) / ctas - 2048) / P.stage_bytes; if (P.stages > 12) P.stages = 12; if (P.stages < 2) P.stages = 2;
-  { const int st = env_int("LIBXSMM_B200_TC_STAGES", (ctas > 1 && pool == nullptr) ? 4 : P.stages); if (st >= 2 && st <= P.stages) P.stages = st; }
-  P.tmem_cols = tmem_for(ctas);
-  P.nslot = P.tmem_cols / P.slot_cols; if (P.nslot > 4) P.nslot = 4;
-  P.evict_first = env_int("LIBXSMM_B200_TC_EVICT_FIRST", 0);
-  P.br = br; P.count = items; P.c = c; P.tile_stride_c = sc; P.ldc = d.ldc;
+  P.kc_elems = 64; P.kinst = 16; P.kchunks = (d.k + 63) / 64;
+  P.a_bytes = wg * 8192; P.stage_bytes = P.a_bytes + nt * 128; P.tx_bytes = P.stage_bytes;
+  P.bf16 = (d.ta == LIBXSMM_DATATYPE_BF16) ? 1 : 0;
+  P.br = br; P.count = L->count; P.c = c; P.tile_stride_c = sc; P.ldc = d.ldc;
   if (pool != nullptr) { P.sets = (const int4*)pool->sets; P.cptrs = (char* const*)pool->cptrs; P.pair = pool->pair; }
-  P.c_type = d.tc; P.a_type = d.ta; P.beta0 = (d.flags & LIBXSMM_GEMM_FLAG_BETA_0) ? 1 : 0;
+  P.beta0 = (d.flags & LIBXSMM_GEMM_FLAG_BETA_0) ? 1 : 0;
   P.ep_mode = xb_ep_mode(d.ta, d.tc, &P.c_esz);
-  // instruction descriptor: D=f32, A/B format, A MN-major, B K-major, N>>3, M>>4
-  const uint32_t fmt = (d.ta == LIBXSMM_DATATYPE_BF16) ? 1u : 0u;
-  P.idesc = (1u << 4) | (fmt << 7) | (fmt << 10) | (1u << 15) | (0u << 16) | ((uint32_t)(P.np >> 3) << 17) | ((uint32_t)(UM >> 4) << 24);
-  // descriptor strides in 16-byte units: A (MN-major) 64-row halves 8192 bytes apart, 8-row groups of k 1024 bytes apart; B (K-major) likewise
-  P.lbo_a = 8192 >> 4; P.sbo_a = 1024 >> 4; P.lbo_b = 1; P.sbo_b = 1024 >> 4;
-  P.a_layout = 2u; P.a_kstep = 2048 >> 4;                    // SWIZZLE_128B: 128-byte rows of 64 elements, 16 k rows = 2048 bytes
-  if (P.grp > 1) {
-    // packed small tiles: every tile is its own block of 64 k-rows x (m elements = 64 or 32 bytes), blocks back to back. That is the
-    // MN-major canonical layout of the 64-byte (m = 32) or 32-byte (m = 16) swizzle mode with the blocks `lbo` apart.
-    const uint32_t rowb = (uint32_t)d.m * 2u;
-    P.a_layout = (d.m == 32) ? 4u : 6u;                       // SWIZZLE_64B : SWIZZLE_32B
-    P.sbo_a = (8u * rowb) >> 4; P.lbo_a = (64u * rowb) >> 4; P.a_kstep = (16u * rowb) >> 4;
-  }
+  int ctas = 1;
+  plan_stages(P, nt, wg, &ctas);
 
-  const CUtensorMapDataType dt = (d.ta == LIBXSMM_DATATYPE_BF16) ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  const CUtensorMapDataType dt = P.bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
   const cuuint32_t estr[4] = {1, 1, 1, 1};
   const size_t ext_a = ((size_t)(d.k - 1) * d.lda + d.m) * es, ext_b = ((size_t)(d.n - 1) * d.ldb + d.k) * es;
   const cuuint64_t pad_a = (ext_a + 15) & ~(size_t)15, pad_b = (ext_b + 15) & ~(size_t)15;
@@ -729,45 +336,92 @@ static int tc_launch_common(const xb_gemm_launch* L, const xb_tc_pool* pool) {
     const cuuint64_t strides[3] = {(cuuint64_t)d.lda * es, pool ? (cuuint64_t)pool->blk_a : ((d.br_type == 3) ? (cuuint64_t)d.br_stride_a : pad_a),
                                    pool ? (cuuint64_t)pool->set_a : ((L->count > 1) ? (cuuint64_t)sa : pad_a)};
     const cuuint32_t box[4] = {64, 64, 1, 1};
-    // packed small tiles: the box spans grp tiles; inner extent m elements = the swizzle span
-    const cuuint32_t pbox[4] = {(cuuint32_t)d.m, 64, 1, (cuuint32_t)P.grp};
-    const CUresult r = (P.grp > 1)
-      ? g_encode(&map_a, dt, 4, (void*)a, dims, strides, pbox, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                 (d.m == 32) ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE)
-      : g_encode(&map_a, dt, 4, (void*)a, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                 CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return (pool != nullptr) ? 1 : xb_gemm_simt_launch(L);
+    if (CUDA_SUCCESS != enc(&map_a, dt, 4, (void*)a, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE))
+      return (pool != nullptr) ? 1 : xb_gemm_simt_launch(L);
   }
   {
     const cuuint64_t dims[4] = {(cuuint64_t)d.k, (cuuint64_t)d.n, (cuuint64_t)br, (cuuint64_t)(pool ? pool->nsets_b : L->count)};
     const cuuint64_t strides[3] = {(cuuint64_t)d.ldb * es, pool ? (cuuint64_t)pool->blk_b : ((d.br_type == 3) ? (cuuint64_t)d.br_stride_b : pad_b),
                                    pool ? (cuuint64_t)pool->set_b : ((L->count > 1) ? (cuuint64_t)sb : pad_b)};
-    const cuuint32_t box[4] = {64, (cuuint32_t)P.npt, 1, (cuuint32_t)P.grp};     // grp > 1: the tiles of an item side by side as N
-    const CUresult r = g_encode(&map_b, dt, 4, (void*)b, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                                CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return (pool != nullptr) ? 1 : xb_gemm_simt_launch(L);
+    const cuuint32_t box[4] = {64, (cuuint32_t)nt, 1, 1};
+    if (CUDA_SUCCESS != enc(&map_b, dt, 4, (void*)b, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE))
+      return (pool != nullptr) ? 1 : xb_gemm_simt_launch(L);
   }
+  return wg_launch(XB_WG_SS16, wg, nt, P, ctas, map_a, map_b, "gemm_tc");
+}
 
-  size_t smem = (size_t)P.stages * P.stage_bytes + 1024 /*align slack*/ + (2 * 16 + 2 * 8) * 8 + 64;
-  const long long tiles_per_cta_unit = (UM == 64) ? 2 : 1;
-  long long grid = (items + tiles_per_cta_unit - 1) / tiles_per_cta_unit; if (grid > (long long)g_num_sms * ctas) grid = (long long)g_num_sms * ctas; if (grid < 1) grid = 1;
-  if (pool != nullptr) {
-    const size_t sets_bytes = (size_t)((L->count + grid - 1) / grid) * sizeof(int4);
-    if (sets_bytes <= 16 * 1024 && smem + sets_bytes <= (size_t)(227 * 1024) / ctas) { P.sets_in_smem = 1; smem += sets_bytes; }
+// ---- VNNI-packed A (register-fragment form) ----------------------------------------------------------------------------
+extern "C" int xb_gemm_ts_supported(const xb_gemm_desc* d) {
+  const unsigned int bad = LIBXSMM_GEMM_FLAG_TRANS_A | LIBXSMM_GEMM_FLAG_TRANS_B | LIBXSMM_GEMM_FLAG_VNNI_B | LIBXSMM_GEMM_FLAG_VNNI_C
+                         | LIBXSMM_GEMM_FLAG_DECOMPRESS_A_VIA_BITMASK | LIBXSMM_GEMM_FLAG_INTLV_A_FORMAT;
+  const int a8 = (d->ta == LIBXSMM_DATATYPE_I8 || d->ta == LIBXSMM_DATATYPE_U8), b8 = (d->tb == LIBXSMM_DATATYPE_I8 || d->tb == LIBXSMM_DATATYPE_U8);
+  static int enabled = -1;
+  if (enabled < 0) enabled = env_int("LIBXSMM_B200_TS", 1) != 0 ? 1 : 0;
+  if (!enabled || (d->flags & bad) != 0 || d->fuse_colbias != 0 || d->cp_op != 0) return 0;
+  if (a8 && b8) {
+    if (d->tcomp != LIBXSMM_DATATYPE_I32 || !(d->tc == LIBXSMM_DATATYPE_I32 || d->tc == LIBXSMM_DATATYPE_F32)) return 0;
+    if ((d->flags & LIBXSMM_GEMM_FLAG_VNNI_A) == 0 && d->tc != LIBXSMM_DATATYPE_F32) return 0;   // flat int8 A: exact-order kernel (the F32-out path is always VNNI4)
+    if ((d->k % 4) != 0 || (d->ldb % 16) != 0) return 0;
+  } else if (d->ta == d->tb && (d->ta == LIBXSMM_DATATYPE_BF16 || d->ta == LIBXSMM_DATATYPE_F16)) {
+    if ((d->flags & LIBXSMM_GEMM_FLAG_VNNI_A) == 0 || d->tcomp != LIBXSMM_DATATYPE_F32) return 0;
+    if (d->ta == LIBXSMM_DATATYPE_BF16 && !(d->tc == LIBXSMM_DATATYPE_F32 || d->tc == LIBXSMM_DATATYPE_BF16)) return 0;
+    if (d->ta == LIBXSMM_DATATYPE_F16 && !(d->tc == LIBXSMM_DATATYPE_F32 || d->tc == LIBXSMM_DATATYPE_F16)) return 0;
+    if ((d->k % 2) != 0 || (d->ldb % 8) != 0) return 0;
+  } else return 0;
+  if (d->m < 4 || d->m > 128 || (d->m % 4) != 0 || (d->lda % 4) != 0 || d->n < 1 || d->n > 128 || d->k > 8192) return 0;
+  if (!(d->br_type == 0 || d->br_type == 3)) return 0;
+  if (d->br_type == 3 && ((d->br_stride_a % 16) != 0 || (d->br_stride_b % 16) != 0 || d->br_stride_a <= 0 || d->br_stride_b <= 0)) return 0;
+  return 1;
+}
+
+extern "C" int xb_gemm_ts_launch(const xb_gemm_launch* L) {
+  const xb_gemm_desc& d = L->d;
+  const char* a = (const char*)L->a; const char* b = (const char*)L->b; char* c = (char*)L->c;
+  long long sa = L->tile_stride_a, sb = L->tile_stride_b, sc = L->tile_stride_c;
+  unsigned long long br = L->br;
+  if (L->recs != nullptr) return xb_gemm_simt_launch(L);
+  if (a == nullptr && c == nullptr) { a = (const char*)L->one.a; b = (const char*)L->one.b; c = (char*)L->one.c; br = L->one.br; sa = sb = sc = 0; }
+  if (d.br_type == 0) br = 1;
+  const bool aligned = (((uintptr_t)a | (uintptr_t)b) & 15) == 0 && (sa % 16) == 0 && (sb % 16) == 0 && (L->count == 1 || (sa > 0 && sb > 0));
+  xb_encode_tiled_fn enc = xb_tma_encoder();
+  if (br == 0 || !aligned || L->count <= 0 || br > 0x7fffffffull || L->count > 0x7fffffffll || enc == nullptr) return xb_gemm_simt_launch(L);
+
+  const int is_i8 = (d.ta == LIBXSMM_DATATYPE_I8 || d.ta == LIBXSMM_DATATYPE_U8);
+  const int v = is_i8 ? 4 : 2, es = is_i8 ? 1 : 2;
+  const int wg = (d.m <= 64) ? 1 : 2, nt = n_tile(d.n);
+  WgParams P; memset(&P, 0, sizeof(P));
+  P.m = d.m; P.n = d.n; P.k = d.k;
+  P.kc_elems = 128 / es; P.kinst = is_i8 ? 32 : 16; P.kchunks = (d.k + P.kc_elems - 1) / P.kc_elems;
+  P.a_bytes = (d.m * 128 + 1023) & ~1023;                        // m words x 32 word-rows; B starts 1024-byte aligned (SWIZZLE_128B atom)
+  P.stage_bytes = P.a_bytes + nt * 128; P.tx_bytes = d.m * 128 + nt * 128;
+  P.bf16 = (d.ta == LIBXSMM_DATATYPE_BF16) ? 1 : 0;
+  P.sgn = ((d.ta == LIBXSMM_DATATYPE_I8) ? 2 : 0) | ((d.tb == LIBXSMM_DATATYPE_I8) ? 1 : 0);
+  P.br = br; P.count = L->count; P.c = c; P.tile_stride_c = sc; P.ldc = d.ldc;
+  P.beta0 = (d.flags & LIBXSMM_GEMM_FLAG_BETA_0) ? 1 : 0; P.scf = L->one.scf;
+  P.ep_mode = xb_ep_mode(d.ta, d.tc, &P.c_esz);
+  int ctas = 1;
+  plan_stages(P, nt, wg, &ctas);
+
+  const cuuint32_t estr[4] = {1, 1, 1, 1};
+  const size_t ext_a = ((size_t)(d.k / v - 1) * d.lda + d.m) * 4, ext_b = ((size_t)(d.n - 1) * d.ldb + d.k) * es;
+  const cuuint64_t pad_a = (ext_a + 15) & ~(size_t)15, pad_b = (ext_b + 15) & ~(size_t)15;
+  CUtensorMap map_a, map_b;
+  {
+    const cuuint64_t dims[4] = {(cuuint64_t)d.m, (cuuint64_t)(d.k / v), (cuuint64_t)br, (cuuint64_t)L->count};
+    const cuuint64_t strides[3] = {(cuuint64_t)d.lda * 4, (d.br_type == 3) ? (cuuint64_t)d.br_stride_a : pad_a, (L->count > 1) ? (cuuint64_t)sa : pad_a};
+    const cuuint32_t box[4] = {(cuuint32_t)d.m, 32, 1, 1};
+    if (CUDA_SUCCESS != enc(&map_a, CU_TENSOR_MAP_DATA_TYPE_UINT32, 4, (void*)a, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                            CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE)) return xb_gemm_simt_launch(L);
   }
-  cudaStream_t stream = (cudaStream_t)xb_rt_stream();
-  cudaError_t e;
-  // one CTA per SM has nothing co-resident to hide its epilogue behind: give it 8 epilogue warps instead of 4
-  const unsigned int threads = (unsigned int)env_int("LIBXSMM_B200_TC_THREADS", (ctas == 1 && P.np >= 64) ? 320 : 192) == 320u ? 320u : 192u;
-#define XB_TC_LAUNCH(SLOT, ...) do { \
-    if (xb_rt_first_use_on_device(&g_attr_set[SLOT])) cudaFuncSetAttribute(gemm_tc_kernel<__VA_ARGS__>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024); \
-    gemm_tc_kernel<__VA_ARGS__><<<(unsigned int)grid, threads, smem, stream>>>(map_a, map_b, P); } while (0)
-  if (threads == 320u) { if (UM == 64) XB_TC_LAUNCH(0, 64, true, 1); else XB_TC_LAUNCH(1, 128, true, 1); }
-  else if (ctas > 4)   { if (UM == 64) XB_TC_LAUNCH(2, 64, false, 6); else XB_TC_LAUNCH(3, 128, false, 6); }
-  else                 { if (UM == 64) XB_TC_LAUNCH(4, 64, false, 4); else XB_TC_LAUNCH(5, 128, false, 4); }
-#undef XB_TC_LAUNCH
-  xb_rt_count_launch();
-  e = cudaGetLastError();
-  if (e != cudaSuccess) { xb_rt_note_error((int)e, "gemm_tc"); return (int)e; }
-  return 0;
+  {
+    const CUtensorMapDataType dt = is_i8 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : (P.bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16);
+    const cuuint64_t dims[4] = {(cuuint64_t)d.k, (cuuint64_t)d.n, (cuuint64_t)br, (cuuint64_t)L->count};
+    const cuuint64_t strides[3] = {(cuuint64_t)d.ldb * es, (d.br_type == 3) ? (cuuint64_t)d.br_stride_b : pad_b, (L->count > 1) ? (cuuint64_t)sb : pad_b};
+    const cuuint32_t box[4] = {(cuuint32_t)P.kc_elems, (cuuint32_t)nt, 1, 1};
+    if (CUDA_SUCCESS != enc(&map_b, dt, 4, (void*)b, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE)) return xb_gemm_simt_launch(L);
+  }
+  return wg_launch(is_i8 ? XB_WG_RS8 : XB_WG_RS16, wg, nt, P, ctas, map_a, map_b, "gemm_ts");
 }

@@ -4,7 +4,7 @@
  * Role in the reference: src/libxsmm_main.c (registry + libxsmm_build + dispatch, :2132-3446) and
  * src/libxsmm_generator.c (descriptor construction, :143-321). There is no code generation here:
  * a handle is one of XB_NTHUNKS pre-compiled trampolines (host_thunks.c) whose index selects a slot
- * holding the normalised descriptor; calling it launches a pre-compiled sm_100a kernel.
+ * holding the normalised descriptor; calling it launches a pre-compiled sm_90a kernel.
  * No CUDA header is included: all device work goes through xb_rt_* and xb_*_launch (C ABI).
  */
 #include <pthread.h>
@@ -16,7 +16,7 @@
 
 /* ---- public state words ------------------------------------------------------------------------ */
 __attribute__((visibility("default"))) unsigned int libxsmm_ninit = 0;
-__attribute__((visibility("default"))) int libxsmm_target_archid = 1000;  /* "sm_100a" */
+__attribute__((visibility("default"))) int libxsmm_target_archid = 1000;  /* the backend's arch id: an ABI value drivers compare with the LIBXSMM_X86_* ids */
 __attribute__((visibility("default"))) int libxsmm_verbosity = 0;
 
 static pthread_mutex_t g_lock = PTHREAD_MUTEX_INITIALIZER;
@@ -130,7 +130,7 @@ LIBXSMM_API void libxsmm_finalize(void) {
   memset(g_reg, 0, sizeof(g_reg));
   g_reg_size = 0; g_nregistered = 0;
   if (libxsmm_verbosity != 0) {
-    fprintf(stderr, "LIBXSMM-B200: %llu kernel launches, target %s\n", xb_rt_launch_count(), "sm_100a");
+    fprintf(stderr, "LIBXSMM-B200: %llu kernel launches, target %s\n", xb_rt_launch_count(), "sm_90a");
   }
   libxsmm_ninit = 0;
   pthread_mutex_unlock(&g_lock);
@@ -138,7 +138,7 @@ LIBXSMM_API void libxsmm_finalize(void) {
 
 LIBXSMM_API int libxsmm_get_target_archid(void) { return libxsmm_target_archid; }
 LIBXSMM_API void libxsmm_set_target_archid(int id) { (void)id; }
-LIBXSMM_API const char* libxsmm_get_target_arch(void) { return "sm_100a"; }
+LIBXSMM_API const char* libxsmm_get_target_arch(void) { return "sm_90a"; }
 LIBXSMM_API void libxsmm_set_target_arch(const char* arch) { (void)arch; }
 LIBXSMM_API int libxsmm_get_verbosity(void) { return libxsmm_verbosity; }
 LIBXSMM_API void libxsmm_set_verbosity(int level) { libxsmm_verbosity = level; }
@@ -668,8 +668,8 @@ struct libxsmm_b200_gemm_plan {
   void* d_arrays;            /* device: per-tile pointer/offset arrays */
   long long count;
   /* address batch-reduce whose blocks form regular block-sets in a pool (base + set*set_stride + r*block_stride): served by the
-   * tcgen05 kernel with the set index as tensor-map coordinate; tiles are visited sorted by set pair so that a CTA re-uses
-   * the operands of equal neighbours from its stage ring (the reference calls the kernel once per tile, the order is free) */
+   * tensor-core kernel with the set index as tensor-map coordinate; tiles are sorted by set pair so that two tiles sharing a B set
+   * form one item (the reference calls the kernel once per tile, the order is free) */
   int pooled; xb_tc_pool pool; unsigned long long br; void* d_sets; void* d_cptrs;
 };
 

@@ -400,8 +400,8 @@ LIBXSMM_API void libxsmm_convert_hf8_f32(const libxsmm_hfloat8* in, float* out, 
 
 /* ---- target queries ------------------------------------------------------------------------------------------------ */
 LIBXSMM_API int libxsmm_cpuid(libxsmm_cpuid_info* info) {
-  if (info != NULL) { memset(info, 0, sizeof(*info)); strncpy(info->model, "NVIDIA B200 (sm_100a)", sizeof(info->model) - 1); }
-  return LIBXSMM_B200_SM100A;
+  if (info != NULL) { memset(info, 0, sizeof(*info)); strncpy(info->model, "NVIDIA H100 (sm_90a)", sizeof(info->model) - 1); }
+  return LIBXSMM_B200_SM90A;
 }
 LIBXSMM_API int libxsmm_cpuid_dot_pack_factor(libxsmm_datatype datatype) {
   const int ts = (int)libxsmm_typesize(datatype);

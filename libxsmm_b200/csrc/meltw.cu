@@ -1,4 +1,4 @@
-// libxsmm_b200 -- matrix-eltwise (TPP) kernels for sm_100a: unary / binary / ternary maps with
+// libxsmm_b200 -- matrix-eltwise (TPP) kernels for sm_90a: unary / binary / ternary maps with
 // row/column/scalar broadcast and bitmasks, reductions, layout transforms, gather/scatter and
 // (de)quantisation. All matrices are column-major, element (i,j) at i + j*ld.
 //
@@ -826,7 +826,7 @@ extern "C" int xb_meltw_launch(const xb_meltw_desc* d, const xb_meltw_args* a) {
     case FAM_MAP: {
       const int n_eff = (d->op_class == LIBXSMM_MELTW_OPERATION_UNARY && d->op == LIBXSMM_MELTW_TYPE_UNARY_REPLICATE_COL_VAR) ? (int)a->n_rt : d->n;
       const long long warps = (long long)((d->m + 31) / 32) * n_eff;
-      long long grid = (warps + 7) / 8; if (grid > 148 * 8) grid = 148 * 8; if (grid < 1) return 0;
+      long long grid = (warps + 7) / 8; if (grid > 132 * 8) grid = 132 * 8; if (grid < 1) return 0;
       if (a->rnd8 != nullptr) {
         meltw_rng8_kernel<<<1, 32, 0, st>>>((unsigned int*)a->rng, a->rnd8, (long long)d->m * n_eff);
         if (launch_done("meltw_rng8") != 0) return 1;
@@ -838,7 +838,7 @@ extern "C" int xb_meltw_launch(const xb_meltw_desc* d, const xb_meltw_args* a) {
       const bool sum_op = (d->op == LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X_OP_ADD || d->op == LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X2_OP_ADD || d->op == LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X_X2_OP_ADD);
       if (sum_op && (d->flags & LIBXSMM_MELTW_FLAG_UNARY_REDUCE_ROWS) == 0 && d->t_in0 != LIBXSMM_DATATYPE_F64 && (long long)d->m * d->n >= (1 << 18) && d->m >= 256) {
         // big column reduction: coalesced two-phase version (partial sums per column slice, then the slices in order)
-        int slices = (int)(((long long)148 * 4 * 128 + d->m - 1) / d->m); if (slices > d->n / 16) slices = d->n / 16; if (slices < 1) slices = 1; if (slices > 256) slices = 256;
+        int slices = (int)(((long long)132 * 4 * 128 + d->m - 1) / d->m); if (slices > d->n / 16) slices = d->n / 16; if (slices < 1) slices = 1; if (slices > 256) slices = 256;
         const int want_x2 = (d->op != LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X_OP_ADD);
         float* part = (float*)xb_rt_scratch((size_t)2 * slices * d->m * sizeof(float));
         if (part != nullptr) {
@@ -854,7 +854,7 @@ extern "C" int xb_meltw_launch(const xb_meltw_desc* d, const xb_meltw_args* a) {
         }
       }
       const int nres = (d->flags & LIBXSMM_MELTW_FLAG_UNARY_REDUCE_ROWS) ? d->n : d->m;
-      int grid = (nres + 7) / 8; if (grid > 148 * 8) grid = 148 * 8;
+      int grid = (nres + 7) / 8; if (grid > 132 * 8) grid = 132 * 8;
       if (d->t_in0 == LIBXSMM_DATATYPE_F64) meltw_reduce_kernel<double><<<grid, 256, 0, st>>>(*d, *a);
       else meltw_reduce_kernel<float><<<grid, 256, 0, st>>>(*d, *a);
       return launch_done("meltw_reduce");
@@ -865,7 +865,7 @@ extern "C" int xb_meltw_launch(const xb_meltw_desc* d, const xb_meltw_args* a) {
       return launch_done("meltw_scalar");
     case FAM_TRANSFORM: case FAM_GS: {
       const long long work = (long long)(d->ldo > d->m ? d->ldo : d->m) * ((d->n + 3) / 4 * 4);
-      long long grid = (work + 255) / 256; if (grid > 148 * 16) grid = 148 * 16; if (grid < 1) grid = 1;
+      long long grid = (work + 255) / 256; if (grid > 132 * 16) grid = 132 * 16; if (grid < 1) grid = 1;
       const int ts = xb_dev_typesize(d->t_in0);
       if (fam == FAM_TRANSFORM && d->op == LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_NORMT && (long long)d->m * d->n >= 4096) {
         const long long tiles = (long long)((d->m + 63) / 64) * ((d->n + 63) / 64);
@@ -881,7 +881,7 @@ extern "C" int xb_meltw_launch(const xb_meltw_desc* d, const xb_meltw_args* a) {
                                   || (ts == 1 && (d->op == LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_VNNI4 || d->op == LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_VNNI4_PAD)))) {
         const int V = (ts == 2) ? 2 : 4;
         const long long workp = (long long)((d->n + V - 1) / V) * ((d->ldo + 3) / 4);
-        long long pg = (workp + 255) / 256; if (pg > 148 * 16) pg = 148 * 16;
+        long long pg = (workp + 255) / 256; if (pg > 132 * 16) pg = 132 * 16;
         const int R = 16 / ts;
         if ((d->m % R) == 0 && (d->ldi % R) == 0 && (d->ldo % R) == 0 && (((uintptr_t)a->in0 | (uintptr_t)a->out) & 15) == 0) {
           const long long items = (long long)((d->n + V - 1) / V) * (d->ldo / R);
@@ -909,7 +909,7 @@ extern "C" int xb_meltw_launch(const xb_meltw_desc* d, const xb_meltw_args* a) {
       return launch_done("meltw_move");
     }
     case FAM_QUANT: {
-      long long grid = ((long long)d->m * d->n + 255) / 256; if (grid > 148 * 16) grid = 148 * 16;
+      long long grid = ((long long)d->m * d->n + 255) / 256; if (grid > 132 * 16) grid = 132 * 16;
       meltw_quant_kernel<<<(unsigned int)grid, 256, 0, st>>>(*d, *a);
       return launch_done("meltw_quant");
     }
@@ -926,7 +926,7 @@ extern "C" int xb_meltw_launch(const xb_meltw_desc* d, const xb_meltw_args* a) {
     }
     case FAM_DROPOUT: {
       const long long warps = (long long)((d->m + 31) / 32) * d->n;
-      long long grid = (warps + 7) / 8; if (grid > 148 * 8) grid = 148 * 8; if (grid < 1) return 0;
+      long long grid = (warps + 7) / 8; if (grid > 132 * 8) grid = 132 * 8; if (grid < 1) return 0;
       if (d->op == LIBXSMM_MELTW_TYPE_UNARY_DROPOUT) {
         meltw_rng_kernel<<<1, 32, 0, st>>>((unsigned int*)a->rng, a->rnd, (long long)((d->m + 15) / 16) * d->n);
         if (launch_done("meltw_rng") != 0) return 1;
@@ -935,7 +935,7 @@ extern "C" int xb_meltw_launch(const xb_meltw_desc* d, const xb_meltw_args* a) {
       return launch_done("meltw_dropout");
     }
     case FAM_SPLIT: {
-      long long grid = ((long long)d->m * d->n + 255) / 256; if (grid > 148 * 16) grid = 148 * 16;
+      long long grid = ((long long)d->m * d->n + 255) / 256; if (grid > 132 * 16) grid = 132 * 16;
       meltw_split_kernel<<<(unsigned int)grid, 256, 0, st>>>(*d, *a);
       return launch_done("meltw_split");
     }

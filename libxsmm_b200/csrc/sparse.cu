@@ -1,4 +1,4 @@
-// libxsmm_b200 -- sparse kernels of the hot path (sm_100a):
+// libxsmm_b200 -- sparse kernels of the hot path (sm_90a):
 //   * sreg_kernel      : fsspmdm -- fixed sparse A (CSR, alpha folded in) times dense row-major B,
 //                        N streamed through shared memory in 512-byte column strips with
 //                        cp.async.bulk (TMA 1D) + mbarrier double buffering. HBM-bound.
@@ -316,7 +316,7 @@ __global__ void __launch_bounds__(256) bcsc_simt_kernel(const BcscParams Q) {
 
 int g_sms = 0;
 int num_sms() {
-  if (g_sms == 0) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&g_sms, cudaDevAttrMultiProcessorCount, dev); if (g_sms <= 0) g_sms = 148; }
+  if (g_sms == 0) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&g_sms, cudaDevAttrMultiProcessorCount, dev); if (g_sms <= 0) g_sms = 132; }
   return g_sms;
 }
 int check_launch(const char* where) {
@@ -393,7 +393,7 @@ extern "C" int xb_packed_sp_launch(const xb_sparse_desc* d, const void* a, const
   const unsigned int grid = (unsigned int)(count < 65535 ? count : 65535);
   if (d->kind == XB_KIND_PK_GEMM || d->kind == XB_KIND_PK_AC_RM || d->kind == XB_KIND_PK_BC_RM) {
     const long long total = (long long)Q.M * Q.N * Q.P;
-    long long gx = (total + 255) / 256; if (gx > 148 * 8) gx = 148 * 8; if (gx < 1) gx = 1;
+    long long gx = (total + 255) / 256; if (gx > 132 * 8) gx = 132 * 8; if (gx < 1) gx = 1;
     const dim3 g2((unsigned int)gx, grid);
     if (Q.is_f64) packed_dense_kernel<double><<<g2, 256, 0, stream>>>(Q); else packed_dense_kernel<float><<<g2, 256, 0, stream>>>(Q);
     return check_launch("packed_dense");

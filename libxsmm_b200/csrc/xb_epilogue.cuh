@@ -1,8 +1,6 @@
-// libxsmm_b200 -- accumulator write-back shared by the tcgen05 GEMM kernels (gemm_tc.cu, gemm_ts.cu).
-// A thread owns one row of the tile and holds 32 consecutive columns of it (one tcgen05.ld 32x32b.x32). Lanes are
-// consecutive rows, so every store instruction of a warp writes one contiguous run of a column of the column-major C.
-// The output type and beta are template parameters and the address is a running pointer: the per-element work is the
-// conversion, one 64-bit add and the store -- nothing is re-derived from kernel parameters inside the loop.
+// libxsmm_b200 -- accumulator write-back shared by the tensor-core GEMM kernels (gemm_tc.cu, bcsc_tc.cu).
+// A thread holds its wgmma accumulator fragment; eight lanes cover eight consecutive rows of a column, so each store
+// instruction of a warp writes full 32-byte sectors of the column-major C. Output type and beta are template parameters.
 // Semantics per type follow libxsmm_ref_matmul (src/generator_gemm_reference_impl.c): f32 accumulate, one rounding at
 // the end (:2367-2419 bf16, :2025-2126 f16), beta = 1 adds the old C in f32 (f16 inputs with f32 C round the old value
 // through f16 first, :2118-2123), int32 wraps (:1452-1555), int8 -> f32 scales by scf (:1556-1683).
@@ -40,56 +38,33 @@ __device__ __forceinline__ void xb_ep_store_one(uint32_t raw, char* p, float scf
   }
 }
 
-// bf16 output, full chunk: the software RNE of xb_f32_to_bf16_rne costs ~16 instructions per value; the hardware conversion
-// (cvt.rn.bf16x2.f32, two values per instruction) gives the same bits for every zero, normal and infinite input. Where
-// libxsmm_convert_f32_to_bf16_rne differs: f32 denormals are flushed to signed zero first -- a multiply by one in .ftz mode
-// does exactly that -- and NaNs keep their upper payload bits; but an accumulator NaN on this machine is always the canonical
-// 0x7fffffff (tensor core and FADD both canonicalise), for which both conversions give 0x7fff.
-template <bool BETA0>
-__device__ __forceinline__ void xb_ep_store_chunk_bf16_full(const uint32_t (&v)[32], char* p, long long ldc_bytes) {
+// one warpgroup's m64 x NC accumulator fragment (xb_wgmma.cuh layout) -> C tile. ctile: column-major C of the tile, rows
+// row0 .. row0 + 63 of it are this warpgroup's, col0 is the fragment's first column; only rows < m and columns < n are stored.
+template <int MODE, bool BETA0, int R>
+__device__ __forceinline__ void xb_ep_store_frag_t(const uint32_t (&v)[R], char* ctile, int row0, int col0, int m, int n, long long ldc_bytes, int esz, float scf) {
+  const int lane = threadIdx.x & 31, r = row0 + 16 * ((threadIdx.x >> 5) & 3) + (lane >> 2), c = col0 + 2 * (lane & 3);
 #pragma unroll
-  for (int j = 0; j < 32; j += 2) {
-    float a0 = __uint_as_float(v[j]), a1 = __uint_as_float(v[j + 1]);
-    if (!BETA0) {
-      a0 += xb_bf16_to_f32(*reinterpret_cast<const unsigned short*>(p));
-      a1 += xb_bf16_to_f32(*reinterpret_cast<const unsigned short*>(p + ldc_bytes));
-    }
-    float f0, f1; uint32_t two;
-    asm("mul.ftz.f32 %0, %1, 0f3F800000;" : "=f"(f0) : "f"(a0));
-    asm("mul.ftz.f32 %0, %1, 0f3F800000;" : "=f"(f1) : "f"(a1));
-    asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(two) : "f"(f1), "f"(f0));                 // upper half <- f1, lower half <- f0
-    *reinterpret_cast<unsigned short*>(p) = (unsigned short)two; p += ldc_bytes;
-    *reinterpret_cast<unsigned short*>(p) = (unsigned short)(two >> 16); p += ldc_bytes;
+  for (int i = 0; i < R; ++i) {
+    const int row = r + 8 * ((i >> 1) & 1), col = c + 8 * (i >> 2) + (i & 1);
+    if (row < m && col < n) xb_ep_store_one<MODE, BETA0>(v[i], ctile + (long long)col * ldc_bytes + (long long)row * esz, scf);
   }
 }
 
-// p: address of (this thread's row, first column of the chunk); ncols: valid columns of the chunk (1..32)
-template <int MODE, bool BETA0>
-__device__ __forceinline__ void xb_ep_store_chunk_t(const uint32_t (&v)[32], char* p, long long ldc_bytes, int ncols, float scf) {
-  if (MODE == XB_EP_BF16 && ncols >= 32) { xb_ep_store_chunk_bf16_full<BETA0>(v, p, ldc_bytes); return; }
-  if (ncols >= 32) {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) { xb_ep_store_one<MODE, BETA0>(v[j], p, scf); p += ldc_bytes; }
-  } else {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) { if (j < ncols) xb_ep_store_one<MODE, BETA0>(v[j], p, scf); p += ldc_bytes; }
-  }
-}
-
-__device__ __forceinline__ void xb_ep_store_chunk(int mode, int beta0, const uint32_t (&v)[32], char* p, long long ldc_bytes, int ncols, float scf) {
+template <int R>
+__device__ __forceinline__ void xb_ep_store_frag(int mode, int beta0, const uint32_t (&v)[R], char* ctile, int row0, int col0, int m, int n, long long ldc_bytes, int esz, float scf) {
   switch (mode * 2 + (beta0 ? 1 : 0)) {
-    case XB_EP_F32 * 2 + 0:          xb_ep_store_chunk_t<XB_EP_F32, false>(v, p, ldc_bytes, ncols, scf); break;
-    case XB_EP_F32 * 2 + 1:          xb_ep_store_chunk_t<XB_EP_F32, true>(v, p, ldc_bytes, ncols, scf); break;
-    case XB_EP_F32_FROM_F16 * 2 + 0: xb_ep_store_chunk_t<XB_EP_F32_FROM_F16, false>(v, p, ldc_bytes, ncols, scf); break;
-    case XB_EP_F32_FROM_F16 * 2 + 1: xb_ep_store_chunk_t<XB_EP_F32, true>(v, p, ldc_bytes, ncols, scf); break;
-    case XB_EP_BF16 * 2 + 0:         xb_ep_store_chunk_t<XB_EP_BF16, false>(v, p, ldc_bytes, ncols, scf); break;
-    case XB_EP_BF16 * 2 + 1:         xb_ep_store_chunk_t<XB_EP_BF16, true>(v, p, ldc_bytes, ncols, scf); break;
-    case XB_EP_F16 * 2 + 0:          xb_ep_store_chunk_t<XB_EP_F16, false>(v, p, ldc_bytes, ncols, scf); break;
-    case XB_EP_F16 * 2 + 1:          xb_ep_store_chunk_t<XB_EP_F16, true>(v, p, ldc_bytes, ncols, scf); break;
-    case XB_EP_I32 * 2 + 0:          xb_ep_store_chunk_t<XB_EP_I32, false>(v, p, ldc_bytes, ncols, scf); break;
-    case XB_EP_I32 * 2 + 1:          xb_ep_store_chunk_t<XB_EP_I32, true>(v, p, ldc_bytes, ncols, scf); break;
-    case XB_EP_I32_TO_F32 * 2 + 0:   xb_ep_store_chunk_t<XB_EP_I32_TO_F32, false>(v, p, ldc_bytes, ncols, scf); break;
-    default:                         xb_ep_store_chunk_t<XB_EP_I32_TO_F32, true>(v, p, ldc_bytes, ncols, scf); break;
+    case XB_EP_F32 * 2 + 0:          xb_ep_store_frag_t<XB_EP_F32, false>(v, ctile, row0, col0, m, n, ldc_bytes, esz, scf); break;
+    case XB_EP_F32 * 2 + 1:          xb_ep_store_frag_t<XB_EP_F32, true>(v, ctile, row0, col0, m, n, ldc_bytes, esz, scf); break;
+    case XB_EP_F32_FROM_F16 * 2 + 0: xb_ep_store_frag_t<XB_EP_F32_FROM_F16, false>(v, ctile, row0, col0, m, n, ldc_bytes, esz, scf); break;
+    case XB_EP_F32_FROM_F16 * 2 + 1: xb_ep_store_frag_t<XB_EP_F32, true>(v, ctile, row0, col0, m, n, ldc_bytes, esz, scf); break;
+    case XB_EP_BF16 * 2 + 0:         xb_ep_store_frag_t<XB_EP_BF16, false>(v, ctile, row0, col0, m, n, ldc_bytes, esz, scf); break;
+    case XB_EP_BF16 * 2 + 1:         xb_ep_store_frag_t<XB_EP_BF16, true>(v, ctile, row0, col0, m, n, ldc_bytes, esz, scf); break;
+    case XB_EP_F16 * 2 + 0:          xb_ep_store_frag_t<XB_EP_F16, false>(v, ctile, row0, col0, m, n, ldc_bytes, esz, scf); break;
+    case XB_EP_F16 * 2 + 1:          xb_ep_store_frag_t<XB_EP_F16, true>(v, ctile, row0, col0, m, n, ldc_bytes, esz, scf); break;
+    case XB_EP_I32 * 2 + 0:          xb_ep_store_frag_t<XB_EP_I32, false>(v, ctile, row0, col0, m, n, ldc_bytes, esz, scf); break;
+    case XB_EP_I32 * 2 + 1:          xb_ep_store_frag_t<XB_EP_I32, true>(v, ctile, row0, col0, m, n, ldc_bytes, esz, scf); break;
+    case XB_EP_I32_TO_F32 * 2 + 0:   xb_ep_store_frag_t<XB_EP_I32_TO_F32, false>(v, ctile, row0, col0, m, n, ldc_bytes, esz, scf); break;
+    default:                         xb_ep_store_frag_t<XB_EP_I32_TO_F32, true>(v, ctile, row0, col0, m, n, ldc_bytes, esz, scf); break;
   }
 }
 

@@ -165,7 +165,7 @@ typedef struct xb_tc_pool {
 } xb_tc_pool;
 int xb_gemm_tc_shape_ok(const xb_gemm_desc* d);           /* everything xb_gemm_tc_supported checks except the batch-reduce mode */
 int xb_gemm_tc_launch_pooled(const xb_gemm_desc* d, const xb_tc_pool* pool, unsigned long long br, long long count);
-int xb_gemm_ts_supported(const xb_gemm_desc* d);          /* VNNI-packed A through tensor memory (gemm_ts.cu); pure host logic */
+int xb_gemm_ts_supported(const xb_gemm_desc* d);          /* VNNI-packed A as wgmma register fragments (gemm_tc.cu); pure host logic */
 int xb_gemm_ts_launch(const xb_gemm_launch* L);
 typedef struct xb_meltw_args {
   const void* in0; const void* in1; const void* in2; void* out;
@@ -187,7 +187,7 @@ int xb_packed_sp_launch(const xb_sparse_desc* d, const void* a, const void* b, v
                         long long stride_a, long long stride_b, long long stride_c);
 int xb_bcsc_launch(xb_sparse_desc* d, const void* a, const void* b_vals, const unsigned int* colptr,
                    const unsigned int* rowidx, unsigned long long n_blocks, unsigned int nnzb, void* c);
-/* 0: exact-order CUDA-core kernel, 1: tcgen05 SS-form (round-1 kernel), 2: tcgen05 TS-form (A operand in tensor memory) */
+/* 0: exact-order CUDA-core kernel, 1: wgmma tensor-core kernel (bcsc_tc.cu) */
 int xb_bcsc_tc_variant(const xb_sparse_desc* d, unsigned long long n_blocks);
 void xb_bcsc_state_free(void* work);
 

@@ -2,7 +2,7 @@
 
  * exact-order CUDA-core kernel: bit-identical to the oracle (and to the reference itself where
    oracle/_ref is present) for every precision tuple / layout flag / batch-reduce mode of the first bar;
- * tcgen05 kernel: within the reference's acceptance norms (samples/xgemm/gemm_kernel.c:5312-5414:
+ * tensor-core (wgmma) kernel: within the reference's acceptance norms (samples/xgemm/gemm_kernel.c:5312-5414:
    f32 out < 1.2e-5, bf16/f16 out < 5e-3 relative Frobenius error)."""
 import ctypes as C
 
@@ -60,7 +60,7 @@ def test_hello_host_pointers_f64_and_f32():
 
 
 TC_SHAPES = [(64, 64, 64), (64, 64, 32), (32, 64, 64), (64, 32, 64), (48, 40, 80), (128, 64, 64), (96, 128, 64),
-             (128, 128, 128), (16, 16, 16), (64, 256, 64), (64, 64, 128), (24, 72, 200), (32, 40, 96), (16, 24, 48), (32, 128, 64)]   # m = 16 / 32: several tiles per instruction
+             (128, 128, 128), (16, 16, 16), (64, 256, 64), (64, 64, 128), (24, 72, 200), (32, 40, 96), (16, 24, 48), (32, 128, 64)]   # m = 16 / 32: small tiles in an m64 instruction
 
 
 @pytest.mark.parametrize("ta,tc", [(gen.BF16, gen.F32), (gen.BF16, gen.BF16), (gen.F16, gen.F32), (gen.F16, gen.F16)])
@@ -286,14 +286,14 @@ def test_bitmap_compressed_a_bit_exact():
                                    (gen.U8, gen.I8, gen.I32, gen.F32), (gen.BF16, gen.BF16, gen.F32, gen.F32), (gen.BF16, gen.BF16, gen.F32, gen.BF16),
                                    (gen.F16, gen.F16, gen.F32, gen.F16)])
 def test_vnni_a_on_tensor_cores(types):
-    """VNNI-packed A (the reference's canonical low-precision layout) through tensor memory (gemm_ts.cu): tcgen05.mma kind::i8 /
-    kind::f16 in TS form. Integer tuples bit-exact against the oracle (integer sums are order-free), I8->F32 exact as well (one
+    """VNNI-packed A (the reference's canonical low-precision layout) as wgmma register fragments (gemm_tc.cu): int8 /
+    16-bit. Integer tuples bit-exact against the oracle (integer sums are order-free), I8->F32 exact as well (one
     int->float conversion and one multiply), 16-bit tuples within the reference drivers' norms. Batches through the strided API."""
     rng = np.random.default_rng(97)
     ta, tb, tcomp, tc = types
     is8 = ta in (gen.I8, gen.U8)
     shapes = [(64, 64, 64, 3, 8, 0), (128, 128, 128, 0, 1, 0), (16, 16, 16, 0, 1, 0), (32, 48, 96, 3, 2, 16), (12, 20, 48 if is8 else 40, 0, 1, 0),
-              (128, 64, 256 + 32, 3, 2, 0), (64, 128, 32, 0, 1, 0), (8, 8, 16, 0, 1, 0), (24, 16, 32, 3, 3, 0), (4, 32, 64, 0, 1, 0)]   # m <= 32: several tiles per instruction
+              (128, 64, 256 + 32, 3, 2, 0), (64, 128, 32, 0, 1, 0), (8, 8, 16, 0, 1, 0), (24, 16, 32, 3, 3, 0), (4, 32, 64, 0, 1, 0)]   # m <= 32: small tiles in an m64 instruction
     for (m, n, k, br_type, br, pad) in shapes:
         for beta0 in (1, 0):
             flags = (cases.FLAG_BETA_0 if beta0 else 0) | cases.FLAG_VNNI_A
@@ -321,8 +321,8 @@ def test_vnni_a_on_tensor_cores(types):
 @pytest.mark.parametrize("tc", [gen.F32, gen.BF16])
 def test_address_mode_pool_on_tensor_cores(tc):
     """ADDRESS batch-reduce whose pointers walk a pool of block-sets (mode R of the benchmark): the plan recognises the pool and
-    runs the tcgen05 kernel (set index = tensor-map coordinate, tiles visited sorted by set pair, operands of equal neighbours
-    shared through the stage ring). Every tile against the oracle called exactly like the reference (pointer arrays)."""
+    runs the tensor-core kernel (set index = tensor-map coordinate, tiles visited sorted by set pair, two tiles that share B
+    in one item). Every tile against the oracle called exactly like the reference (pointer arrays)."""
     rng = np.random.default_rng(98)
     for (m, n, k, br, nsets, count) in ((64, 64, 64, 8, 5, 300), (32, 48, 64, 2, 3, 41), (128, 64, 128, 3, 4, 57), (64, 64, 64, 1, 2, 9),
                                         (64, 64, 64, 2, 7, 3001), (48, 80, 96, 2, 6, 2000)):   # many items per CTA: set changes, buffer swaps, odd tails
@@ -362,7 +362,7 @@ def test_address_mode_pool_on_tensor_cores(tc):
 
 def test_offset_mode_pool_on_tensor_cores():
     """OFFSET batch-reduce (block r = a.primary + a.secondary[r]) over the same kind of operand pool: recognised by the plan like the
-    ADDRESS form and run by the resident-set tcgen05 kernel"""
+    ADDRESS form and run by the tensor-core kernel"""
     rng = np.random.default_rng(99)
     tc = gen.BF16
     for (m, n, k, br, nsets, count) in ((64, 64, 64, 4, 4, 777), (32, 32, 128, 2, 3, 50)):

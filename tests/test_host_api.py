@@ -41,7 +41,7 @@ def test_typesize_typename_and_arch():
     for t, sz in ((gen.F64, 8), (gen.F32, 4), (gen.BF16, 2), (gen.F16, 2), (gen.I32, 4), (gen.I16, 2), (gen.I8, 1), (gen.U8, 1)):
         assert X.libxsmm_typesize(t) == sz
     assert X.libxsmm_get_typename(gen.F32) == b"f32" and X.libxsmm_get_typename(gen.BF16) == b"bf16"
-    assert X.libxsmm_get_target_arch() == b"sm_100a"
+    assert X.libxsmm_get_target_arch() == b"sm_90a"
     v = X.libxsmm_get_verbosity(); X.libxsmm_set_verbosity(v)
 
 

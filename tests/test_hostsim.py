@@ -21,7 +21,7 @@ from test_meqn import EQUATIONS
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "libxsmm_b200", "csrc")
 OUT = os.path.join(ROOT, "tests", "c", "_hostsim")
-DRV = os.path.join(ROOT, "tests", "c", "_drivers")
+DRV = os.path.join(ROOT, "oracle", "_ref", "drivers")
 ORACLE = os.path.join(ROOT, "oracle")
 F32, BF16 = gen.F32, gen.BF16
 HOST_C = ["host_core.c", "host_thunks.c", "host_sparse.c", "host_meltw.c", "host_utils.c", "host_meqn.c"]
@@ -234,7 +234,7 @@ DRIVER_RUNS = [("equation_simple", (64, 32)), ("equation_relu", (64, 32)), ("equ
 
 @pytest.mark.parametrize("name,args", DRIVER_RUNS)
 def test_reference_equation_drivers_against_the_simulated_device(name, args):
-    """the reference's unmodified samples/equation/*.c (prebuilt by test_ref_drivers.build_drivers) with the simulation library
+    """the reference's unmodified samples/equation/*.c (built by oracle/ref_drivers.py) with the simulation library
     first on the loader's path: each driver checks itself and returns EXIT_FAILURE on a mismatch"""
     exe = os.path.join(DRV, name)
     if not os.path.exists(exe):
@@ -247,7 +247,7 @@ def test_reference_equation_drivers_against_the_simulated_device(name, args):
 
 
 def test_reference_eltwise_drivers_against_the_simulated_device():
-    """every (driver, arguments) pair of test_ref_drivers.ELTWISE_RUNS (the B200 pass list) plus the ternary driver, with host operands:
+    """every (driver, arguments) pair of test_ref_drivers.ELTWISE_RUNS (the GPU pass list) plus the ternary driver, with host operands:
     the staging rules of host_meltw.c (extents per operation, secondary operands, generator state in and out, padding kept) against
     the oracle's answers. Gather / scatter insist on device-accessible operands, so those runs declare the memory pinned."""
     from test_ref_drivers import ELTWISE_RUNS

@@ -1,71 +1,24 @@
 """The reference's OWN sample drivers, unmodified, compiled against this repository's include/ and linked with -lxsmm
 (libxsmm_b200/lib): the drop-in boundary of SURVEY.md 8b.
 
-  * CPU (`-m "not gpu"`): where /root/reference exists, every driver in DRIVERS must compile and link (build container).
-    The binaries land in tests/c/_drivers/ (git-ignored, travels to the GPU box like the built library).
-  * GPU (`-m gpu`): the prebuilt binaries run on the box and must report success by their own criteria (each driver
+  * CPU (`-m "not gpu"`): where the reference sources exist, every driver in DRIVERS must compile and link.
+    The binaries land in oracle/_ref/drivers/ (oracle/ref_drivers.py, built by __graft_entry__.build()).
+  * GPU (`-m gpu`): the built binaries run on the GPU and must report success by their own criteria (each driver
     compares against its own dense/scalar gold and prints/returns the verdict).
 """
 import os
 import subprocess
+import sys
 
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = "/root/reference"
-OUT = os.path.join(ROOT, "tests", "c", "_drivers")
-LIBDIR = os.path.join(ROOT, "libxsmm_b200", "lib")
+sys.path.insert(0, os.path.join(ROOT, "oracle"))
+from ref_drivers import DRIVERS, LIBDIR, OUT, build_drivers, have_sources  # noqa: E402,F401
 MTX = os.path.join(ROOT, "tests", "golden", "mtx")
 
-# name -> source (relative to the reference tree)
-DRIVERS = {
-    "hello": "samples/hello/hello.c",
-    "pyfr_driver_asp_reg": "samples/xgemm_sparse_Ainregs/pyfr_driver_asp_reg.c",
-    "spmm_kernel": "samples/xgemm_sparse/spmm_kernel.c",
-    "gemm_kernel": "samples/xgemm/gemm_kernel.c",
-    "gemm_kernel_fused": "samples/xgemm/gemm_kernel_fused.c",
-    "eltwise_unary_relu": "samples/eltwise/eltwise_unary_relu.c",
-    "eltwise_unary_transform": "samples/eltwise/eltwise_unary_transform.c",
-    "eltwise_unary_simple": "samples/eltwise/eltwise_unary_simple.c",
-    "eltwise_binary_simple": "samples/eltwise/eltwise_binary_simple.c",
-    "eltwise_ternary_simple": "samples/eltwise/eltwise_ternary_simple.c",
-    "eltwise_unary_dropout": "samples/eltwise/eltwise_unary_dropout.c",
-    "eltwise_unary_gather_scatter": "samples/eltwise/eltwise_unary_gather_scatter.c",
-    "eltwise_unary_quantization": "samples/eltwise/eltwise_unary_quantization.c",
-    "eltwise_unary_quantization_to_mxbf8": "samples/eltwise/eltwise_unary_quantization_to_mxbf8.c",
-    "eltwise_unary_quantization_to_mxfp4": "samples/eltwise/eltwise_unary_quantization_to_mxfp4.c",
-    "eltwise_unary_quantization_to_nvfp4": "samples/eltwise/eltwise_unary_quantization_to_nvfp4.c",
-    "eltwise_unary_reduce": "samples/eltwise/eltwise_unary_reduce.c",
-    "equation_simple": "samples/equation/equation_simple.c",
-    "equation_relu": "samples/equation/equation_relu.c",
-    "equation_softmax": "samples/equation/equation_softmax.c",
-    "equation_simple_layernorm": "samples/equation/equation_simple_layernorm.c",
-    "equation_bf16_x3_split_f32": "samples/equation/equation_bf16_x3_split_f32.c",
-    "gimmik": "samples/xgemm_sparse_Ainregs/gimmik.c",
-    "gemm_kernel_parallel": "samples/xgemm/gemm_kernel_parallel.c",
-    # the reference's unit tests that pin dispatch-level behaviour (SURVEY.md section 4: threadsafety, registry, gemmflags) + matdiff
-    "ut_threadsafety": "tests/threadsafety.c",
-    "ut_registry": "tests/registry.c",
-    "ut_gemmflags": "tests/gemmflags.c",
-    "ut_matdiff": "tests/matdiff.c",
-}
 
-
-def build_drivers(names=None):
-    """compile the listed reference drivers; returns {name: (rc, stderr tail)}"""
-    os.makedirs(OUT, exist_ok=True)
-    res = {}
-    for name, src in DRIVERS.items():
-        if names and name not in names:
-            continue
-        cmd = ["gcc", "-O2", "-fopenmp", "-I" + os.path.join(ROOT, "include"), os.path.join(REF, src), "-o", os.path.join(OUT, name),
-               "-L" + LIBDIR, "-lxsmm", "-lm", "-Wl,-rpath," + LIBDIR]
-        p = subprocess.run(cmd, capture_output=True, text=True)
-        res[name] = (p.returncode, p.stderr[-2000:])
-    return res
-
-
-@pytest.mark.skipif(not os.path.isdir(os.path.join(REF, "samples")), reason="the reference tree is not present here")
+@pytest.mark.skipif(not have_sources(), reason="the reference sources are not present here")
 def test_reference_drivers_compile_and_link_unmodified():
     res = build_drivers()
     bad = {k: v[1] for k, v in res.items() if v[0] != 0}
@@ -75,7 +28,7 @@ def test_reference_drivers_compile_and_link_unmodified():
 def _run(name, *args, timeout=300):
     exe = os.path.join(OUT, name)
     if not os.path.exists(exe):
-        pytest.skip("%s was not prebuilt (no reference tree in the build container?)" % name)
+        pytest.skip("%s was not built: build() compiles the drivers into oracle/_ref/drivers where the reference sources exist" % name)
     env = dict(os.environ, LD_LIBRARY_PATH=LIBDIR + ":" + os.environ.get("LD_LIBRARY_PATH", ""), OMP_NUM_THREADS="4")
     return subprocess.run([exe] + [str(a) for a in args], capture_output=True, text=True, timeout=timeout, env=env, cwd=OUT)
 
@@ -140,8 +93,7 @@ def test_spmm_kernel_driver_f32_and_int8():
         assert p.returncode == 0, (types, p.stdout[-1500:], p.stderr[-800:])
 
 
-# (driver, arguments) sets that the unmodified reference drivers accept and PASS by their own criteria on the B200
-# (profiles/r02_reference_drivers_run.txt is the log of exactly these invocations)
+# (driver, arguments) sets that the unmodified reference drivers accept and PASS by their own criteria on the GPU
 ELTWISE_RUNS = [
     ("eltwise_unary_simple", (1, 0, "F32", "F32", "F32", 37, 11, 40, 40, 0)), ("eltwise_unary_simple", (2, 0, "F32", "F32", "F32", 37, 11, 40, 40, 0)),
     ("eltwise_unary_simple", (3, 0, "F32", "F32", "F32", 37, 11, 40, 40, 0)), ("eltwise_unary_simple", (11, 0, "F32", "F32", "F32", 37, 11, 40, 40, 0)),

@@ -122,7 +122,7 @@ def _bcsc_bf16_run(rng, mblocks, M, K, N, bk, bn, dens, beta0, expect_variant, t
     d_a, d_b, d_cp, d_ri, d_c = dev(a), dev(bvals), dev(colptr), dev(rowidx), dev(c0)
     want = c0.copy()
     assert _run_bcsc(oracle, types, (mblocks, M, K, N, bk, bn), flags, a, bvals, colptr, rowidx, want) == 0
-    for rep in range(2):     # the second call takes the cached-pattern path of the prep kernel
+    for rep in range(2):     # a second call on the same handle gives the same result
         d_c.copy_(dev(c0))
         X.call_gemm(kernel, d_a, d_b, d_c, colptr=d_cp, rowidx=d_ri, nblocks=N // bn); X.check()
         err = gen.normf_rel(gen.to_f64(want, ta), gen.to_f64(host(d_c, np.uint16), ta))
@@ -137,24 +137,21 @@ _BCSC_TC_GEOMETRIES = ((4, 32, 64, 64, 32, 32, 1.0), (4, 32, 128, 64, 32, 32, 0.
                        (7, 32, 512, 512, 32, 32, 0.1), (6, 64, 448, 384, 64, 128, 0.7), (11, 16, 192, 48, 16, 48, 0.8))
 
 
-@pytest.mark.parametrize("force_v1", [0, 1])
-def test_bcsc_bf16_tcgen05_kernels(force_v1, monkeypatch):
-    """both tensor-core BCSC kernels (TS-form: A in tensor memory; round-1 SS-form) against the oracle, incl. the BASELINE configs[3]
-    geometry (M=32, N=K=512, 32x32 blocks, 50%) at a small m_blocks; thresholds of samples/xgemm_sparse/spmm_kernel.c:1019-1029"""
-    monkeypatch.setenv("LIBXSMM_B200_BCSC_V1", str(force_v1))
-    rng = np.random.default_rng(77 + force_v1)
+def test_bcsc_bf16_tensor_core_kernel():
+    """the wgmma BCSC kernel against the oracle, incl. the BASELINE configs[3] geometry (M=32, N=K=512, 32x32 blocks, 50%) at a
+    small m_blocks; thresholds of samples/xgemm_sparse/spmm_kernel.c:1019-1029"""
+    rng = np.random.default_rng(77)
     for geo in _BCSC_TC_GEOMETRIES:
         for beta0 in (1, 0):
-            _bcsc_bf16_run(rng, *geo, beta0, expect_variant=1 if force_v1 else 2)
+            _bcsc_bf16_run(rng, *geo, beta0, expect_variant=1)
 
 
 def test_bcsc_bf16_kernel_selection_by_geometry(monkeypatch):
-    """K > 512 does not fit the TMEM-resident A operand -> round-1 kernel; N > 512 is served by the TS-form kernel only;
-    bn > 128 -> round-1 kernel; K < 64 or an unsupported block shape -> exact-order kernel"""
-    monkeypatch.delenv("LIBXSMM_B200_BCSC_V1", raising=False)
+    """K > 512, N > 512 and bn > 128 are all served by the tensor-core kernel; K < 64 or an unsupported block shape -> exact-order
+    kernel"""
     rng = np.random.default_rng(5)
     _bcsc_bf16_run(rng, 5, 32, 640, 256, 32, 32, 0.5, 1, expect_variant=1)
-    _bcsc_bf16_run(rng, 5, 32, 256, 1024, 32, 32, 0.4, 1, expect_variant=2)
+    _bcsc_bf16_run(rng, 5, 32, 256, 1024, 32, 32, 0.4, 1, expect_variant=1)
     _bcsc_bf16_run(rng, 3, 32, 128, 512, 32, 256, 0.6, 0, expect_variant=1)
     _bcsc_bf16_run(rng, 3, 32, 32, 64, 16, 16, 0.6, 0, expect_variant=0)
     _bcsc_bf16_run(rng, 3, 8, 64, 64, 32, 32, 0.6, 1, expect_variant=0)
