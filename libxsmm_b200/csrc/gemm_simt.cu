@@ -104,11 +104,108 @@ template <typename T> __device__ inline T ldg_as(const char* base, long long idx
   return reinterpret_cast<const T*>(base)[idx];
 }
 
+// Loop invariants of the dot_* loops, read from the descriptor once at kernel entry. Derived from `d` inside the loops instead,
+// they are reloaded and recomputed per element: the fused kernel then needs more registers and ran up to 1.9x slower (H100 SXM,
+// 400 W power limit).
+struct DotGeom {
+  int k; long long lda, ldb;
+  bool trans_a, trans_b, vnni_a, vnni_b, ua, ub;
+};
+__device__ __forceinline__ DotGeom dot_geom(const xb_gemm_desc& d) {
+  DotGeom g;
+  g.k = d.k; g.lda = d.lda; g.ldb = d.ldb;
+  g.trans_a = (d.flags & LIBXSMM_GEMM_FLAG_TRANS_A) != 0; g.trans_b = (d.flags & LIBXSMM_GEMM_FLAG_TRANS_B) != 0;
+  g.vnni_a = (d.flags & LIBXSMM_GEMM_FLAG_VNNI_A) != 0; g.vnni_b = (d.flags & LIBXSMM_GEMM_FLAG_VNNI_B) != 0;
+  g.ua = (d.ta == LIBXSMM_DATATYPE_U8); g.ub = (d.tb == LIBXSMM_DATATYPE_U8);
+  return g;
+}
+
+// ---- the reference's accumulation loops, shared by gemm_simt_kernel and gemm_simt_fused_kernel ---------------------------
+// Each returns `acc` after the batch-reduce and k loops of element (i, j), in the reference's order and rounding points; the
+// seed, the scale, the epilogue and the store stay with the caller.
+__device__ __forceinline__ float dot_f32(const xb_gemm_desc& d, const DotGeom& g, const TileCtx& x, int i, int j, float acc) {   // reference :1359-1426
+  const int k = g.k;
+  const long long lda = g.lda, ldb = g.ldb;
+  const bool trans_a = g.trans_a, trans_b = g.trans_b;
+  const bool cvt = (d.ta == LIBXSMM_DATATYPE_BF32);   // BF32: operands rounded to bf16 first
+  for (unsigned long long r = 0; r < x.br; ++r) {
+    const char *pa, *pb; br_ptrs(d, x, r, 4, 4, pa, pb);
+    for (int s = 0; s < k; ++s) {
+      float av = ldg_as<float>(pa, trans_a ? (i * lda + s) : (s * lda + i));
+      float bv = ldg_as<float>(pb, trans_b ? (s * ldb + j) : (j * ldb + s));
+      if (cvt) { av = xb_bf16_to_f32(xb_f32_to_bf16_rne(av)); bv = xb_bf16_to_f32(xb_f32_to_bf16_rne(bv)); }
+      acc = __fadd_rn(acc, __fmul_rn(av, bv));
+    }
+  }
+  return acc;
+}
+
+// reference :1452-1683 (four sign combinations); an f32 C always reads A as VNNI4
+__device__ __forceinline__ unsigned int dot_i8(const xb_gemm_desc& d, const DotGeom& g, const TileCtx& x, int i, int j, unsigned int acc) {
+  const int k = g.k;
+  const long long lda = g.lda, ldb = g.ldb;
+  const bool ua = g.ua, ub = g.ub;
+  const int kb = (d.tc == LIBXSMM_DATATYPE_F32 || g.vnni_a) ? 4 : 1;
+  for (unsigned long long r = 0; r < x.br; ++r) {
+    const char *pa, *pb; br_ptrs(d, x, r, 1, 1, pa, pb);
+    for (int s = 0; s < k / kb; ++s) for (int k2 = 0; k2 < kb; ++k2) {
+      const unsigned char ar = ldg_as<unsigned char>(pa, s * (lda * kb) + (long long)i * kb + k2);
+      const unsigned char brw = ldg_as<unsigned char>(pb, j * ldb + (long long)s * kb + k2);
+      const int av = ua ? (int)ar : (int)(signed char)ar;
+      const int bv = ub ? (int)brw : (int)(signed char)brw;
+      acc += (unsigned int)(av * bv);      // wrap-around like the reference's int accumulator
+    }
+  }
+  return acc;
+}
+
+__device__ __forceinline__ float dot_f16(const xb_gemm_desc& d, const DotGeom& g, const TileCtx& x, int i, int j, float acc) {   // reference :2025-2126
+  const int k = g.k;
+  const long long lda = g.lda, ldb = g.ldb;
+  const bool trans_b = g.trans_b;
+  const int kb = g.vnni_a ? 2 : 1;
+  // comp F16 (or IMPLICIT, resolved like an SPR host) rounds the accumulator to f16 per FMA
+  const bool round_each = (d.tcomp == LIBXSMM_DATATYPE_F16 || d.tcomp == LIBXSMM_DATATYPE_IMPLICIT);
+  for (unsigned long long r = 0; r < x.br; ++r) {
+    const char *pa, *pb; br_ptrs(d, x, r, 2, 2, pa, pb);
+    for (int s = 0; s < k / kb; ++s) for (int k2 = 0; k2 < kb; ++k2) {
+      const float av = xb_f16_to_f32(ldg_as<unsigned short>(pa, s * (lda * kb) + (long long)i * kb + k2));
+      const long long kk = (long long)s * kb + k2;
+      const float bv = xb_f16_to_f32(ldg_as<unsigned short>(pb, trans_b ? (kk * ldb + j) : (j * ldb + kk)));
+      acc = __fadd_rn(acc, __fmul_rn(av, bv));
+      if (round_each) acc = xb_f16_to_f32(xb_f32_to_f16(acc));
+    }
+  }
+  return acc;
+}
+
+__device__ __forceinline__ float dot_bf16(const xb_gemm_desc& d, const DotGeom& g, const TileCtx& x, int i, int j, float acc) {   // reference :2127-2170 and :2367-2419
+  const int k = g.k;
+  const long long lda = g.lda, ldb = g.ldb;
+  const bool trans_a = g.trans_a, trans_b = g.trans_b;
+  const bool vnni_a = g.vnni_a, vnni_b = g.vnni_b;
+  const int kb = vnni_a ? 2 : 1;
+  for (unsigned long long r = 0; r < x.br; ++r) {
+    const char *pa, *pb; br_ptrs(d, x, r, 2, 2, pa, pb);
+    for (int s = 0; s < k / kb; ++s) for (int k2 = kb - 1; k2 >= 0; --k2) {   // high k of a pair first
+      const long long kk = (long long)s * kb + k2;
+      unsigned short ar = 0, brw = 0;
+      if (!trans_a) ar = ldg_as<unsigned short>(pa, s * (lda * kb) + (long long)i * kb + k2);
+      else if (!vnni_a) ar = ldg_as<unsigned short>(pa, i * lda + kk);
+      if (trans_b && vnni_b) brw = ldg_as<unsigned short>(pb, (long long)j * kb + s * (ldb * kb) + k2);
+      else if (trans_b) brw = ldg_as<unsigned short>(pb, kk * ldb + j);
+      else if (!vnni_b) brw = ldg_as<unsigned short>(pb, j * ldb + kk);
+      acc = __fadd_rn(acc, __fmul_rn(xb_bf16_to_f32(ar), xb_bf16_to_f32(brw)));
+    }
+  }
+  return acc;
+}
+
 // ---- fused form: column-bias pre-op, ReLU (+bitmask) / sigmoid post-op (reference :255-372) -----------------------------
 // The reference builds an f32 image of C (bias column broadcast, + old C when beta = 1), lets the GEMM accumulate into it
-// with beta = 1 and C type F32, applies the post-op and rounds ONCE into C. Per element that is: seed -> same loop as the
-// F32-output variant of the precision path -> activation -> one conversion. The pre-ops are mateltwise kernels, hence their
-// bf16 load (flushes bf16 subnormals).
+// with beta = 1 and C type F32, applies the post-op and rounds ONCE into C. Per element that is: seed -> the precision path's
+// dot_* loop, as gemm_simt_kernel runs it for an F32 C -> activation -> one conversion. The pre-ops are mateltwise kernels,
+// hence their bf16 load (flushes bf16 subnormals).
 __device__ __forceinline__ float fuse_ld(const void* p, long long i, int t) {
   if (t == LIBXSMM_DATATYPE_F32) return ((const float*)p)[i];
   if (t == LIBXSMM_DATATYPE_BF16) { unsigned short h = ((const unsigned short*)p)[i]; if ((h & 0x7f80) == 0) h &= 0x8000; return xb_bf16_to_f32(h); }
@@ -122,12 +219,9 @@ __device__ __forceinline__ void fuse_st(void* p, long long i, int t, float v) {
 
 __global__ void __launch_bounds__(256) gemm_simt_fused_kernel(const xb_gemm_launch L, const int path) {
   const xb_gemm_desc& d = L.d;
-  const int m = d.m, n = d.n, k = d.k;
-  const long long lda = d.lda, ldb = d.ldb, ldc = d.ldc;
-  const bool trans_a = (d.flags & LIBXSMM_GEMM_FLAG_TRANS_A) != 0, trans_b = (d.flags & LIBXSMM_GEMM_FLAG_TRANS_B) != 0;
-  const bool vnni_a = (d.flags & LIBXSMM_GEMM_FLAG_VNNI_A) != 0, vnni_b = (d.flags & LIBXSMM_GEMM_FLAG_VNNI_B) != 0;
-  const bool ua = (d.ta == LIBXSMM_DATATYPE_U8), ub = (d.tb == LIBXSMM_DATATYPE_U8);
-  const int tsa = xb_dev_typesize(d.ta), tsb = xb_dev_typesize(d.tb);
+  const DotGeom g = dot_geom(d);
+  const int m = d.m, n = d.n;
+  const long long ldc = d.ldc;
   const bool bias = d.fuse_colbias != 0, relu = d.cp_op == LIBXSMM_MELTW_TYPE_UNARY_RELU, sigm = d.cp_op == LIBXSMM_MELTW_TYPE_UNARY_SIGMOID;
   const bool bitm = relu && (d.cp_flags & LIBXSMM_MELTW_FLAG_UNARY_BITMASK_2BYTEMULT) != 0;
   const bool beta0 = (d.flags & LIBXSMM_GEMM_FLAG_BETA_0) != 0, beta0_eff = beta0 && !bias;
@@ -144,66 +238,19 @@ __global__ void __launch_bounds__(256) gemm_simt_fused_kernel(const xb_gemm_laun
       if (act) {
         if (bias) { const float bv = fuse_ld(x.colbias, i, d.tc); seed = beta0 ? bv : __fadd_rn(bv, fuse_ld(x.c, ci, d.tc)); }
         else if (!beta0) seed = (d.tc == LIBXSMM_DATATYPE_F32) ? ((const float*)x.c)[ci] : fuse_ld(x.c, ci, d.tc);
-        float acc = 0.0f;
+        float acc;
         switch (path) {
-          case P_F32: {
-            const bool cvt = (d.ta == LIBXSMM_DATATYPE_BF32);
-            acc = beta0_eff ? 0.0f : seed;
-            for (unsigned long long r = 0; r < x.br; ++r) {
-              const char *pa, *pb; br_ptrs(d, x, r, 4, 4, pa, pb);
-              for (int s2 = 0; s2 < k; ++s2) {
-                float av = ldg_as<float>(pa, trans_a ? (i * lda + s2) : (s2 * lda + i));
-                float bv = ldg_as<float>(pb, trans_b ? (s2 * ldb + j) : (j * ldb + s2));
-                if (cvt) { av = xb_bf16_to_f32(xb_f32_to_bf16_rne(av)); bv = xb_bf16_to_f32(xb_f32_to_bf16_rne(bv)); }
-                acc = __fadd_rn(acc, __fmul_rn(av, bv));
-              }
-            }
-          } break;
-          case P_I8_F32: {
-            unsigned int ia = 0u;
-            for (unsigned long long r = 0; r < x.br; ++r) {
-              const char *pa, *pb; br_ptrs(d, x, r, 1, 1, pa, pb);
-              for (int s2 = 0; s2 < k / 4; ++s2) for (int k2 = 0; k2 < 4; ++k2) {
-                const unsigned char ar = ldg_as<unsigned char>(pa, s2 * (lda * 4) + (long long)i * 4 + k2);
-                const unsigned char brw = ldg_as<unsigned char>(pb, j * ldb + (long long)s2 * 4 + k2);
-                ia += (unsigned int)((ua ? (int)ar : (int)(signed char)ar) * (ub ? (int)brw : (int)(signed char)brw));
-              }
-            }
-            acc = __fmul_rn((float)(int)ia, x.scf);
+          case P_F32: acc = dot_f32(d, g, x, i, j, beta0_eff ? 0.0f : seed); break;
+          case P_I8_F32:
+            __builtin_assume(d.tc == LIBXSMM_DATATYPE_F32);   // xb_path_of: P_I8_F32 has an f32 C, so dot_i8 reads VNNI4
+            acc = __fmul_rn((float)(int)dot_i8(d, g, x, i, j, 0u), x.scf);
             if (!beta0_eff) acc = __fadd_rn(acc, seed);
-          } break;
-          case P_F16_F16: case P_F16_F32: {
-            const int kb = vnni_a ? 2 : 1;
-            const bool round_each = (d.tcomp == LIBXSMM_DATATYPE_F16 || d.tcomp == LIBXSMM_DATATYPE_IMPLICIT);
-            for (unsigned long long r = 0; r < x.br; ++r) {
-              const char *pa, *pb; br_ptrs(d, x, r, 2, 2, pa, pb);
-              for (int s2 = 0; s2 < k / kb; ++s2) for (int k2 = 0; k2 < kb; ++k2) {
-                const float av = xb_f16_to_f32(ldg_as<unsigned short>(pa, s2 * (lda * kb) + (long long)i * kb + k2));
-                const long long kk = (long long)s2 * kb + k2;
-                const float bv = xb_f16_to_f32(ldg_as<unsigned short>(pb, trans_b ? (kk * ldb + j) : (j * ldb + kk)));
-                acc = __fadd_rn(acc, __fmul_rn(av, bv));
-                if (round_each) acc = xb_f16_to_f32(xb_f32_to_f16(acc));
-              }
-            }
+            break;
+          case P_F16_F16: case P_F16_F32:
+            acc = dot_f16(d, g, x, i, j, 0.0f);
             if (!beta0_eff) acc = __fadd_rn(acc, xb_f16_to_f32(xb_f32_to_f16(seed)));   // the F32-C variant rounds the old C through f16 (:2118-2124)
-          } break;
-          default: {   // P_BF16_F32 / P_BF16_BF16
-            const int kb = vnni_a ? 2 : 1;
-            acc = beta0_eff ? 0.0f : seed;
-            for (unsigned long long r = 0; r < x.br; ++r) {
-              const char *pa, *pb; br_ptrs(d, x, r, 2, 2, pa, pb);
-              for (int s2 = 0; s2 < k / kb; ++s2) for (int k2 = kb - 1; k2 >= 0; --k2) {
-                const long long kk = (long long)s2 * kb + k2;
-                unsigned short ar = 0, brw = 0;
-                if (!trans_a) ar = ldg_as<unsigned short>(pa, s2 * (lda * kb) + (long long)i * kb + k2);
-                else if (!vnni_a) ar = ldg_as<unsigned short>(pa, i * lda + kk);
-                if (trans_b && vnni_b) brw = ldg_as<unsigned short>(pb, (long long)j * kb + s2 * (ldb * kb) + k2);
-                else if (trans_b) brw = ldg_as<unsigned short>(pb, kk * ldb + j);
-                else if (!vnni_b) brw = ldg_as<unsigned short>(pb, j * ldb + kk);
-                acc = __fadd_rn(acc, __fmul_rn(xb_bf16_to_f32(ar), xb_bf16_to_f32(brw)));
-              }
-            }
-          } break;
+            break;
+          default: acc = dot_bf16(d, g, x, i, j, beta0_eff ? 0.0f : seed); break;   // P_BF16_F32 / P_BF16_BF16
         }
         y = relu ? ((acc <= 0.0f) ? 0.0f : acc) : (sigm ? (tanhf(acc / 2.0f) + 1.0f) / 2.0f : acc);
         fuse_st(x.c, ci, d.tc, y);
@@ -223,20 +270,17 @@ __global__ void __launch_bounds__(256) gemm_simt_fused_kernel(const xb_gemm_laun
       }
     }
   }
-  (void)tsa; (void)tsb;
 }
 
 __global__ void __launch_bounds__(256) gemm_simt_kernel(const xb_gemm_launch L, const int path) {
   const xb_gemm_desc& d = L.d;
+  const DotGeom g = dot_geom(d);
   const int m = d.m, n = d.n, k = d.k;
   const long long lda = d.lda, ldb = d.ldb, ldc = d.ldc;
   const bool beta0 = (d.flags & LIBXSMM_GEMM_FLAG_BETA_0) != 0;
   const bool trans_a = (d.flags & LIBXSMM_GEMM_FLAG_TRANS_A) != 0;
   const bool trans_b = (d.flags & LIBXSMM_GEMM_FLAG_TRANS_B) != 0;
   const bool vnni_a = (d.flags & LIBXSMM_GEMM_FLAG_VNNI_A) != 0;
-  const bool vnni_b = (d.flags & LIBXSMM_GEMM_FLAG_VNNI_B) != 0;
-  const bool ua = (d.ta == LIBXSMM_DATATYPE_U8), ub = (d.tb == LIBXSMM_DATATYPE_U8);
-  const int tsa = xb_dev_typesize(d.ta), tsb = xb_dev_typesize(d.tb);
 
   for (long long t = blockIdx.x; t < L.count; t += gridDim.x) {
     TileCtx x; resolve_tile(L, t, x);
@@ -256,20 +300,9 @@ __global__ void __launch_bounds__(256) gemm_simt_kernel(const xb_gemm_launch L, 
           }
           reinterpret_cast<double*>(x.c)[ci] = acc;
         } break;
-        case P_F32: {   // reference :1359-1426 (BF32: operands rounded to bf16 first)
-          const bool cvt = (d.ta == LIBXSMM_DATATYPE_BF32);
-          float acc = beta0 ? 0.0f : ldg_as<float>(x.c, ci);
-          for (unsigned long long r = 0; r < x.br; ++r) {
-            const char *pa, *pb; br_ptrs(d, x, r, 4, 4, pa, pb);
-            for (int s = 0; s < k; ++s) {
-              float av = ldg_as<float>(pa, trans_a ? (i * lda + s) : (s * lda + i));
-              float bv = ldg_as<float>(pb, trans_b ? (s * ldb + j) : (j * ldb + s));
-              if (cvt) { av = xb_bf16_to_f32(xb_f32_to_bf16_rne(av)); bv = xb_bf16_to_f32(xb_f32_to_bf16_rne(bv)); }
-              acc = __fadd_rn(acc, __fmul_rn(av, bv));
-            }
-          }
-          reinterpret_cast<float*>(x.c)[ci] = acc;
-        } break;
+        case P_F32:
+          reinterpret_cast<float*>(x.c)[ci] = dot_f32(d, g, x, i, j, beta0 ? 0.0f : ldg_as<float>(x.c, ci));
+          break;
         case P_I16: {   // reference :1427-1451 (trans flags ignored, VNNI2 A optional)
           const int kb = vnni_a ? 2 : 1;
           int acc = beta0 ? 0 : ldg_as<int>(x.c, ci);
@@ -283,19 +316,8 @@ __global__ void __launch_bounds__(256) gemm_simt_kernel(const xb_gemm_launch L, 
           }
           reinterpret_cast<int*>(x.c)[ci] = acc;
         } break;
-        case P_I8_I32: case P_I8_F32: {   // reference :1452-1683 (four sign combinations)
-          const int kb = (path == P_I8_F32) ? 4 : (vnni_a ? 4 : 1);
-          unsigned int acc = (path == P_I8_I32 && !beta0) ? (unsigned int)ldg_as<int>(x.c, ci) : 0u;
-          for (unsigned long long r = 0; r < x.br; ++r) {
-            const char *pa, *pb; br_ptrs(d, x, r, 1, 1, pa, pb);
-            for (int s = 0; s < k / kb; ++s) for (int k2 = 0; k2 < kb; ++k2) {
-              const unsigned char ar = ldg_as<unsigned char>(pa, s * (lda * kb) + (long long)i * kb + k2);
-              const unsigned char brw = ldg_as<unsigned char>(pb, j * ldb + (long long)s * kb + k2);
-              const int av = ua ? (int)ar : (int)(signed char)ar;
-              const int bv = ub ? (int)brw : (int)(signed char)brw;
-              acc += (unsigned int)(av * bv);      // wrap-around like the reference's int accumulator
-            }
-          }
+        case P_I8_I32: case P_I8_F32: {
+          const unsigned int acc = dot_i8(d, g, x, i, j, (path == P_I8_I32 && !beta0) ? (unsigned int)ldg_as<int>(x.c, ci) : 0u);
           if (path == P_I8_I32) reinterpret_cast<int*>(x.c)[ci] = (int)acc;
           else {
             float f = __fmul_rn((float)(int)acc, x.scf);
@@ -303,21 +325,8 @@ __global__ void __launch_bounds__(256) gemm_simt_kernel(const xb_gemm_launch L, 
             reinterpret_cast<float*>(x.c)[ci] = f;
           }
         } break;
-        case P_F16_F16: case P_F16_F32: {   // reference :2025-2126
-          const int kb = vnni_a ? 2 : 1;
-          // comp F16 (or IMPLICIT, resolved like an SPR host) rounds the accumulator to f16 per FMA
-          const bool round_each = (d.tcomp == LIBXSMM_DATATYPE_F16 || d.tcomp == LIBXSMM_DATATYPE_IMPLICIT);
-          float acc = 0.0f;
-          for (unsigned long long r = 0; r < x.br; ++r) {
-            const char *pa, *pb; br_ptrs(d, x, r, 2, 2, pa, pb);
-            for (int s = 0; s < k / kb; ++s) for (int k2 = 0; k2 < kb; ++k2) {
-              const float av = xb_f16_to_f32(ldg_as<unsigned short>(pa, s * (lda * kb) + (long long)i * kb + k2));
-              const long long kk = (long long)s * kb + k2;
-              const float bv = xb_f16_to_f32(ldg_as<unsigned short>(pb, trans_b ? (kk * ldb + j) : (j * ldb + kk)));
-              acc = __fadd_rn(acc, __fmul_rn(av, bv));
-              if (round_each) acc = xb_f16_to_f32(xb_f32_to_f16(acc));
-            }
-          }
+        case P_F16_F16: case P_F16_F32: {
+          float acc = dot_f16(d, g, x, i, j, 0.0f);
           if (path == P_F16_F16) {
             if (!beta0) acc = __fadd_rn(acc, xb_f16_to_f32(ldg_as<unsigned short>(x.c, ci)));
             reinterpret_cast<unsigned short*>(x.c)[ci] = xb_f32_to_f16(acc);
@@ -326,24 +335,11 @@ __global__ void __launch_bounds__(256) gemm_simt_kernel(const xb_gemm_launch L, 
             reinterpret_cast<float*>(x.c)[ci] = acc;
           }
         } break;
-        case P_BF16_F32: case P_BF16_BF16: {   // reference :2127-2170 and :2367-2419
-          const int kb = vnni_a ? 2 : 1;
+        case P_BF16_F32: case P_BF16_BF16: {
           float acc;
           if (path == P_BF16_F32) acc = beta0 ? 0.0f : ldg_as<float>(x.c, ci);
           else acc = beta0 ? 0.0f : xb_bf16_to_f32(ldg_as<unsigned short>(x.c, ci));
-          for (unsigned long long r = 0; r < x.br; ++r) {
-            const char *pa, *pb; br_ptrs(d, x, r, 2, 2, pa, pb);
-            for (int s = 0; s < k / kb; ++s) for (int k2 = kb - 1; k2 >= 0; --k2) {   // high k of a pair first
-              const long long kk = (long long)s * kb + k2;
-              unsigned short ar = 0, brw = 0;
-              if (!trans_a) ar = ldg_as<unsigned short>(pa, s * (lda * kb) + (long long)i * kb + k2);
-              else if (!vnni_a) ar = ldg_as<unsigned short>(pa, i * lda + kk);
-              if (trans_b && vnni_b) brw = ldg_as<unsigned short>(pb, (long long)j * kb + s * (ldb * kb) + k2);
-              else if (trans_b) brw = ldg_as<unsigned short>(pb, kk * ldb + j);
-              else if (!vnni_b) brw = ldg_as<unsigned short>(pb, j * ldb + kk);
-              acc = __fadd_rn(acc, __fmul_rn(xb_bf16_to_f32(ar), xb_bf16_to_f32(brw)));
-            }
-          }
+          acc = dot_bf16(d, g, x, i, j, acc);
           if (path == P_BF16_F32) reinterpret_cast<float*>(x.c)[ci] = acc;
           else reinterpret_cast<unsigned short*>(x.c)[ci] = xb_f32_to_bf16_rne(acc);
         } break;

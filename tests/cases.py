@@ -168,7 +168,7 @@ def run_gemm_ext(side, case, ops, fuse, colbias, mask, c):
     """one fused call on tile 0 of `ops` (stride / plain modes); c in/out"""
     from oracle_ffi import iarr
     return side["gemm_ext"](iarr(*case.dims), iarr(*case.types), case.flags, case.br_type, ops.stride_a, ops.stride_b, case.br,
-                            ops.a.ctypes.data, ops.b.ctypes.data, c.ctypes.data, None, None, 0.0, iarr(*fuse),
+                            ops.a.ctypes.data, ops.b.ctypes.data, c.ctypes.data, None, None, ops.scf, iarr(*fuse),
                             colbias.ctypes.data if colbias is not None else None, mask.ctypes.data if mask is not None else None)
 
 

@@ -166,7 +166,7 @@ def test_host_resident_batch_goes_through_the_copy_pipeline(pinned, monkeypatch)
 
 
 @pytest.mark.parametrize("types", [(gen.F32, gen.F32, gen.F32, gen.F32), (gen.BF16, gen.BF16, gen.F32, gen.BF16), (gen.BF16, gen.BF16, gen.F32, gen.F32),
-                                   (gen.F16, gen.F16, gen.F32, gen.F16)])
+                                   (gen.F16, gen.F16, gen.F32, gen.F16), (gen.U8, gen.I8, gen.I32, gen.F32)])
 def test_fused_brgemm_ext_matches_oracle(types):
     """libxsmm_dispatch_brgemm_ext: column-bias pre-op, ReLU (+bitmask) / sigmoid post-op, VNNI-packed C, over the matrix of
     samples/xgemm/kernel_test/gemm_kernel_fused.tpl (beta x batch-reduce mode x fusion). ReLU / bias / packing are bit-exact
@@ -181,11 +181,13 @@ def test_fused_brgemm_ext_matches_oracle(types):
                 for fuse in cases.fused_variants():
                     if fuse[3] and (tc == gen.F32 or n % 2):
                         continue
-                    flags = (cases.FLAG_BETA_0 if beta0 else 0) | (cases.FLAG_VNNI_A if ta != gen.F32 and k % 2 == 0 and m % 2 == 0 else 0)
+                    vnni_a = ta in (gen.I8, gen.U8) or (ta != gen.F32 and k % 2 == 0 and m % 2 == 0)   # int8: VNNI4 A, k % 4 == 0
+                    flags = (cases.FLAG_BETA_0 if beta0 else 0) | (cases.FLAG_VNNI_A if vnni_a else 0)
                     case = cases.GemmCase(m, n, k, ta, tb, tcomp, tc, flags=flags, br_type=br_type, br=br, pad=pad)
                     ops = cases.Operands(case, seed=int(rng.integers(1 << 30)))
                     bias = gen.values(rng, m, tc)
                     mask0 = rng.integers(0, 256, size=((case.ldc + 15) // 16 * 16) // 8 * n + 8, dtype=np.uint8)
+                    scf = C.c_float(ops.scf)     # int8 -> f32 scale, read from c.tertiary
                     want, wmask = ops.c0.copy(), mask0.copy()
                     assert cases.run_gemm_ext(oracle, case, ops, fuse, bias if fuse[0] else None, wmask if fuse[2] else None, want) == 0
                     argops = X.libxsmm_create_gemm_ext_unary_argops(0, 0, 0, 0, 0, 0, 0, 0, case.ldc, fuse[1], X.MELTW_FLAG_UNARY_BITMASK_2BYTEMULT if fuse[2] else 0, 0)
@@ -204,6 +206,7 @@ def test_fused_brgemm_ext_matches_oracle(types):
                             pa, pb, pc, pd, pm = ops.a.ctypes.data, ops.b.ctypes.data, hc.ctypes.data, bias.ctypes.data, hm.ctypes.data
                         p = X.GemmExtParam(); brv = C.c_ulonglong(case.br)
                         p.op.tertiary = C.addressof(brv); p.a.primary, p.b.primary, p.c.primary = pa, pb, pc
+                        p.c.tertiary = C.addressof(scf)
                         if fuse[0]:
                             p.d.primary = pd
                         if fuse[2]:

@@ -157,10 +157,11 @@ def test_packed_sparse_oracle_matches_reference_jit(kind):
 
 @needs_ref
 @pytest.mark.parametrize("types", [(gen.F32, gen.F32, gen.F32, gen.F32), (gen.BF16, gen.BF16, gen.F32, gen.BF16), (gen.BF16, gen.BF16, gen.F32, gen.F32),
-                                   (gen.F16, gen.F16, gen.F32, gen.F16)])
+                                   (gen.F16, gen.F16, gen.F32, gen.F16), (gen.U8, gen.I8, gen.I32, gen.F32)])
 def test_fused_gemm_restatement_matches_reference(types):
     """oracle_gemm_ext against libxsmm_reference_gemm on the extended ABI: column-bias pre-op, ReLU (+bitmask) / sigmoid post-op,
-    VNNI-packed C (generator_gemm_reference_impl.c:255-372, 2803-2842) -- bit for bit (same libm on the same host)"""
+    VNNI-packed C (generator_gemm_reference_impl.c:255-372, 2803-2842) -- bit for bit (same libm on the same host).
+    int8 -> f32 reads A as VNNI4 (every k here is a multiple of 4) and scales the product by c.tertiary."""
     rng = np.random.default_rng(88)
     ta, tb, tcomp, tc = types
     for (m, n, k, pad) in ((32, 16, 32, 0), (13, 6, 8, 3), (64, 64, 64, 0)):
@@ -169,7 +170,8 @@ def test_fused_gemm_restatement_matches_reference(types):
                 for fuse in cases.fused_variants():
                     if fuse[3] and (tc == gen.F32 or n % 2):
                         continue
-                    flags = (cases.FLAG_BETA_0 if beta0 else 0) | (cases.FLAG_VNNI_A if ta != gen.F32 and k % 2 == 0 and m % 2 == 0 else 0)
+                    vnni_a = ta in (gen.I8, gen.U8) or (ta != gen.F32 and k % 2 == 0 and m % 2 == 0)
+                    flags = (cases.FLAG_BETA_0 if beta0 else 0) | (cases.FLAG_VNNI_A if vnni_a else 0)
                     case = cases.GemmCase(m, n, k, ta, tb, tcomp, tc, flags=flags, br_type=br_type, br=br, pad=pad)
                     ops = cases.Operands(case, seed=int(rng.integers(1 << 30)))
                     bias = gen.values(rng, m, tc)
