@@ -39,6 +39,9 @@ LIBXSMM_API int libxsmm_b200_sync(void);                       /* 0, or the stic
 LIBXSMM_API int libxsmm_b200_last_error(void);
 LIBXSMM_API const char* libxsmm_b200_last_error_string(void);
 LIBXSMM_API unsigned long long libxsmm_b200_launch_count(void); /* kernels launched by this library */
+/* the same, counted per kernel family: TCGEN05 (wgmma GEMM and BCSC kernels), SIMT (exact-order GEMM, int8 dp4a, bitmap-A and
+ * BCSC kernels), STREAM (everything else); tells which kernel a call really ran, after any launch-time fallback */
+LIBXSMM_API unsigned long long libxsmm_b200_launch_count_backend(int backend);
 LIBXSMM_API int libxsmm_b200_kernel_backend(const void* kernel);
 /* BCSC handles (libxsmm_create_packed_spgemm_bcsc): the kernel a call with `n_block_columns` (= *b.quaternary) takes:
  * 0 exact-order CUDA-core kernel, 1 wgmma tensor-core kernel; -1: not BCSC */
@@ -58,6 +61,10 @@ LIBXSMM_API int libxsmm_b200_memcpy(void* dst, const void* src, size_t size); /*
  *   A + t*stride_a, B + t*stride_b, C + t*stride_c          (strides in BYTES)
  * and, inside a tile, the handle's own batch-reduce addressing (stride mode: the dispatch-time
  * br_stride hints; br_count as given). Returns 0 on success. */
+/* returned by every batch form (and a NULL plan) for a handle a batch cannot run like a single call: a fused column bias or ReLU
+ * bit mask (libxsmm_dispatch_brgemm_ext), VNNI-packed C, and for the strided forms int8 -> f32 (the scale travels in c.tertiary
+ * of a call); nothing is launched and C is left untouched */
+#define LIBXSMM_B200_ERROR_NOT_BATCHABLE (-6)
 LIBXSMM_API int libxsmm_b200_gemm_batch_strided(libxsmm_gemmfunction kernel,
   const void* a, const void* b, void* c, long long stride_a, long long stride_b, long long stride_c,
   unsigned long long br_count, long long count);

@@ -285,6 +285,7 @@ libxsmm_b200_sync = _sig("libxsmm_b200_sync", _I, [])
 libxsmm_b200_last_error = _sig("libxsmm_b200_last_error", _I, [])
 libxsmm_b200_last_error_string = _sig("libxsmm_b200_last_error_string", C.c_char_p, [])
 libxsmm_b200_launch_count = _sig("libxsmm_b200_launch_count", _ULL, [])
+libxsmm_b200_launch_count_backend = _sig("libxsmm_b200_launch_count_backend", _ULL, [_I])
 libxsmm_b200_kernel_backend = _sig("libxsmm_b200_kernel_backend", _I, [_P])
 libxsmm_b200_bcsc_variant = _sig("libxsmm_b200_bcsc_variant", _I, [_P, _ULL])
 libxsmm_b200_set_force_simt = _sig("libxsmm_b200_set_force_simt", None, [_I])

@@ -187,7 +187,7 @@ extern "C" int xb_bcsc_tc_launch(const xb_sparse_desc* d, void** work, const voi
     case 128: e = launch<64, 2>(grid, smem, stream, P); break;
     default:  e = launch<64, 4>(grid, smem, stream, P); break;
   }
-  xb_rt_count_launch();
+  xb_rt_count_launch_backend(LIBXSMM_B200_BACKEND_TCGEN05);
   if (e != cudaSuccess) { xb_rt_note_error((int)e, "bcsc_tc"); return (int)e; }
   return 0;
 }

@@ -625,7 +625,7 @@ extern "C" int xb_gemm_simt_launch(const xb_gemm_launch* L) {
     unsigned int* prefix = (unsigned int*)xb_rt_scratch((size_t)(((long long)L->d.m * L->d.k + 31) / 32) * 4 + 16);
     if (prefix == nullptr) return 2;
     gemm_bitmap_kernel<<<1, 1024, 0, (cudaStream_t)xb_rt_stream()>>>(*L, prefix);
-    xb_rt_count_launch();
+    xb_rt_count_launch_backend(LIBXSMM_B200_BACKEND_SIMT);
     const cudaError_t be = cudaGetLastError();
     if (be != cudaSuccess) { xb_rt_note_error((int)be, "gemm_bitmap"); return (int)be; }
     return 0;
@@ -634,7 +634,7 @@ extern "C" int xb_gemm_simt_launch(const xb_gemm_launch* L) {
   if (L->d.fuse_colbias != 0 || L->d.cp_op != 0) {
     const long long fgrid = L->count < (1 << 20) ? L->count : (1 << 20);
     gemm_simt_fused_kernel<<<(unsigned int)fgrid, 256, 0, (cudaStream_t)xb_rt_stream()>>>(*L, path);
-    xb_rt_count_launch();
+    xb_rt_count_launch_backend(LIBXSMM_B200_BACKEND_SIMT);
     const cudaError_t fe = cudaGetLastError();
     if (fe != cudaSuccess) { xb_rt_note_error((int)fe, "gemm_simt_fused"); return (int)fe; }
     return 0;
@@ -661,14 +661,14 @@ extern "C" int xb_gemm_simt_launch(const xb_gemm_launch* L) {
       if (tm == 4) e = launch_i8<4, 8>(*L, path, wpt, words, smem, (unsigned int)grid, st);
       else if (tm == 2) e = launch_i8<2, 4>(*L, path, wpt, words, smem, (unsigned int)grid, st);
       else e = launch_i8<1, 2>(*L, path, wpt, words, smem, (unsigned int)grid, st);
-      xb_rt_count_launch();
+      xb_rt_count_launch_backend(LIBXSMM_B200_BACKEND_SIMT);
       if (e != cudaSuccess) { xb_rt_note_error((int)e, "gemm_i8"); return (int)e; }
       return 0;
     }
   }
   const long long grid = L->count < (1 << 20) ? L->count : (1 << 20);
   gemm_simt_kernel<<<(unsigned int)grid, 256, 0, (cudaStream_t)xb_rt_stream()>>>(*L, path);
-  xb_rt_count_launch();
+  xb_rt_count_launch_backend(LIBXSMM_B200_BACKEND_SIMT);
   const cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) { xb_rt_note_error((int)e, "gemm_simt"); return (int)e; }
   return 0;

@@ -256,7 +256,7 @@ int wg_launch(int amode, int wg, int nt, const WgParams& P, int ctas, const CUte
   if (amode == XB_WG_SS16) e = (wg == 2) ? launch_n<XB_WG_SS16, 2>(nt, grid, smem, stream, ma, mb, P) : launch_n<XB_WG_SS16, 1>(nt, grid, smem, stream, ma, mb, P);
   else if (amode == XB_WG_RS16) e = (wg == 2) ? launch_n<XB_WG_RS16, 2>(nt, grid, smem, stream, ma, mb, P) : launch_n<XB_WG_RS16, 1>(nt, grid, smem, stream, ma, mb, P);
   else e = (wg == 2) ? launch_n<XB_WG_RS8, 2>(nt, grid, smem, stream, ma, mb, P) : launch_n<XB_WG_RS8, 1>(nt, grid, smem, stream, ma, mb, P);
-  xb_rt_count_launch();
+  xb_rt_count_launch_backend(LIBXSMM_B200_BACKEND_TCGEN05);
   if (e != cudaSuccess) { xb_rt_note_error((int)e, where); return (int)e; }
   return 0;
 }

@@ -528,6 +528,16 @@ static const xb_slot* xb_gemm_slot(const void* kernel) {
   return (s != NULL && (s->kind == XB_KIND_GEMM || s->kind == XB_KIND_GEMM_EXT)) ? s : NULL;
 }
 
+/* 1 if a batch entry point cannot run this handle as a single call would: a fused handle's bias column and ReLU bit mask are
+ * per-call operands (libxsmm_gemm_ext_param) that no batch form carries, VNNI-packed C is re-packed by a pass after a single
+ * call only, and the strided forms have no argument struct for the int8 -> f32 scale (c.tertiary) */
+static int xb_batch_refused(const xb_gemm_desc* d, int strided) {
+  const int i8 = (d->ta == LIBXSMM_DATATYPE_I8 || d->ta == LIBXSMM_DATATYPE_U8);
+  if (d->fuse_colbias != 0 || (d->flags & LIBXSMM_GEMM_FLAG_VNNI_C) != 0) return 1;
+  if (d->cp_op == LIBXSMM_MELTW_TYPE_UNARY_RELU && (d->cp_flags & LIBXSMM_MELTW_FLAG_UNARY_BITMASK_2BYTEMULT) != 0) return 1;
+  return (strided && i8 && d->tc == LIBXSMM_DATATYPE_F32) ? 1 : 0;
+}
+
 /* host-resident strided batch: chunked H2D -> kernel -> D2H through device scratch */
 static int xb_gemm_batch_strided_host(const xb_slot* s, const void* a, const void* b, void* c,
   long long sa, long long sb, long long sc, unsigned long long br, long long count);
@@ -539,6 +549,7 @@ LIBXSMM_API int libxsmm_b200_gemm_batch_strided(libxsmm_gemmfunction kernel, con
   xb_gemm_launch L;
   int rc;
   if (s == NULL || count < 0) return -1;
+  if (xb_batch_refused(&s->u.gemm, 1)) return LIBXSMM_B200_ERROR_NOT_BATCHABLE;
   if (s->u.gemm.br_type == 1 || s->u.gemm.br_type == 2) return -2;   /* address / offset mode need per-tile arrays: use libxsmm_b200_gemm_batch */
   if (count == 0) return 0;
   {
@@ -588,6 +599,7 @@ LIBXSMM_API int libxsmm_b200_gemm_batch_strided_multi(libxsmm_gemmfunction kerne
   int d, rc = 0, started = 0, prev_dev;
   const int avail = xb_rt_device_count();
   if (xb_gemm_slot((const void*)kernel) == NULL || count < 0 || ndevices <= 0) return -1;
+  if (xb_batch_refused(&xb_gemm_slot((const void*)kernel)->u.gemm, 1)) return LIBXSMM_B200_ERROR_NOT_BATCHABLE;
   if (ndevices > avail) ndevices = avail;
   if (ndevices > 64) ndevices = 64;
   if (ndevices <= 0) return -1;
@@ -764,7 +776,7 @@ LIBXSMM_API libxsmm_b200_gemm_plan* libxsmm_b200_gemm_plan_create(libxsmm_gemmfu
   xb_gemm_rec* recs;
   char* arrays = NULL; size_t arrays_bytes = 0, off = 0;
   long long t;
-  if (s == NULL || params == NULL || count <= 0) return NULL;
+  if (s == NULL || params == NULL || count <= 0 || xb_batch_refused(&s->u.gemm, 0)) return NULL;
   plan = (libxsmm_b200_gemm_plan*)calloc(1, sizeof(*plan));
   if (plan != NULL && xb_plan_try_pool(plan, s, params, count)) return plan;
   recs = (xb_gemm_rec*)calloc((size_t)count, sizeof(xb_gemm_rec));
@@ -830,8 +842,10 @@ LIBXSMM_API void libxsmm_b200_gemm_plan_destroy(libxsmm_b200_gemm_plan* plan) {
 }
 
 LIBXSMM_API int libxsmm_b200_gemm_batch(libxsmm_gemmfunction kernel, const libxsmm_gemm_param* params, long long count) {
+  const xb_slot* s = xb_gemm_slot((const void*)kernel);
   libxsmm_b200_gemm_plan* plan;
   int rc;
+  if (s != NULL && xb_batch_refused(&s->u.gemm, 0)) return LIBXSMM_B200_ERROR_NOT_BATCHABLE;
   if (count == 0) return 0;
   plan = libxsmm_b200_gemm_plan_create(kernel, params, count);
   if (plan == NULL) return -1;

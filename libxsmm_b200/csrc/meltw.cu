@@ -808,7 +808,7 @@ __global__ void __launch_bounds__(256) meltw_split_kernel(const xb_meltw_desc d,
 }
 
 int launch_done(const char* where) {
-  xb_rt_count_launch();
+  xb_rt_count_launch_backend(LIBXSMM_B200_BACKEND_STREAM);
   const cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) { xb_rt_note_error((int)e, where); return (int)e; }
   return 0;

@@ -20,6 +20,7 @@ struct ThreadState {
 thread_local ThreadState tls;
 std::atomic<int> g_last_error{0};
 std::atomic<unsigned long long> g_launches{0};
+std::atomic<unsigned long long> g_launches_by[LIBXSMM_B200_BACKEND_NOOP + 1];   // per kernel family (libxsmm_b200_backend)
 char g_error_where[128] = {0};
 int g_have_gpu = -1;
 }  // namespace
@@ -83,6 +84,13 @@ const char* xb_rt_last_error_string(void) {
 
 unsigned long long xb_rt_launch_count(void) { return g_launches.load(); }
 void xb_rt_count_launch(void) { g_launches.fetch_add(1, std::memory_order_relaxed); }
+void xb_rt_count_launch_backend(int backend) {
+  xb_rt_count_launch();
+  if (backend >= 0 && backend <= LIBXSMM_B200_BACKEND_NOOP) g_launches_by[backend].fetch_add(1, std::memory_order_relaxed);
+}
+LIBXSMM_API unsigned long long libxsmm_b200_launch_count_backend(int backend) {
+  return (backend >= 0 && backend <= LIBXSMM_B200_BACKEND_NOOP) ? g_launches_by[backend].load() : 0ull;
+}
 
 void* xb_rt_device_malloc(size_t size) {
   void* p = nullptr;

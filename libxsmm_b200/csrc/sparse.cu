@@ -288,6 +288,7 @@ __global__ void __launch_bounds__(256) bcsc_simt_kernel(const BcscParams Q) {
       }
       for (unsigned int z = Q.colptr[jb]; z < Q.colptr[jb + 1]; ++z) {
         const int kb = (int)Q.rowidx[z];
+        if (kb >= Q.K / Q.bk) continue;            // block-row outside A: ignored, like the tensor-core kernel
         for (int kk = 0; kk < Q.bk; ++kk) {
           const int k = kb * Q.bk + kk;
           size_t ai;
@@ -319,8 +320,8 @@ int num_sms() {
   if (g_sms == 0) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&g_sms, cudaDevAttrMultiProcessorCount, dev); if (g_sms <= 0) g_sms = 132; }
   return g_sms;
 }
-int check_launch(const char* where) {
-  xb_rt_count_launch();
+int check_launch(const char* where, int backend = LIBXSMM_B200_BACKEND_STREAM) {
+  xb_rt_count_launch_backend(backend);
   const cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) { xb_rt_note_error((int)e, where); return (int)e; }
   return 0;
@@ -428,5 +429,5 @@ extern "C" int xb_bcsc_launch(xb_sparse_desc* d, const void* a, const void* b_va
   const long long work = Q.m_blocks * (long long)n_blocks;
   const unsigned int grid = (unsigned int)(work < (1 << 20) ? work : (1 << 20));
   bcsc_simt_kernel<<<grid, 256, 0, (cudaStream_t)xb_rt_stream()>>>(Q);
-  return check_launch("bcsc_simt");
+  return check_launch("bcsc_simt", LIBXSMM_B200_BACKEND_SIMT);
 }

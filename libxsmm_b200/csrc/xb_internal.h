@@ -122,6 +122,9 @@ const char* xb_rt_last_error_string(void);
 void xb_rt_note_error(int code, const char* where);
 unsigned long long xb_rt_launch_count(void);
 void xb_rt_count_launch(void);
+/* xb_rt_count_launch() plus one in the count of the kernel's family `backend` (libxsmm_b200_backend); the per-family counts and
+ * libxsmm_b200_launch_count_backend live in runtime.cu next to the launchers that feed them */
+void xb_rt_count_launch_backend(int backend);
 void* xb_rt_device_malloc(size_t size);
 void xb_rt_device_free(void* p);
 void* xb_rt_host_malloc(size_t size);

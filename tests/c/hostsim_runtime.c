@@ -17,7 +17,7 @@ extern int oracle_meltw(const int* desc, void* param, int mode);
 /* ---- runtime ------------------------------------------------------------------------------------------------------------- */
 static __thread void* g_blocks[4096]; static __thread int g_nblocks = 0;
 static __thread int g_err = 0; static __thread char g_errs[256];
-static unsigned long long g_launches = 0;
+static unsigned long long g_launches = 0, g_launches_by[LIBXSMM_B200_BACKEND_NOOP + 1];   /* all, and per kernel family */
 
 int xb_rt_device_count(void) { return 1; }
 int xb_rt_set_device(int ordinal) { return ordinal == 0 ? 0 : 1; }
@@ -31,6 +31,10 @@ const char* xb_rt_last_error_string(void) { return g_errs; }
 void xb_rt_note_error(int code, const char* where) { g_err = code; snprintf(g_errs, sizeof(g_errs), "%s", where); fprintf(stderr, "hostsim: error %d: %s\n", code, where); }
 unsigned long long xb_rt_launch_count(void) { return g_launches; }
 void xb_rt_count_launch(void) { ++g_launches; }
+/* the library defines this next to its launchers (runtime.cu); here every GEMM tile is an exact-order launch, everything else streams */
+LIBXSMM_API unsigned long long libxsmm_b200_launch_count_backend(int backend) {
+  return (backend >= 0 && backend <= LIBXSMM_B200_BACKEND_NOOP) ? g_launches_by[backend] : 0ull;
+}
 void* xb_rt_device_malloc(size_t size) { return malloc(size); }
 void xb_rt_device_free(void* p) { free(p); }
 void* xb_rt_host_malloc(size_t size) { return malloc(size); }
@@ -94,7 +98,7 @@ extern int oracle_gemm_bitmap(const int* dims, const int* types, unsigned int fl
 static int sim_gemm_tile(const xb_gemm_desc* d, const xb_gemm_rec* r) {
   const int dims[6] = { d->m, d->n, d->k, d->lda, d->ldb, d->ldc }, types[4] = { d->ta, d->tb, d->tcomp, d->tc };
   const unsigned int flags = d->flags & ~(unsigned int)LIBXSMM_GEMM_FLAG_VNNI_C;
-  ++g_launches;
+  ++g_launches; ++g_launches_by[LIBXSMM_B200_BACKEND_SIMT];
   if ((d->flags & LIBXSMM_GEMM_FLAG_DECOMPRESS_A_VIA_BITMASK) != 0) return oracle_gemm_bitmap(dims, types, flags, r->a, r->b, r->c, (const unsigned char*)r->a_q);
   if (d->ta == LIBXSMM_DATATYPE_I4X2 || d->ta == LIBXSMM_DATATYPE_U4X2) {
     return oracle_gemm_i4(dims, flags, d->br_type, d->br_stride_a, d->br_stride_b, r->br, (const unsigned char*)r->a, (const unsigned char*)r->b, (int*)r->c, (const unsigned char*)r->a_q);
@@ -130,7 +134,7 @@ int xb_gemm_ts_launch(const xb_gemm_launch* L) { (void)L; return 1; }
  * ({value, 512 * column}); the accumulation order per element is the row order, like the library's direct kernel */
 int xb_sreg_launch(const xb_sparse_desc* d, const void* b, void* c, long long n_total) {
   const int f64 = (d->ta == LIBXSMM_DATATYPE_F64); int row; long long col; unsigned int z;
-  ++g_launches;
+  ++g_launches; ++g_launches_by[LIBXSMM_B200_BACKEND_STREAM];
   for (row = 0; row < d->m; ++row) for (col = 0; col < n_total; ++col) {
     if (f64) {
       double acc = 0, *dst = (double*)c + (size_t)row * d->ldc + col;
@@ -168,7 +172,7 @@ int xb_meltw_launch(const xb_meltw_desc* d, const xb_meltw_args* a) {
   desc[0] = d->op_class; desc[1] = d->op; desc[2] = (int)d->flags; desc[3] = d->m; desc[4] = d->n; desc[5] = d->ldi; desc[6] = d->ldi2; desc[7] = d->ldi3;
   desc[8] = d->ldo; desc[9] = d->t_in0; desc[10] = d->t_in1; desc[11] = d->t_in2; desc[12] = d->t_out; desc[13] = d->t_comp;
   if (a->n_rt != 0) return 1;
-  ++g_launches;
+  ++g_launches; ++g_launches_by[LIBXSMM_B200_BACKEND_STREAM];
   if (d->op_class == LIBXSMM_MELTW_OPERATION_UNARY) {
     libxsmm_meltw_unary_param p; memset(&p, 0, sizeof(p));
     p.in.primary = (void*)(uintptr_t)a->in0; p.in.secondary = (void*)(uintptr_t)a->in_aux; p.out.primary = a->out; p.out.secondary = a->out_aux; p.op.primary = &alpha;

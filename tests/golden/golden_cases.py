@@ -20,6 +20,18 @@ def gemm_cases():
     return out
 
 
+def int8_full_range():
+    """(GemmCase, Operands): U8 in [0, 255] x I8 in [-128, 127] -> I32 over VNNI4 A with a stride batch-reduce, and an old C spread over
+    the whole int32 range so that beta = 1 wraps; gen.values keeps 8-bit operands within +-20"""
+    case = cases.GemmCase(48, 20, 128, gen.U8, gen.I8, gen.I32, gen.I32, flags=cases.FLAG_VNNI_A, br_type=3, br=3)
+    ops = cases.Operands(case, seed=80, count=2)
+    rng = np.random.default_rng(81)
+    ops.a = rng.integers(0, 256, size=ops.a.size).astype(np.uint8)
+    ops.b = rng.integers(-128, 128, size=ops.b.size).astype(np.int8)
+    ops.c0 = rng.integers(-2 ** 31, 2 ** 31, size=ops.c0.size).astype(np.int32)
+    return case, ops
+
+
 # ---- BCSC (reference: x86 JIT of libxsmm_create_packed_spgemm_bcsc; gold loop samples/xgemm_sparse/spmm_kernel.c:74-217)
 def bcsc_cases():
     T_BF, T_F32, T_U8I8, T_I8U8 = (gen.BF16, gen.BF16, gen.F32, gen.BF16), (gen.F32,) * 4, (gen.U8, gen.I8, gen.I32, gen.I32), (gen.I8, gen.U8, gen.I32, gen.I32)

@@ -29,10 +29,10 @@ def crc(*arrs):
 
 
 def main():
-    """usage: make_golden.py [gemm] [sparse] [mtx]  (default: all). The sparse sections need a host whose ISA the reference's JIT can build
+    """usage: make_golden.py [gemm] [int8] [sparse] [mtx]  (default: all). The sparse sections need a host whose ISA the reference's JIT can build
     BCSC bf16 for (AVX512-BF16 / AMX: the GPU box); the GEMM section runs on any x86-64 host."""
     import sys
-    want = set(sys.argv[1:]) or {"gemm", "sparse", "mtx"}
+    want = set(sys.argv[1:]) or {"gemm", "int8", "sparse", "mtx"}
     assert ref is not None, "oracle/_ref/libxsmm_ref.so is missing: run `make ref` where /root/reference exists"
     out = {}
     for i, (case, seed, count) in enumerate(G.gemm_cases() if "gemm" in want else []):
@@ -42,6 +42,10 @@ def main():
     if "gemm" in want:
         np.savez_compressed(os.path.join(HERE, "gemm.npz"), **out)
         print("gemm.npz: %d cases" % (len(out) // 2))
+    if "int8" in want:
+        case, ops = G.int8_full_range()
+        np.savez_compressed(os.path.join(HERE, "int8.npz"), gemm=cases.ref_result(ref, case, ops, run_gemm), crc=crc(ops.a, ops.b, ops.c0))
+        print("int8.npz: 1 case")
     if "sparse" not in want and "mtx" not in want:
         return
 

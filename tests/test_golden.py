@@ -20,6 +20,7 @@ import golden_cases as G  # noqa: E402
 from oracle_ffi import oracle, run_gemm  # noqa: E402
 
 GEMM = np.load(os.path.join(HERE, "golden", "gemm.npz"))
+INT8 = np.load(os.path.join(HERE, "golden", "int8.npz"))
 SPARSE = np.load(os.path.join(HERE, "golden", "sparse.npz"))
 MTX = np.load(os.path.join(HERE, "golden", "mtx.npz"))
 
@@ -45,6 +46,12 @@ def test_gemm_golden_pins_the_oracle():
         assert crc(ops.a, ops.b, ops.c0) == GEMM["gemm_%03d_crc" % i], "input generator drifted: regenerate the fixtures"
         got = cases.ref_result(oracle, case, ops, run_gemm)
         assert np.array_equal(got.view(np.uint8), GEMM["gemm_%03d" % i].view(np.uint8)), case
+
+
+def test_int8_full_range_golden_pins_the_oracle():
+    case, ops = G.int8_full_range()
+    assert crc(ops.a, ops.b, ops.c0) == INT8["crc"], "input generator drifted: regenerate the fixtures"
+    assert np.array_equal(cases.ref_result(oracle, case, ops, run_gemm), INT8["gemm"]), case
 
 
 def test_sparse_golden_pins_the_oracle():
@@ -128,6 +135,27 @@ def test_gemm_golden_on_gpu():
                     assert np.array_equal(got.view(np.uint8), want.view(np.uint8)), case
         finally:
             X.libxsmm_b200_set_force_simt(0)
+
+
+@pytest.mark.gpu
+def test_int8_full_range_golden_on_gpu():
+    """the full-range int8 vector on the wgmma kernel (strided batch) and on the dp4a kernel (forced exact-order): bit for bit"""
+    import libxsmm_b200 as X
+    from gpu_util import dev, dispatch, host
+    case, ops = G.int8_full_range()
+    for force_simt, backend in ((0, X.BACKEND_TCGEN05), (1, X.BACKEND_SIMT)):
+        X.libxsmm_b200_set_force_simt(force_simt)
+        try:
+            kernel = dispatch(case, ops)
+        finally:
+            X.libxsmm_b200_set_force_simt(0)
+        assert kernel and X.libxsmm_b200_kernel_backend(kernel) == backend
+        d_a, d_b, d_c = dev(ops.a), dev(ops.b), dev(ops.c0)
+        before = X.libxsmm_b200_launch_count_backend(backend)
+        assert X.libxsmm_b200_gemm_batch_strided(kernel, d_a.data_ptr(), d_b.data_ptr(), d_c.data_ptr(), ops.tile_a, ops.tile_b, ops.tile_c, case.br, ops.count) == 0
+        X.check()
+        assert X.libxsmm_b200_launch_count_backend(backend) > before
+        assert np.array_equal(host(d_c, np.int32), INT8["gemm"]), backend
 
 
 @pytest.mark.gpu

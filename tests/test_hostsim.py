@@ -339,3 +339,66 @@ def test_host_resident_strided_batch_through_the_chunked_pipeline(sim):
                 acc += b[t, r, :, :k].astype(np.float64) @ a[t, r, :, :m].astype(np.float64)        # C^T[n][m] = B^T[n][k] A^T[k][m]
             assert np.allclose(c[t, :, :m], acc, rtol=1e-5, atol=1e-5), (beta0, t)
             assert np.array_equal(c[t, :, m:], c0[t, :, m:]), "padding rows of C survive"
+
+
+def test_batch_entry_points_refuse_handles_they_cannot_run_like_a_single_call(sim):
+    """A fused handle's bias column and ReLU bit mask are operands of one call (libxsmm_gemm_ext_param), VNNI-packed C is re-packed after a
+    single call only, and the strided forms have no place for the int8 -> f32 scale of c.tertiary. Every batch form refuses such a handle with
+    LIBXSMM_B200_ERROR_NOT_BATCHABLE before anything runs: C keeps its bytes and no kernel is counted. The int8 -> f32 handle stays usable
+    through libxsmm_b200_gemm_batch, whose argument structs carry one scale per tile."""
+    lib = sim.lib
+    I, U, P, LL, ULL, UB = C.c_int, C.c_uint, C.c_void_p, C.c_longlong, C.c_ulonglong, C.c_ubyte
+    for name, res, args in (("libxsmm_create_gemm_shape", X.GemmShape, [I] * 10), ("libxsmm_create_gemm_batch_reduce_config", X.BatchReduceConfig, [I, I, I, UB]),
+                            ("libxsmm_create_gemm_ext_unary_argops", X.GemmExtUnaryArgops, [I, I, U, I, I, I, U, I, I, I, U, I]),
+                            ("libxsmm_create_gemm_ext_binary_postops", X.GemmExtBinaryPostops, [I, I, I, U]),
+                            ("libxsmm_dispatch_gemm", P, [X.GemmShape, U, U]),
+                            ("libxsmm_dispatch_brgemm_ext", P, [X.GemmShape, U, U, X.BatchReduceConfig, X.GemmExtUnaryArgops, X.GemmExtBinaryPostops]),
+                            ("libxsmm_b200_gemm_batch_strided", I, [P, P, P, P, LL, LL, LL, ULL, LL]),
+                            ("libxsmm_b200_gemm_batch_strided_multi", I, [P, P, P, P, LL, LL, LL, ULL, LL, I]),
+                            ("libxsmm_b200_gemm_batch", I, [P, C.POINTER(X.GemmParam), LL]), ("libxsmm_b200_gemm_plan_create", P, [P, C.POINTER(X.GemmParam), LL]),
+                            ("libxsmm_b200_launch_count", ULL, []), ("libxsmm_b200_launch_count_backend", ULL, [I])):
+        fn = getattr(lib, name); fn.restype = res; fn.argtypes = args
+    NOT_BATCHABLE = -6          # include/libxsmm_b200.h
+    m, n, k, count = 16, 8, 16, 3
+    nobr = lib.libxsmm_create_gemm_batch_reduce_config(X.GEMM_BATCH_REDUCE_NONE, 0, 0, 0)
+    no_post = lib.libxsmm_create_gemm_ext_binary_postops(0, 0, 0, 0)
+    no_arg = lib.libxsmm_create_gemm_ext_unary_argops(0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0)
+    f32 = lib.libxsmm_create_gemm_shape(m, n, k, m, k, m, F32, F32, F32, F32)
+    handles = {
+        "column bias": lib.libxsmm_dispatch_brgemm_ext(f32, 0, 0, nobr, no_arg,
+                                                       lib.libxsmm_create_gemm_ext_binary_postops(m, F32, X.MELTW_TYPE_BINARY_ADD, X.MELTW_FLAG_BINARY_BCAST_COL_IN_0)),
+        "relu bit mask": lib.libxsmm_dispatch_brgemm_ext(f32, 0, 0, nobr, lib.libxsmm_create_gemm_ext_unary_argops(
+            0, 0, 0, 0, 0, 0, 0, 0, m, X.MELTW_TYPE_UNARY_RELU, X.MELTW_FLAG_UNARY_BITMASK_2BYTEMULT, 0), no_post),
+        "vnni c": lib.libxsmm_dispatch_gemm(lib.libxsmm_create_gemm_shape(m, n, k, m, k, m, BF16, BF16, BF16, F32), X.GEMM_FLAG_VNNI_A | X.GEMM_FLAG_VNNI_C, 0),
+        "int8 to f32": lib.libxsmm_dispatch_gemm(lib.libxsmm_create_gemm_shape(m, n, k, m, k, m, gen.U8, gen.I8, F32, gen.I32), X.GEMM_FLAG_VNNI_A, 0),
+    }
+    rng = np.random.default_rng(12)
+    a = rng.integers(0, 256, size=count * m * k * 4, dtype=np.uint8); b = rng.integers(0, 256, size=count * k * n * 4, dtype=np.uint8)
+    sa, sb, sc = m * k * 4, k * n * 4, m * n * 4
+    scales = [C.c_float(2.0 ** -(t + 1)) for t in range(count)]
+    for what, fn in handles.items():
+        assert fn, what
+        c = rng.integers(0, 256, size=count * sc, dtype=np.uint8); c0 = c.copy()
+        params = (X.GemmParam * count)()
+        for t in range(count):
+            params[t].a.primary, params[t].b.primary, params[t].c.primary = a.ctypes.data + t * sa, b.ctypes.data + t * sb, c.ctypes.data + t * sc
+            params[t].c.tertiary = C.addressof(scales[t])
+        before = [lib.libxsmm_b200_launch_count()] + [lib.libxsmm_b200_launch_count_backend(x) for x in (X.BACKEND_SIMT, X.BACKEND_TCGEN05, X.BACKEND_STREAM)]
+        assert lib.libxsmm_b200_gemm_batch_strided(fn, a.ctypes.data, b.ctypes.data, c.ctypes.data, sa, sb, sc, 1, count) == NOT_BATCHABLE, what
+        assert lib.libxsmm_b200_gemm_batch_strided_multi(fn, a.ctypes.data, b.ctypes.data, c.ctypes.data, sa, sb, sc, 1, count, 1) == NOT_BATCHABLE, what
+        if what != "int8 to f32":
+            assert lib.libxsmm_b200_gemm_batch(fn, params, count) == NOT_BATCHABLE, what
+            assert not lib.libxsmm_b200_gemm_plan_create(fn, params, count), what
+        after = [lib.libxsmm_b200_launch_count()] + [lib.libxsmm_b200_launch_count_backend(x) for x in (X.BACKEND_SIMT, X.BACKEND_TCGEN05, X.BACKEND_STREAM)]
+        assert after == before, (what, before, after)
+        assert np.array_equal(c, c0), what
+        if what == "int8 to f32":     # one scale per argument struct: this form runs, one exact-order tile per struct
+            assert lib.libxsmm_b200_gemm_batch(fn, params, count) == 0
+            assert lib.libxsmm_b200_launch_count_backend(X.BACKEND_SIMT) == before[1] + count
+            want = c0.copy()
+            for t in range(count):
+                p = X.GemmParam()
+                p.a.primary, p.b.primary, p.c.primary, p.c.tertiary = a.ctypes.data + t * sa, b.ctypes.data + t * sb, want.ctypes.data + t * sc, C.addressof(scales[t])
+                X.GEMMFUNCTION(fn)(C.byref(p))
+            assert np.array_equal(c, want)
+            assert not np.array_equal(c, c0)

@@ -57,6 +57,32 @@ def test_reference_jit_agrees_with_reference_kernel():
         assert gen.normf_rel(gen.to_f64(c_ref, t[3]), gen.to_f64(c_jit, t[3])) <= thr
 
 
+@needs_ref
+def test_int8_full_range_restatement_is_bit_exact():
+    """U8 in [0, 255] and I8 in [-128, 127] in all four sign combinations (gen.values stays within +-20), VNNI4 and flat A, I32 C over the
+    whole int32 range (beta = 1 wraps) and the scaled F32 C; plus one U8 x U8 case of 255s whose sums pass 2^31 and wrap"""
+    rng = np.random.default_rng(23)
+    for ta, tb in ((gen.U8, gen.U8), (gen.U8, gen.I8), (gen.I8, gen.U8), (gen.I8, gen.I8)):
+        for tc, vnni in ((gen.I32, 1), (gen.I32, 0), (gen.F32, 1)):
+            for beta0 in (0, 1):
+                flags = (cases.FLAG_BETA_0 if beta0 else 0) | (cases.FLAG_VNNI_A if vnni else 0)
+                case = cases.GemmCase(24, 13, 36, ta, tb, gen.I32, tc, flags=flags, br_type=3, br=3, pad=2)
+                ops = cases.Operands(case, seed=int(rng.integers(1 << 30)), count=2)
+                ops.a = rng.integers(-128 if ta == gen.I8 else 0, 128 if ta == gen.I8 else 256, size=ops.a.size).astype(gen.NP_OF[ta])
+                ops.b = rng.integers(-128 if tb == gen.I8 else 0, 128 if tb == gen.I8 else 256, size=ops.b.size).astype(gen.NP_OF[tb])
+                if tc == gen.I32:
+                    ops.c0 = rng.integers(-2 ** 31, 2 ** 31, size=ops.c0.size).astype(np.int32)
+                want = cases.ref_result(ref, case, ops, run_gemm)
+                got = cases.ref_result(oracle, case, ops, run_gemm)
+                assert np.array_equal(want.view(np.uint8), got.view(np.uint8)), case
+    case = cases.GemmCase(16, 4, 1024, gen.U8, gen.U8, gen.I32, gen.I32, flags=cases.FLAG_BETA_0 | cases.FLAG_VNNI_A, br_type=3, br=36)
+    ops = cases.Operands(case, count=1)
+    ops.a[:] = 255; ops.b[:] = 255
+    want = cases.ref_result(ref, case, ops, run_gemm)
+    assert np.all(want == np.int32(255 * 255 * 1024 * 36 - 2 ** 32)), "255^2 * 36864 wraps to a negative int32"
+    assert np.array_equal(want, cases.ref_result(oracle, case, ops, run_gemm))
+
+
 def _bcsc_inputs(rng, ta, tb, tc, mblocks, M, K, N, bk, bn, density, vnni_a=True, trans_a=False):
     nbr, nbc = K // bk, N // bn
     keep = rng.random((nbc, nbr)) < density
