@@ -14,6 +14,7 @@
 #define LIBXSMM_B200_H
 
 #include "libxsmm_typedefs.h"
+#include "libxsmm_fsspmdm.h"
 
 #if defined(__cplusplus)
 extern "C" {
@@ -46,6 +47,10 @@ LIBXSMM_API int libxsmm_b200_kernel_backend(const void* kernel);
 /* BCSC handles (libxsmm_create_packed_spgemm_bcsc): the kernel a call with `n_block_columns` (= *b.quaternary) takes:
  * 0 exact-order CUDA-core kernel, 1 wgmma tensor-core kernel; -1: not BCSC */
 LIBXSMM_API int libxsmm_b200_bcsc_variant(const void* kernel, unsigned long long n_block_columns);
+/* fsspmdm handles: the kernel libxsmm_fsspmdm_execute(handle, B, C) takes: 0 direct kernel (no shared-memory staging), S = 1..3 the
+ * TMA-staged kernel with S shared-memory stages; -1: NULL handle. Pageable host B / C are answered for the device buffers they are
+ * staged through. */
+LIBXSMM_API int libxsmm_b200_fsspmdm_variant(const libxsmm_fsspmdm* handle, const void* B, const void* C);
 /* force the SIMT kernel for dense GEMM handles dispatched afterwards (debug / parity checking) */
 LIBXSMM_API void libxsmm_b200_set_force_simt(int on);
 

@@ -288,6 +288,7 @@ libxsmm_b200_launch_count = _sig("libxsmm_b200_launch_count", _ULL, [])
 libxsmm_b200_launch_count_backend = _sig("libxsmm_b200_launch_count_backend", _ULL, [_I])
 libxsmm_b200_kernel_backend = _sig("libxsmm_b200_kernel_backend", _I, [_P])
 libxsmm_b200_bcsc_variant = _sig("libxsmm_b200_bcsc_variant", _I, [_P, _ULL])
+libxsmm_b200_fsspmdm_variant = _sig("libxsmm_b200_fsspmdm_variant", _I, [_P, _P, _P])
 libxsmm_b200_set_force_simt = _sig("libxsmm_b200_set_force_simt", None, [_I])
 libxsmm_b200_device_malloc = _sig("libxsmm_b200_device_malloc", _P, [C.c_size_t])
 libxsmm_b200_device_free = _sig("libxsmm_b200_device_free", None, [_P])

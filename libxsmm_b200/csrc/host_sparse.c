@@ -375,6 +375,10 @@ LIBXSMM_API void libxsmm_fsspmdm_execute(const libxsmm_fsspmdm* handle, const vo
   p.b.primary = (void*)(uintptr_t)B; p.c.primary = C;
   handle->kernel(&p);
 }
+const xb_sparse_desc* xb_fsspmdm_desc(const libxsmm_fsspmdm* handle) {
+  const xb_slot* s = (handle != NULL) ? xb_slot_of((const void*)handle->kernel) : NULL;
+  return (s != NULL && s->kind == XB_KIND_SREG) ? &s->u.sp : NULL;
+}
 LIBXSMM_API void libxsmm_dfsspmdm_execute(const libxsmm_dfsspmdm* handle, const double* B, double* C) { libxsmm_fsspmdm_execute(handle, B, C); }
 LIBXSMM_API void libxsmm_sfsspmdm_execute(const libxsmm_sfsspmdm* handle, const float* B, float* C) { libxsmm_fsspmdm_execute(handle, B, C); }
 

@@ -1,7 +1,7 @@
 // libxsmm_b200 -- sparse kernels of the hot path (sm_90a):
 //   * sreg_kernel      : fsspmdm -- fixed sparse A (CSR, alpha folded in) times dense row-major B,
 //                        N streamed through shared memory in 512-byte column strips with
-//                        cp.async.bulk (TMA 1D) + mbarrier double buffering. HBM-bound.
+//                        TMA 2D tensor copies into a ring of 1 to 3 mbarrier-guarded stages. HBM-bound.
 //                        Replaces src/generator_spgemm_csr_asparse_reg.c (A kept in registers on x86).
 //   * packed_sp_kernel : SOA-packed sparse x dense with `packed_width` innermost
 //                        (src/generator_packed_spgemm_cs*.c; golds in samples/xgemm_norm_packed/*.c)
@@ -92,15 +92,13 @@ __global__ void __launch_bounds__(1024, 1) sreg_kernel(const __grid_constant__ C
   T* Cg = (T*)P.c;
   const int S = P.stages;
 
-  // producer: one TMA tensor copy per strip (box = 512 bytes x min(K,256) rows; columns past N are zero-filled)
+  // producer: one TMA tensor copy per strip (box = 512 bytes x K rows, K <= 256; columns past N are zero-filled)
   auto issue = [&](long long strip, int stage) {
     if (lane == 0) {
       const uint32_t bar = smem_u32(&bars[stage]);
       mbar_expect_tx(bar, (uint32_t)stage_bytes);
-      for (int k0 = 0; k0 < P.K; k0 += 256) {
-        asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
-                     :: "r"(smem_u32(sB + (size_t)stage * stage_bytes + (size_t)k0 * 512)), "l"(&map_b), "r"((int)(strip * STRIP)), "r"(k0), "r"(bar) : "memory");
-      }
+      asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
+                   :: "r"(smem_u32(sB + (size_t)stage * stage_bytes)), "l"(&map_b), "r"((int)(strip * STRIP)), "r"(0), "r"(bar) : "memory");
     }
   };
 
@@ -330,47 +328,71 @@ unsigned long long g_sreg_attr[2] = {0ull, 0ull};   // one bit per device ordina
 
 }  // namespace
 
-extern "C" int xb_sreg_launch(const xb_sparse_desc* d, const void* b, void* c, long long n_total) {
-  SregParams P;
-  P.M = d->m; P.K = d->k; P.N = n_total; P.ldb = d->ldb; P.ldc = d->ldc; P.nnz = d->nnz;
-  P.rowptr = d->d_ptr; P.entries = d->d_val; P.b = b; P.c = c; P.beta0 = d->beta0; P.stages = 3;
-  const bool f64 = (d->ta == LIBXSMM_DATATYPE_F64);
-  const size_t ts = f64 ? 8 : 4, es = f64 ? 16 : 8;
-  const size_t meta = 1024 + (size_t)d->nnz * es + (size_t)(d->m + 1) * 4 + 16;
+// shared memory sreg_kernel needs besides its stages: barriers, the entries of A, the row pointers
+static size_t sreg_meta_bytes(const xb_sparse_desc* d) {
+  const size_t es = (d->ta == LIBXSMM_DATATYPE_F64) ? 16 : 8;
+  return 1024 + (size_t)d->nnz * es + (size_t)(d->m + 1) * 4 + 16;
+}
+
+// The one decision of which kernel an fsspmdm call runs: 0 = sreg_direct_kernel, S = 1..3 = sreg_kernel with S stages. The staged
+// kernel needs 16-byte aligned B, C and rows (TMA), one TMA box per strip (K <= 256 rows) and S stages of K x 512 bytes plus the
+// pattern within 226 KB of shared memory; it takes as many stages up to 3 as fit.
+static int xb_sreg_variant(const xb_sparse_desc* d, const void* b, const void* c, long long n_total) {
+  const size_t ts = (d->ta == LIBXSMM_DATATYPE_F64) ? 8 : 4;
   const size_t limit = 226 * 1024;
-  cudaStream_t stream = (cudaStream_t)xb_rt_stream();
   const bool aligned = ((uintptr_t)b % 16 == 0) && ((uintptr_t)c % 16 == 0) && ((d->ldb * ts) % 16 == 0) && ((d->ldc * ts) % 16 == 0)
                     && ((n_total * ts) % 16 == 0);
+  if (!aligned || d->k > 256 || xb_tma_encoder() == nullptr) return 0;
+  int stages = 3;
+  while (stages > 0 && (size_t)stages * d->k * 512 + sreg_meta_bytes(d) > limit) --stages;
+  return stages;
+}
+
+// the same answer for a handle and the operands of a call (include/libxsmm_b200.h). Defined here, next to the decision, so that the
+// host objects need nothing new from the CUDA side.
+LIBXSMM_API int libxsmm_b200_fsspmdm_variant(const libxsmm_fsspmdm* handle, const void* B, const void* C) {
+  const xb_sparse_desc* d = xb_fsspmdm_desc(handle);
+  const void* staged = (const void*)(uintptr_t)256;   // pageable operands travel through the scratch arena, 256-byte aligned
+  if (d == nullptr) return -1;
+  if (B == nullptr || xb_rt_ptr_kind(B) == 0) B = staged;
+  if (C == nullptr || xb_rt_ptr_kind(C) == 0) C = staged;
+  return xb_sreg_variant(d, B, C, d->max_n);
+}
+
+extern "C" int xb_sreg_launch(const xb_sparse_desc* d, const void* b, void* c, long long n_total) {
   if (n_total <= 0) return 0;
-  { const char* e = getenv("LIBXSMM_B200_SREG_STAGES"); if (e != nullptr && *e) P.stages = atoi(e); }
-  while (P.stages > 1 && (size_t)P.stages * d->k * 512 + meta > limit) --P.stages;
-  if (!aligned || (size_t)P.stages * d->k * 512 + meta > limit) {
+  SregParams P;
+  P.M = d->m; P.K = d->k; P.N = n_total; P.ldb = d->ldb; P.ldc = d->ldc; P.nnz = d->nnz;
+  P.rowptr = d->d_ptr; P.entries = d->d_val; P.b = b; P.c = c; P.beta0 = d->beta0;
+  P.stages = xb_sreg_variant(d, b, c, n_total);
+  const bool f64 = (d->ta == LIBXSMM_DATATYPE_F64);
+  const size_t ts = f64 ? 8 : 4;
+  cudaStream_t stream = (cudaStream_t)xb_rt_stream();
+  if (P.stages == 0) {
     const long long total = (long long)d->m * n_total;
     long long grid = (total + 255) / 256; if (grid > num_sms() * 16) grid = num_sms() * 16;
     if (f64) sreg_direct_kernel<double><<<(unsigned int)grid, 256, 0, stream>>>(P);
     else sreg_direct_kernel<float><<<(unsigned int)grid, 256, 0, stream>>>(P);
     return check_launch("sreg_direct");
   }
-  const size_t smem = (size_t)P.stages * d->k * 512 + meta;
+  const size_t smem = (size_t)P.stages * d->k * 512 + sreg_meta_bytes(d);
   const long long strip = f64 ? 64 : 128;
   long long grid = (n_total + strip - 1) / strip; if (grid > num_sms()) grid = num_sms();
-  int warps = d->m < 4 ? 4 : (d->m > 32 ? 32 : d->m);      // one row per warp and pass
-  { const char* e = getenv("LIBXSMM_B200_SREG_WARPS"); if (e != nullptr && *e) warps = atoi(e); }
+  const int warps = d->m < 4 ? 4 : (d->m > 32 ? 32 : d->m);      // one row per warp and pass
   const int threads = warps * 32;
+  // the encoder is a driver-API call and needs the device's context current on this thread. The runtime binds it lazily, so in a
+  // thread whose first CUDA work is this call (an OpenMP worker on managed B and C) encoding fails unless it is bound here first.
+  { int dev = 0; if (cudaGetDevice(&dev) == cudaSuccess) cudaSetDevice(dev); }
   CUtensorMap map_b;
   {
-    xb_encode_tiled_fn enc = xb_tma_encoder();
     const cuuint64_t dims[2] = {(cuuint64_t)n_total, (cuuint64_t)d->k};
     const cuuint64_t strides[1] = {(cuuint64_t)d->ldb * ts};
-    const cuuint32_t box[2] = {(cuuint32_t)strip, (cuuint32_t)(d->k < 256 ? d->k : 256)};
+    const cuuint32_t box[2] = {(cuuint32_t)strip, (cuuint32_t)d->k};
     const cuuint32_t estr[2] = {1, 1};
-    if (enc == nullptr || (d->k > 256 && (d->k % 256) != 0) || CUDA_SUCCESS != enc(&map_b, f64 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT64 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void*)b,
-          dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE)) {
-      const long long total = (long long)d->m * n_total;
-      long long g2 = (total + 255) / 256; if (g2 > num_sms() * 16) g2 = num_sms() * 16;
-      if (f64) sreg_direct_kernel<double><<<(unsigned int)g2, 256, 0, stream>>>(P); else sreg_direct_kernel<float><<<(unsigned int)g2, 256, 0, stream>>>(P);
-      return check_launch("sreg_direct");
-    }
+    // xb_sreg_variant accepted these operands: a tensor map that still cannot be encoded is a bug, not a reason to fall back
+    const CUresult r = xb_tma_encoder()(&map_b, f64 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT64 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void*)b,
+          dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) { xb_rt_note_error((int)r, "sreg: TMA tensor map"); return (int)r; }
   }
   if (f64) {
     if (xb_rt_first_use_on_device(&g_sreg_attr[1])) cudaFuncSetAttribute(sreg_kernel<double>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);

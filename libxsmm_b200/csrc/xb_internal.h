@@ -196,6 +196,7 @@ void xb_bcsc_state_free(void* work);
 
 /* ---- host runtime (host_core.c) ---------------------------------------------------------------- */
 xb_slot* xb_slot_of(const void* fnptr);    /* NULL if not one of our thunks */
+const xb_sparse_desc* xb_fsspmdm_desc(const libxsmm_fsspmdm* handle);   /* host_sparse.c: the descriptor of an fsspmdm handle, or NULL */
 void xb_invoke(int slot, const void* param);
 const void* xb_thunk(int slot);
 #define XB_NTHUNKS 8192

@@ -182,3 +182,64 @@ def packed_dense_case(rng, kind, dtype, M, N, K, P, pad=0):
         a = gen.values(rng, M * lda * (P if kind == 1 else 1), dtype); b = gen.values(rng, K * ldb * (1 if kind == 1 else P), dtype)
         c0 = gen.values(rng, M * ldc * P, dtype)
     return (M, N, K, lda, ldb, ldc), a, b, c0
+
+
+# ---- fsspmdm "family E", exact by construction: A, B and the old C are dyadic on one grid 2^-q and every element satisfies
+# sum_z |v_z b| + |c0| < 2^(p - q) (p = 24 for f32, 53 for f64). Every partial sum is then a value of the type, so the result cannot
+# depend on the summation order: any correct kernel equals the float64 reference bit for bit. A is +-(1..7)/8, alpha is 1, -2 or 0.75
+# (the folded values stay on the grid 2^-5), B has `fb` fraction bits, |c0| <= 2 on the grid 2^-q.
+FSSPMDM_EXACT = {gen.F32: (24, 9, 4), gen.F64: (53, 25, 20)}     # dtype -> (p, q, fb)
+FSSPMDM_EXACT_ALPHAS = (1.0, -2.0, 0.75)
+
+
+def fsspmdm_pattern(rng, M, K, density=None, row_nnz=None):
+    """boolean M x K pattern: Bernoulli(density), or exactly row_nnz[i] non-zeros in row i"""
+    if row_nnz is None:
+        return rng.random((M, K)) < density
+    mask = np.zeros((M, K), dtype=bool)
+    for i, z in enumerate(row_nnz):
+        mask[i, rng.choice(K, size=z, replace=False)] = True
+    return mask
+
+
+def fsspmdm_exact_operands(rng, dtype, mask, N, ldb, ldc, alpha, lda=None):
+    """(a [M][lda], b [K][ldb], c0 [M][ldc]) of family E; columns N.. of B and C hold NaN"""
+    p, q, fb = FSSPMDM_EXACT[dtype]
+    npdt = gen.NP_OF[dtype]
+    M, K = mask.shape
+    lda = lda or K
+    a = np.zeros((M, lda), dtype=npdt)
+    a[:, :K] = np.where(mask, rng.integers(1, 8, size=(M, K)) * rng.choice([-1.0, 1.0], size=(M, K)), 0.0) / 8.0
+    bmax = 2 ** (fb + 1) - 1
+    b = np.full((K, ldb), np.nan, dtype=npdt)
+    for k in range(K):                                         # row by row: N may be 10^6
+        b[k, :N] = rng.integers(-bmax, bmax + 1, size=N) * 2.0 ** -fb
+    c0 = np.full((M, ldc), np.nan, dtype=npdt)
+    for i in range(M):
+        c0[i, :N] = rng.integers(-2 ** (q + 1), 2 ** (q + 1) + 1, size=N) * 2.0 ** -q
+    worst = np.abs(fsspmdm_fold(dtype, a[:, :K], alpha)).sum(axis=1).max() * bmax * 2.0 ** -fb + 2.0
+    assert worst < 2.0 ** (p - q), ("family E bound", worst)
+    return a, b, c0
+
+
+def fsspmdm_fold(dtype, a, alpha):
+    """A (M x K) with alpha folded in as libxsmm_fsspmdm_create does it (f32: float32(alpha) * a in float32), as float64"""
+    if dtype == gen.F32:
+        return (np.float32(alpha) * np.asarray(a, dtype=np.float32)).astype(np.float64)
+    return np.float64(alpha) * np.asarray(a, dtype=np.float64)
+
+
+def fsspmdm_reference(v, b, c0, N, beta, magnitude=True, chunk=1 << 16):
+    """float64 beta*C0 + V B over columns 0..N-1 (V = folded A, M x K) and, if asked for, the per-element magnitude sum
+    |V||B| + |beta C0|; column chunk by column chunk"""
+    M, K = v.shape
+    exact, mag = np.empty((M, N)), (np.empty((M, N)) if magnitude else None)
+    av = np.abs(v)
+    for j0 in range(0, N, chunk):
+        j1 = min(N, j0 + chunk)
+        bj = b[:K, j0:j1].astype(np.float64)
+        cj = c0[:, j0:j1].astype(np.float64) if beta else np.zeros((M, j1 - j0))
+        exact[:, j0:j1] = v @ bj + cj
+        if magnitude:
+            mag[:, j0:j1] = av @ np.abs(bj) + np.abs(cj)
+    return exact, mag

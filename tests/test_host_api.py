@@ -105,6 +105,13 @@ def test_unsupported_descriptors_return_null():
     assert not X.libxsmm_dispatch_tilecfg_gemm(_shape(16, 16, 16), both)
 
 
+def test_fsspmdm_variant_of_no_handle():
+    """libxsmm_b200_fsspmdm_variant answers -1 without a handle (0 / 1..3 name the direct and the staged kernel)"""
+    b = np.zeros(64, dtype=np.float32)
+    assert X.libxsmm_b200_fsspmdm_variant(None, None, None) == -1
+    assert X.libxsmm_b200_fsspmdm_variant(None, b.ctypes.data, b.ctypes.data) == -1
+
+
 def test_meltw_dispatch_host_logic():
     sh = X.libxsmm_create_meltw_unary_shape(10, 7, 10, 10, gen.F32, gen.F32, gen.F32)
     k = X.libxsmm_dispatch_meltw_unary(X.MELTW_TYPE_UNARY_RELU, sh, 0)

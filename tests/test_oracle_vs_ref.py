@@ -151,6 +151,29 @@ def test_fsspmdm_oracle_matches_reference():
 
 
 @needs_ref
+@pytest.mark.parametrize("dtype", [gen.F32, gen.F64])
+def test_fsspmdm_oracle_is_bit_exact_on_exact_operands(dtype):
+    """Family E of tests/test_fsspmdm_exact_gpu.py (cases.fsspmdm_exact_operands: every partial sum exact), on which the GPU kernels are
+    compared with oracle["fsspmdm"] bit for bit: the oracle, the reference and the float64 product must agree exactly, every alpha of the
+    family, beta 0 and 1, rows with 0 to 9 non-zeros. Zeros compare by value (the reference's dense kernel may produce -0)."""
+    rng = np.random.default_rng(6)
+    npdt = gen.NP_OF[dtype]
+    M, K, N = 24, 40, 96
+    for alpha in cases.FSSPMDM_EXACT_ALPHAS:
+        for beta in (0.0, 1.0):
+            mask = cases.fsspmdm_pattern(rng, M, K, row_nnz=[(3 + 7 * i) % 10 for i in range(M)])
+            a, b, c0 = cases.fsspmdm_exact_operands(rng, dtype, mask, N, N, N, alpha)
+            al, bt = np.array([alpha], dtype=npdt), np.array([beta], dtype=npdt)
+            args = (dtype, M, N, K, K, N, N, al.ctypes.data, bt.ctypes.data, a.ctypes.data, b.ctypes.data)
+            c_o, c_r = c0.copy(), c0.copy()
+            assert oracle["fsspmdm"](*args, c_o.ctypes.data) == 0
+            assert ref["fsspmdm"](*args, c_r.ctypes.data) == 0
+            exact, _ = cases.fsspmdm_reference(cases.fsspmdm_fold(dtype, a, alpha), b, c0, N, beta)
+            assert np.array_equal(c_r, exact.astype(npdt)), (alpha, beta, "reference vs float64")
+            assert np.array_equal(c_o, c_r), (alpha, beta, "oracle vs reference")
+
+
+@needs_ref
 @pytest.mark.parametrize("kind", ["a_csr", "b_csr", "b_csc", "c_csc"])
 def test_packed_sparse_oracle_matches_reference_jit(kind):
     """oracle_packed_sp (restated driver golds, samples/xgemm_norm_packed/*.c) against the reference's own JIT of
