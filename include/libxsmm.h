@@ -157,6 +157,21 @@ LIBXSMM_API libxsmm_gemmfunction libxsmm_create_spgemm_csr_areg(const libxsmm_ge
   const unsigned int* row_ptr, const unsigned int* column_idx, const double* values);
 LIBXSMM_API void libxsmm_release_kernel(const void* kernel);      /* reference include/libxsmm.h:229 */
 
+/* ---- BLAS-style GEMM (reference include/libxsmm.h:231-242, src/libxsmm_main.c:3933-3949): C (+)= op(A) * op(B) through the
+ * dispatched handle. As in the reference, alpha is ignored and beta only selects between beta = 0 and accumulate (any non-zero
+ * beta acts as 1); NULL transa/transb mean "as is", NULL k/n/ld* take the reference's defaults. The Fortran-77 symbols
+ * libxsmm_dgemm_ / libxsmm_sgemm_ are exported as well. */
+LIBXSMM_API void libxsmm_dgemm(const char* transa, const char* transb,
+  const libxsmm_blasint* m, const libxsmm_blasint* n, const libxsmm_blasint* k,
+  const double* alpha, const double* a, const libxsmm_blasint* lda,
+  const double* b, const libxsmm_blasint* ldb,
+  const double* beta, double* c, const libxsmm_blasint* ldc);
+LIBXSMM_API void libxsmm_sgemm(const char* transa, const char* transb,
+  const libxsmm_blasint* m, const libxsmm_blasint* n, const libxsmm_blasint* k,
+  const float* alpha, const float* a, const libxsmm_blasint* lda,
+  const float* b, const libxsmm_blasint* ldb,
+  const float* beta, float* c, const libxsmm_blasint* ldc);
+
 /* ---- memory (reference include/libxsmm_malloc.h:17-31): backed by CUDA managed memory so that
  * buffers obtained here are valid on host and device ------------------------------------------- */
 LIBXSMM_API void* libxsmm_malloc(size_t size);
@@ -171,5 +186,19 @@ LIBXSMM_API libxsmm_float16 libxsmm_convert_f32_to_f16(float in);
 
 #if defined(__cplusplus)
 }
-#endif
+
+/* ---- C++ overloads of the BLAS-style GEMM (reference include/libxsmm.h:370-404): m, n, k by pointer or by value -------------- */
+inline void libxsmm_gemm(const char* transa, const char* transb, const libxsmm_blasint* m, const libxsmm_blasint* n, const libxsmm_blasint* k,
+  const double* alpha, const double* a, const libxsmm_blasint* lda, const double* b, const libxsmm_blasint* ldb,
+  const double* beta, double* c, const libxsmm_blasint* ldc) { libxsmm_dgemm(transa, transb, m, n, k, alpha, a, lda, b, ldb, beta, c, ldc); }
+inline void libxsmm_gemm(const char* transa, const char* transb, libxsmm_blasint m, libxsmm_blasint n, libxsmm_blasint k,
+  const double* alpha, const double* a, const libxsmm_blasint* lda, const double* b, const libxsmm_blasint* ldb,
+  const double* beta, double* c, const libxsmm_blasint* ldc) { libxsmm_dgemm(transa, transb, &m, &n, &k, alpha, a, lda, b, ldb, beta, c, ldc); }
+inline void libxsmm_gemm(const char* transa, const char* transb, const libxsmm_blasint* m, const libxsmm_blasint* n, const libxsmm_blasint* k,
+  const float* alpha, const float* a, const libxsmm_blasint* lda, const float* b, const libxsmm_blasint* ldb,
+  const float* beta, float* c, const libxsmm_blasint* ldc) { libxsmm_sgemm(transa, transb, m, n, k, alpha, a, lda, b, ldb, beta, c, ldc); }
+inline void libxsmm_gemm(const char* transa, const char* transb, libxsmm_blasint m, libxsmm_blasint n, libxsmm_blasint k,
+  const float* alpha, const float* a, const libxsmm_blasint* lda, const float* b, const libxsmm_blasint* ldb,
+  const float* beta, float* c, const libxsmm_blasint* ldc) { libxsmm_sgemm(transa, transb, &m, &n, &k, alpha, a, lda, b, ldb, beta, c, ldc); }
+#endif /* __cplusplus */
 #endif /* LIBXSMM_H */

@@ -27,7 +27,13 @@
 #if !defined(LIBXSMM_API)
 # define LIBXSMM_API LIBXSMM_EXTERN_C __attribute__((visibility("default")))
 #endif
-#define LIBXSMM_APIVAR_PUBLIC(DECL) LIBXSMM_EXTERN_C __attribute__((visibility("default"))) extern DECL
+/* declares (never defines) a public variable; in C++ the linkage specification of a single declaration already implies extern,
+ * and a second extern after it is ill-formed */
+#if defined(__cplusplus)
+# define LIBXSMM_APIVAR_PUBLIC(DECL) extern "C" __attribute__((visibility("default"))) DECL
+#else
+# define LIBXSMM_APIVAR_PUBLIC(DECL) __attribute__((visibility("default"))) extern DECL
+#endif
 
 /* LP64 build only (reference: LIBXSMM_CONFIG_ILP64 0) */
 #define LIBXSMM_ILP64 0

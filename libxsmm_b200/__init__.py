@@ -260,6 +260,9 @@ libxsmm_create_packed_spgemm_bcsc = _sig("libxsmm_create_packed_spgemm_bcsc", _P
 libxsmm_create_tilecfg_packed_spgemm_bcsc = _sig("libxsmm_create_tilecfg_packed_spgemm_bcsc", _P, [GemmShape, _U, SpgemmConfig])
 libxsmm_create_spgemm_csr_areg = _sig("libxsmm_create_spgemm_csr_areg", _P, [GemmShape, _U, _U, _I, _P, _P, _P])
 libxsmm_release_kernel = _sig("libxsmm_release_kernel", None, [_P])
+# BLAS-style GEMM: every argument by reference (char*, blasint*, scalar*), a/b/c as addresses
+libxsmm_dgemm = _sig("libxsmm_dgemm", None, [C.c_char_p, C.c_char_p, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P])
+libxsmm_sgemm = _sig("libxsmm_sgemm", None, [C.c_char_p, C.c_char_p, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P])
 libxsmm_malloc = _sig("libxsmm_malloc", _P, [C.c_size_t])
 libxsmm_aligned_malloc = _sig("libxsmm_aligned_malloc", _P, [C.c_size_t, C.c_size_t])
 libxsmm_free = _sig("libxsmm_free", None, [_P])

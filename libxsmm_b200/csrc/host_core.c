@@ -517,9 +517,81 @@ static void xb_invoke_gemm(const xb_slot* s, const libxsmm_gemm_param* p) {
     if (0 != xb_meltw_launch(&md, &ma)) { xb_rt_scratch_reset(); return; }
     staged = 1;
   }
-  if (need_cb) xb_rt_memcpy_async(cb.host, cb.dev, cb.bytes);
+  if (need_cb) {
+    /* only the m x n block this call owns goes back: callers update row blocks of ONE host C from several threads (ldc > m), and the
+     * contiguous span would carry the neighbours' rows back stale over their results. VNNI-packed C is re-packed as a whole ldc x n image. */
+    if (vnni_c) xb_rt_memcpy_async(cb.host, cb.dev, cb.bytes);
+    else xb_rt_memcpy2d_async(cb.host, cb.dev, (size_t)d->ldc * tsc, (size_t)d->m * tsc, (size_t)d->n);
+  }
   if (need_cb_mask) xb_rt_memcpy_async(cb_mask.host, cb_mask.dev, cb_mask.bytes);
   if (staged || xb_rt_blocking()) { xb_rt_sync(); xb_rt_scratch_reset(); }
+}
+
+/* ---- BLAS-style entry points (reference src/libxsmm_main.c:3933-3949) ----------------------------------------------------------
+ * LIBXSMM_XGEMM (reference src/libxsmm_main.h:215-240) with its quirks, so that a relinked caller gets the reference's numbers rather
+ * than BLAS's: alpha is never read; beta only chooses between BETA_0 (beta == 0) and accumulate (any other value, 0.5 included, acts
+ * as 1; NULL means LIBXSMM_BETA); k defaults to m and n to k; lda defaults to m (k under TRANS_A), ldb to k (n under TRANS_B), ldc to
+ * m, and every leading dimension is at least 1. A shape the descriptor rejects prints "LIBXSMM_GEMM failed" and leaves C alone. */
+static void xb_blas_gemm(libxsmm_datatype type, const char* transa, const char* transb,
+  const libxsmm_blasint* m, const libxsmm_blasint* n, const libxsmm_blasint* k,
+  const void* a, const libxsmm_blasint* lda, const void* b, const libxsmm_blasint* ldb,
+  const void* beta, void* c, const libxsmm_blasint* ldc)
+{
+  const int beta0 = (beta != NULL) && ((type == LIBXSMM_DATATYPE_F64) ? (*(const double*)beta == 0) : (*(const float*)beta == 0));
+  const libxsmm_bitfield flags = LIBXSMM_GEMM_PFLAGS(transa, transb, LIBXSMM_FLAGS) | (beta0 ? LIBXSMM_GEMM_FLAG_BETA_0 : 0);
+  const libxsmm_blasint* kk = (k != NULL) ? k : m;
+  const libxsmm_blasint* nn = (n != NULL) ? n : kk;
+  const libxsmm_blasint ld_a = LIBXSMM_MAX((lda != NULL) ? *lda : *((flags & LIBXSMM_GEMM_FLAG_TRANS_A) == 0 ? m : kk), 1);
+  const libxsmm_blasint ld_b = LIBXSMM_MAX((ldb != NULL) ? *ldb : *((flags & LIBXSMM_GEMM_FLAG_TRANS_B) == 0 ? kk : nn), 1);
+  const libxsmm_blasint ld_c = LIBXSMM_MAX((ldc != NULL) ? *ldc : *m, 1);
+  const libxsmm_gemm_shape shape = libxsmm_create_gemm_shape(*m, *nn, *kk, ld_a, ld_b, ld_c, type, type, type, type);
+  const libxsmm_gemmfunction kernel = xb_dispatch_gemm_common(&shape, flags, LIBXSMM_PREFETCH, NULL);
+  if (kernel != NULL) {
+    libxsmm_gemm_param p;
+    memset(&p, 0, sizeof(p));
+    p.a.primary = (void*)(uintptr_t)a; p.b.primary = (void*)(uintptr_t)b; p.c.primary = c;
+    xb_invoke_gemm(xb_slot_of((const void*)kernel), &p);
+  }
+  else printf("LIBXSMM_GEMM failed\n");
+}
+
+LIBXSMM_API void libxsmm_dgemm(const char* transa, const char* transb,
+  const libxsmm_blasint* m, const libxsmm_blasint* n, const libxsmm_blasint* k,
+  const double* alpha, const double* a, const libxsmm_blasint* lda,
+  const double* b, const libxsmm_blasint* ldb,
+  const double* beta, double* c, const libxsmm_blasint* ldc)
+{
+  (void)alpha;
+  xb_blas_gemm(LIBXSMM_DATATYPE_F64, transa, transb, m, n, k, a, lda, b, ldb, beta, c, ldc);
+}
+
+LIBXSMM_API void libxsmm_sgemm(const char* transa, const char* transb,
+  const libxsmm_blasint* m, const libxsmm_blasint* n, const libxsmm_blasint* k,
+  const float* alpha, const float* a, const libxsmm_blasint* lda,
+  const float* b, const libxsmm_blasint* ldb,
+  const float* beta, float* c, const libxsmm_blasint* ldc)
+{
+  (void)alpha;
+  xb_blas_gemm(LIBXSMM_DATATYPE_F32, transa, transb, m, n, k, a, lda, b, ldb, beta, c, ldc);
+}
+
+/* Fortran-77 symbols (reference src/libxsmm_main.c:4313-4340, LIBXSMM_FSYMBOL): every argument by reference already */
+LIBXSMM_API void libxsmm_dgemm_(const char* transa, const char* transb,
+  const libxsmm_blasint* m, const libxsmm_blasint* n, const libxsmm_blasint* k,
+  const double* alpha, const double* a, const libxsmm_blasint* lda,
+  const double* b, const libxsmm_blasint* ldb,
+  const double* beta, double* c, const libxsmm_blasint* ldc)
+{
+  libxsmm_dgemm(transa, transb, m, n, k, alpha, a, lda, b, ldb, beta, c, ldc);
+}
+
+LIBXSMM_API void libxsmm_sgemm_(const char* transa, const char* transb,
+  const libxsmm_blasint* m, const libxsmm_blasint* n, const libxsmm_blasint* k,
+  const float* alpha, const float* a, const libxsmm_blasint* lda,
+  const float* b, const libxsmm_blasint* ldb,
+  const float* beta, float* c, const libxsmm_blasint* ldc)
+{
+  libxsmm_sgemm(transa, transb, m, n, k, alpha, a, lda, b, ldb, beta, c, ldc);
 }
 
 /* ---- batch entry points -------------------------------------------------------------------------- */
