@@ -67,8 +67,9 @@ LIBXSMM_API int libxsmm_b200_memcpy(void* dst, const void* src, size_t size); /*
  * and, inside a tile, the handle's own batch-reduce addressing (stride mode: the dispatch-time
  * br_stride hints; br_count as given). Returns 0 on success. */
 /* returned by every batch form (and a NULL plan) for a handle a batch cannot run like a single call: a fused column bias or ReLU
- * bit mask (libxsmm_dispatch_brgemm_ext), VNNI-packed C, and for the strided forms int8 -> f32 (the scale travels in c.tertiary
- * of a call); nothing is launched and C is left untouched */
+ * bit mask (libxsmm_dispatch_brgemm_ext), VNNI-packed C, MX handles (their block scales travel per call: use
+ * libxsmm_b200_gemm_batch_strided_scaled), and for the strided forms int8 -> f32 (the scale travels in c.tertiary of a call);
+ * nothing is launched and C is left untouched */
 #define LIBXSMM_B200_ERROR_NOT_BATCHABLE (-6)
 LIBXSMM_API int libxsmm_b200_gemm_batch_strided(libxsmm_gemmfunction kernel,
   const void* a, const void* b, void* c, long long stride_a, long long stride_b, long long stride_c,
@@ -78,6 +79,15 @@ LIBXSMM_API int libxsmm_b200_gemm_batch_strided(libxsmm_gemmfunction kernel,
 LIBXSMM_API int libxsmm_b200_gemm_batch_strided_multi(libxsmm_gemmfunction kernel,
   const void* a, const void* b, void* c, long long stride_a, long long stride_b, long long stride_c,
   unsigned long long br_count, long long count, int ndevices);
+/* MX GEMM (MXBF8 / MXHF8 handles) over a strided batch: the E8M0 block scales of tile t are scf_a + t*stride_scf_a (a.tertiary
+ * of a single call), scf_b + t*stride_scf_b (b.tertiary) and, for an MXBF8 C, scf_c + t*stride_scf_c (c.tertiary); strides in
+ * BYTES. Every operand must be device-accessible (-4 for pageable host memory); -1 for a handle without per-call scales.
+ * An MXBF8 C is quantised from an f32 image in device scratch: the batch then runs in chunks of at most 64 MiB of image and the
+ * call returns after the device has finished. */
+LIBXSMM_API int libxsmm_b200_gemm_batch_strided_scaled(libxsmm_gemmfunction kernel,
+  const void* a, const void* b, void* c, long long stride_a, long long stride_b, long long stride_c,
+  const void* scf_a, const void* scf_b, void* scf_c, long long stride_scf_a, long long stride_scf_b, long long stride_scf_c,
+  unsigned long long br_count, long long count);
 /* general form: one reference argument struct per tile (address/offset batch-reduce modes, scale
  * factors...). All matrix pointers must be device-accessible. */
 LIBXSMM_API int libxsmm_b200_gemm_batch(libxsmm_gemmfunction kernel, const libxsmm_gemm_param* params, long long count);

@@ -23,7 +23,7 @@ _DT = ("F64 F32 BF16 F16 BF8 HF8 I64 U64 I32 U32 I16 U16 I8 U8 MXBF8 MXHF8 MXBF6
        "MXFP4X2 NVFP4X2 I2X4 I1X8 BF32 IMPLICIT UNSUPPORTED").split()
 for _i, _n in enumerate(_DT):
     globals()["DATATYPE_" + _n] = _i
-TYPESIZE = {0: 8, 1: 4, 2: 2, 3: 2, 4: 1, 5: 1, 6: 8, 7: 8, 8: 4, 9: 4, 10: 2, 11: 2, 12: 1, 13: 1, 24: 4}
+TYPESIZE = {0: 8, 1: 4, 2: 2, 3: 2, 4: 1, 5: 1, 6: 8, 7: 8, 8: 4, 9: 4, 10: 2, 11: 2, 12: 1, 13: 1, 14: 1, 15: 1, 24: 4}
 
 GEMM_FLAG_NONE = 0
 GEMM_FLAG_TRANS_A = 1
@@ -299,6 +299,8 @@ libxsmm_b200_host_malloc = _sig("libxsmm_b200_host_malloc", _P, [C.c_size_t])
 libxsmm_b200_host_free = _sig("libxsmm_b200_host_free", None, [_P])
 libxsmm_b200_memcpy = _sig("libxsmm_b200_memcpy", _I, [_P, _P, C.c_size_t])
 libxsmm_b200_gemm_batch_strided = _sig("libxsmm_b200_gemm_batch_strided", _I, [_P, _P, _P, _P, _LL, _LL, _LL, _ULL, _LL])
+libxsmm_b200_gemm_batch_strided_scaled = _sig("libxsmm_b200_gemm_batch_strided_scaled", _I,
+                                              [_P, _P, _P, _P, _LL, _LL, _LL, _P, _P, _P, _LL, _LL, _LL, _ULL, _LL])
 libxsmm_b200_gemm_batch_strided_multi = _sig("libxsmm_b200_gemm_batch_strided_multi", _I, [_P, _P, _P, _P, _LL, _LL, _LL, _ULL, _LL, _I])
 libxsmm_b200_gemm_batch = _sig("libxsmm_b200_gemm_batch", _I, [_P, C.POINTER(GemmParam), _LL])
 libxsmm_b200_gemm_plan_create = _sig("libxsmm_b200_gemm_plan_create", _P, [_P, C.POINTER(GemmParam), _LL])
@@ -323,8 +325,10 @@ def ptr(x):
     return C.addressof(x)
 
 
-def call_gemm(kernel, a, b, c, br_count=None, a_aux=None, b_aux=None, scf=None, colptr=None, rowidx=None, nblocks=None):
-    """Invoke a GEMM-family handle like the reference drivers do (fill libxsmm_gemm_param, call)."""
+def call_gemm(kernel, a, b, c, br_count=None, a_aux=None, b_aux=None, scf=None, colptr=None, rowidx=None, nblocks=None,
+              a_scales=None, b_scales=None, c_scales=None):
+    """Invoke a GEMM-family handle like the reference drivers do (fill libxsmm_gemm_param, call).
+    a_scales / b_scales / c_scales: the E8M0 block scales of an MX handle (a/b/c.tertiary)."""
     p = GemmParam()
     keep = []
     if br_count is not None:
@@ -346,6 +350,12 @@ def call_gemm(kernel, a, b, c, br_count=None, a_aux=None, b_aux=None, scf=None, 
         nb = C.c_ulonglong(nblocks)
         keep.append(nb)
         p.b.quaternary = C.addressof(nb)
+    if a_scales is not None:
+        p.a.tertiary = ptr(a_scales)
+    if b_scales is not None:
+        p.b.tertiary = ptr(b_scales)
+    if c_scales is not None:
+        p.c.tertiary = ptr(c_scales)
     GEMMFUNCTION(kernel)(C.byref(p))
     return keep
 

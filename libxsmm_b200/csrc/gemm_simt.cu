@@ -22,12 +22,16 @@
 
 namespace {
 
-enum { P_F64 = 0, P_F32, P_I16, P_I8_I32, P_I8_F32, P_F16_F16, P_F16_F32, P_BF16_F32, P_BF16_BF16, P_I4_I32, P_BITMAP, P_FP8, P_NONE };
+enum { P_F64 = 0, P_F32, P_I16, P_I8_I32, P_I8_F32, P_F16_F16, P_F16_F32, P_BF16_F32, P_BF16_BF16, P_I4_I32, P_BITMAP, P_FP8, P_MX8, P_NONE };
 
 __host__ __device__ inline int xb_path_of(const xb_gemm_desc& d) {
   const int a = d.ta, b = d.tb, c = d.tc, comp = d.tcomp;
   const bool a8 = (a == LIBXSMM_DATATYPE_I8 || a == LIBXSMM_DATATYPE_U8);
   const bool b8 = (b == LIBXSMM_DATATYPE_I8 || b == LIBXSMM_DATATYPE_U8);
+  if (a == LIBXSMM_DATATYPE_MXBF8 || a == LIBXSMM_DATATYPE_MXHF8) {   // MX fp8 (reference :2620-2679); the layout rules live in host_core.c
+    const bool cok = (c == LIBXSMM_DATATYPE_F32) || (c == LIBXSMM_DATATYPE_MXBF8 && a == LIBXSMM_DATATYPE_MXBF8);
+    return (b == a && comp == LIBXSMM_DATATYPE_F32 && cok && (d.br_type == 0 || d.br_type == 3) && d.fuse_colbias == 0 && d.cp_op == 0) ? P_MX8 : P_NONE;
+  }
   if ((d.flags & LIBXSMM_GEMM_FLAG_DECOMPRESS_A_VIA_BITMASK) != 0) {   // bitmap-compressed A (reference :857-948): float operands, no batch reduce
     const bool fa = (a == LIBXSMM_DATATYPE_F32 || a == LIBXSMM_DATATYPE_BF16 || a == LIBXSMM_DATATYPE_F16);
     const bool fb = (b == LIBXSMM_DATATYPE_F32 || b == LIBXSMM_DATATYPE_BF16 || b == LIBXSMM_DATATYPE_F16);
@@ -68,6 +72,7 @@ struct TileCtx {
   float scf;
   const void* colbias; unsigned char* relu_mask;          // fused form (libxsmm_dispatch_brgemm_ext)
   const unsigned char* a_q;                                // int4: zero points; bitmap-compressed A: the bitmap
+  const unsigned char* a_s; const unsigned char* b_s; unsigned char* c_s;   // MX fp8: E8M0 block scales
 };
 
 __device__ inline void resolve_tile(const xb_gemm_launch& L, long long t, TileCtx& x) {
@@ -86,6 +91,12 @@ __device__ inline void resolve_tile(const xb_gemm_launch& L, long long t, TileCt
   x.a_offs = (const long long*)r.a_aux; x.b_offs = (const long long*)r.b_aux;
   x.br = (L.d.br_type == 0) ? 1ull : r.br; x.scf = r.scf;
   x.colbias = r.d; x.relu_mask = (unsigned char*)r.c_aux; x.a_q = (const unsigned char*)r.a_q;
+}
+
+// MX fp8 block scales of tile t; kept out of resolve_tile, whose other callers would carry the extra registers
+__device__ inline void resolve_scales(const xb_gemm_launch& L, long long t, TileCtx& x) {
+  x.a_s = (const unsigned char*)L.one.a_s; x.b_s = (const unsigned char*)L.one.b_s; x.c_s = (unsigned char*)L.one.c_s;
+  if (!(L.a == nullptr && L.c == nullptr)) { x.a_s += t * L.tile_stride_as; x.b_s += t * L.tile_stride_bs; if (x.c_s != nullptr) x.c_s += t * L.tile_stride_cs; }
 }
 
 // base pointers of the r-th batch-reduce operand pair; mirrors libxsmm_calculate_brgemm_offsets
@@ -447,6 +458,93 @@ __global__ void __launch_bounds__(1024) gemm_bitmap_kernel(const xb_gemm_launch 
 }
 
 
+// ---- MX fp8: MXBF8 x MXBF8 / MXHF8 x MXHF8 with E8M0 block scales (reference :2620-2679) -------------------------------
+// A is VNNI4 [k/4][lda][4], B is VNNI4-transposed [k/4][ldb][4]; one scale byte per (row, 32 k): A's [r][k/32][lda], B's
+// [r][k/32][ldb]. A scale byte widens as bits = s << 23 (0 -> +0, 0xFF -> +inf). Per element and 4-k group: tmp = sum of a*b
+// over k2 = 3..0 from 0, then acc += (tmp * sa) * sb; acc runs over (r, group) from 0 and C = (beta0 ? 0 : C) + acc. Block r of
+// a batch-reduce sits at r*lda*k (A) and r*ldb*k (B): the reference ignores the stride hints, dispatch accepts stride mode only
+// where they agree with that.
+__device__ __forceinline__ float mx_scale(unsigned char s) { return __uint_as_float((unsigned int)s << 23); }
+
+__device__ __forceinline__ float dot_mx8(const xb_gemm_desc& d, const TileCtx& x, int i, int j) {
+  const int k = d.k, groups = d.k / 4;
+  const long long lda = d.lda, ldb = d.ldb;
+  const bool hf = (d.ta == LIBXSMM_DATATYPE_MXHF8);
+  float acc = 0.0f;
+  for (unsigned long long r = 0; r < x.br; ++r) {
+    const unsigned char* pa = (const unsigned char*)x.a0 + (long long)r * lda * k + (long long)i * 4;
+    const unsigned char* pb = (const unsigned char*)x.b0 + (long long)r * ldb * k + (long long)j * 4;
+    const unsigned char* psa = x.a_s + (long long)r * lda * (k / 32) + i;
+    const unsigned char* psb = x.b_s + (long long)r * ldb * (k / 32) + j;
+    for (int s = 0; s < groups; ++s) {
+      float tmp = 0.0f;
+      for (int k2 = 3; k2 >= 0; --k2) {
+        const unsigned char ab = pa[(long long)s * lda * 4 + k2], bb = pb[(long long)s * ldb * 4 + k2];
+        tmp = __fadd_rn(tmp, __fmul_rn(hf ? xb_hf8_to_f32(ab) : xb_bf8_to_f32(ab), hf ? xb_hf8_to_f32(bb) : xb_bf8_to_f32(bb)));
+      }
+      acc = __fadd_rn(acc, __fmul_rn(__fmul_rn(tmp, mx_scale(psa[(long long)(s / 8) * lda])), mx_scale(psb[(long long)(s / 8) * ldb])));
+    }
+  }
+  return acc;
+}
+
+// F32 C: written in place. MXBF8 C: the f32 image (0 + acc, BETA_0 only) goes to img [tile][n][m] for gemm_mx8_quant_kernel.
+__global__ void __launch_bounds__(256) gemm_mx8_kernel(const xb_gemm_launch L, float* __restrict__ img) {
+  const xb_gemm_desc& d = L.d;
+  const int m = d.m, n = d.n;
+  const long long ldc = d.ldc;
+  const bool beta0 = (d.flags & LIBXSMM_GEMM_FLAG_BETA_0) != 0;
+  for (long long t = blockIdx.x; t < L.count; t += gridDim.x) {
+    TileCtx x; resolve_tile(L, t, x); resolve_scales(L, t, x);
+    for (int e = threadIdx.x; e < m * n; e += blockDim.x) {
+      const int i = e % m, j = e / m;
+      const float acc = dot_mx8(d, x, i, j);
+      if (img != nullptr) img[(t * n + j) * (long long)m + i] = __fadd_rn(0.0f, acc);
+      else { float* c = reinterpret_cast<float*>(x.c) + (long long)j * ldc + i; *c = __fadd_rn(beta0 ? 0.0f : *c, acc); }
+    }
+  }
+}
+
+// MXBF8 C (reference :757-, one 32-row block of one column per thread): each value rounded to bf16 (nearest-even, subnormals
+// flushed); the block's amax (NaN wins); shared exponent e = biased exponent of amax - 15, clamped to [0, 254], 0 for amax = 0,
+// stored as the scale byte; the scale 2^(e-127) (2^-127 for e = 0) rounded to bf16 and its reciprocal rounded to bf16; each value
+// times that reciprocal, rounded to bf16, then to bf8 (E5M2) nearest-even, Inf and NaN bytes clamped to +-0x7B. The flushes
+// matter: e = 0 gives a zero scale and an infinite reciprocal, e = 254 a zero reciprocal. The elementwise MXBF8 quantiser
+// (meltw.cu) divides by the unrounded scale and writes a NaN block as 0x7B with scale 0xFF, so it does not give these bytes.
+__device__ __forceinline__ float mx_bf16_rne(float f) { return xb_bf16_to_f32(xb_f32_to_bf16_rne(f)); }
+// the reference runs on x86: an invalid product (0 * inf) is the negative default NaN there, and a NaN operand passes through
+__device__ __forceinline__ float mx_x86_mul(float a, float b) {
+  if (a != a) return __uint_as_float(__float_as_uint(a) | 0x400000u);
+  const float p = __fmul_rn(a, b);
+  return (p != p) ? __uint_as_float(0xffc00000u) : p;
+}
+__global__ void __launch_bounds__(128) gemm_mx8_quant_kernel(const xb_gemm_launch L, const float* __restrict__ img) {
+  const int m = L.d.m, n = L.d.n, bm = L.d.m / 32;
+  const long long ldc = L.d.ldc, per_tile = (long long)n * bm;
+  const long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (e >= L.count * per_tile) return;
+  const long long t = e / per_tile;
+  const int j = (int)((e % per_tile) / bm), b = (int)(e % bm);
+  TileCtx x; resolve_tile(L, t, x); resolve_scales(L, t, x);
+  const float* src = img + (t * n + j) * (long long)m + b * 32;
+  float v[32], amax = 0.0f;
+#pragma unroll
+  for (int q = 0; q < 32; ++q) { v[q] = mx_bf16_rne(src[q]); const float a = fabsf(v[q]); if (a > amax || a != a) amax = a; }
+  int se = (amax == 0.0f) ? 0 : (int)((__float_as_uint(amax) >> 23) & 0xffu);
+  se = (se - 15 < 0) ? 0 : ((se - 15 > 254) ? 254 : se - 15);
+  x.c_s[(long long)j * (ldc / 32) + b] = (unsigned char)se;
+  const float scale = __uint_as_float(((unsigned int)se << 23) | (se == 0 ? 0x400000u : 0u));
+  const float rcp = mx_bf16_rne(__fdiv_rn(1.0f, mx_bf16_rne(scale)));
+  unsigned char* dst = reinterpret_cast<unsigned char*>(x.c) + (long long)j * ldc + b * 32;
+#pragma unroll
+  for (int q = 0; q < 32; ++q) {
+    unsigned char o = xb_f32_to_bf8(mx_bf16_rne(mx_x86_mul(v[q], rcp)));
+    if ((o & 0x7c) == 0x7c) o = (unsigned char)((o & 0x80) | 0x7b);
+    dst[q] = o;
+  }
+}
+
+
 // ---- 8-bit integer tiles: dp4a kernel ------------------------------------------------------------------------------
 // Integer sums wrap modulo 2^32 and are therefore exact in ANY order: the int8 paths need not follow the reference's
 // loop order to stay bit-identical (reference :1452-1683). One WARP per tile: the VNNI4 A words [k/4][m] and the
@@ -628,6 +726,24 @@ extern "C" int xb_gemm_simt_launch(const xb_gemm_launch* L) {
     xb_rt_count_launch_backend(LIBXSMM_B200_BACKEND_SIMT);
     const cudaError_t be = cudaGetLastError();
     if (be != cudaSuccess) { xb_rt_note_error((int)be, "gemm_bitmap"); return (int)be; }
+    return 0;
+  }
+  if (path == P_MX8) {
+    if (L->recs != nullptr || L->one.a_s == nullptr || L->one.b_s == nullptr || (L->d.tc == LIBXSMM_DATATYPE_MXBF8 && L->one.c_s == nullptr)) {
+      xb_rt_note_error(1, "MX fp8: block scales missing (a/b.tertiary, c.tertiary for an MXBF8 C)"); return 1;
+    }
+    float* img = nullptr;                        // MXBF8 C: f32 image in the caller's scratch arena (reset after the sync)
+    if (L->d.tc == LIBXSMM_DATATYPE_MXBF8 && nullptr == (img = (float*)xb_rt_scratch((size_t)L->count * L->d.m * L->d.n * 4))) return 2;
+    cudaStream_t st = (cudaStream_t)xb_rt_stream();
+    gemm_mx8_kernel<<<(unsigned int)(L->count < (1 << 20) ? L->count : (1 << 20)), 256, 0, st>>>(*L, img);
+    xb_rt_count_launch_backend(LIBXSMM_B200_BACKEND_SIMT);
+    if (img != nullptr) {
+      const long long blocks = L->count * L->d.n * (L->d.m / 32);
+      gemm_mx8_quant_kernel<<<(unsigned int)((blocks + 127) / 128), 128, 0, st>>>(*L, img);
+      xb_rt_count_launch_backend(LIBXSMM_B200_BACKEND_SIMT);
+    }
+    const cudaError_t me = cudaGetLastError();
+    if (me != cudaSuccess) { xb_rt_note_error((int)me, "gemm_mx8"); return (int)me; }
     return 0;
   }
   if (path == P_I4_I32 && L->one.a_q == nullptr && L->recs == nullptr) { xb_rt_note_error(1, "int4 A: zero points missing (a.quaternary)"); return 1; }

@@ -256,6 +256,28 @@ static int xb_tilecfg_inconsistent(unsigned int flags) {
   return nr != ns;
 }
 
+static int xb_is_mx8(int t) { return t == LIBXSMM_DATATYPE_MXBF8 || t == LIBXSMM_DATATYPE_MXHF8; }
+
+/* MXBF8 x MXBF8 and MXHF8 x MXHF8 with E8M0 block scales (reference src/generator_gemm_reference_impl.c:2620-2679); 1 if the
+ * reference kernel defines a result for the descriptor. Every other MX tuple (MXHF8 -> MXHF8, mixed, MX6, MX4) matches no branch. */
+static int xb_mx8_desc_ok(const xb_gemm_desc* d, int ext) {
+  const unsigned int need = LIBXSMM_GEMM_FLAG_VNNI_A | LIBXSMM_GEMM_FLAG_VNNI_B | LIBXSMM_GEMM_FLAG_TRANS_B;
+  const int mx_c = (d->tc == LIBXSMM_DATATYPE_MXBF8);
+  if (ext) return 0;                                                           /* fused MX does not exist */
+  if (!xb_is_mx8(d->ta) || d->tb != d->ta || d->tcomp != LIBXSMM_DATATYPE_F32) return 0;
+  if (!(d->tc == LIBXSMM_DATATYPE_F32 || (mx_c && d->ta == LIBXSMM_DATATYPE_MXBF8))) return 0;
+  if ((d->flags & need) != need || (d->flags & LIBXSMM_GEMM_FLAG_TRANS_A) != 0) return 0;   /* the reference prints an error and leaves C (:2632-2635) */
+  if ((d->flags & (LIBXSMM_GEMM_FLAG_VNNI_C | LIBXSMM_GEMM_FLAG_DECOMPRESS_A_VIA_BITMASK)) != 0) return 0;                   /* not served for MX */
+  if ((d->k % 32) != 0 || d->lda < d->m || d->ldb < d->n) return 0;
+  /* block r is read at r*lda*k and r*ldb*k whatever the batch-reduce type says (:2646-2655): stride mode only where the hints agree;
+   * address and offset mode would read the pointer / offset arrays as data, which defines no result */
+  if (d->br_type == 1 || d->br_type == 2) return 0;
+  if (d->br_type == 3 && (d->br_stride_a != (long long)d->lda * d->k || d->br_stride_b != (long long)d->ldb * d->k)) return 0;
+  /* MXBF8 C: the reference accumulates into an uninitialised image unless beta = 0, and quantises whole 32-row blocks (:757-) */
+  if (mx_c && ((d->flags & LIBXSMM_GEMM_FLAG_BETA_0) == 0 || (d->m % 32) != 0 || (d->ldc % 32) != 0)) return 0;
+  return 1;
+}
+
 static int xb_make_gemm_desc(xb_gemm_desc* d, const libxsmm_gemm_shape* shape, unsigned int flags, unsigned int prefetch,
                              const libxsmm_gemm_batch_reduce_config* br, int ext)
 {
@@ -275,6 +297,11 @@ static int xb_make_gemm_desc(xb_gemm_desc* d, const libxsmm_gemm_shape* shape, u
       default: d->br_type = 0;
     }
     if (d->br_type != 0) d->br_unroll = (br->br_unroll_hint > 0 && br->br_unroll_hint < 255) ? br->br_unroll_hint : 0;
+  }
+  if (xb_is_mx8(d->ta) || xb_is_mx8(d->tb) || xb_is_mx8(d->tc)) {   /* MX fp8: its own layout rules, exact-order kernel only */
+    if (!xb_mx8_desc_ok(d, ext) || !xb_gemm_simt_supported(d)) return 0;
+    d->backend = LIBXSMM_B200_BACKEND_SIMT;
+    return 1;
   }
   /* leading-dimension sanity for the layout in use (the reference JIT rejects these too) */
   {
@@ -372,6 +399,7 @@ typedef struct xb_copyback { void* host; const void* dev; size_t bytes; } xb_cop
 
 static size_t xb_extent_a(const xb_gemm_desc* d) {   /* elements touched in one A operand */
   if (d->ta == LIBXSMM_DATATYPE_I4X2 || d->ta == LIBXSMM_DATATYPE_U4X2) return (size_t)(d->k / 8 - 1) * d->lda * 4 + (size_t)d->m * 4;   /* bytes: 8 k per 4 bytes */
+  if (xb_is_mx8(d->ta)) return (size_t)(d->k / 4 - 1) * d->lda * 4 + (size_t)d->m * 4;                                                 /* VNNI4 */
   const int trans_a = (d->flags & LIBXSMM_GEMM_FLAG_TRANS_A) != 0, vnni_a = (d->flags & LIBXSMM_GEMM_FLAG_VNNI_A) != 0;
   const int is8 = (d->ta == LIBXSMM_DATATYPE_I8 || d->ta == LIBXSMM_DATATYPE_U8);
   const int is_f8 = (d->ta == LIBXSMM_DATATYPE_BF8 || d->ta == LIBXSMM_DATATYPE_HF8);
@@ -386,12 +414,18 @@ static size_t xb_extent_a(const xb_gemm_desc* d) {   /* elements touched in one 
 }
 
 static size_t xb_extent_b(const xb_gemm_desc* d) {
+  if (xb_is_mx8(d->tb)) return (size_t)(d->k / 4 - 1) * d->ldb * 4 + (size_t)d->n * 4;                                                 /* VNNI4-T */
   const int trans_b = (d->flags & LIBXSMM_GEMM_FLAG_TRANS_B) != 0, vnni_b = (d->flags & LIBXSMM_GEMM_FLAG_VNNI_B) != 0;
   const int honours = (d->tb == LIBXSMM_DATATYPE_F64 || d->tb == LIBXSMM_DATATYPE_F32 || d->tb == LIBXSMM_DATATYPE_BF32
                     || d->tb == LIBXSMM_DATATYPE_BF16 || d->tb == LIBXSMM_DATATYPE_F16 || d->tb == LIBXSMM_DATATYPE_BF8 || d->tb == LIBXSMM_DATATYPE_HF8);
   if (honours && trans_b && vnni_b && d->tb == LIBXSMM_DATATYPE_BF16) return (size_t)(d->k / 2 - 1) * d->ldb * 2 + (size_t)d->n * 2;
   if (honours && trans_b) return (size_t)(d->k - 1) * d->ldb + d->n;
   return (size_t)(d->n - 1) * d->ldb + d->k;
+}
+
+/* MX block scales touched by one call of br blocks: [br][k/32][ld] bytes, up to the last row in use */
+static size_t xb_extent_mx_scales(const xb_gemm_desc* d, unsigned long long br, int ld, int rows) {
+  return (size_t)((br ? br : 1) * (unsigned long long)(d->k / 32) - 1) * (size_t)ld + (size_t)rows;
 }
 
 /* returns a device-usable pointer for `p`: itself if the device can read it, else a staged copy */
@@ -419,7 +453,7 @@ static void xb_invoke_gemm(const xb_slot* s, const libxsmm_gemm_param* p) {
   const size_t ext_a = xb_extent_a(d) * tsa, ext_b = xb_extent_b(d) * tsb, ext_c = (vnni_c ? (size_t)d->n * d->ldc : ((size_t)(d->n - 1) * d->ldc + d->m)) * tsc;
   const unsigned long long br = (d->br_type != 0 && p->op.tertiary != NULL) ? *(const unsigned long long*)p->op.tertiary : 1ull;
   xb_gemm_launch L;
-  xb_copyback cb, cb_mask; int staged = 0, need_cb = 0, need_cb_mask = 0;
+  xb_copyback cb, cb_mask; int staged = 0, need_cb = 0, need_cb_mask = 0, need_cb_scf = 0;
   memset(&L, 0, sizeof(L)); memset(&cb, 0, sizeof(cb)); memset(&cb_mask, 0, sizeof(cb_mask));
   L.d = *d; L.count = 1;
   L.one.br = br;
@@ -487,6 +521,18 @@ static void xb_invoke_gemm(const xb_slot* s, const libxsmm_gemm_param* p) {
   if (d->tc == LIBXSMM_DATATYPE_F32 && (d->ta == LIBXSMM_DATATYPE_I8 || d->ta == LIBXSMM_DATATYPE_U8) && p->c.tertiary != NULL) {
     L.one.scf = *(const float*)p->c.tertiary;
   }
+  if (xb_is_mx8(d->ta)) {   /* E8M0 block scales: a.tertiary, b.tertiary and, for an MXBF8 C, c.tertiary [n][ldc/32] */
+    L.one.a_s = xb_stage_in(p->a.tertiary, xb_extent_mx_scales(d, br, d->lda, d->m), &staged);
+    L.one.b_s = xb_stage_in(p->b.tertiary, xb_extent_mx_scales(d, br, d->ldb, d->n), &staged);
+    if (d->tc == LIBXSMM_DATATYPE_MXBF8) {
+      staged = 1;                      /* the f32 image lives in the scratch arena until the sync below */
+      if (p->c.tertiary != NULL && xb_rt_ptr_kind(p->c.tertiary) == 0) {
+        L.one.c_s = xb_rt_scratch((size_t)(d->n - 1) * (d->ldc / 32) + (size_t)(d->m / 32));
+        if (L.one.c_s == NULL) { xb_rt_scratch_reset(); return; }
+        need_cb_scf = 1;
+      } else L.one.c_s = p->c.tertiary;
+    }
+  }
   if (s->kind == XB_KIND_GEMM_EXT && (d->fuse_colbias != 0 || d->cp_op != 0)) {   /* d.primary: bias column; c.secondary: ReLU bitmask */
     const libxsmm_gemm_ext_param* pe = (const libxsmm_gemm_ext_param*)p;
     if (d->fuse_colbias != 0) {
@@ -524,6 +570,7 @@ static void xb_invoke_gemm(const xb_slot* s, const libxsmm_gemm_param* p) {
     else xb_rt_memcpy2d_async(cb.host, cb.dev, (size_t)d->ldc * tsc, (size_t)d->m * tsc, (size_t)d->n);
   }
   if (need_cb_mask) xb_rt_memcpy_async(cb_mask.host, cb_mask.dev, cb_mask.bytes);
+  if (need_cb_scf) xb_rt_memcpy2d_async(p->c.tertiary, L.one.c_s, (size_t)(d->ldc / 32), (size_t)(d->m / 32), (size_t)d->n);   /* the m/32 scale bytes of each column */
   if (staged || xb_rt_blocking()) { xb_rt_sync(); xb_rt_scratch_reset(); }
 }
 
@@ -602,10 +649,12 @@ static const xb_slot* xb_gemm_slot(const void* kernel) {
 
 /* 1 if a batch entry point cannot run this handle as a single call would: a fused handle's bias column and ReLU bit mask are
  * per-call operands (libxsmm_gemm_ext_param) that no batch form carries, VNNI-packed C is re-packed by a pass after a single
- * call only, and the strided forms have no argument struct for the int8 -> f32 scale (c.tertiary) */
+ * call only, the strided forms have no argument struct for the int8 -> f32 scale (c.tertiary), and no form but the scaled one carries
+ * the MX block scales */
 static int xb_batch_refused(const xb_gemm_desc* d, int strided) {
   const int i8 = (d->ta == LIBXSMM_DATATYPE_I8 || d->ta == LIBXSMM_DATATYPE_U8);
   if (d->fuse_colbias != 0 || (d->flags & LIBXSMM_GEMM_FLAG_VNNI_C) != 0) return 1;
+  if (xb_is_mx8(d->ta)) return 1;      /* MX block scales travel per call: libxsmm_b200_gemm_batch_strided_scaled */
   if (d->cp_op == LIBXSMM_MELTW_TYPE_UNARY_RELU && (d->cp_flags & LIBXSMM_MELTW_FLAG_UNARY_BITMASK_2BYTEMULT) != 0) return 1;
   return (strided && i8 && d->tc == LIBXSMM_DATATYPE_F32) ? 1 : 0;
 }
@@ -643,6 +692,57 @@ LIBXSMM_API int libxsmm_b200_gemm_batch_strided(libxsmm_gemmfunction kernel, con
   rc = xb_run_gemm_launch(&L);
   if (rc == 0 && xb_rt_blocking()) rc = xb_rt_sync();
   return rc;
+}
+
+#define XB_MX_IMAGE_BYTES (64ll << 20)   /* f32 image of an MXBF8-C batch: scratch per chunk */
+
+LIBXSMM_API int libxsmm_b200_gemm_batch_strided_scaled(libxsmm_gemmfunction kernel,
+  const void* a, const void* b, void* c, long long stride_a, long long stride_b, long long stride_c,
+  const void* scf_a, const void* scf_b, void* scf_c, long long stride_scf_a, long long stride_scf_b, long long stride_scf_c,
+  unsigned long long br_count, long long count)
+{
+  const xb_slot* s = xb_gemm_slot((const void*)kernel);
+  xb_gemm_launch L;
+  int rc;
+  if (s == NULL || count < 0 || s->kind != XB_KIND_GEMM || !xb_is_mx8(s->u.gemm.ta)) return -1;   /* only MX handles take per-call scales */
+  if (count == 0) return 0;
+  {
+    const int mx_c = (s->u.gemm.tc == LIBXSMM_DATATYPE_MXBF8);
+    if (a == NULL || b == NULL || c == NULL || scf_a == NULL || scf_b == NULL || (mx_c && scf_c == NULL)) return -1;
+    if (xb_rt_ptr_kind(a) == 0 || xb_rt_ptr_kind(b) == 0 || xb_rt_ptr_kind(c) == 0 || xb_rt_ptr_kind(scf_a) == 0
+     || xb_rt_ptr_kind(scf_b) == 0 || (mx_c && xb_rt_ptr_kind(scf_c) == 0)) return -4;               /* device-accessible operands only */
+  }
+  memset(&L, 0, sizeof(L));
+  L.d = s->u.gemm;
+  L.tile_stride_a = stride_a; L.tile_stride_b = stride_b; L.tile_stride_c = stride_c;
+  L.tile_stride_as = stride_scf_a; L.tile_stride_bs = stride_scf_b; L.tile_stride_cs = stride_scf_c;
+  L.br = (s->u.gemm.br_type == 0) ? 1ull : br_count;
+  if (L.d.tc != LIBXSMM_DATATYPE_MXBF8) {
+    L.count = count; L.a = a; L.b = b; L.c = c; L.one.a_s = scf_a; L.one.b_s = scf_b;
+    rc = xb_run_gemm_launch(&L);
+    if (rc == 0 && xb_rt_blocking()) rc = xb_rt_sync();
+    return rc;
+  }
+  {
+    /* MXBF8 C: the product goes through an f32 image of m*n*4 bytes per tile in the thread's scratch arena, which keeps its size
+     * once grown. The batch runs in chunks of at most XB_MX_IMAGE_BYTES of image, each synchronised before the arena is reused. */
+    const long long per_tile = (long long)L.d.m * L.d.n * 4;
+    const long long chunk = (per_tile < XB_MX_IMAGE_BYTES) ? XB_MX_IMAGE_BYTES / per_tile : 1;
+    long long t0;
+    rc = 0;
+    for (t0 = 0; t0 < count && rc == 0; t0 += chunk) {
+      int rs;
+      L.count = (count - t0 < chunk) ? (count - t0) : chunk;
+      L.a = (const char*)a + t0 * stride_a; L.b = (const char*)b + t0 * stride_b; L.c = (char*)c + t0 * stride_c;
+      L.one.a_s = (const char*)scf_a + t0 * stride_scf_a; L.one.b_s = (const char*)scf_b + t0 * stride_scf_b;
+      L.one.c_s = (char*)scf_c + t0 * stride_scf_c;
+      rc = xb_run_gemm_launch(&L);
+      rs = xb_rt_sync();
+      if (rc == 0) rc = rs;
+      xb_rt_scratch_reset();
+    }
+    return rc;
+  }
 }
 
 /* ---- one process, several GPUs: the batch is the only shard axis (SURVEY.md 8e). Host-resident operands are cut into

@@ -94,6 +94,9 @@ typedef struct xb_gemm_rec {
   unsigned long long br;
   float scf;            /* I8 x I8 -> F32 scalar scale */
   int pad_;
+  /* MXBF8 / MXHF8: E8M0 block scales, one byte per (row, 32 k); a.tertiary [br][k/32][lda], b.tertiary [br][k/32][ldb],
+   * and for an MXBF8 C c.tertiary [n][ldc/32] */
+  const void* a_s; const void* b_s; void* c_s;
 } xb_gemm_rec;
 
 /* launch description handed to the CUDA side */
@@ -103,6 +106,7 @@ typedef struct xb_gemm_launch {
   /* mode 0: uniform strided batch */
   const void* a; const void* b; void* c;
   long long tile_stride_a, tile_stride_b, tile_stride_c;   /* bytes */
+  long long tile_stride_as, tile_stride_bs, tile_stride_cs; /* MX block scales (bases in one.a_s / b_s / c_s), bytes */
   unsigned long long br;
   /* mode 1: per-tile records (device array of xb_gemm_rec[count]) */
   const xb_gemm_rec* recs;
