@@ -22,7 +22,7 @@
 
 namespace {
 
-enum { P_F64 = 0, P_F32, P_I16, P_I8_I32, P_I8_F32, P_F16_F16, P_F16_F32, P_BF16_F32, P_BF16_BF16, P_I4_I32, P_BITMAP, P_FP8, P_MX8, P_NONE };
+enum { P_F64 = 0, P_F32, P_I16, P_I8_I32, P_I8_F32, P_F16_F16, P_F16_F32, P_BF16_F32, P_BF16_BF16, P_I4_I32, P_BITMAP, P_FP8, P_MX8, P_DQ, P_NONE };
 
 __host__ __device__ inline int xb_path_of(const xb_gemm_desc& d) {
   const int a = d.ta, b = d.tb, c = d.tc, comp = d.tcomp;
@@ -31,6 +31,9 @@ __host__ __device__ inline int xb_path_of(const xb_gemm_desc& d) {
   if (a == LIBXSMM_DATATYPE_MXBF8 || a == LIBXSMM_DATATYPE_MXHF8) {   // MX fp8 (reference :2620-2679); the layout rules live in host_core.c
     const bool cok = (c == LIBXSMM_DATATYPE_F32) || (c == LIBXSMM_DATATYPE_MXBF8 && a == LIBXSMM_DATATYPE_MXBF8);
     return (b == a && comp == LIBXSMM_DATATYPE_F32 && cok && (d.br_type == 0 || d.br_type == 3) && d.fuse_colbias == 0 && d.cp_op == 0) ? P_MX8 : P_NONE;
+  }
+  if (xb_dq_form(&d) != XB_DQ_NONE) {   // dequantising A (reference :1684-2024); the layout rules live in host_core.c
+    return (d.fuse_colbias == 0 && d.cp_op == 0 && (d.flags & LIBXSMM_GEMM_FLAG_DECOMPRESS_A_VIA_BITMASK) == 0) ? P_DQ : P_NONE;
   }
   if ((d.flags & LIBXSMM_GEMM_FLAG_DECOMPRESS_A_VIA_BITMASK) != 0) {   // bitmap-compressed A (reference :857-948): float operands, no batch reduce
     const bool fa = (a == LIBXSMM_DATATYPE_F32 || a == LIBXSMM_DATATYPE_BF16 || a == LIBXSMM_DATATYPE_F16);
@@ -545,6 +548,87 @@ __global__ void __launch_bounds__(128) gemm_mx8_quant_kernel(const xb_gemm_launc
 }
 
 
+// ---- dequantising A: I8 x BF16, I8 / I4 / U4 / BF8 x F16 with per-row scales and zero points (reference :1684-2024) -----------
+// One thread per C element, the reference's order: acc runs from 0 over (r, k) with acc += a * b, where a is A's element widened
+// and dequantised with row i's scale sc (a.tertiary) and zero point zp (a.quaternary):
+//   I8 x BF16 (:1684-1730)  a = bf16_rne((float)int8 * sc), sc f32      A flat [k][lda], B [n][ldb]
+//   I8 x F16  (:1881-2024)  a = (float)int8 * sc, sc f16                 A flat; no zero point (the reference's fuse_zpt_sub is 0)
+//   I4 x F16  (:1793-1880)  a = ((float)nibble - zp) * sc, both f16       A bytes [k/2][lda]: low nibble even k, high nibble odd k,
+//                                                                          sign-extended unless U4
+//   BF8 x F16 (:1731-1792)  a = bf8 widened through f16                  A flat, or VNNI2 [k/2][lda][2]
+// An F16 B honours TRANS_B. Comp F16, or IMPLICIT resolved like an SPR host (as dot_f16), is the reference's "replacement FMA":
+// a is rounded to f16 after the subtraction and after the scaling, and acc after every add (the integer itself is exact in f16).
+// Then C: a 16-bit C adds its old value widened (beta = 1) and rounds once; an F32 C adds the old value as is, except next to an
+// I8 / I4 A and an F16 B, where the old value is first rounded to f16 (:1871-1876, :2016-2021).
+__device__ __forceinline__ float dq_f16r(float v) { return xb_f16_to_f32(xb_f32_to_f16(v)); }
+
+// row scales of tile t; kept out of resolve_tile like resolve_scales (the zero points travel in TileCtx::a_q)
+__device__ inline const void* dq_scales(const xb_gemm_launch& L, long long t) {
+  if (L.recs != nullptr) return L.recs[t].a_s;
+  if (L.a == nullptr && L.c == nullptr) return L.one.a_s;
+  return (const char*)L.one.a_s + t * L.tile_stride_as;
+}
+
+__global__ void __launch_bounds__(256) gemm_dq_kernel(const xb_gemm_launch L) {
+  const xb_gemm_desc& d = L.d;
+  const int form = xb_dq_form(&d);
+  const int m = d.m, n = d.n, k = d.k;
+  const long long lda = d.lda, ldb = d.ldb, ldc = d.ldc;
+  const bool beta0 = (d.flags & LIBXSMM_GEMM_FLAG_BETA_0) != 0, trans_b = (d.flags & LIBXSMM_GEMM_FLAG_TRANS_B) != 0;
+  const bool round_each = form != XB_DQ_I8_BF16 && (d.tcomp == LIBXSMM_DATATYPE_F16 || d.tcomp == LIBXSMM_DATATYPE_IMPLICIT);
+  const bool u4 = (d.ta == LIBXSMM_DATATYPE_U4X2), i4 = (form == XB_DQ_I4_F16), b16 = (form == XB_DQ_I8_BF16);
+  const int kb = (i4 || (form == XB_DQ_BF8_F16 && (d.flags & LIBXSMM_GEMM_FLAG_VNNI_A) != 0)) ? 2 : 1;
+  for (long long t = blockIdx.x; t < L.count; t += gridDim.x) {
+    TileCtx x; resolve_tile(L, t, x);
+    const void* scl = dq_scales(L, t);
+    for (int e = threadIdx.x; e < m * n; e += blockDim.x) {
+      const int i = e % m, j = e / m;
+      const long long ci = (long long)j * ldc + i;
+      float sc = 1.0f, zp = 0.0f;
+      if (b16) sc = reinterpret_cast<const float*>(scl)[i];
+      else if (form != XB_DQ_BF8_F16) sc = xb_f16_to_f32(reinterpret_cast<const unsigned short*>(scl)[i]);
+      if (i4) zp = xb_f16_to_f32(reinterpret_cast<const unsigned short*>(x.a_q)[i]);
+      float acc = 0.0f;
+      for (unsigned long long r = 0; r < x.br; ++r) {
+        const char *pa, *pb; br_ptrs(d, x, r, 1, 2, pa, pb);
+        for (int s = 0; s < k / kb; ++s) for (int k2 = 0; k2 < kb; ++k2) {
+          const long long kk = (long long)s * kb + k2;
+          float av;
+          if (form == XB_DQ_BF8_F16) av = xb_bf8_to_f32(ldg_as<unsigned char>(pa, s * (lda * kb) + (long long)i * kb + k2));
+          else {
+            const unsigned char by = ldg_as<unsigned char>(pa, s * lda + i);
+            int q;
+            if (!i4) q = (signed char)by;
+            else if (u4) q = (k2 == 0) ? (by & 0x0f) : (by >> 4);
+            else q = (k2 == 0) ? ((signed char)(by << 4)) >> 4 : ((signed char)by) >> 4;
+            av = (float)q;
+            if (b16) av = xb_bf16_to_f32(xb_f32_to_bf16_rne(__fmul_rn(av, sc)));
+            else {
+              if (i4) { av = __fsub_rn(av, zp); if (round_each) av = dq_f16r(av); }
+              av = __fmul_rn(av, sc);
+              if (round_each) av = dq_f16r(av);
+            }
+          }
+          const unsigned short bw = trans_b ? ldg_as<unsigned short>(pb, kk * ldb + j) : ldg_as<unsigned short>(pb, j * ldb + kk);
+          acc = __fadd_rn(acc, __fmul_rn(av, b16 ? xb_bf16_to_f32(bw) : xb_f16_to_f32(bw)));
+          if (round_each) acc = dq_f16r(acc);
+        }
+      }
+      if (d.tc == LIBXSMM_DATATYPE_F32) {
+        if (!beta0) { const float old = ldg_as<float>(x.c, ci); acc = __fadd_rn(acc, (b16 || form == XB_DQ_BF8_F16) ? old : dq_f16r(old)); }
+        reinterpret_cast<float*>(x.c)[ci] = acc;
+      } else if (b16) {
+        if (!beta0) acc = __fadd_rn(acc, xb_bf16_to_f32(ldg_as<unsigned short>(x.c, ci)));
+        reinterpret_cast<unsigned short*>(x.c)[ci] = xb_f32_to_bf16_rne(acc);
+      } else {
+        if (!beta0) acc = __fadd_rn(acc, xb_f16_to_f32(ldg_as<unsigned short>(x.c, ci)));
+        reinterpret_cast<unsigned short*>(x.c)[ci] = xb_f32_to_f16(acc);
+      }
+    }
+  }
+}
+
+
 // ---- 8-bit integer tiles: dp4a kernel ------------------------------------------------------------------------------
 // Integer sums wrap modulo 2^32 and are therefore exact in ANY order: the int8 paths need not follow the reference's
 // loop order to stay bit-identical (reference :1452-1683). One WARP per tile: the VNNI4 A words [k/4][m] and the
@@ -744,6 +828,17 @@ extern "C" int xb_gemm_simt_launch(const xb_gemm_launch* L) {
     }
     const cudaError_t me = cudaGetLastError();
     if (me != cudaSuccess) { xb_rt_note_error((int)me, "gemm_mx8"); return (int)me; }
+    return 0;
+  }
+  if (path == P_DQ) {
+    const int form = xb_dq_form(&L->d);
+    if (L->recs == nullptr && ((form != XB_DQ_BF8_F16 && L->one.a_s == nullptr) || (form == XB_DQ_I4_F16 && L->one.a_q == nullptr))) {
+      xb_rt_note_error(1, "dequantising A: row scales (a.tertiary) or int4 zero points (a.quaternary) missing"); return 1;
+    }
+    gemm_dq_kernel<<<(unsigned int)(L->count < (1 << 20) ? L->count : (1 << 20)), 256, 0, (cudaStream_t)xb_rt_stream()>>>(*L);
+    xb_rt_count_launch_backend(LIBXSMM_B200_BACKEND_SIMT);
+    const cudaError_t qe = cudaGetLastError();
+    if (qe != cudaSuccess) { xb_rt_note_error((int)qe, "gemm_dq"); return (int)qe; }
     return 0;
   }
   if (path == P_I4_I32 && L->one.a_q == nullptr && L->recs == nullptr) { xb_rt_note_error(1, "int4 A: zero points missing (a.quaternary)"); return 1; }

@@ -278,6 +278,32 @@ static int xb_mx8_desc_ok(const xb_gemm_desc* d, int ext) {
   return 1;
 }
 
+/* a narrow A next to a 16-bit float B: the dequantising tuples and their unsigned / mis-typed neighbours (none of which dispatched before) */
+static int xb_is_dq_family(const xb_gemm_desc* d) {
+  const int a = d->ta, b = d->tb;
+  return ((a == LIBXSMM_DATATYPE_I8 || a == LIBXSMM_DATATYPE_U8 || a == LIBXSMM_DATATYPE_I4X2 || a == LIBXSMM_DATATYPE_U4X2)
+          && (b == LIBXSMM_DATATYPE_BF16 || b == LIBXSMM_DATATYPE_F16)) || (a == LIBXSMM_DATATYPE_BF8 && b == LIBXSMM_DATATYPE_F16);
+}
+
+/* dequantising A (xb_dq_form; reference src/generator_gemm_reference_impl.c:1684-2024, operand slots :551-630): 1 if the reference
+ * defines a result for the descriptor in the layout the flags ask for. A flag the reference would ignore rather than obey is declined,
+ * so that no caller gets a layout other than the one asked for. */
+static int xb_dq_desc_ok(const xb_gemm_desc* d, int ext) {
+  const int form = xb_dq_form(d);
+  const int trans_b = (d->flags & LIBXSMM_GEMM_FLAG_TRANS_B) != 0, vnni_a = (d->flags & LIBXSMM_GEMM_FLAG_VNNI_A) != 0;
+  if (ext || form == XB_DQ_NONE) return 0;                 /* no fused form; U8 A (see xb_dq_form), other comp / C types */
+  /* no branch reads A transposed or B / C VNNI-packed; bitmap A is the sparse branch (:857-948); INTLV_A_FORMAT makes int4 the
+   * int8-B form (:472-480) */
+  if ((d->flags & (LIBXSMM_GEMM_FLAG_TRANS_A | LIBXSMM_GEMM_FLAG_VNNI_B | LIBXSMM_GEMM_FLAG_VNNI_C | LIBXSMM_GEMM_FLAG_DECOMPRESS_A_VIA_BITMASK
+                   | LIBXSMM_GEMM_FLAG_INTLV_A_FORMAT)) != 0) return 0;
+  if (form == XB_DQ_I8_BF16 && trans_b) return 0;          /* B is read [n][ldb] whatever the flag says (:1709) */
+  if ((form == XB_DQ_I8_BF16 || form == XB_DQ_I8_F16) && vnni_a) return 0;   /* A is read flat (l_k_block = 1, :1691, :1891, :1963) */
+  if (form == XB_DQ_I4_F16 && !vnni_a) return 0;           /* int4 x f16 is the VNNI_A form only (:472) */
+  if ((form == XB_DQ_I4_F16 || (form == XB_DQ_BF8_F16 && vnni_a)) && (d->k % 2) != 0) return 0;   /* k in pairs: an odd k would drop the last */
+  if (d->lda < d->m || d->ldb < (trans_b ? d->n : d->k)) return 0;
+  return 1;
+}
+
 static int xb_make_gemm_desc(xb_gemm_desc* d, const libxsmm_gemm_shape* shape, unsigned int flags, unsigned int prefetch,
                              const libxsmm_gemm_batch_reduce_config* br, int ext)
 {
@@ -300,6 +326,11 @@ static int xb_make_gemm_desc(xb_gemm_desc* d, const libxsmm_gemm_shape* shape, u
   }
   if (xb_is_mx8(d->ta) || xb_is_mx8(d->tb) || xb_is_mx8(d->tc)) {   /* MX fp8: its own layout rules, exact-order kernel only */
     if (!xb_mx8_desc_ok(d, ext) || !xb_gemm_simt_supported(d)) return 0;
+    d->backend = LIBXSMM_B200_BACKEND_SIMT;
+    return 1;
+  }
+  if (xb_is_dq_family(d)) {   /* dequantising A: its own layout rules, exact-order kernel only */
+    if (!xb_dq_desc_ok(d, ext) || !xb_gemm_simt_supported(d)) return 0;
     d->backend = LIBXSMM_B200_BACKEND_SIMT;
     return 1;
   }
@@ -398,6 +429,11 @@ LIBXSMM_API libxsmm_tilecfgfunction libxsmm_dispatch_tilecfg_gemm(const libxsmm_
 typedef struct xb_copyback { void* host; const void* dev; size_t bytes; } xb_copyback;
 
 static size_t xb_extent_a(const xb_gemm_desc* d) {   /* elements touched in one A operand */
+  if (xb_dq_form(d) != XB_DQ_NONE) {                  /* bytes: int4 pairs [k/2][lda], bf8 VNNI2 [k/2][lda][2], else flat [k][lda] */
+    if (xb_dq_form(d) == XB_DQ_I4_F16) return (size_t)(d->k / 2 - 1) * d->lda + (size_t)d->m;
+    if ((d->flags & LIBXSMM_GEMM_FLAG_VNNI_A) != 0) return (size_t)(d->k / 2 - 1) * d->lda * 2 + (size_t)d->m * 2;
+    return (size_t)(d->k - 1) * d->lda + d->m;
+  }
   if (d->ta == LIBXSMM_DATATYPE_I4X2 || d->ta == LIBXSMM_DATATYPE_U4X2) return (size_t)(d->k / 8 - 1) * d->lda * 4 + (size_t)d->m * 4;   /* bytes: 8 k per 4 bytes */
   if (xb_is_mx8(d->ta)) return (size_t)(d->k / 4 - 1) * d->lda * 4 + (size_t)d->m * 4;                                                 /* VNNI4 */
   const int trans_a = (d->flags & LIBXSMM_GEMM_FLAG_TRANS_A) != 0, vnni_a = (d->flags & LIBXSMM_GEMM_FLAG_VNNI_A) != 0;
@@ -505,7 +541,11 @@ static void xb_invoke_gemm(const xb_slot* s, const libxsmm_gemm_param* p) {
     L.one.a = xb_stage_in(p->a.primary, span_a ? span_a : 1, &staged);
     L.one.b = xb_stage_in(p->b.primary, span_b, &staged);
   }
-  if (d->ta == LIBXSMM_DATATYPE_I4X2 || d->ta == LIBXSMM_DATATYPE_U4X2) {   /* a.quaternary: one zero-point byte per row (and per reduce step) */
+  if (xb_dq_form(d) != XB_DQ_NONE && xb_dq_form(d) != XB_DQ_BF8_F16) {   /* a.tertiary: m row scales (f32 next to a bf16 B, else f16);
+                                                                          * int4: a.quaternary, m f16 zero points. One set for every r. */
+    L.one.a_s = xb_stage_in(p->a.tertiary, (size_t)d->m * (xb_dq_form(d) == XB_DQ_I8_BF16 ? 4 : 2), &staged);
+    if (xb_dq_form(d) == XB_DQ_I4_F16) L.one.a_q = xb_stage_in(p->a.quaternary, (size_t)d->m * 2, &staged);
+  } else if (d->ta == LIBXSMM_DATATYPE_I4X2 || d->ta == LIBXSMM_DATATYPE_U4X2) {   /* a.quaternary: one zero-point byte per row (and per reduce step) */
     const size_t zb = (size_t)d->m + ((d->br_type == 3 && br > 0) ? (size_t)(br - 1) * (size_t)((d->br_stride_a * 2) / d->k) : 0);
     L.one.a_q = xb_stage_in(p->a.quaternary, zb, &staged);
     if (L.one.a_q == NULL) { xb_rt_note_error(2, "invoke_gemm: int4 A needs zero points in a.quaternary"); xb_rt_scratch_reset(); return; }
@@ -650,11 +690,14 @@ static const xb_slot* xb_gemm_slot(const void* kernel) {
 /* 1 if a batch entry point cannot run this handle as a single call would: a fused handle's bias column and ReLU bit mask are
  * per-call operands (libxsmm_gemm_ext_param) that no batch form carries, VNNI-packed C is re-packed by a pass after a single
  * call only, the strided forms have no argument struct for the int8 -> f32 scale (c.tertiary), and no form but the scaled one carries
- * the MX block scales */
+ * the MX block scales. The row scales of a dequantising A travel in the per-tile form and the scaled one (see xb_dq_scaled). */
+static int xb_dq_scaled(const xb_gemm_desc* d) { return xb_dq_form(d) != XB_DQ_NONE && xb_dq_form(d) != XB_DQ_BF8_F16; }
+
 static int xb_batch_refused(const xb_gemm_desc* d, int strided) {
   const int i8 = (d->ta == LIBXSMM_DATATYPE_I8 || d->ta == LIBXSMM_DATATYPE_U8);
   if (d->fuse_colbias != 0 || (d->flags & LIBXSMM_GEMM_FLAG_VNNI_C) != 0) return 1;
   if (xb_is_mx8(d->ta)) return 1;      /* MX block scales travel per call: libxsmm_b200_gemm_batch_strided_scaled */
+  if (strided && xb_dq_scaled(d)) return 1;   /* row scales: libxsmm_b200_gemm_batch_strided_scaled or libxsmm_b200_gemm_batch */
   if (d->cp_op == LIBXSMM_MELTW_TYPE_UNARY_RELU && (d->cp_flags & LIBXSMM_MELTW_FLAG_UNARY_BITMASK_2BYTEMULT) != 0) return 1;
   return (strided && i8 && d->tc == LIBXSMM_DATATYPE_F32) ? 1 : 0;
 }
@@ -703,9 +746,25 @@ LIBXSMM_API int libxsmm_b200_gemm_batch_strided_scaled(libxsmm_gemmfunction kern
 {
   const xb_slot* s = xb_gemm_slot((const void*)kernel);
   xb_gemm_launch L;
-  int rc;
-  if (s == NULL || count < 0 || s->kind != XB_KIND_GEMM || !xb_is_mx8(s->u.gemm.ta)) return -1;   /* only MX handles take per-call scales */
+  int rc, dq;
+  if (s == NULL || count < 0 || s->kind != XB_KIND_GEMM) return -1;
+  /* only MX handles and int8 dequantising ones take per-call scales here; int4 needs zero points as well: libxsmm_b200_gemm_batch */
+  dq = xb_dq_form(&s->u.gemm);
+  if (!xb_is_mx8(s->u.gemm.ta) && dq != XB_DQ_I8_BF16 && dq != XB_DQ_I8_F16) return -1;
   if (count == 0) return 0;
+  if (dq != XB_DQ_NONE) {   /* row scales of tile t: scf_a + t*stride_scf_a (stride 0: shared weights' scales) */
+    if (a == NULL || b == NULL || c == NULL || scf_a == NULL) return -1;
+    if (s->u.gemm.br_type == 1 || s->u.gemm.br_type == 2) return -2;   /* per-tile arrays: libxsmm_b200_gemm_batch */
+    if (xb_rt_ptr_kind(a) == 0 || xb_rt_ptr_kind(b) == 0 || xb_rt_ptr_kind(c) == 0 || xb_rt_ptr_kind(scf_a) == 0) return -4;
+    memset(&L, 0, sizeof(L));
+    L.d = s->u.gemm; L.count = count; L.a = a; L.b = b; L.c = c;
+    L.tile_stride_a = stride_a; L.tile_stride_b = stride_b; L.tile_stride_c = stride_c;
+    L.one.a_s = scf_a; L.tile_stride_as = stride_scf_a;
+    L.br = (s->u.gemm.br_type == 0) ? 1ull : br_count;
+    rc = xb_run_gemm_launch(&L);
+    if (rc == 0 && xb_rt_blocking()) rc = xb_rt_sync();
+    return rc;
+  }
   {
     const int mx_c = (s->u.gemm.tc == LIBXSMM_DATATYPE_MXBF8);
     if (a == NULL || b == NULL || c == NULL || scf_a == NULL || scf_b == NULL || (mx_c && scf_c == NULL)) return -1;
@@ -940,15 +999,18 @@ static int xb_plan_try_pool(libxsmm_b200_gemm_plan* plan, const xb_slot* s, cons
   return 1;
 }
 
-LIBXSMM_API libxsmm_b200_gemm_plan* libxsmm_b200_gemm_plan_create(libxsmm_gemmfunction kernel,
-  const libxsmm_gemm_param* params, long long count)
-{
-  const xb_slot* s = xb_gemm_slot((const void*)kernel);
+/* the per-tile records of a batch: libxsmm_b200_gemm_batch and libxsmm_b200_gemm_plan_create */
+static libxsmm_b200_gemm_plan* xb_plan_make(const xb_slot* s, const libxsmm_gemm_param* params, long long count) {
   libxsmm_b200_gemm_plan* plan;
   xb_gemm_rec* recs;
   char* arrays = NULL; size_t arrays_bytes = 0, off = 0;
   long long t;
   if (s == NULL || params == NULL || count <= 0 || xb_batch_refused(&s->u.gemm, 0)) return NULL;
+  if (xb_dq_scaled(&s->u.gemm)) {   /* every tile brings its row scales (a.tertiary) and, for int4, zero points (a.quaternary) */
+    for (t = 0; t < count; ++t) {
+      if (params[t].a.tertiary == NULL || (xb_dq_form(&s->u.gemm) == XB_DQ_I4_F16 && params[t].a.quaternary == NULL)) return NULL;
+    }
+  }
   plan = (libxsmm_b200_gemm_plan*)calloc(1, sizeof(*plan));
   if (plan != NULL && xb_plan_try_pool(plan, s, params, count)) return plan;
   recs = (xb_gemm_rec*)calloc((size_t)count, sizeof(xb_gemm_rec));
@@ -979,6 +1041,7 @@ LIBXSMM_API libxsmm_b200_gemm_plan* libxsmm_b200_gemm_plan_create(libxsmm_gemmfu
     }
     if (s->u.gemm.tc == LIBXSMM_DATATYPE_F32 && (s->u.gemm.ta == LIBXSMM_DATATYPE_I8 || s->u.gemm.ta == LIBXSMM_DATATYPE_U8)
         && p->c.tertiary != NULL) r->scf = *(const float*)p->c.tertiary;
+    if (xb_dq_scaled(&s->u.gemm)) { r->a_s = p->a.tertiary; r->a_q = p->a.quaternary; }
   }
   plan->d_recs = (xb_gemm_rec*)xb_rt_device_malloc((size_t)count * sizeof(xb_gemm_rec));
   if (plan->d_recs == NULL) { free(arrays); free(recs); xb_rt_device_free(plan->d_arrays); free(plan); return NULL; }
@@ -987,6 +1050,15 @@ LIBXSMM_API libxsmm_b200_gemm_plan* libxsmm_b200_gemm_plan_create(libxsmm_gemmfu
   free(arrays); free(recs);
   plan->slot = s; plan->count = count;
   return plan;
+}
+
+/* a plan is prepared once and replayed: the row scales of a dequantising A are per-call operands, so such a handle gets no plan */
+LIBXSMM_API libxsmm_b200_gemm_plan* libxsmm_b200_gemm_plan_create(libxsmm_gemmfunction kernel,
+  const libxsmm_gemm_param* params, long long count)
+{
+  const xb_slot* s = xb_gemm_slot((const void*)kernel);
+  if (s == NULL || xb_dq_scaled(&s->u.gemm)) return NULL;
+  return xb_plan_make(s, params, count);
 }
 
 LIBXSMM_API int libxsmm_b200_gemm_plan_run(const libxsmm_b200_gemm_plan* plan) {
@@ -1019,7 +1091,7 @@ LIBXSMM_API int libxsmm_b200_gemm_batch(libxsmm_gemmfunction kernel, const libxs
   int rc;
   if (s != NULL && xb_batch_refused(&s->u.gemm, 0)) return LIBXSMM_B200_ERROR_NOT_BATCHABLE;
   if (count == 0) return 0;
-  plan = libxsmm_b200_gemm_plan_create(kernel, params, count);
+  plan = xb_plan_make(s, params, count);   /* unlike a plan, one batch call also carries dequantising A's row scales */
   if (plan == NULL) return -1;
   rc = libxsmm_b200_gemm_plan_run(plan);
   if (rc == 0 && !xb_rt_blocking()) rc = xb_rt_sync();   /* the plan's arrays must outlive the launch */

@@ -90,14 +90,35 @@ typedef struct xb_gemm_rec {
   const void* b_aux;
   const void* d;        /* ext: colbias */
   void* c_aux;          /* ext: relu bitmask out */
-  const void* a_q;      /* int4 A: zero points (a.quaternary); bitmap-compressed A: the bitmap (a.secondary) */
+  const void* a_q;      /* int4 A: zero points (a.quaternary: bytes next to an 8-bit B, m f16 next to an f16 B); bitmap-compressed A:
+                         * the bitmap (a.secondary) */
   unsigned long long br;
   float scf;            /* I8 x I8 -> F32 scalar scale */
   int pad_;
   /* MXBF8 / MXHF8: E8M0 block scales, one byte per (row, 32 k); a.tertiary [br][k/32][lda], b.tertiary [br][k/32][ldb],
-   * and for an MXBF8 C c.tertiary [n][ldc/32] */
+   * and for an MXBF8 C c.tertiary [n][ldc/32]. Dequantising A (xb_dq_form): a_s holds the m row scales of a.tertiary. */
   const void* a_s; const void* b_s; void* c_s;
 } xb_gemm_rec;
+
+/* dequantising GEMM: a narrow A widened to B's 16-bit float type inside the kernel, with per-row scales (and, for int4, zero
+ * points) of the call (reference src/generator_gemm_reference_impl.c:1684-2024). The form of a descriptor by its types, or 0.
+ * U8 A is not a form: the reference reads those bytes as signed char (:1703, :1907, :1979), so a U8 caller would get the
+ * results of the I8 bytes; dispatch declines it instead. */
+enum { XB_DQ_NONE = 0, XB_DQ_I8_BF16, XB_DQ_I8_F16, XB_DQ_I4_F16, XB_DQ_BF8_F16 };
+#if defined(__CUDACC__)
+__host__ __device__
+#endif
+static inline int xb_dq_form(const xb_gemm_desc* d) {
+  const int f16comp = (d->tcomp == LIBXSMM_DATATYPE_F16 || d->tcomp == LIBXSMM_DATATYPE_F32 || d->tcomp == LIBXSMM_DATATYPE_IMPLICIT);
+  if (d->ta == LIBXSMM_DATATYPE_I8 && d->tb == LIBXSMM_DATATYPE_BF16) {            /* :1684-1730, comp F32 */
+    return (d->tcomp == LIBXSMM_DATATYPE_F32 && (d->tc == LIBXSMM_DATATYPE_F32 || d->tc == LIBXSMM_DATATYPE_BF16)) ? XB_DQ_I8_BF16 : XB_DQ_NONE;
+  }
+  if (d->tb != LIBXSMM_DATATYPE_F16 || !f16comp || (d->tc != LIBXSMM_DATATYPE_F16 && d->tc != LIBXSMM_DATATYPE_F32)) return XB_DQ_NONE;
+  if (d->ta == LIBXSMM_DATATYPE_I8) return XB_DQ_I8_F16;                                                 /* :1881-2024 */
+  if (d->ta == LIBXSMM_DATATYPE_I4X2 || d->ta == LIBXSMM_DATATYPE_U4X2) return XB_DQ_I4_F16;             /* :1793-1880 */
+  if (d->ta == LIBXSMM_DATATYPE_BF8) return XB_DQ_BF8_F16;                                               /* :1731-1792 */
+  return XB_DQ_NONE;
+}
 
 /* launch description handed to the CUDA side */
 typedef struct xb_gemm_launch {
@@ -106,7 +127,7 @@ typedef struct xb_gemm_launch {
   /* mode 0: uniform strided batch */
   const void* a; const void* b; void* c;
   long long tile_stride_a, tile_stride_b, tile_stride_c;   /* bytes */
-  long long tile_stride_as, tile_stride_bs, tile_stride_cs; /* MX block scales (bases in one.a_s / b_s / c_s), bytes */
+  long long tile_stride_as, tile_stride_bs, tile_stride_cs; /* MX block scales, dequantising A's row scales (bases in one.a_s / b_s / c_s), bytes */
   unsigned long long br;
   /* mode 1: per-tile records (device array of xb_gemm_rec[count]) */
   const xb_gemm_rec* recs;
