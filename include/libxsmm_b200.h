@@ -51,6 +51,11 @@ LIBXSMM_API int libxsmm_b200_bcsc_variant(const void* kernel, unsigned long long
  * TMA-staged kernel with S shared-memory stages; -1: NULL handle. Pageable host B / C are answered for the device buffers they are
  * staged through. */
 LIBXSMM_API int libxsmm_b200_fsspmdm_variant(const libxsmm_fsspmdm* handle, const void* B, const void* C);
+/* matrix-eltwise handles: the kernel a call with this libxsmm_meltw_unary_param (NULL: aligned device operands) runs. 0 generic
+ * transform, 1 tiled transpose, 2 VNNI pack, 3 VNNI pack with 16-byte accesses, 4 warp reduction, 5 two-phase column reduction,
+ * 6 two-phase column reduction with the float4 partial pass, 7 any other kernel (map, to-scalar, gather / scatter, quantisers,
+ * dropout, unzip / decomp); -1: not a matrix-eltwise handle. Pageable operands are answered for the buffers they are staged through. */
+LIBXSMM_API int libxsmm_b200_meltw_variant(const void* kernel, const void* param);
 /* force the SIMT kernel for dense GEMM handles dispatched afterwards (debug / parity checking) */
 LIBXSMM_API void libxsmm_b200_set_force_simt(int on);
 

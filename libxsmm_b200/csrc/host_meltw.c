@@ -263,6 +263,12 @@ void xb_invoke_meltw(const xb_slot* s, const void* param) {
       if (op != LIBXSMM_MELTW_TYPE_UNARY_GATHER && op != LIBXSMM_MELTW_TYPE_UNARY_SCATTER) {
         a.n_rt = *(const unsigned long long*)p->in.tertiary;
         a.in_aux = stage_in(&st, p->in.secondary, (size_t)a.n_rt * ((d->flags & LIBXSMM_MELTW_FLAG_UNARY_IDX_SIZE_4BYTES) ? 4 : 8));
+        /* MAX / MIN with RECORD_ARGOP write one column index per row to out.secondary (reference :1243-1275): staged in and out like
+         * the REDUCE_X_OP_* branch below, so that a pageable index buffer is never handed to the kernel */
+        if (op != LIBXSMM_MELTW_TYPE_UNARY_REDUCE_COLS_IDX_OP_ADD && (d->flags & LIBXSMM_MELTW_FLAG_UNARY_REDUCE_RECORD_ARGOP) != 0) {
+          a.out_aux = stage_inout(&st, p->out.secondary, (size_t)d->m * ((d->flags & LIBXSMM_MELTW_FLAG_UNARY_IDX_SIZE_4BYTES) ? 4 : 8));
+          if (a.out_aux == NULL) st.failed = 1;
+        }
       } else {
         const size_t isz = (d->flags & LIBXSMM_MELTW_FLAG_UNARY_IDX_SIZE_8BYTES) ? 8 : 4;
         const size_t cnt = (d->flags & LIBXSMM_MELTW_FLAG_UNARY_GS_COLS) ? (size_t)d->n : ((d->flags & LIBXSMM_MELTW_FLAG_UNARY_GS_ROWS) ? (size_t)d->m : (size_t)d->m * d->n);

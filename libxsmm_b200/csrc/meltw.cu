@@ -13,6 +13,7 @@
 // and stores are coalesced along i and a bitmask byte is assembled with one __ballot_sync.
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <string.h>
 #include <float.h>
 #include "xb_internal.h"
 #include "xb_device.cuh"
@@ -315,17 +316,67 @@ __global__ void __launch_bounds__(256) meltw_map_kernel(const xb_meltw_desc d, c
   }
 }
 
-// ---- reductions: one warp per result element, lanes stride the reduced dimension, shuffle combine -------------------
+// ---- reductions: one warp per result element ------------------------------------------------------------------------
+// Sums: lanes stride the reduced dimension, shuffle combine. Max / min / absmax give the reference's sequential fold bit for bit
+// (:1215-1428 with LIBXSMM_MAX(A,B) = A < B ? B : A, LIBXSMM_MIN(A,B) = A < B ? A : B, LIBXSMM_ABS(A) = 0 <= A ? A : -A):
+//   line   op       start       equal values      NaN element
+//   rows   MAX      element 0   earlier kept      ignored; a NaN element 0 sticks
+//   rows   ABSMAX   element 0   earlier kept      ignored; a NaN element 0 sticks, its sign flipped once per element folded
+//   rows   MIN      element 0   later taken       taken, and the next element replaces it (the fold restarts after it)
+//   cols   MAX      -FLT_MAX    later taken       taken, the fold restarts after it (without the -FLT_MAX start)
+//   cols   ABSMAX   +0          later taken       like cols MAX, on ABS values (ABS(-0) = -0, ABS flips a NaN's sign)
+//   cols   MIN      +FLT_MAX    earlier kept      ignored
+//   argop  any      as cols     later taken       ignored (x >= tmp / x <= tmp is false); an index never taken is not written
+// Each lane folds one contiguous segment of the line with these rules; the segments combine in lane order (a segment holding a
+// NaN that restarts the fold discards everything before it), so the result is the sequential one whatever the segment cut.
+// Values are compared through integer keys and moved as bits: a float select could be fused into FMNMX, which returns +0 for
+// (-0, +0) and canonicalises NaN payloads.
+__device__ __forceinline__ unsigned int mm_bits(float x) { return __float_as_uint(x); }
+__device__ __forceinline__ unsigned long long mm_bits(double x) { return (unsigned long long)__double_as_longlong(x); }
+__device__ __forceinline__ float mm_from(unsigned int u, float) { return __uint_as_float(u); }
+__device__ __forceinline__ double mm_from(unsigned long long u, double) { return __longlong_as_double((long long)u); }
+template <typename T> struct mm_traits;
+template <> struct mm_traits<float> { typedef unsigned int U; static constexpr U SIGN = 0x80000000u, INF = 0x7f800000u; };
+template <> struct mm_traits<double> { typedef unsigned long long U; static constexpr U SIGN = 0x8000000000000000ull, INF = 0x7ff0000000000000ull; };
+template <typename T> __device__ __forceinline__ bool mm_isnan(T x) {
+  typedef typename mm_traits<T>::U U; return (mm_bits(x) & ~mm_traits<T>::SIGN) > mm_traits<T>::INF;
+}
+// LIBXSMM_ABS: negative non-zero values and NaNs get their sign flipped, +-0 stay
+template <typename T> __device__ __forceinline__ T mm_abs(T x) {
+  typedef typename mm_traits<T>::U U; const U u = mm_bits(x);
+  const bool flip = mm_isnan(x) || ((u & mm_traits<T>::SIGN) != 0 && (u & ~mm_traits<T>::SIGN) != 0);
+  return mm_from(flip ? (u ^ mm_traits<T>::SIGN) : u, x);
+}
+// order key of a non-NaN value with -0 == +0
+template <typename T> __device__ __forceinline__ typename mm_traits<T>::U mm_key(T x) {
+  typedef typename mm_traits<T>::U U; U u = mm_bits(x);
+  if ((u & ~mm_traits<T>::SIGN) == 0) u = 0;
+  return (u & mm_traits<T>::SIGN) ? ~u : (u | mm_traits<T>::SIGN);
+}
+// x replaces the running value v: max or min, the later one on equal values or the earlier one
+template <typename T> __device__ __forceinline__ bool mm_better(T x, T v, bool is_min, bool later) {
+  const typename mm_traits<T>::U kx = mm_key(x), kv = mm_key(v);
+  return is_min ? (later ? kx <= kv : kx < kv) : (later ? kx >= kv : kx > kv);
+}
+template <typename T> struct mm_state { T v, nanv; long long pos; int have, reset; };
+template <typename T> __device__ __forceinline__ mm_state<T> mm_combine(mm_state<T> l, const mm_state<T>& r, bool is_min, bool later) {
+  if (r.reset) return r;
+  if (r.have && (!l.have || mm_better(r.v, l.v, is_min, later))) { l.v = r.v; l.pos = r.pos; l.have = 1; }
+  return l;
+}
+
+template <typename T>
+__device__ __forceinline__ T reduce_load(const xb_meltw_desc& d, const xb_meltw_args& a, long long idx) {
+  return (sizeof(T) == 8) ? (T)((const double*)a.in0)[idx] : (T)ld_f32(a.in0, idx, d.t_in0);
+}
 template <typename T> __device__ __forceinline__ T warp_sum(T v) { for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o); return v; }
-template <typename T> __device__ __forceinline__ T warp_max(T v) { for (int o = 16; o > 0; o >>= 1) { const T u = __shfl_xor_sync(0xffffffffu, v, o); v = (u > v) ? u : v; } return v; }
-template <typename T> __device__ __forceinline__ T warp_min(T v) { for (int o = 16; o > 0; o >>= 1) { const T u = __shfl_xor_sync(0xffffffffu, v, o); v = (u < v) ? u : v; } return v; }
 
 template <typename T>
 __global__ void __launch_bounds__(256) meltw_reduce_kernel(const xb_meltw_desc d, const xb_meltw_args a) {
   const int lane = threadIdx.x & 31;
   const bool rows = (d.flags & LIBXSMM_MELTW_FLAG_UNARY_REDUCE_ROWS) != 0;
   const bool init_acc = (d.flags & LIBXSMM_MELTW_FLAG_UNARY_REDUCE_INIT_ACC) != 0;
-  const bool argop = (d.flags & LIBXSMM_MELTW_FLAG_UNARY_REDUCE_RECORD_ARGOP) != 0;
+  const bool argop = !rows && (d.flags & LIBXSMM_MELTW_FLAG_UNARY_REDUCE_RECORD_ARGOP) != 0;
   const bool idx4 = (d.flags & LIBXSMM_MELTW_FLAG_UNARY_IDX_SIZE_4BYTES) != 0;
   const bool f64 = sizeof(T) == 8;
   const int op = d.op;
@@ -337,35 +388,23 @@ __global__ void __launch_bounds__(256) meltw_reduce_kernel(const xb_meltw_desc d
   const bool want_x2 = (op == LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X2_OP_ADD || op == LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X_X2_OP_ADD);
   const int nres = rows ? d.n : d.m;
   const int result_size = rows ? d.n : d.ldo;                 // offset of the x^2 plane (reference :1073-1076)
-  const int len = rows ? d.m : (by_idx ? (int)a.n_rt : d.n);
+  const long long len = rows ? d.m : (by_idx ? (long long)a.n_rt : d.n);
+  // fold rules of the table above
+  const bool is_min = (kind == 2);
+  const bool later = argop || (rows ? kind == 2 : kind != 2);
+  const bool nan_restarts = !argop && (rows ? kind == 2 : kind != 2);
   for (int o = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); o < nres; o += gridDim.x * (blockDim.x >> 5)) {
-    T sx = 0, sx2 = 0, best = (kind == 1) ? (T)-FLT_MAX : ((kind == 2) ? (T)FLT_MAX : (T)0);
-    long long best_j = 0;
-    if (kind != 0 && rows) best = f64 ? (T)((const double*)a.in0)[(long long)o * d.ldi] : (T)ld_f32(a.in0, (long long)o * d.ldi, d.t_in0);
-    if (argop && kind != 0 && !rows) {                        // order-dependent (last extremum wins): one lane scans
-      if (lane == 0) {
-        for (int t = 0; t < len; ++t) {
-          const long long j = by_idx ? (idx4 ? (long long)((const unsigned int*)a.in_aux)[t] : (long long)((const unsigned long long*)a.in_aux)[t]) : t;
-          T v = f64 ? (T)((const double*)a.in0)[o + j * d.ldi] : (T)ld_f32(a.in0, o + j * d.ldi, d.t_in0);
-          if (kind == 3) v = (v < 0) ? -v : v;
-          if ((kind == 2) ? (v <= best) : (v >= best)) { best = v; best_j = j; }
-        }
-        if (a.out_aux != nullptr) { if (idx4) ((unsigned int*)a.out_aux)[o] = (unsigned int)best_j; else ((unsigned long long*)a.out_aux)[o] = (unsigned long long)best_j; }
-      }
-      best = __shfl_sync(0xffffffffu, best, 0);
-    } else {
-      for (int t = lane; t < len; t += 32) {
+    if (kind == 0) {
+      T sx = 0, sx2 = 0;
+      for (long long t = lane; t < len; t += 32) {
         long long idx;
         if (rows) idx = t + (long long)o * d.ldi;
         else { const long long j = by_idx ? (idx4 ? (long long)((const unsigned int*)a.in_aux)[t] : (long long)((const unsigned long long*)a.in_aux)[t]) : t; idx = o + j * d.ldi; }
-        T v = f64 ? (T)((const double*)a.in0)[idx] : (T)ld_f32(a.in0, idx, d.t_in0);
-        if (kind == 0) { sx += v; sx2 += v * v; }
-        else { if (kind == 3) { v = (v < 0) ? -v : v; best = (best < 0) ? -best : best; } best = (kind == 2) ? ((v < best) ? v : best) : ((v > best) ? v : best); }
+        const T v = reduce_load<T>(d, a, idx);
+        sx += v; sx2 += v * v;
       }
-      if (kind == 0) { sx = warp_sum(sx); sx2 = warp_sum(sx2); } else best = (kind == 2) ? warp_min(best) : warp_max(best);
-    }
-    if (lane == 0) {
-      if (kind == 0) {
+      sx = warp_sum(sx); sx2 = warp_sum(sx2);
+      if (lane == 0) {
         if (f64) {
           double* ox = (double*)a.out; double* ox2 = want_x ? ox + result_size : ox;
           if (want_x) ox[o] = (double)sx + ((init_acc) ? ox[o] : 0.0);
@@ -375,8 +414,43 @@ __global__ void __launch_bounds__(256) meltw_reduce_kernel(const xb_meltw_desc d
           if (want_x) { float r = (float)sx; if (init_acc && !by_idx) r += ld_f32(a.out, o, d.t_out); st_f32(a.out, o, d.t_out, r); }
           if (want_x2) { float r = (float)sx2; if (init_acc) r += ld_f32(base2, o, d.t_out); st_f32(base2, o, d.t_out, r); }
         }
-      } else {
-        if (f64) ((double*)a.out)[o] = (double)best; else st_f32(a.out, o, d.t_out, (float)best);
+      }
+      continue;
+    }
+    const long long seg = (len + 31) / 32, t0 = lane * seg, t1 = (t0 + seg < len) ? t0 + seg : len;
+    mm_state<T> st; st.v = st.nanv = (T)0; st.pos = 0; st.have = 0; st.reset = 0;
+    for (long long t = t0; t < t1; ++t) {
+      const long long j = rows ? t : (by_idx ? (idx4 ? (long long)((const unsigned int*)a.in_aux)[t] : (long long)((const unsigned long long*)a.in_aux)[t]) : t);
+      T v = reduce_load<T>(d, a, rows ? (t + (long long)o * d.ldi) : (o + j * d.ldi));
+      if (kind == 3) v = mm_abs(v);
+      if (mm_isnan(v)) { if (nan_restarts) { st.reset = 1; st.have = 0; st.nanv = v; } }
+      else if (!st.have || mm_better(v, st.v, is_min, later)) { st.v = v; st.pos = j; st.have = 1; }
+    }
+#pragma unroll
+    for (int off = 1; off < 32; off <<= 1) {
+      mm_state<T> r;
+      r.v = __shfl_down_sync(0xffffffffu, st.v, off); r.nanv = __shfl_down_sync(0xffffffffu, st.nanv, off);
+      r.pos = __shfl_down_sync(0xffffffffu, st.pos, off);
+      r.have = __shfl_down_sync(0xffffffffu, st.have, off); r.reset = __shfl_down_sync(0xffffffffu, st.reset, off);
+      if ((lane & (2 * off - 1)) == 0 && lane + off < 32) st = mm_combine(st, r, is_min, later);
+    }
+    if (lane == 0) {
+      T res; bool taken = false;
+      if (rows) {
+        const T x0 = reduce_load<T>(d, a, (long long)o * d.ldi);
+        if (kind != 2 && mm_isnan(x0)) {                       // a NaN start sticks; ABS flips it once per element folded
+          typedef typename mm_traits<T>::U U;
+          res = (kind == 3 && (len & 1)) ? mm_from((U)(mm_bits(x0) ^ mm_traits<T>::SIGN), x0) : x0;
+        } else res = st.have ? st.v : st.nanv;
+      } else if (st.reset) res = st.have ? st.v : st.nanv;    // after a NaN the fold has no start value
+      else {
+        const T start = (kind == 1) ? (T)-FLT_MAX : ((kind == 2) ? (T)FLT_MAX : (T)0);
+        taken = st.have && mm_better(st.v, start, is_min, later);
+        res = taken ? st.v : start;
+      }
+      if (f64) ((double*)a.out)[o] = (double)res; else st_f32(a.out, o, d.t_out, (float)res);
+      if (argop && taken && a.out_aux != nullptr) {
+        if (idx4) ((unsigned int*)a.out_aux)[o] = (unsigned int)st.pos; else ((unsigned long long*)a.out_aux)[o] = (unsigned long long)st.pos;
       }
     }
   }
@@ -818,10 +892,65 @@ int launch_done(const char* where) {
 
 extern "C" int xb_meltw_supported(const xb_meltw_desc* d) { return family_of(*d) != FAM_NONE; }
 
+// which kernel a call runs (the variant numbers of libxsmm_b200_meltw_variant, include/libxsmm_b200.h). The choice depends on the
+// shape and, for the vector kernels, on the alignment of the operands the kernel reads and writes:
+//   NORM_TO_NORMT with m*n >= 4096 ................................................. 1 tiled transpose (64 x 64 tiles)
+//   NORM_TO_VNNI2(_PAD) 16-bit / NORM_TO_VNNI4(_PAD) 8-bit with ldo*n >= 4096 ........ 2 VNNI pack, or 3 with 16-byte accesses when
+//                                                                                      m, ldi, ldo are multiples of 16/size and in0, out
+//                                                                                      are 16-byte aligned
+//   other transforms ................................................................ 0 generic transform
+//   column sum / sum of squares, not F64, m >= 256, m*n >= 2^18 ...................... 5 two-phase column reduction, or 6 with the float4
+//                                                                                      partial pass (F32, m % 4 = 0, ldi % 4 = 0, in0
+//                                                                                      16-byte aligned)
+//   other reductions (rows, max / min / absmax, column-index, F64) ................... 4 warp reduction
+//   maps, to-scalar, gather / scatter, quantisers, dropout, unzip / decomp ........... 7
+extern "C" int xb_meltw_variant(const xb_meltw_desc* d, const xb_meltw_args* a) {
+  const int fam = family_of(*d);
+  if (fam == FAM_TRANSFORM) {
+    const int ts = xb_dev_typesize(d->t_in0);
+    if (d->op == LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_NORMT && (long long)d->m * d->n >= 4096) return 1;
+    if ((long long)d->ldo * d->n >= 4096 && ((ts == 2 && (d->op == LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_VNNI2 || d->op == LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_VNNI2_PAD))
+                                          || (ts == 1 && (d->op == LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_VNNI4 || d->op == LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_VNNI4_PAD)))) {
+      const int V = (ts == 2) ? 2 : 4, R = 16 / ts;
+      const long long items = (long long)((d->n + V - 1) / V) * (d->ldo / R);
+      const bool vec = (d->m % R) == 0 && (d->ldi % R) == 0 && (d->ldo % R) == 0 && (((uintptr_t)a->in0 | (uintptr_t)a->out) & 15) == 0
+                    && (items + 255) / 256 <= 0x7fffffffll;
+      return vec ? 3 : 2;
+    }
+    return 0;
+  }
+  if (fam == FAM_REDUCE) {
+    const bool sum_op = (d->op == LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X_OP_ADD || d->op == LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X2_OP_ADD || d->op == LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X_X2_OP_ADD);
+    if (sum_op && (d->flags & LIBXSMM_MELTW_FLAG_UNARY_REDUCE_ROWS) == 0 && d->t_in0 != LIBXSMM_DATATYPE_F64 && (long long)d->m * d->n >= (1 << 18) && d->m >= 256) {
+      return (d->t_in0 == LIBXSMM_DATATYPE_F32 && (d->m % 4) == 0 && (d->ldi % 4) == 0 && ((uintptr_t)a->in0 & 15) == 0) ? 6 : 5;
+    }
+    return 4;
+  }
+  return 7;
+}
+
+// the same answer for a handle and the argument struct of a call. Pageable operands are answered for the scratch buffers they are
+// staged through (256-byte aligned); a NULL param stands for aligned device operands. -1: not a matrix-eltwise handle.
+LIBXSMM_API int libxsmm_b200_meltw_variant(const void* kernel, const void* param) {
+  const xb_slot* s = xb_slot_of(kernel);
+  const void* staged = (const void*)(uintptr_t)256;
+  xb_meltw_args a;
+  if (s == nullptr || s->kind != XB_KIND_MELTW) return -1;
+  memset(&a, 0, sizeof(a));
+  a.in0 = staged; a.out = (void*)(uintptr_t)staged;
+  if (param != nullptr && s->u.meltw.op_class == LIBXSMM_MELTW_OPERATION_UNARY) {
+    const libxsmm_meltw_unary_param* p = (const libxsmm_meltw_unary_param*)param;
+    if (p->in.primary != nullptr && xb_rt_ptr_kind(p->in.primary) != 0) a.in0 = p->in.primary;
+    if (p->out.primary != nullptr && xb_rt_ptr_kind(p->out.primary) != 0) a.out = p->out.primary;
+  }
+  return xb_meltw_variant(&s->u.meltw, &a);
+}
+
 extern "C" int xb_meltw_launch(const xb_meltw_desc* d, const xb_meltw_args* a) {
   cudaStream_t st = (cudaStream_t)xb_rt_stream();
   const int fam = family_of(*d);
   if (d->m <= 0 || d->n <= 0) return 0;
+  const int variant = xb_meltw_variant(d, a);
   switch (fam) {
     case FAM_MAP: {
       const int n_eff = (d->op_class == LIBXSMM_MELTW_OPERATION_UNARY && d->op == LIBXSMM_MELTW_TYPE_UNARY_REPLICATE_COL_VAR) ? (int)a->n_rt : d->n;
@@ -835,23 +964,22 @@ extern "C" int xb_meltw_launch(const xb_meltw_desc* d, const xb_meltw_args* a) {
       return launch_done("meltw_map");
     }
     case FAM_REDUCE: {
-      const bool sum_op = (d->op == LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X_OP_ADD || d->op == LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X2_OP_ADD || d->op == LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X_X2_OP_ADD);
-      if (sum_op && (d->flags & LIBXSMM_MELTW_FLAG_UNARY_REDUCE_ROWS) == 0 && d->t_in0 != LIBXSMM_DATATYPE_F64 && (long long)d->m * d->n >= (1 << 18) && d->m >= 256) {
+      if (variant == 5 || variant == 6) {
         // big column reduction: coalesced two-phase version (partial sums per column slice, then the slices in order)
         int slices = (int)(((long long)132 * 4 * 128 + d->m - 1) / d->m); if (slices > d->n / 16) slices = d->n / 16; if (slices < 1) slices = 1; if (slices > 256) slices = 256;
         const int want_x2 = (d->op != LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X_OP_ADD);
         float* part = (float*)xb_rt_scratch((size_t)2 * slices * d->m * sizeof(float));
-        if (part != nullptr) {
+        if (part == nullptr) { xb_rt_note_error(2, "meltw_reduce: no scratch for the partial sums"); return 1; }
+        if (variant == 6) {
+          const dim3 gv((d->m + 127) / 128, slices);
+          meltw_reduce_cols_partial_vec_kernel<<<gv, 256, 0, st>>>((const float*)a->in0, d->m, d->n, d->ldi, part, want_x2);
+        } else {
           const dim3 g((d->m + 255) / 256, slices);
-          if (d->t_in0 == LIBXSMM_DATATYPE_F32 && (d->m % 4) == 0 && (d->ldi % 4) == 0 && ((uintptr_t)a->in0 & 15) == 0) {
-            const dim3 gv((d->m + 127) / 128, slices);
-            meltw_reduce_cols_partial_vec_kernel<<<gv, 256, 0, st>>>((const float*)a->in0, d->m, d->n, d->ldi, part, want_x2);
-          } else
           meltw_reduce_cols_partial_kernel<<<g, 256, 0, st>>>(*d, *a, part, want_x2);
-          if (launch_done("meltw_reduce_partial") != 0) return 1;
-          meltw_reduce_cols_final_kernel<<<(d->m + 255) / 256, 256, 0, st>>>(*d, *a, part, slices);
-          return launch_done("meltw_reduce_final");
         }
+        if (launch_done("meltw_reduce_partial") != 0) return 1;
+        meltw_reduce_cols_final_kernel<<<(d->m + 255) / 256, 256, 0, st>>>(*d, *a, part, slices);
+        return launch_done("meltw_reduce_final");
       }
       const int nres = (d->flags & LIBXSMM_MELTW_FLAG_UNARY_REDUCE_ROWS) ? d->n : d->m;
       int grid = (nres + 7) / 8; if (grid > 132 * 8) grid = 132 * 8;
@@ -867,7 +995,7 @@ extern "C" int xb_meltw_launch(const xb_meltw_desc* d, const xb_meltw_args* a) {
       const long long work = (long long)(d->ldo > d->m ? d->ldo : d->m) * ((d->n + 3) / 4 * 4);
       long long grid = (work + 255) / 256; if (grid > 132 * 16) grid = 132 * 16; if (grid < 1) grid = 1;
       const int ts = xb_dev_typesize(d->t_in0);
-      if (fam == FAM_TRANSFORM && d->op == LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_NORMT && (long long)d->m * d->n >= 4096) {
+      if (variant == 1) {
         const long long tiles = (long long)((d->m + 63) / 64) * ((d->n + 63) / 64);
         if (tiles > 0x7fffffffll) return 1;
         const unsigned int tg = (unsigned int)tiles;
@@ -877,21 +1005,17 @@ extern "C" int xb_meltw_launch(const xb_meltw_desc* d, const xb_meltw_args* a) {
         else meltw_transpose_tiled_kernel<unsigned char><<<tg, 256, 0, st>>>((const unsigned char*)a->in0, (unsigned char*)a->out, d->m, d->n, d->ldi, d->ldo);
         return launch_done("meltw_transpose");
       }
-      if (fam == FAM_TRANSFORM && (long long)d->ldo * d->n >= 4096 && ((ts == 2 && (d->op == LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_VNNI2 || d->op == LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_VNNI2_PAD))
-                                  || (ts == 1 && (d->op == LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_VNNI4 || d->op == LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_VNNI4_PAD)))) {
+      if (variant == 3) {
+        const long long items = (long long)((d->n + (ts == 2 ? 2 : 4) - 1) / (ts == 2 ? 2 : 4)) * (d->ldo / (16 / ts));
+        const unsigned int vg = (unsigned int)((items + 255) / 256);
+        if (ts == 2) meltw_vnni_pack_vec_kernel<unsigned short, 2><<<vg, 256, 0, st>>>((const unsigned short*)a->in0, (unsigned short*)a->out, d->m, d->n, d->ldi, d->ldo);
+        else meltw_vnni_pack_vec_kernel<unsigned char, 4><<<vg, 256, 0, st>>>((const unsigned char*)a->in0, (unsigned char*)a->out, d->m, d->n, d->ldi, d->ldo);
+        return launch_done("meltw_vnni_pack_vec");
+      }
+      if (variant == 2) {
         const int V = (ts == 2) ? 2 : 4;
         const long long workp = (long long)((d->n + V - 1) / V) * ((d->ldo + 3) / 4);
         long long pg = (workp + 255) / 256; if (pg > 132 * 16) pg = 132 * 16;
-        const int R = 16 / ts;
-        if ((d->m % R) == 0 && (d->ldi % R) == 0 && (d->ldo % R) == 0 && (((uintptr_t)a->in0 | (uintptr_t)a->out) & 15) == 0) {
-          const long long items = (long long)((d->n + V - 1) / V) * (d->ldo / R);
-          const long long vg = (items + 255) / 256;
-          if (vg <= 0x7fffffffll) {
-            if (ts == 2) meltw_vnni_pack_vec_kernel<unsigned short, 2><<<(unsigned int)vg, 256, 0, st>>>((const unsigned short*)a->in0, (unsigned short*)a->out, d->m, d->n, d->ldi, d->ldo);
-            else meltw_vnni_pack_vec_kernel<unsigned char, 4><<<(unsigned int)vg, 256, 0, st>>>((const unsigned char*)a->in0, (unsigned char*)a->out, d->m, d->n, d->ldi, d->ldo);
-            return launch_done("meltw_vnni_pack_vec");
-          }
-        }
         if (ts == 2) meltw_vnni_pack_kernel<unsigned short, 2><<<(unsigned int)pg, 256, 0, st>>>((const unsigned short*)a->in0, (unsigned short*)a->out, d->m, d->n, d->ldi, d->ldo);
         else meltw_vnni_pack_kernel<unsigned char, 4><<<(unsigned int)pg, 256, 0, st>>>((const unsigned char*)a->in0, (unsigned char*)a->out, d->m, d->n, d->ldi, d->ldo);
         return launch_done("meltw_vnni_pack");

@@ -136,10 +136,16 @@ static int unary_map(const mdesc* d, const libxsmm_meltw_unary_param* p) {
   const int bitm = (d->flags & LIBXSMM_MELTW_FLAG_UNARY_BITMASK_2BYTEMULT) != 0;
   const float alpha = (p->op.primary != NULL && (op == LIBXSMM_MELTW_TYPE_UNARY_LEAKY_RELU || op == LIBXSMM_MELTW_TYPE_UNARY_LEAKY_RELU_INV
                        || op == LIBXSMM_MELTW_TYPE_UNARY_ELU || op == LIBXSMM_MELTW_TYPE_UNARY_ELU_INV)) ? *(const float*)p->op.primary : 0.0f;
+  /* REPLICATE_COL_VAR copies the column in0[0..m) into N columns, N = *(unsigned long long*)op.primary at call time (:249, :2084) */
+  const int rep = (op == LIBXSMM_MELTW_TYPE_UNARY_REPLICATE_COL_VAR);
+  const long long n_eff = rep ? (p->op.primary != NULL ? (long long)*(const unsigned long long*)p->op.primary : -1) : d->n;
+  mdesc dc = *d;
   int i, j;
   if (!f64 && !(is_f(d->t0) && is_f(d->to))) return 2;
-  if (f64 && op == LIBXSMM_MELTW_TYPE_UNARY_DUMP) return 2;      /* not in the reference's F64 op list (:116-138) */
-  for (j = 0; j < d->n; ++j) for (i = 0; i < d->m; ++i) {
+  if (f64 && (op == LIBXSMM_MELTW_TYPE_UNARY_DUMP || rep)) return 2;      /* not in the reference's F64 op list (:116-138) */
+  if (n_eff < 0) return 1;
+  if (rep) { dc.flags |= LIBXSMM_MELTW_FLAG_UNARY_BCAST_COL; d = &dc; }
+  for (j = 0; j < n_eff; ++j) for (i = 0; i < d->m; ++i) {
     const long long oi = i + (long long)j * d->ldo;
     if (f64) { ((double*)p->out.primary)[oi] = unary_f64(((const double*)p->in.primary)[bidx(d, 0, i, j, d->ldi)], op); continue; }
     {
@@ -172,27 +178,68 @@ static int unary_map(const mdesc* d, const libxsmm_meltw_unary_param* p) {
 }
 
 /* reductions: reference :1065-1443. REDUCE_ROWS collapses i (n results), otherwise j (m results, buffer pitch ldo);
- * X_X2 stores the sums, then the sums of squares at element offset result_size (:1073-1076); INIT_ACC adds the old output */
+ * X_X2 stores the sums, then the sums of squares at element offset result_size (:1073-1076); INIT_ACC adds the old output.
+ * COLS_IDX_OP_* reduce the columns listed in in.secondary (*in.tertiary of them, 4- or 8-byte indices) and ignore INIT_ACC
+ * (:1121-1138, :1347-1356). Max / min / absmax are the reference's sequential folds with its macros (include/libxsmm_macros.h:635-637):
+ * MAX(A,B) = A < B ? B : A, MIN(A,B) = A < B ? A : B, ABS(A) = 0 <= A ? A : -A (so ABS(-0) = -0 and ABS flips a NaN's sign).
+ *   rows (:1215-1224, :1360-1369): tmp = first element, then tmp = f(tmp, x) for EVERY element, the first included;
+ *   cols (:1226-1284, :1371-1428): tmp = -FLT_MAX (max), 0 (absmax) or FLT_MAX (min), then tmp = f(x, tmp) -- operands swapped;
+ *   RECORD_ARGOP, columns only: x >= tmp (max, absmax) / x <= tmp (min) takes x and records its column in out.secondary,
+ *   an index that is never taken is not written. */
+#define RMAX(A, B) ((A) < (B) ? (B) : (A))
+#define RMIN(A, B) ((A) < (B) ? (A) : (B))
+#define RABS(A) (0 <= (A) ? (A) : -(A))
 static int unary_reduce(const mdesc* d, const libxsmm_meltw_unary_param* p) {
-  const int op = d->op, rows = (d->flags & LIBXSMM_MELTW_FLAG_UNARY_REDUCE_ROWS) != 0, init = (d->flags & LIBXSMM_MELTW_FLAG_UNARY_REDUCE_INIT_ACC) != 0;
+  const int op = d->op, rows = (d->flags & LIBXSMM_MELTW_FLAG_UNARY_REDUCE_ROWS) != 0;
+  const int by_idx = (op == LIBXSMM_MELTW_TYPE_UNARY_REDUCE_COLS_IDX_OP_ADD || op == LIBXSMM_MELTW_TYPE_UNARY_REDUCE_COLS_IDX_OP_MAX
+                   || op == LIBXSMM_MELTW_TYPE_UNARY_REDUCE_COLS_IDX_OP_MIN);
+  const int init = !by_idx && (d->flags & LIBXSMM_MELTW_FLAG_UNARY_REDUCE_INIT_ACC) != 0;
+  const int argop = !rows && (d->flags & LIBXSMM_MELTW_FLAG_UNARY_REDUCE_RECORD_ARGOP) != 0;
+  const int idx4 = (d->flags & LIBXSMM_MELTW_FLAG_UNARY_IDX_SIZE_4BYTES) != 0;    /* the reference's default is 8 bytes (:1088) */
   const int f64 = (d->t0 == LIBXSMM_DATATYPE_F64 && d->to == LIBXSMM_DATATYPE_F64);
-  const int kind = (op == LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X_OP_MAX) ? 1 : ((op == LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X_OP_MIN) ? 2
-                 : ((op == LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X_OP_ABSMAX) ? 3 : 0));   /* ABSMAX: max over |x| */
+  const int kind = (op == LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X_OP_MAX || op == LIBXSMM_MELTW_TYPE_UNARY_REDUCE_COLS_IDX_OP_MAX) ? 1
+                 : ((op == LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X_OP_MIN || op == LIBXSMM_MELTW_TYPE_UNARY_REDUCE_COLS_IDX_OP_MIN) ? 2
+                 : ((op == LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X_OP_ABSMAX) ? 3 : 0));
   const int want_x = (op != LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X2_OP_ADD), want_x2 = (op == LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X2_OP_ADD || op == LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X_X2_OP_ADD);
-  const int nres = rows ? d->n : d->m, len = rows ? d->m : d->n;
+  const long long ncols = by_idx ? (p->in.tertiary != NULL ? (long long)*(const unsigned long long*)p->in.tertiary : -1) : d->n;
+  const int nres = rows ? d->n : d->m;
+  const long long len = rows ? d->m : ncols;
   const long long result_size = rows ? d->n : d->ldo;
-  int o, t;
-  if (d->flags & LIBXSMM_MELTW_FLAG_UNARY_REDUCE_RECORD_ARGOP) return 2;
+  long long t;
+  int o;
   if (!f64 && !(is_f(d->t0) && is_f(d->to))) return 2;
+  if ((by_idx && (rows || ncols < 0 || p->in.secondary == NULL)) || (argop && kind != 0 && p->out.secondary == NULL)) return 1;
   for (o = 0; o < nres; ++o) {
     double sx = 0.0, sx2 = 0.0, best = 0.0; float fsx = 0.0f, fsx2 = 0.0f, fbest = 0.0f;
+    long long arg = -1;
+    if (kind != 0 && rows) { if (f64) best = ((const double*)p->in.primary)[(long long)o * d->ldi]; else fbest = ldf(p->in.primary, (long long)o * d->ldi, d->t0); }
+    else if (kind != 0) { best = (kind == 1) ? -FLT_MAX : ((kind == 2) ? FLT_MAX : 0); fbest = (kind == 1) ? -FLT_MAX : ((kind == 2) ? FLT_MAX : 0); }
     for (t = 0; t < len; ++t) {
-      const long long idx = rows ? (t + (long long)o * d->ldi) : (o + (long long)t * d->ldi);
-      if (f64) { double v = ((const double*)p->in.primary)[idx]; sx += v; sx2 += v * v; if (kind == 3) v = fabs(v); if (t == 0 || (kind == 2 ? v < best : v > best)) best = v; }
-      else { float v = ldf(p->in.primary, idx, d->t0); fsx += v; fsx2 += v * v; if (kind == 3) v = fabsf(v); if (t == 0 || (kind == 2 ? v < fbest : v > fbest)) fbest = v; }
+      const long long j = !by_idx ? t : (idx4 ? (long long)((const uint32_t*)p->in.secondary)[t] : (long long)((const uint64_t*)p->in.secondary)[t]);
+      const long long idx = rows ? (t + (long long)o * d->ldi) : (o + j * d->ldi);
+      if (f64) {
+        double v = ((const double*)p->in.primary)[idx];
+        if (kind == 0) { sx += v; sx2 += v * v; }
+        else if (rows) best = (kind == 1) ? RMAX(best, v) : ((kind == 3) ? RMAX(RABS(best), RABS(v)) : RMIN(best, v));
+        else {
+          if (kind == 3) v = RABS(v);
+          if (argop) { if (kind == 2 ? (v <= best) : (v >= best)) { best = v; arg = j; } }
+          else best = (kind == 2) ? RMIN(v, best) : RMAX(v, best);
+        }
+      } else {
+        float v = ldf(p->in.primary, idx, d->t0);
+        if (kind == 0) { fsx += v; fsx2 += v * v; }
+        else if (rows) fbest = (kind == 1) ? RMAX(fbest, v) : ((kind == 3) ? RMAX(RABS(fbest), RABS(v)) : RMIN(fbest, v));
+        else {
+          if (kind == 3) v = RABS(v);
+          if (argop) { if (kind == 2 ? (v <= fbest) : (v >= fbest)) { fbest = v; arg = j; } }
+          else fbest = (kind == 2) ? RMIN(v, fbest) : RMAX(v, fbest);
+        }
+      }
     }
     if (kind != 0) {
       if (f64) ((double*)p->out.primary)[o] = best; else stf(p->out.primary, o, d->to, fbest);
+      if (argop && arg >= 0) { if (idx4) ((uint32_t*)p->out.secondary)[o] = (uint32_t)arg; else ((uint64_t*)p->out.secondary)[o] = (uint64_t)arg; }
     } else if (f64) {
       double* ox = (double*)p->out.primary; double* ox2 = want_x ? ox + result_size : ox;
       if (want_x) ox[o] = sx + (init ? ox[o] : 0.0);
@@ -205,6 +252,9 @@ static int unary_reduce(const mdesc* d, const libxsmm_meltw_unary_param* p) {
   }
   return 0;
 }
+#undef RMAX
+#undef RMIN
+#undef RABS
 
 /* layout transforms, pure data movement: reference :377-1062. Formulas (elements, E = element of 1/2/4/8 bytes):
  *   NORM_TO_NORMT      out[j*ldo + i] = in[i*ldi + j]                      i < n, j < m               (:390-417)
@@ -627,10 +677,11 @@ ORACLE_API int oracle_meltw(const int* desc, void* param, int mode) {
       case LIBXSMM_MELTW_TYPE_UNARY_TANH: case LIBXSMM_MELTW_TYPE_UNARY_TANH_INV: case LIBXSMM_MELTW_TYPE_UNARY_SIGMOID: case LIBXSMM_MELTW_TYPE_UNARY_SIGMOID_INV:
       case LIBXSMM_MELTW_TYPE_UNARY_GELU: case LIBXSMM_MELTW_TYPE_UNARY_GELU_INV: case LIBXSMM_MELTW_TYPE_UNARY_EXP:
       case LIBXSMM_MELTW_TYPE_UNARY_RELU: case LIBXSMM_MELTW_TYPE_UNARY_RELU_INV: case LIBXSMM_MELTW_TYPE_UNARY_LEAKY_RELU: case LIBXSMM_MELTW_TYPE_UNARY_LEAKY_RELU_INV:
-      case LIBXSMM_MELTW_TYPE_UNARY_ELU: case LIBXSMM_MELTW_TYPE_UNARY_ELU_INV:
+      case LIBXSMM_MELTW_TYPE_UNARY_ELU: case LIBXSMM_MELTW_TYPE_UNARY_ELU_INV: case LIBXSMM_MELTW_TYPE_UNARY_REPLICATE_COL_VAR:
         return unary_map(&d, (const libxsmm_meltw_unary_param*)param);
       case LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X_OP_ADD: case LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X2_OP_ADD: case LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X_X2_OP_ADD:
       case LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X_OP_MAX: case LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X_OP_MIN: case LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X_OP_ABSMAX:
+      case LIBXSMM_MELTW_TYPE_UNARY_REDUCE_COLS_IDX_OP_ADD: case LIBXSMM_MELTW_TYPE_UNARY_REDUCE_COLS_IDX_OP_MAX: case LIBXSMM_MELTW_TYPE_UNARY_REDUCE_COLS_IDX_OP_MIN:
         return unary_reduce(&d, (const libxsmm_meltw_unary_param*)param);
       case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_NORMT: case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_VNNI2: case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_VNNI2_PAD:
       case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_VNNI4: case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_VNNI4_PAD:

@@ -112,6 +112,26 @@ def test_fsspmdm_variant_of_no_handle():
     assert X.libxsmm_b200_fsspmdm_variant(None, b.ctypes.data, b.ctypes.data) == -1
 
 
+def test_meltw_variant_query():
+    """libxsmm_b200_meltw_variant: -1 without a matrix-eltwise handle; the shape thresholds of the kernel choice for aligned operands
+    (a NULL param), both sides of each"""
+    assert X.libxsmm_b200_meltw_variant(None, None) == -1
+    F32, BF16, F64 = 1, 2, 0
+
+    def var(op, m, n, ldi, ldo, t, flags=0):
+        k = X.libxsmm_dispatch_meltw_unary(op, X.libxsmm_create_meltw_unary_shape(m, n, ldi, ldo, t, t, F64 if t == F64 else F32), flags)
+        assert k
+        return X.libxsmm_b200_meltw_variant(k, None)
+    T, V2, ADD, MAX = X.MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_NORMT, X.MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_VNNI2, X.MELTW_TYPE_UNARY_REDUCE_X_OP_ADD, X.MELTW_TYPE_UNARY_REDUCE_X_OP_MAX
+    assert (var(T, 63, 65, 63, 65, F32), var(T, 64, 64, 64, 64, F32)) == (0, 1)                     # m*n = 4095 / 4096
+    assert (var(V2, 48, 63, 48, 64, BF16), var(V2, 64, 64, 64, 64, BF16), var(V2, 60, 70, 60, 64, BF16)) == (0, 3, 2)
+    assert (var(ADD, 255, 1100, 255, 255, F32), var(ADD, 256, 1100, 256, 256, F32)) == (4, 6)       # m = 255 / 256
+    assert (var(ADD, 513, 511, 513, 513, F32), var(ADD, 512, 512, 512, 512, F32)) == (4, 6)         # m*n = 2^18 - 1 / 2^18
+    assert (var(ADD, 258, 1024, 258, 258, F32), var(ADD, 256, 1024, 258, 256, F32), var(ADD, 512, 512, 512, 512, BF16)) == (5, 5, 5)
+    assert var(ADD, 512, 512, 512, 512, F64) == 4 and var(ADD, 512, 512, 512, 512, F32, X.MELTW_FLAG_UNARY_REDUCE_ROWS) == 4
+    assert var(MAX, 512, 512, 512, 512, F32) == 4 and var(X.MELTW_TYPE_UNARY_RELU, 8, 8, 8, 8, F32) == 7
+
+
 def test_meltw_dispatch_host_logic():
     sh = X.libxsmm_create_meltw_unary_shape(10, 7, 10, 10, gen.F32, gen.F32, gen.F32)
     k = X.libxsmm_dispatch_meltw_unary(X.MELTW_TYPE_UNARY_RELU, sh, 0)
