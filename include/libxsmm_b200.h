@@ -110,6 +110,31 @@ LIBXSMM_API int libxsmm_b200_gemm_plan_run(const libxsmm_b200_gemm_plan* plan);
 LIBXSMM_API int libxsmm_b200_gemm_plan_is_pooled(const libxsmm_b200_gemm_plan* plan);
 LIBXSMM_API void libxsmm_b200_gemm_plan_destroy(libxsmm_b200_gemm_plan* plan);
 
+/* ---- batched matrix-eltwise and matrix equations -----------------------------------------------
+ * count calls of one handle in one launch (an equation: one launch per node). Call t is the single call with every pointer of
+ * *param advanced by t times its stride (BYTES; 0 = one operand shared by every call). Values a single call reads by value are
+ * read once, from call 0: op.primary (alpha, drop probability) and the QUANT / DEQUANT scale in in.secondary. Returns 0; -1 for a
+ * NULL or foreign handle, count < 0, a negative stride, or an output stride smaller than the bytes one call writes through that
+ * pointer; -4 if an operand is pageable host memory (device, managed or pinned only); LIBXSMM_B200_ERROR_NOT_BATCHABLE for calls
+ * with per-call state or run-time extents: DROPOUT forward, STOCHASTIC_ROUND, REPLICATE_COL_VAR, GATHER / SCATTER, the COLS_IDX
+ * reductions, UNZIP and DECOMP_FP32_TO_BF16X2 / X3 (and an equation holding one); the positive CUDA error (2: out of device
+ * scratch) if a launch fails. count == 0 does nothing. The meltw form honours
+ * libxsmm_b200_set_blocking; the equation form returns after the device has finished, like a single equation call. */
+typedef struct libxsmm_b200_meltw_strides {
+  long long in0, in1, in2;   /* in.primary (unary) / in0, in1, in2 .primary */
+  long long in_aux;          /* unary in.secondary: bit mask (RELU_INV, LEAKY_RELU_INV, DROPOUT_INV), forward output (ELU_INV) */
+  long long out, out_aux;    /* out.primary; unary out.secondary: bit mask, argop indices, MX block scales, DUMP copy */
+} libxsmm_b200_meltw_strides;
+LIBXSMM_API int libxsmm_b200_meltw_batch_strided(const void* kernel, const void* param,
+  const libxsmm_b200_meltw_strides* strides, long long count);
+/* input_strides[i] applies to inputs[i], ops_strides[pos] to the ops_args[pos].primary a DUMP writes (NULL without DUMP),
+ * output_aux_stride to the relu bit mask of the head (output.secondary); an argument a DUMP writes must have the DUMP's stride (-1
+ * otherwise), and a NULL input is -1. Temporaries live in one device scratch block per chunk; past 64 MiB of them
+ * the calls run in chunks, each one launch per node. */
+LIBXSMM_API int libxsmm_b200_meqn_batch_strided(libxsmm_meqn_function kernel, const libxsmm_meqn_param* param,
+  const long long* input_strides, long long output_stride, long long output_aux_stride,
+  const long long* ops_strides, long long count);
+
 #if defined(__cplusplus)
 }
 #endif

@@ -309,6 +309,15 @@ libxsmm_b200_gemm_plan_run = _sig("libxsmm_b200_gemm_plan_run", _I, [_P])
 libxsmm_b200_gemm_plan_destroy = _sig("libxsmm_b200_gemm_plan_destroy", None, [_P])
 libxsmm_b200_gemm_plan_is_pooled = _sig("libxsmm_b200_gemm_plan_is_pooled", _I, [_P])
 
+
+class MeltwStrides(C.Structure):
+    _fields_ = [(n, C.c_longlong) for n in ("in0", "in1", "in2", "in_aux", "out", "out_aux")]
+
+
+libxsmm_b200_meltw_batch_strided = _sig("libxsmm_b200_meltw_batch_strided", _I, [_P, _P, C.POINTER(MeltwStrides), _LL])
+libxsmm_b200_meqn_batch_strided = _sig("libxsmm_b200_meqn_batch_strided", _I,
+                                       [_P, C.POINTER(MeqnParam), C.POINTER(_LL), _LL, _LL, C.POINTER(_LL), _LL])
+
 EXPORTED = [n for n in dir() if n.startswith("libxsmm_") and callable(globals()[n])]
 
 

@@ -146,9 +146,12 @@ LIBXSMM_API libxsmm_xmeltwfunction libxsmm_dispatch_meltw(const libxsmm_meltw_de
 
 /* ---- invocation -------------------------------------------------------------------------------------------- */
 typedef struct xb_stage { void* host; void* dev; size_t bytes; } xb_stage;
-typedef struct xb_stager { xb_stage out[4]; int nout; int staged; int failed; } xb_stager;
+/* batch: nothing is staged; operands pass through, a pageable one sets `pageable`, and every output is recorded in out[] with the
+ * bytes one call writes through it (the batch form checks its stride against them) */
+typedef struct xb_stager { xb_stage out[4]; int nout; int staged; int failed; int batch; int pageable; } xb_stager;
 
 static const void* stage_in(xb_stager* st, const void* p, size_t bytes) {
+  if (st->batch) { if (p != NULL && xb_rt_ptr_kind(p) == 0) st->pageable = 1; return p; }
   if (p == NULL || xb_rt_ptr_kind(p) != 0) return p;
   else {
     void* d = xb_rt_scratch(bytes ? bytes : 1);
@@ -160,6 +163,13 @@ static const void* stage_in(xb_stager* st, const void* p, size_t bytes) {
 }
 /* output staged in AND out (partial writes must preserve what the kernel does not touch) */
 static void* stage_inout(xb_stager* st, void* p, size_t bytes) {
+  if (st->batch) {
+    if (p == NULL) return p;
+    if (xb_rt_ptr_kind(p) == 0) st->pageable = 1;
+    if (st->nout >= 4) { st->failed = 1; return p; }
+    st->out[st->nout].host = st->out[st->nout].dev = p; st->out[st->nout].bytes = bytes; ++st->nout;
+    return p;
+  }
   if (p == NULL || xb_rt_ptr_kind(p) != 0) return p;
   else {
     void* d = xb_rt_scratch(bytes ? bytes : 1);
@@ -199,13 +209,13 @@ static void stage_stochastic(xb_stager* st, xb_meltw_args* a, const void* state,
   if (a->rng == NULL || a->rnd8 == NULL) st->failed = 1;
 }
 
-void xb_invoke_meltw(const xb_slot* s, const void* param) {
-  const xb_meltw_desc* d = &s->u.meltw;
-  xb_meltw_args a; xb_stager st;
+/* the kernel arguments of one call: operands staged through `st` (or, for a batch, checked and recorded there). Returns 1 if the
+ * call cannot run; the error is noted and the scratch arena reset. */
+static int meltw_args(const xb_meltw_desc* d, const void* param, xb_meltw_args* out_args, xb_stager* pst) {
+  xb_meltw_args a; xb_stager st = *pst;
   const size_t ts_in = libxsmm_typesize((libxsmm_datatype)d->t_in0), ts_out = libxsmm_typesize((libxsmm_datatype)d->t_out);
   const size_t mask_ld_o = (size_t)LIBXSMM_UP(d->ldo, 16), mask_ld_i = (size_t)LIBXSMM_UP(d->ldi, 16);
-  int rc, i;
-  memset(&a, 0, sizeof(a)); memset(&st, 0, sizeof(st));
+  memset(&a, 0, sizeof(a));
   if (d->op_class == LIBXSMM_MELTW_OPERATION_UNARY) {
     const libxsmm_meltw_unary_param* p = (const libxsmm_meltw_unary_param*)param;
     const int op = d->op;
@@ -258,7 +268,7 @@ void xb_invoke_meltw(const xb_slot* s, const void* param) {
     if (op == LIBXSMM_MELTW_TYPE_UNARY_GATHER || op == LIBXSMM_MELTW_TYPE_UNARY_SCATTER || op == LIBXSMM_MELTW_TYPE_UNARY_REDUCE_COLS_IDX_OP_ADD
      || op == LIBXSMM_MELTW_TYPE_UNARY_REDUCE_COLS_IDX_OP_MAX || op == LIBXSMM_MELTW_TYPE_UNARY_REDUCE_COLS_IDX_OP_MIN) {
       /* extents depend on run-time indices: operands must be device-accessible (device, managed or pinned) */
-      if (xb_rt_ptr_kind(p->in.primary) == 0 || xb_rt_ptr_kind(p->out.primary) == 0) { xb_rt_note_error(1, "meltw: indexed op needs device-accessible memory"); return; }
+      if (xb_rt_ptr_kind(p->in.primary) == 0 || xb_rt_ptr_kind(p->out.primary) == 0) { xb_rt_note_error(1, "meltw: indexed op needs device-accessible memory"); return 1; }
       a.in0 = p->in.primary; a.out = p->out.primary; a.in_aux = p->in.secondary; a.out_aux = p->out.secondary;
       if (op != LIBXSMM_MELTW_TYPE_UNARY_GATHER && op != LIBXSMM_MELTW_TYPE_UNARY_SCATTER) {
         a.n_rt = *(const unsigned long long*)p->in.tertiary;
@@ -281,7 +291,7 @@ void xb_invoke_meltw(const xb_slot* s, const void* param) {
         /* several bf16 planes behind ONE output pointer at caller-given byte distances (out.secondary): the output must be
          * device-accessible, there is no single extent to stage */
         const unsigned long long* offs = (const unsigned long long*)p->out.secondary;
-        if (offs == NULL || xb_rt_ptr_kind(p->out.primary) == 0) { xb_rt_note_error(1, "meltw: unzip/decomp need a device-accessible output and plane offsets"); xb_rt_scratch_reset(); return; }
+        if (offs == NULL || xb_rt_ptr_kind(p->out.primary) == 0) { xb_rt_note_error(1, "meltw: unzip/decomp need a device-accessible output and plane offsets"); xb_rt_scratch_reset(); return 1; }
         if (xb_rt_ptr_kind(offs) == 1) xb_rt_memcpy(a.off, offs, (op == LIBXSMM_MELTW_TYPE_UNARY_DECOMP_FP32_TO_BF16X3 ? 2 : 1) * sizeof(unsigned long long));
         else { a.off[0] = offs[0]; if (op == LIBXSMM_MELTW_TYPE_UNARY_DECOMP_FP32_TO_BF16X3) a.off[1] = offs[1]; }
         a.out = p->out.primary;
@@ -341,9 +351,72 @@ void xb_invoke_meltw(const xb_slot* s, const void* param) {
     a.out = stage_inout(&st, p->out.primary, ((size_t)(d->n - 1) * d->ldo + d->m) * ts_out);
     if ((d->flags & LIBXSMM_MELTW_FLAG_TERNARY_STOCHASTIC_ROUND) != 0 && d->t_out == LIBXSMM_DATATYPE_BF8) stage_stochastic(&st, &a, p->op.secondary, (long long)d->m * d->n);
   }
-  if (st.failed) { xb_rt_note_error(2, "meltw: staging failed"); xb_rt_scratch_reset(); return; }
+  *pst = st; *out_args = a;
+  if (st.failed) { xb_rt_note_error(2, "meltw: staging failed"); xb_rt_scratch_reset(); return 1; }
+  return 0;
+}
+
+void xb_invoke_meltw(const xb_slot* s, const void* param) {
+  const xb_meltw_desc* d = &s->u.meltw;
+  xb_meltw_args a; xb_stager st;
+  int rc, i;
+  memset(&st, 0, sizeof(st));
+  if (meltw_args(d, param, &a, &st) != 0) return;
   rc = xb_meltw_launch(d, &a);
   if (rc != 0) { xb_rt_scratch_reset(); return; }
   for (i = 0; i < st.nout; ++i) xb_rt_memcpy_async(st.out[i].host, st.out[i].dev, st.out[i].bytes);
   if (st.staged || xb_rt_blocking()) { xb_rt_sync(); xb_rt_scratch_reset(); }
+}
+
+/* ---- strided batch: `count` calls of one handle in one launch ------------------------------------------------------------
+ * Calls whose kernel carries per-call state or run-time extents are refused: the dropout generator chains call to call, stochastic
+ * rounding draws from a state in op.secondary, REPLICATE_COL_VAR / the COLS_IDX reductions / gather and scatter read their extents
+ * or indices at run time, unzip and decomp write planes at caller-given offsets. */
+int xb_meltw_batchable(const xb_meltw_desc* d) {
+  if (d->op_class == LIBXSMM_MELTW_OPERATION_UNARY) {
+    if ((d->flags & LIBXSMM_MELTW_FLAG_UNARY_STOCHASTIC_ROUND) != 0) return 0;
+    switch (d->op) {
+      case LIBXSMM_MELTW_TYPE_UNARY_DROPOUT: case LIBXSMM_MELTW_TYPE_UNARY_REPLICATE_COL_VAR:
+      case LIBXSMM_MELTW_TYPE_UNARY_GATHER: case LIBXSMM_MELTW_TYPE_UNARY_SCATTER:
+      case LIBXSMM_MELTW_TYPE_UNARY_REDUCE_COLS_IDX_OP_ADD: case LIBXSMM_MELTW_TYPE_UNARY_REDUCE_COLS_IDX_OP_MAX: case LIBXSMM_MELTW_TYPE_UNARY_REDUCE_COLS_IDX_OP_MIN:
+      case LIBXSMM_MELTW_TYPE_UNARY_UNZIP: case LIBXSMM_MELTW_TYPE_UNARY_DECOMP_FP32_TO_BF16X2: case LIBXSMM_MELTW_TYPE_UNARY_DECOMP_FP32_TO_BF16X3: return 0;
+      default: return 1;
+    }
+  }
+  if (d->op_class == LIBXSMM_MELTW_OPERATION_BINARY) return (d->flags & LIBXSMM_MELTW_FLAG_BINARY_STOCHASTIC_ROUND) == 0;
+  return (d->flags & LIBXSMM_MELTW_FLAG_TERNARY_STOCHASTIC_ROUND) == 0;
+}
+
+LIBXSMM_API int libxsmm_b200_meltw_batch_strided(const void* kernel, const void* param, const libxsmm_b200_meltw_strides* strides, long long count) {
+  const xb_slot* s = xb_slot_of(kernel);
+  const xb_meltw_desc* d;
+  xb_meltw_args a; xb_stager st;
+  void* outs[2] = { NULL, NULL }; long long out_strides[2] = { 0, 0 };
+  int rc, i, k;
+  if (s == NULL || s->kind != XB_KIND_MELTW || param == NULL || strides == NULL || count < 0) return -1;
+  d = &s->u.meltw;
+  if (!xb_meltw_batchable(d)) return LIBXSMM_B200_ERROR_NOT_BATCHABLE;
+  if (strides->in0 < 0 || strides->in1 < 0 || strides->in2 < 0 || strides->in_aux < 0 || strides->out < 0 || strides->out_aux < 0) return -1;
+  if (count == 0) return 0;
+  memset(&st, 0, sizeof(st)); st.batch = 1;
+  if (meltw_args(d, param, &a, &st) != 0) return -1;
+  if (st.pageable) return -4;                           /* no staging path: device, managed or pinned operands only */
+  /* every output a call writes must not reach into the next call's */
+  if (d->op_class == LIBXSMM_MELTW_OPERATION_UNARY) {
+    const libxsmm_meltw_unary_param* p = (const libxsmm_meltw_unary_param*)param;
+    outs[0] = p->out.primary; outs[1] = p->out.secondary; out_strides[0] = strides->out; out_strides[1] = strides->out_aux;
+    a.s_in0 = strides->in0; a.s_in_aux = strides->in_aux; a.s_out = strides->out; a.s_out_aux = strides->out_aux;
+  } else {
+    outs[0] = (d->op_class == LIBXSMM_MELTW_OPERATION_BINARY) ? ((const libxsmm_meltw_binary_param*)param)->out.primary
+                                                               : ((const libxsmm_meltw_ternary_param*)param)->out.primary;
+    out_strides[0] = strides->out;
+    a.s_in0 = strides->in0; a.s_in1 = strides->in1; a.s_in2 = strides->in2; a.s_out = strides->out;
+  }
+  if (count > 1) for (i = 0; i < st.nout; ++i) for (k = 0; k < 2; ++k) {
+    if (outs[k] != NULL && st.out[i].host == outs[k] && out_strides[k] < (long long)st.out[i].bytes) return -1;
+  }
+  a.count = count;
+  rc = xb_meltw_launch(d, &a);
+  if (rc == 0 && xb_rt_blocking()) rc = xb_rt_sync();
+  return rc;
 }

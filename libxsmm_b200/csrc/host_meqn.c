@@ -347,6 +347,123 @@ void xb_invoke_meqn(const xb_slot* s, const void* param) {
   xb_rt_sync(); xb_rt_scratch_reset();
 }
 
+/* ---- strided batch: the tree evaluated once for `count` calls, every node one launch over all of them ------------------------
+ * Call t reads inputs[i] + t*input_strides[i] and writes output.primary + t*output_stride (the relu bit mask of the head:
+ * output.secondary + t*output_aux_stride, a DUMP: ops_args[pos].primary + t*ops_strides[pos]). A temporary holds its node's value for
+ * every call of a chunk at 256-byte aligned strides; when all temporaries of a batch would exceed XB_MEQN_BATCH_SCRATCH_BYTES the
+ * calls run in chunks, each one launch per node, then a sync and a scratch reset. */
+#define XB_MEQN_BATCH_SCRATCH_BYTES (64ll << 20)
+
+typedef struct xb_beval {
+  const xb_eqn* e; const libxsmm_meqn_param* p; const long long* in_s; const long long* ops_s; long long out_s, aux_s, t0, cnt; int failed, rc;
+  char* pool; size_t used;      /* the chunk's temporaries: one scratch block, carved in visiting order */
+} xb_beval;
+
+static long long tmp_stride(const xb_eqn_node* nd) { return (long long)LIBXSMM_UP(span(nd) ? span(nd) : 16, 256); }
+static int is_dump(const xb_eqn_node* nd) { return nd->type == EQ_UNARY && nd->op == LIBXSMM_MELTW_TYPE_UNARY_DUMP; }
+
+static const void* beval_node(xb_beval* ev, int at, int is_root, long long* stride) {
+  const xb_eqn_node* nd = &ev->e->node[at];
+  if (nd->type == EQ_ARG) {
+    /* an argument that a DUMP of this evaluation writes is the DUMP's strided buffer (the entry point checked the strides agree) */
+    *stride = ev->in_s[nd->pos];
+    return (const char*)ev->p->inputs[nd->pos].primary + ev->t0 * *stride;
+  } else {
+    xb_meltw_desc d; xb_meltw_args a; char* out;
+    const void* in[3] = { NULL, NULL, NULL }; long long s[3] = { 0, 0, 0 }; int c, k, order[3] = { 0, 1, 2 };
+    memset(&a, 0, sizeof(a));
+    for (c = 1; c < arity(nd->type); ++c) for (k = c; k > 0 && ev->e->node[nd->child[order[k]]].score > ev->e->node[nd->child[order[k - 1]]].score; --k) {
+      const int t = order[k]; order[k] = order[k - 1]; order[k - 1] = t;
+    }
+    for (c = 0; c < arity(nd->type); ++c) in[order[c]] = beval_node(ev, nd->child[order[c]], 0, &s[order[c]]);
+    if (ev->failed) return NULL;
+    *stride = is_root ? ev->out_s : tmp_stride(nd);
+    if (is_root) out = (char*)ev->p->output.primary + ev->t0 * ev->out_s;
+    else { out = ev->pool + ev->used; ev->used += (size_t)(ev->cnt * *stride); }
+    node_desc(ev->e, at, &d);
+    a.in0 = in[0]; a.in1 = in[1]; a.in2 = in[2]; a.s_in0 = s[0]; a.s_in1 = s[1]; a.s_in2 = s[2];
+    a.out = out; a.s_out = *stride; a.alpha = 1.0f; a.count = ev->cnt;
+    if (nd->type == EQ_UNARY && ev->p->ops_args != NULL && nd->pos >= 0) {       /* read once, from call 0 */
+      const void* op1 = ev->p->ops_args[nd->pos].primary;
+      if (op1 != NULL && (nd->op == LIBXSMM_MELTW_TYPE_UNARY_LEAKY_RELU || nd->op == LIBXSMM_MELTW_TYPE_UNARY_ELU)) {
+        if (xb_rt_ptr_kind(op1) == 1) xb_rt_memcpy(&a.alpha, op1, sizeof(float)); else a.alpha = *(const float*)op1;
+      }
+    }
+    if (has_bitmask_out(nd)) { a.out_aux = (char*)ev->p->output.secondary + ev->t0 * ev->aux_s; a.s_out_aux = ev->aux_s; }
+    else if (is_dump(nd)) { a.out_aux = (char*)ev->p->ops_args[nd->pos].primary + ev->t0 * ev->ops_s[nd->pos]; a.s_out_aux = ev->ops_s[nd->pos]; }
+    if (0 != (ev->rc = xb_meltw_launch(&d, &a))) ev->failed = 1;
+    return out;
+  }
+}
+
+LIBXSMM_API int libxsmm_b200_meqn_batch_strided(libxsmm_meqn_function kernel, const libxsmm_meqn_param* param,
+  const long long* input_strides, long long output_stride, long long output_aux_stride, const long long* ops_strides, long long count)
+{
+  const xb_slot* s = xb_slot_of((const void*)kernel);
+  const xb_eqn_plan* plan; const xb_eqn* e;
+  long long per_tile = 0, chunk, t0;
+  int i, rc = 0;
+  if (s == NULL || s->kind != XB_KIND_MEQN || param == NULL || param->output.primary == NULL || count < 0) return -1;
+  plan = (const xb_eqn_plan*)s->u.sp.work; e = &plan->eqn;
+  for (i = 0; i < e->nnodes; ++i) {
+    const xb_eqn_node* nd = &e->node[i]; xb_meltw_desc d;
+    if (nd->type == EQ_ARG) continue;
+    node_desc(e, i, &d);
+    if (!xb_meltw_batchable(&d)) return LIBXSMM_B200_ERROR_NOT_BATCHABLE;
+  }
+  if (output_stride < 0 || output_aux_stride < 0) return -1;
+  for (i = 0; i < e->nnodes; ++i) {
+    const xb_eqn_node* nd = &e->node[i];
+    if (nd->type == EQ_ARG && (input_strides == NULL || param->inputs == NULL || input_strides[nd->pos] < 0 || param->inputs[nd->pos].primary == NULL)) return -1;
+    if (is_dump(nd) && (nd->pos < 0 || ops_strides == NULL || param->ops_args == NULL || ops_strides[nd->pos] < 0)) return -1;
+    if (has_bitmask_out(nd) && param->output.secondary == NULL) return -1;
+    if (is_dump(nd) && param->ops_args[nd->pos].primary == NULL) return -1;
+  }
+  /* an argument that a DUMP writes is read through the DUMP's buffer: both strides must describe the same tiles */
+  for (i = 0; i < e->nnodes; ++i) if (is_dump(&e->node[i])) {
+    const int dp = e->node[i].pos; int j;
+    for (j = 0; j < e->nnodes; ++j) {
+      const xb_eqn_node* x = &e->node[j];
+      if (x->type == EQ_ARG && param->inputs[x->pos].primary == param->ops_args[dp].primary && input_strides[x->pos] != ops_strides[dp]) return -1;
+    }
+  }
+  if (count == 0) return 0;
+  if (count > 1) {                      /* calls must not overlap in what they write */
+    const size_t out_bytes = ((size_t)(plan->out_n - 1) * plan->out_ld + plan->out_m) * libxsmm_typesize((libxsmm_datatype)plan->out_type);
+    if (output_stride < (long long)out_bytes) return -1;
+    for (i = 0; i < e->nnodes; ++i) {
+      const xb_eqn_node* nd = &e->node[i];
+      if (has_bitmask_out(nd) && output_aux_stride < (long long)(LIBXSMM_UP(nd->ld, 16) / 8 * nd->n)) return -1;
+      if (is_dump(nd) && ops_strides[nd->pos] < (long long)span(nd)) return -1;
+    }
+  }
+  /* device-accessible operands only: there is no staging path */
+  if (xb_rt_ptr_kind(param->output.primary) == 0) return -4;
+  for (i = 0; i < e->nnodes; ++i) {
+    const xb_eqn_node* nd = &e->node[i];
+    if (nd->type == EQ_ARG && xb_rt_ptr_kind(param->inputs[nd->pos].primary) == 0) return -4;
+    if (is_dump(nd) && xb_rt_ptr_kind(param->ops_args[nd->pos].primary) == 0) return -4;
+    if (has_bitmask_out(nd) && xb_rt_ptr_kind(param->output.secondary) == 0) return -4;
+    if (nd->type != EQ_ARG && i != 0) per_tile += tmp_stride(nd);
+  }
+  chunk = (per_tile > 0 && per_tile < XB_MEQN_BATCH_SCRATCH_BYTES) ? XB_MEQN_BATCH_SCRATCH_BYTES / per_tile : (per_tile > 0 ? 1 : count);
+  for (t0 = 0; t0 < count && rc == 0; t0 += chunk) {
+    xb_beval ev; long long st; int rs;
+    memset(&ev, 0, sizeof(ev));
+    ev.e = e; ev.p = param; ev.in_s = input_strides; ev.ops_s = ops_strides; ev.out_s = output_stride; ev.aux_s = output_aux_stride;
+    ev.t0 = t0; ev.cnt = (count - t0 < chunk) ? count - t0 : chunk;
+    ev.pool = (per_tile > 0) ? (char*)xb_rt_scratch((size_t)(per_tile * ev.cnt)) : NULL;
+    if (per_tile > 0 && ev.pool == NULL) { xb_rt_note_error(2, "meqn batch: out of scratch"); return 2; }
+    (void)beval_node(&ev, 0, 1, &st);
+    rc = ev.failed ? (ev.rc != 0 ? ev.rc : 2) : 0;
+    if (ev.failed) xb_rt_note_error(rc, "meqn batch: evaluation failed");
+    rs = xb_rt_sync();
+    if (rc == 0) rc = rs;
+    xb_rt_scratch_reset();
+  }
+  return rc;
+}
+
 /* ---- user registry: libxsmm_xregister / xdispatch / xrelease (src/libxsmm_main.c:3010-3120) --------------------------------
  * binary keys of up to LIBXSMM_DESCRIPTOR_MAXSIZE bytes; the value is copied and owned here. A released entry stays in the list as
  * a tombstone (its memory too) until the same key is registered again: tests/registry.c:133-137 walks the registry releasing each

@@ -15,6 +15,7 @@
 #include <stdint.h>
 #include <string.h>
 #include <float.h>
+#include <type_traits>
 #include "xb_internal.h"
 #include "xb_device.cuh"
 
@@ -114,6 +115,16 @@ __host__ __device__ inline int family_of(const xb_meltw_desc& d) {
   return FAM_NONE;
 }
 
+// what a kernel sees of a call: xb_meltw_args without the tile axis, which only the batch instantiations take (as mtiles). The
+// kernels' argument struct keeps its former size, so the single-call kernels compile as they did before the axis existed.
+struct margs {
+  const void* in0; const void* in1; const void* in2; void* out;
+  const void* in_aux; void* out_aux;
+  float alpha; unsigned long long n_rt; unsigned long long off[2];
+  void* rng; float* rnd; unsigned char* rnd8;
+};
+struct mtiles { long long count, s_in0, s_in1, s_in2, s_in_aux, s_out, s_out_aux; };
+
 // ---- typed load/store -----------------------------------------------------------------------------------
 __device__ __forceinline__ float ld_f32(const void* p, long long idx, int t) {
   if (t == LIBXSMM_DATATYPE_F32) return ((const float*)p)[idx];
@@ -139,7 +150,7 @@ __device__ __forceinline__ unsigned char bf8_stochastic(float v, unsigned int rn
   return (unsigned char)(h >> 8);
 }
 // store of the map kernels: element (i, j) is the (j*m + i)-th the reference visits, which selects its random byte
-__device__ __forceinline__ void st_map(const xb_meltw_desc& d, const xb_meltw_args& a, long long oi, int i, int j, float v) {
+__device__ __forceinline__ void st_map(const xb_meltw_desc& d, const margs& a, long long oi, int i, int j, float v) {
   if (a.rnd8 != nullptr) ((unsigned char*)a.out)[oi] = bf8_stochastic(v, a.rnd8[(long long)j * d.m + i]);
   else st_f32(a.out, oi, d.t_out, v);
 }
@@ -237,13 +248,31 @@ __device__ __forceinline__ void mask_store(void* mask, int i0, int j, long long 
   }
 }
 
+// ---- tile axis (margs.count): a batch of calls in one launch. blockIdx.y strides the calls, blockIdx.x keeps the
+// single call's work split; call t reads and writes through its operands advanced by t times their byte strides. Every kernel
+// that takes the axis has a template flag B: a single call launches B = false, whose loop over the calls is the one iteration
+// t = 0 and folds away at compile time, so its code and registers are those of the kernel without the axis.
+
+template <typename P> __device__ __forceinline__ P adv(P p, long long t, long long s) { return (P)((const char*)p + t * s); }
+__device__ __forceinline__ margs tile_args(const margs& a, const mtiles& s, long long t) {
+  margs r = a;
+  r.in0 = adv(a.in0, t, s.s_in0); r.in1 = adv(a.in1, t, s.s_in1); r.in2 = adv(a.in2, t, s.s_in2);
+  r.in_aux = adv(a.in_aux, t, s.s_in_aux); r.out = (void*)adv(a.out, t, s.s_out); r.out_aux = (void*)adv(a.out_aux, t, s.s_out_aux);
+  return r;
+}
+#define XB_FOR_TILES(A0) _Pragma("unroll 1") for (long long t_ = B ? blockIdx.y : 0; t_ < (B ? tl.count : 1); t_ += B ? gridDim.y : 1)
+#define XB_FOR_CALLS(T, COUNT) _Pragma("unroll 1") for (long long T = B ? blockIdx.y : 0; T < (B ? (COUNT) : 1); T += B ? gridDim.y : 1)
+
 // ---- map kernel: unary / binary / ternary elementwise (with masks) ---------------------------------------------
-__global__ void __launch_bounds__(256) meltw_map_kernel(const xb_meltw_desc d, const xb_meltw_args a, const int n_eff) {
+template <bool B>
+__global__ void __launch_bounds__(256) meltw_map_kernel(const xb_meltw_desc d, const margs a0, const mtiles tl, const int n_eff) {
   const int lane = threadIdx.x & 31;
   const int chunks = (d.m + 31) / 32;
   const long long nwork = (long long)chunks * n_eff;
   const long long wstride = (long long)gridDim.x * (blockDim.x >> 5);
   const bool f64 = (d.t_out == LIBXSMM_DATATYPE_F64);
+  XB_FOR_TILES(a0) {
+  const margs a = B ? tile_args(a0, tl, t_) : a0;
   for (long long w = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); w < nwork; w += wstride) {
     const int j = (int)(w / chunks), i0 = (int)(w % chunks) * 32, i = i0 + lane;
     const bool act = i < d.m;
@@ -314,6 +343,7 @@ __global__ void __launch_bounds__(256) meltw_map_kernel(const xb_meltw_desc d, c
       }
     }
   }
+  }
 }
 
 // ---- reductions: one warp per result element ------------------------------------------------------------------------
@@ -366,13 +396,13 @@ template <typename T> __device__ __forceinline__ mm_state<T> mm_combine(mm_state
 }
 
 template <typename T>
-__device__ __forceinline__ T reduce_load(const xb_meltw_desc& d, const xb_meltw_args& a, long long idx) {
-  return (sizeof(T) == 8) ? (T)((const double*)a.in0)[idx] : (T)ld_f32(a.in0, idx, d.t_in0);
+__device__ __forceinline__ T reduce_load(const xb_meltw_desc& d, const void* in0, long long idx) {
+  return (sizeof(T) == 8) ? (T)((const double*)in0)[idx] : (T)ld_f32(in0, idx, d.t_in0);
 }
 template <typename T> __device__ __forceinline__ T warp_sum(T v) { for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o); return v; }
 
-template <typename T>
-__global__ void __launch_bounds__(256) meltw_reduce_kernel(const xb_meltw_desc d, const xb_meltw_args a) {
+template <typename T, bool B>
+__global__ void __launch_bounds__(256) meltw_reduce_kernel(const xb_meltw_desc d, const margs a, const mtiles tl) {
   const int lane = threadIdx.x & 31;
   const bool rows = (d.flags & LIBXSMM_MELTW_FLAG_UNARY_REDUCE_ROWS) != 0;
   const bool init_acc = (d.flags & LIBXSMM_MELTW_FLAG_UNARY_REDUCE_INIT_ACC) != 0;
@@ -393,25 +423,28 @@ __global__ void __launch_bounds__(256) meltw_reduce_kernel(const xb_meltw_desc d
   const bool is_min = (kind == 2);
   const bool later = argop || (rows ? kind == 2 : kind != 2);
   const bool nan_restarts = !argop && (rows ? kind == 2 : kind != 2);
+  XB_FOR_CALLS(t_, tl.count) {                              // the operands of call t_ (a single call: t_ = 0, the kernel's own)
+  const void* const in0 = adv(a.in0, t_, tl.s_in0); const void* const in_aux = adv(a.in_aux, t_, tl.s_in_aux);
+  void* const out = adv(a.out, t_, tl.s_out); void* const out_aux = adv(a.out_aux, t_, tl.s_out_aux);
   for (int o = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); o < nres; o += gridDim.x * (blockDim.x >> 5)) {
     if (kind == 0) {
       T sx = 0, sx2 = 0;
       for (long long t = lane; t < len; t += 32) {
         long long idx;
         if (rows) idx = t + (long long)o * d.ldi;
-        else { const long long j = by_idx ? (idx4 ? (long long)((const unsigned int*)a.in_aux)[t] : (long long)((const unsigned long long*)a.in_aux)[t]) : t; idx = o + j * d.ldi; }
-        const T v = reduce_load<T>(d, a, idx);
+        else { const long long j = by_idx ? (idx4 ? (long long)((const unsigned int*)in_aux)[t] : (long long)((const unsigned long long*)in_aux)[t]) : t; idx = o + j * d.ldi; }
+        const T v = reduce_load<T>(d, in0, idx);
         sx += v; sx2 += v * v;
       }
       sx = warp_sum(sx); sx2 = warp_sum(sx2);
       if (lane == 0) {
         if (f64) {
-          double* ox = (double*)a.out; double* ox2 = want_x ? ox + result_size : ox;
+          double* ox = (double*)out; double* ox2 = want_x ? ox + result_size : ox;
           if (want_x) ox[o] = (double)sx + ((init_acc) ? ox[o] : 0.0);
           if (want_x2) ox2[o] = (double)sx2 + ((init_acc) ? ox2[o] : 0.0);
         } else {
-          char* base2 = (char*)a.out + (want_x ? (size_t)result_size * xb_dev_typesize(d.t_out) : 0);
-          if (want_x) { float r = (float)sx; if (init_acc && !by_idx) r += ld_f32(a.out, o, d.t_out); st_f32(a.out, o, d.t_out, r); }
+          char* base2 = (char*)out + (want_x ? (size_t)result_size * xb_dev_typesize(d.t_out) : 0);
+          if (want_x) { float r = (float)sx; if (init_acc && !by_idx) r += ld_f32(out, o, d.t_out); st_f32(out, o, d.t_out, r); }
           if (want_x2) { float r = (float)sx2; if (init_acc) r += ld_f32(base2, o, d.t_out); st_f32(base2, o, d.t_out, r); }
         }
       }
@@ -420,8 +453,8 @@ __global__ void __launch_bounds__(256) meltw_reduce_kernel(const xb_meltw_desc d
     const long long seg = (len + 31) / 32, t0 = lane * seg, t1 = (t0 + seg < len) ? t0 + seg : len;
     mm_state<T> st; st.v = st.nanv = (T)0; st.pos = 0; st.have = 0; st.reset = 0;
     for (long long t = t0; t < t1; ++t) {
-      const long long j = rows ? t : (by_idx ? (idx4 ? (long long)((const unsigned int*)a.in_aux)[t] : (long long)((const unsigned long long*)a.in_aux)[t]) : t);
-      T v = reduce_load<T>(d, a, rows ? (t + (long long)o * d.ldi) : (o + j * d.ldi));
+      const long long j = rows ? t : (by_idx ? (idx4 ? (long long)((const unsigned int*)in_aux)[t] : (long long)((const unsigned long long*)in_aux)[t]) : t);
+      T v = reduce_load<T>(d, in0, rows ? (t + (long long)o * d.ldi) : (o + j * d.ldi));
       if (kind == 3) v = mm_abs(v);
       if (mm_isnan(v)) { if (nan_restarts) { st.reset = 1; st.have = 0; st.nanv = v; } }
       else if (!st.have || mm_better(v, st.v, is_min, later)) { st.v = v; st.pos = j; st.have = 1; }
@@ -437,7 +470,7 @@ __global__ void __launch_bounds__(256) meltw_reduce_kernel(const xb_meltw_desc d
     if (lane == 0) {
       T res; bool taken = false;
       if (rows) {
-        const T x0 = reduce_load<T>(d, a, (long long)o * d.ldi);
+        const T x0 = reduce_load<T>(d, in0, (long long)o * d.ldi);
         if (kind != 2 && mm_isnan(x0)) {                       // a NaN start sticks; ABS flips it once per element folded
           typedef typename mm_traits<T>::U U;
           res = (kind == 3 && (len & 1)) ? mm_from((U)(mm_bits(x0) ^ mm_traits<T>::SIGN), x0) : x0;
@@ -448,20 +481,23 @@ __global__ void __launch_bounds__(256) meltw_reduce_kernel(const xb_meltw_desc d
         taken = st.have && mm_better(st.v, start, is_min, later);
         res = taken ? st.v : start;
       }
-      if (f64) ((double*)a.out)[o] = (double)res; else st_f32(a.out, o, d.t_out, (float)res);
-      if (argop && taken && a.out_aux != nullptr) {
-        if (idx4) ((unsigned int*)a.out_aux)[o] = (unsigned int)st.pos; else ((unsigned long long*)a.out_aux)[o] = (unsigned long long)st.pos;
+      if (f64) ((double*)out)[o] = (double)res; else st_f32(out, o, d.t_out, (float)res);
+      if (argop && taken && out_aux != nullptr) {
+        if (idx4) ((unsigned int*)out_aux)[o] = (unsigned int)st.pos; else ((unsigned long long*)out_aux)[o] = (unsigned long long)st.pos;
       }
     }
   }
+  }
 }
 
-// whole-matrix reductions to one scalar (single CTA; the tests' sizes are tiny, the large case is a dot product)
-template <typename T>
-__global__ void __launch_bounds__(1024) meltw_scalar_kernel(const xb_meltw_desc d, const xb_meltw_args a) {
+// whole-matrix reductions to one scalar (one CTA per call; the tests' sizes are tiny, the large case is a dot product)
+template <typename T, bool B>
+__global__ void __launch_bounds__(1024) meltw_scalar_kernel(const xb_meltw_desc d, const margs a0, const mtiles tl) {
   __shared__ T part[32];
   const bool f64 = sizeof(T) == 8;
   const bool dot = (d.op_class == LIBXSMM_MELTW_OPERATION_BINARY);
+  XB_FOR_TILES(a0) {
+  const margs a = B ? tile_args(a0, tl, t_) : a0;
   T acc = 0;
   for (long long e = threadIdx.x; e < (long long)d.m * d.n; e += blockDim.x) {
     const int i = (int)(e % d.m), j = (int)(e / d.m);
@@ -477,17 +513,22 @@ __global__ void __launch_bounds__(1024) meltw_scalar_kernel(const xb_meltw_desc 
     acc = warp_sum(acc);
     if (threadIdx.x == 0) { if (f64) ((double*)a.out)[0] = (double)acc; else st_f32(a.out, 0, d.t_out, (float)acc); }
   }
+  if (B && t_ + gridDim.y < tl.count) __syncthreads();       // part[] is reused by the next call of the batch
+  }
 }
 
 // ---- transforms: one thread per OUTPUT element, pure data movement -------------------------------------------------
-template <typename E>
-__global__ void __launch_bounds__(256) meltw_transform_kernel(const xb_meltw_desc d, const xb_meltw_args a) {
-  const E* in = (const E*)a.in0; E* out = (E*)a.out;
+template <typename E, bool B>
+__global__ void __launch_bounds__(256) meltw_transform_kernel(const xb_meltw_desc d, const margs a0, const mtiles tl) {
   const long long M = d.m, N = d.n, ldi = d.ldi, ldo = d.ldo;
   const long long tid = blockIdx.x * (long long)blockDim.x + threadIdx.x, nth = (long long)gridDim.x * blockDim.x;
+  const E* in0 = (const E*)a0.in0; E* out0 = (E*)a0.out;
+  // the element's indices are worked out once and the move repeats for every call of the batch (a single call: once, t_ = 0)
+#define XB_PUT(OI, COND, II) { const long long oi_ = (OI), ii_ = (II); const bool c_ = (COND); \
+    XB_FOR_CALLS(t_, tl.count) adv(out0, t_, tl.s_out)[oi_] = c_ ? adv(in0, t_, tl.s_in0)[ii_] : (E)0; }
   switch (d.op) {
     case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_NORMT:          // out[j*ldo+i] = in[i*ldi+j], i<N, j<M (:390-417)
-      for (long long e = tid; e < M * N; e += nth) { const long long i = e % N, j = e / N; out[j * ldo + i] = in[i * ldi + j]; }
+      for (long long e = tid; e < M * N; e += nth) { const long long i = e % N, j = e / N; XB_PUT(j * ldo + i, true, i * ldi + j); }
       break;
     case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_VNNI2: case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_VNNI2_PAD:
     case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_VNNI4: case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_VNNI4_PAD: {
@@ -496,51 +537,51 @@ __global__ void __launch_bounds__(256) meltw_transform_kernel(const xb_meltw_des
       const long long Nn = ((N + v - 1) / v) * v;
       for (long long e = tid; e < ldo * Nn; e += nth) {
         const long long j = e / (ldo * v), rem = e % (ldo * v), i = rem / v, j2 = rem % v, col = j * v + j2;
-        out[e] = (i < M && col < N) ? in[col * ldi + i] : (E)0;   // rows >= N of the last group are zero padding
+        XB_PUT(e, i < M && col < N, col * ldi + i);   // rows >= N of the last group are zero padding
       }
     } break;
     case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_VNNI2T: case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_VNNI4T: {
       const long long v = (d.op == LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_VNNI2T) ? 2 : 4;   // out[(i*ldo*v)+(j*v)+i2] = in[(j*ldi)+(i*v+i2)]
-      for (long long e = tid; e < (M / v) * N * v; e += nth) { const long long i2 = e % v, j = (e / v) % N, i = e / (v * N); out[i * ldo * v + j * v + i2] = in[j * ldi + i * v + i2]; }
+      for (long long e = tid; e < (M / v) * N * v; e += nth) { const long long i2 = e % v, j = (e / v) % N, i = e / (v * N); XB_PUT(i * ldo * v + j * v + i2, true, j * ldi + i * v + i2); }
     } break;
     case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_VNNI2_TO_VNNI2T: case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_VNNI4_TO_VNNI4T: {
       const long long v = (d.op == LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_VNNI2_TO_VNNI2T) ? 2 : 4;  // out[j*ldo*v+j2+(i*v+i2)*v] = in[i*ldi*v+i2+(j*v+j2)*v]
       for (long long e = tid; e < (M / v) * (N / v) * v * v; e += nth) {
         const long long i2 = e % v, j2 = (e / v) % v, i = (e / (v * v)) % (N / v), j = e / (v * v * (N / v));
-        out[j * ldo * v + j2 + (i * v + i2) * v] = in[i * ldi * v + i2 + (j * v + j2) * v];
+        XB_PUT(j * ldo * v + j2 + (i * v + i2) * v, true, i * ldi * v + i2 + (j * v + j2) * v);
       }
     } break;
     case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_VNNI2T_TO_NORM: case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_VNNI4T_TO_NORM: {
       const long long v = (d.op == LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_VNNI2T_TO_NORM) ? 2 : 4;   // roles of m/n swapped (:620-660)
       const long long Mr = d.n, Nr = d.m;                                                          // out[(j*ldo)+(i*v)+i2] = in[(i*ldi*v)+(j*v+i2)]
-      for (long long e = tid; e < (Mr / v) * Nr * v; e += nth) { const long long i2 = e % v, j = (e / v) % Nr, i = e / (v * Nr); out[j * ldo + i * v + i2] = in[i * ldi * v + j * v + i2]; }
+      for (long long e = tid; e < (Mr / v) * Nr * v; e += nth) { const long long i2 = e % v, j = (e / v) % Nr, i = e / (v * Nr); XB_PUT(j * ldo + i * v + i2, true, i * ldi * v + j * v + i2); }
     } break;
     case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_VNNI4_TO_NORM:            // out[(i*ldo)+j] = in[((i/4)*ldi*4)+j*4+(i%4)], i<N, j<M (:787-803)
-      for (long long e = tid; e < M * N; e += nth) { const long long j = e % M, i = e / M; out[i * ldo + j] = in[(i / 4) * ldi * 4 + j * 4 + (i % 4)]; }
+      for (long long e = tid; e < M * N; e += nth) { const long long j = e % M, i = e / M; XB_PUT(i * ldo + j, true, (i / 4) * ldi * 4 + j * 4 + (i % 4)); }
       break;
     case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_VNNI8: case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_VNNI8_PAD: {
       // :712-786 -- like VNNI2/VNNI4 with groups of 8 columns; columns past N read as zero here (the reference reads past its input)
       const long long v = 8, Nn = ((N + v - 1) / v) * v;
       for (long long e = tid; e < ldo * Nn; e += nth) {
         const long long j = e / (ldo * v), rem = e % (ldo * v), i = rem / v, j2 = rem % v, col = j * v + j2;
-        out[e] = (i < M && col < N) ? in[col * ldi + i] : (E)0;
+        XB_PUT(e, i < M && col < N, col * ldi + i);
       }
     } break;
     case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_VNNI8T:           // out[(i*ldo*8)+(j*8)+i2] = in[(j*ldi)+(i*8+i2)] (:666-686)
-      for (long long e = tid; e < (M / 8) * N * 8; e += nth) { const long long i2 = e % 8, j = (e / 8) % N, i = e / (8 * N); out[i * ldo * 8 + j * 8 + i2] = in[j * ldi + i * 8 + i2]; }
+      for (long long e = tid; e < (M / 8) * N * 8; e += nth) { const long long i2 = e % 8, j = (e / 8) % N, i = e / (8 * N); XB_PUT(i * ldo * 8 + j * 8 + i2, true, j * ldi + i * 8 + i2); }
       break;
     case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_VNNI8_TO_VNNI8T:          // out[j*ldo*8+j2+(i*8+i2)*8] = in[i*ldi*8+i2+(j*8+j2)*8] (:489-531)
       for (long long e = tid; e < (M / 8) * (N / 8) * 64; e += nth) {
         const long long i2 = e % 8, j2 = (e / 8) % 8, i = (e / 64) % (N / 8), j = e / (64 * (N / 8));
-        out[j * ldo * 8 + j2 + (i * 8 + i2) * 8] = in[i * ldi * 8 + i2 + (j * 8 + j2) * 8];
+        XB_PUT(j * ldo * 8 + j2 + (i * 8 + i2) * 8, true, i * ldi * 8 + i2 + (j * 8 + j2) * 8);
       }
       break;
     case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_VNNI8T_TO_NORM: {         // roles of m/n swapped (:581-601)
       const long long Mr = d.n, Nr = d.m;                              // out[(j*ldo)+(i*8)+i2] = in[(i*ldi*8)+(j*8+i2)]
-      for (long long e = tid; e < (Mr / 8) * Nr * 8; e += nth) { const long long i2 = e % 8, j = (e / 8) % Nr, i = e / (8 * Nr); out[j * ldo + i * 8 + i2] = in[i * ldi * 8 + j * 8 + i2]; }
+      for (long long e = tid; e < (Mr / 8) * Nr * 8; e += nth) { const long long i2 = e % 8, j = (e / 8) % Nr, i = e / (8 * Nr); XB_PUT(j * ldo + i * 8 + i2, true, i * ldi * 8 + j * 8 + i2); }
     } break;
     case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_VNNI4_TO_VNNI2:            // out[((i/2)*ldo*2)+j*2+(i%2)] = in[((i/4)*ldi*4)+j*4+(i%4)], i<N, j<M (:806-823)
-      for (long long e = tid; e < M * N; e += nth) { const long long j = e % M, i = e / M; out[(i / 2) * ldo * 2 + j * 2 + (i % 2)] = in[(i / 4) * ldi * 4 + j * 4 + (i % 4)]; }
+      for (long long e = tid; e < M * N; e += nth) { const long long j = e % M, i = e / M; XB_PUT((i / 2) * ldo * 2 + j * 2 + (i % 2), true, (i / 4) * ldi * 4 + j * 4 + (i % 4)); }
       break;
     case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_PADM_MOD2: case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_PADN_MOD2: case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_PADNM_MOD2:
     case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_PADM_MOD4: case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_PADN_MOD4: case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_PADNM_MOD4: {
@@ -548,22 +589,27 @@ __global__ void __launch_bounds__(256) meltw_transform_kernel(const xb_meltw_des
       const bool mod4 = (d.op == LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_PADM_MOD4 || d.op == LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_PADN_MOD4 || d.op == LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_PADNM_MOD4);
       const bool padm_only = (d.op == LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_PADM_MOD2 || d.op == LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_PADM_MOD4);
       const long long v = mod4 ? 4 : 2, Nn = padm_only ? N : ((N + v - 1) / v) * v;
-      for (long long e = tid; e < ldo * Nn; e += nth) { const long long i = e % ldo, j = e / ldo; out[e] = (i < M && j < N) ? in[j * ldi + i] : (E)0; }
+      for (long long e = tid; e < ldo * Nn; e += nth) { const long long i = e % ldo, j = e / ldo; XB_PUT(e, i < M && j < N, j * ldi + i); }
     } break;
     default: break;
   }
+#undef XB_PUT
 }
 
 // ---- bandwidth versions of the three layout/reduction kernels that matter at size (K7 of SURVEY.md 2.3) ------------------------
 // transpose: 64 x 64 tiles through shared memory, one tile per CTA; both the read (rows of the input) and the write (rows of
 // the output) are coalesced and every thread has its 16 loads in flight before the first store
-template <typename E>
-__global__ void __launch_bounds__(256) meltw_transpose_tiled_kernel(const E* __restrict__ in, E* __restrict__ out, long long M, long long N, long long ldi, long long ldo) {
+template <typename E, bool B>
+__global__ void __launch_bounds__(256) meltw_transpose_tiled_kernel(const E* __restrict__ in0, E* __restrict__ out0, long long M, long long N, long long ldi, long long ldo,
+                                                                    long long count, long long s_in, long long s_out) {
   __shared__ E tile[64][65];
   const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;                 // 32 x 8 threads
   const long long tiles_j = (M + 63) / 64;
   const long long t = blockIdx.x;
   const long long j0 = (t % tiles_j) * 64, i0 = (t / tiles_j) * 64;       // in[i*ldi + j], j contiguous, j < M, i < N
+  XB_FOR_CALLS(c, count) {                                                // calls of a batch
+  const E* __restrict__ in = adv(in0, c, s_in);
+  E* __restrict__ out = adv(out0, c, s_out);
   E v[16];
 #pragma unroll
   for (int r = 0; r < 8; ++r) {
@@ -580,12 +626,18 @@ __global__ void __launch_bounds__(256) meltw_transpose_tiled_kernel(const E* __r
 #pragma unroll
     for (int h = 0; h < 2; ++h) if (j < M && i0 + tx + 32 * h < N) out[j * ldo + i0 + tx + 32 * h] = tile[tx + 32 * h][ty + 8 * r];
   }
+  if (B && c + gridDim.y < count) __syncthreads();                        // the next call refills the tile
+  }
 }
 // NORM -> VNNI-v pack: a thread takes 4 consecutive rows of one group of v columns: v loads of 4 elements, 4 stores of one
 // v-element word each (16 contiguous bytes); zero padding of the last group and of rows [m, ldo) like the generic kernel
-template <typename E, int V>
-__global__ void __launch_bounds__(256) meltw_vnni_pack_kernel(const E* __restrict__ in, E* __restrict__ out, long long M, long long N, long long ldi, long long ldo) {
+template <typename E, int V, bool B>
+__global__ void __launch_bounds__(256) meltw_vnni_pack_kernel(const E* __restrict__ in0, E* __restrict__ out0, long long M, long long N, long long ldi, long long ldo,
+                                                              long long count, long long s_in, long long s_out) {
   const long long groups = (N + V - 1) / V, quads = (ldo + 3) / 4;
+  XB_FOR_CALLS(t, count) {
+  const E* __restrict__ in = adv(in0, t, s_in);
+  E* __restrict__ out = adv(out0, t, s_out);
   for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < groups * quads; e += (long long)gridDim.x * blockDim.x) {
     const long long g = e / quads, i0 = (e % quads) * 4;
     E v[V][4];
@@ -601,16 +653,21 @@ __global__ void __launch_bounds__(256) meltw_vnni_pack_kernel(const E* __restric
       for (int c = 0; c < V; ++c) out[(g * ldo + i0 + r) * V + c] = v[c][r];
     }
   }
+  }
 }
 // the same pack with 16-byte accesses: a thread takes R = 16/sizeof(E) consecutive rows of one group of v columns (v loads of
 // 16 bytes, v stores of 16 contiguous bytes); needs M, ldi, ldo multiples of R and 16-byte aligned bases
-template <typename E, int V>
-__global__ void __launch_bounds__(256) meltw_vnni_pack_vec_kernel(const E* __restrict__ in, E* __restrict__ out, long long M, long long N, long long ldi, long long ldo) {
+template <typename E, int V, bool B>
+__global__ void __launch_bounds__(256) meltw_vnni_pack_vec_kernel(const E* __restrict__ in0, E* __restrict__ out0, long long M, long long N, long long ldi, long long ldo,
+                                                                  long long count, long long s_in, long long s_out) {
   constexpr int R = 16 / (int)sizeof(E);
   const long long groups = (N + V - 1) / V, chunks = ldo / R;
   const long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   if (e >= groups * chunks) return;
   const long long g = e / chunks, i0 = (e % chunks) * R;
+  XB_FOR_CALLS(t, count) {
+  const E* __restrict__ in = adv(in0, t, s_in);
+  E* __restrict__ out = adv(out0, t, s_out);
   union { uint4 q; E e[R]; } src[V];
   union { uint4 q[V]; E e[R * V]; } dst;
 #pragma unroll
@@ -626,6 +683,7 @@ __global__ void __launch_bounds__(256) meltw_vnni_pack_vec_kernel(const E* __res
   uint4* o = reinterpret_cast<uint4*>(out + (g * ldo + i0) * V);
 #pragma unroll
   for (int c = 0; c < V; ++c) o[c] = dst.q[c];
+  }
 }
 // column sums of an f32 matrix with 16-byte loads: a warp covers 128 consecutive rows (one float4 per lane), the 8 warps of a
 // CTA take the columns of the CTA's slice round-robin, four columns in flight per warp; the CTA's eight partial sums are added
@@ -669,7 +727,7 @@ __global__ void __launch_bounds__(256) meltw_reduce_cols_partial_vec_kernel(cons
 // column reduction (one result per ROW i, the input's contiguous index): lanes take consecutive rows, so every load of a
 // warp is one 128-byte line; the columns are cut into gridDim.y slices whose partial sums go to `part` and are added up, in
 // slice order, by a second small kernel
-__global__ void __launch_bounds__(256) meltw_reduce_cols_partial_kernel(const xb_meltw_desc d, const xb_meltw_args a, float* __restrict__ part, int want_x2) {
+__global__ void __launch_bounds__(256) meltw_reduce_cols_partial_kernel(const xb_meltw_desc d, const margs a, float* __restrict__ part, int want_x2) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   const int per = (d.n + gridDim.y - 1) / gridDim.y, j0 = blockIdx.y * per, j1 = (j0 + per < d.n) ? j0 + per : d.n;
   if (i >= d.m) return;
@@ -678,7 +736,7 @@ __global__ void __launch_bounds__(256) meltw_reduce_cols_partial_kernel(const xb
   part[(size_t)blockIdx.y * d.m + i] = sx;
   if (want_x2) part[(size_t)(gridDim.y + blockIdx.y) * d.m + i] = sx2;
 }
-__global__ void __launch_bounds__(256) meltw_reduce_cols_final_kernel(const xb_meltw_desc d, const xb_meltw_args a, const float* __restrict__ part, int slices) {
+__global__ void __launch_bounds__(256) meltw_reduce_cols_final_kernel(const xb_meltw_desc d, const margs a, const float* __restrict__ part, int slices) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= d.m) return;
   const bool init_acc = (d.flags & LIBXSMM_MELTW_FLAG_UNARY_REDUCE_INIT_ACC) != 0;
@@ -693,7 +751,7 @@ __global__ void __launch_bounds__(256) meltw_reduce_cols_final_kernel(const xb_m
 
 // ---- gather / scatter (:1444-1794) ------------------------------------------------------------------------------------
 template <typename E>
-__global__ void __launch_bounds__(256) meltw_gs_kernel(const xb_meltw_desc d, const xb_meltw_args a) {
+__global__ void __launch_bounds__(256) meltw_gs_kernel(const xb_meltw_desc d, const margs a) {
   const E* in = (const E*)a.in0; E* out = (E*)a.out;
   const bool gather = (d.op == LIBXSMM_MELTW_TYPE_UNARY_GATHER);
   const void* idxp = gather ? a.in_aux : (const void*)a.out_aux;
@@ -737,13 +795,18 @@ __device__ __forceinline__ unsigned int mx_e4m3_scale(float v) {       // RNE, c
   return (m >= 8u) ? (sign | 0x08u) : (sign | (m & 7u));
 }
 __device__ __forceinline__ float mx_bf16_round(float f) { return __uint_as_float((unsigned int)xb_f32_to_bf16_rne(f) << 16); }
-template <int BLK, int KIND>     // KIND 0: MXFP4, 1: NVFP4, 2: MXBF8
-__global__ void __launch_bounds__(128) meltw_mxquant_kernel(const unsigned short* __restrict__ in, unsigned char* __restrict__ out, unsigned char* __restrict__ scl,
-                                                            int m, int n, long long ldi, long long ldo) {
+template <int BLK, int KIND, bool B>     // KIND 0: MXFP4, 1: NVFP4, 2: MXBF8
+__global__ void __launch_bounds__(128) meltw_mxquant_kernel(const unsigned short* __restrict__ in0, unsigned char* __restrict__ out0, unsigned char* __restrict__ scl0,
+                                                            int m, int n, long long ldi, long long ldo,
+                                                            long long count, long long s_in, long long s_out, long long s_scl) {
   const long long blocks_m = m / BLK, ld_data = (KIND == 2) ? ldo : ldo / 2, ld_scl = ldo / BLK;
   const long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   if (e >= blocks_m * n) return;
   const long long b = e % blocks_m, j = e / blocks_m;
+  XB_FOR_CALLS(t, count) {
+  const unsigned short* __restrict__ in = adv(in0, t, s_in);
+  unsigned char* __restrict__ out = adv(out0, t, s_out);
+  unsigned char* __restrict__ scl = adv(scl0, t, s_scl);
   const unsigned short* src = in + j * ldi + b * BLK;
   float x[BLK];
   float amax = 0.0f;
@@ -780,12 +843,16 @@ __global__ void __launch_bounds__(128) meltw_mxquant_kernel(const unsigned short
       for (int k = 0; k < BLK; ++k) o[k] = special ? (unsigned char)0x7b : (unsigned char)xb_f32_to_bf8(__fdiv_rn(x[k], scale));
     }
   }
+  }
 }
 
 // ---- quant / dequant (:2195-2360) ----------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) meltw_quant_kernel(const xb_meltw_desc d, const xb_meltw_args a) {
+template <bool B>
+__global__ void __launch_bounds__(256) meltw_quant_kernel(const xb_meltw_desc d, const margs a0, const mtiles tl) {
   const bool quant = (d.op == LIBXSMM_MELTW_TYPE_UNARY_QUANT);
   const bool sat = (d.flags & LIBXSMM_MELTW_FLAG_UNARY_SIGN_SAT_QUANT) != 0;
+  XB_FOR_TILES(a0) {
+  const margs a = B ? tile_args(a0, tl, t_) : a0;
   for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < (long long)d.m * d.n; e += (long long)gridDim.x * blockDim.x) {
     const int i = (int)(e % d.m), j = (int)(e / d.m);
     const long long ii = bidx(d, 0, i, j, d.ldi), oi = i + (long long)j * d.ldo;
@@ -801,6 +868,7 @@ __global__ void __launch_bounds__(256) meltw_quant_kernel(const xb_meltw_desc d,
       else v = (float)((const int*)a.in0)[ii];
       ((float*)a.out)[oi] = v * a.alpha;
     }
+  }
   }
 }
 
@@ -833,13 +901,16 @@ __global__ void __launch_bounds__(32) meltw_rng8_kernel(unsigned int* __restrict
   }
   state[w] = s0; state[16 + w] = s1; state[32 + w] = s2; state[48 + w] = s3;
 }
-__global__ void __launch_bounds__(256) meltw_dropout_kernel(const xb_meltw_desc d, const xb_meltw_args a) {
+template <bool B>
+__global__ void __launch_bounds__(256) meltw_dropout_kernel(const xb_meltw_desc d, const margs a0, const mtiles tl) {
   const int lane = threadIdx.x & 31;
   const int chunks = (d.m + 31) / 32, gpc = (d.m + 15) / 16;
   const bool fwd = (d.op == LIBXSMM_MELTW_TYPE_UNARY_DROPOUT);
   const bool bitm = (d.flags & LIBXSMM_MELTW_FLAG_UNARY_BITMASK_2BYTEMULT) != 0;
-  const float pn = 1.0f - a.alpha, pi = 1.0f / pn;
+  const float pn = 1.0f - a0.alpha, pi = 1.0f / pn;
   const long long nwork = (long long)chunks * d.n, wstride = (long long)gridDim.x * (blockDim.x >> 5);
+  XB_FOR_TILES(a0) {                                        // batches: DROPOUT_INV only (the forward generator chains call to call)
+  const margs a = B ? tile_args(a0, tl, t_) : a0;
   for (long long w = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); w < nwork; w += wstride) {
     const int j = (int)(w / chunks), i0 = (int)(w % chunks) * 32, i = i0 + lane;
     const bool act = i < d.m;
@@ -853,10 +924,11 @@ __global__ void __launch_bounds__(256) meltw_dropout_kernel(const xb_meltw_desc 
       st_f32(a.out, i + (long long)j * d.ldo, d.t_out, mask_bit(a.in_aux, i, j, mld) ? x * pi : 0.0f);
     }
   }
+  }
 }
 
 // ---- f32 -> bf16 planes: UNZIP (low/high halves), DECOMP_FP32_TO_BF16X2/X3 (truncated head + rounded remainders) (:2423-2469)
-__global__ void __launch_bounds__(256) meltw_split_kernel(const xb_meltw_desc d, const xb_meltw_args a) {
+__global__ void __launch_bounds__(256) meltw_split_kernel(const xb_meltw_desc d, const margs a) {
   const float* in = (const float*)a.in0;
   unsigned short* out = (unsigned short*)a.out;
   for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < (long long)d.m * d.n; e += (long long)gridDim.x * blockDim.x) {
@@ -879,6 +951,16 @@ __global__ void __launch_bounds__(256) meltw_split_kernel(const xb_meltw_desc d,
       } else out[o + (long long)(a.off[0] / 2)] = xb_f32_to_bf16_rne(r1);
     }
   }
+}
+
+// grid of a launch: `gx` blocks per call (the single call's grid), and as many calls side by side in y as keep the whole grid within
+// `cap` blocks; the kernels stride the remaining calls through blockIdx.y. A single call gets gridDim.y = 1.
+dim3 batch_grid(long long gx, long long count, long long cap) {
+  long long gy = cap / (gx > 0 ? gx : 1);
+  if (gy > count) gy = count;
+  if (gy > 65535) gy = 65535;
+  if (gy < 1) gy = 1;
+  return dim3((unsigned int)gx, (unsigned int)gy);
 }
 
 int launch_done(const char* where) {
@@ -904,8 +986,11 @@ extern "C" int xb_meltw_supported(const xb_meltw_desc* d) { return family_of(*d)
 //                                                                                      16-byte aligned)
 //   other reductions (rows, max / min / absmax, column-index, F64) ................... 4 warp reduction
 //   maps, to-scalar, gather / scatter, quantisers, dropout, unzip / decomp ........... 7
+// A batch (a->count > 1) takes the same kernel as its single call, except: the 16-byte VNNI pack also needs both byte strides to be
+// multiples of 16, and column sums take the warp reduction (4) -- the two-phase reduction's scratch is sized for one call.
 extern "C" int xb_meltw_variant(const xb_meltw_desc* d, const xb_meltw_args* a) {
   const int fam = family_of(*d);
+  const bool batch = a->count > 1;
   if (fam == FAM_TRANSFORM) {
     const int ts = xb_dev_typesize(d->t_in0);
     if (d->op == LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_NORMT && (long long)d->m * d->n >= 4096) return 1;
@@ -913,7 +998,8 @@ extern "C" int xb_meltw_variant(const xb_meltw_desc* d, const xb_meltw_args* a) 
                                           || (ts == 1 && (d->op == LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_VNNI4 || d->op == LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_VNNI4_PAD)))) {
       const int V = (ts == 2) ? 2 : 4, R = 16 / ts;
       const long long items = (long long)((d->n + V - 1) / V) * (d->ldo / R);
-      const bool vec = (d->m % R) == 0 && (d->ldi % R) == 0 && (d->ldo % R) == 0 && (((uintptr_t)a->in0 | (uintptr_t)a->out) & 15) == 0
+      const uintptr_t strides = batch ? (uintptr_t)(a->s_in0 | a->s_out) : 0;
+      const bool vec = (d->m % R) == 0 && (d->ldi % R) == 0 && (d->ldo % R) == 0 && (((uintptr_t)a->in0 | (uintptr_t)a->out | strides) & 15) == 0
                     && (items + 255) / 256 <= 0x7fffffffll;
       return vec ? 3 : 2;
     }
@@ -921,7 +1007,7 @@ extern "C" int xb_meltw_variant(const xb_meltw_desc* d, const xb_meltw_args* a) 
   }
   if (fam == FAM_REDUCE) {
     const bool sum_op = (d->op == LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X_OP_ADD || d->op == LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X2_OP_ADD || d->op == LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X_X2_OP_ADD);
-    if (sum_op && (d->flags & LIBXSMM_MELTW_FLAG_UNARY_REDUCE_ROWS) == 0 && d->t_in0 != LIBXSMM_DATATYPE_F64 && (long long)d->m * d->n >= (1 << 18) && d->m >= 256) {
+    if (!batch && sum_op && (d->flags & LIBXSMM_MELTW_FLAG_UNARY_REDUCE_ROWS) == 0 && d->t_in0 != LIBXSMM_DATATYPE_F64 && (long long)d->m * d->n >= (1 << 18) && d->m >= 256) {
       return (d->t_in0 == LIBXSMM_DATATYPE_F32 && (d->m % 4) == 0 && (d->ldi % 4) == 0 && ((uintptr_t)a->in0 & 15) == 0) ? 6 : 5;
     }
     return 4;
@@ -951,6 +1037,16 @@ extern "C" int xb_meltw_launch(const xb_meltw_desc* d, const xb_meltw_args* a) {
   const int fam = family_of(*d);
   if (d->m <= 0 || d->n <= 0) return 0;
   const int variant = xb_meltw_variant(d, a);
+  const long long count = (a->count > 1) ? a->count : 1;   // calls in this launch: every grid below is the single call's in x, calls in y
+  const margs ka = { a->in0, a->in1, a->in2, a->out, a->in_aux, a->out_aux, a->alpha, a->n_rt, { a->off[0], a->off[1] }, a->rng, a->rnd, a->rnd8 };
+  const mtiles tl = { count, a->s_in0, a->s_in1, a->s_in2, a->s_in_aux, a->s_out, a->s_out_aux };
+  if (count > 1 && (fam == FAM_GS || fam == FAM_SPLIT || a->rnd8 != nullptr || a->n_rt != 0
+                    || (fam == FAM_DROPOUT && d->op == LIBXSMM_MELTW_TYPE_UNARY_DROPOUT))) {
+    xb_rt_note_error(1, "meltw: this operation has per-call state or run-time extents and runs one call per launch"); return 1;
+  }
+  // the kernels' tile-axis flag: a batch launches <.., true>, a single call <.., false>
+  const auto run = [&](auto batched) -> int {
+  constexpr bool B = decltype(batched)::value;
   switch (fam) {
     case FAM_MAP: {
       const int n_eff = (d->op_class == LIBXSMM_MELTW_OPERATION_UNARY && d->op == LIBXSMM_MELTW_TYPE_UNARY_REPLICATE_COL_VAR) ? (int)a->n_rt : d->n;
@@ -960,7 +1056,7 @@ extern "C" int xb_meltw_launch(const xb_meltw_desc* d, const xb_meltw_args* a) {
         meltw_rng8_kernel<<<1, 32, 0, st>>>((unsigned int*)a->rng, a->rnd8, (long long)d->m * n_eff);
         if (launch_done("meltw_rng8") != 0) return 1;
       }
-      meltw_map_kernel<<<(unsigned int)grid, 256, 0, st>>>(*d, *a, n_eff);
+      meltw_map_kernel<B><<<batch_grid(grid, count, 132 * 8), 256, 0, st>>>(*d, ka, tl, n_eff);
       return launch_done("meltw_map");
     }
     case FAM_REDUCE: {
@@ -975,77 +1071,83 @@ extern "C" int xb_meltw_launch(const xb_meltw_desc* d, const xb_meltw_args* a) {
           meltw_reduce_cols_partial_vec_kernel<<<gv, 256, 0, st>>>((const float*)a->in0, d->m, d->n, d->ldi, part, want_x2);
         } else {
           const dim3 g((d->m + 255) / 256, slices);
-          meltw_reduce_cols_partial_kernel<<<g, 256, 0, st>>>(*d, *a, part, want_x2);
+          meltw_reduce_cols_partial_kernel<<<g, 256, 0, st>>>(*d, ka, part, want_x2);
         }
         if (launch_done("meltw_reduce_partial") != 0) return 1;
-        meltw_reduce_cols_final_kernel<<<(d->m + 255) / 256, 256, 0, st>>>(*d, *a, part, slices);
+        meltw_reduce_cols_final_kernel<<<(d->m + 255) / 256, 256, 0, st>>>(*d, ka, part, slices);
         return launch_done("meltw_reduce_final");
       }
       const int nres = (d->flags & LIBXSMM_MELTW_FLAG_UNARY_REDUCE_ROWS) ? d->n : d->m;
       int grid = (nres + 7) / 8; if (grid > 132 * 8) grid = 132 * 8;
-      if (d->t_in0 == LIBXSMM_DATATYPE_F64) meltw_reduce_kernel<double><<<grid, 256, 0, st>>>(*d, *a);
-      else meltw_reduce_kernel<float><<<grid, 256, 0, st>>>(*d, *a);
+      const dim3 g = batch_grid(grid, count, 132 * 8);
+      if (d->t_in0 == LIBXSMM_DATATYPE_F64) meltw_reduce_kernel<double, B><<<g, 256, 0, st>>>(*d, ka, tl);
+      else meltw_reduce_kernel<float, B><<<g, 256, 0, st>>>(*d, ka, tl);
       return launch_done("meltw_reduce");
     }
-    case FAM_SCALAR:
-      if (d->t_in0 == LIBXSMM_DATATYPE_F64) meltw_scalar_kernel<double><<<1, 1024, 0, st>>>(*d, *a);
-      else meltw_scalar_kernel<float><<<1, 1024, 0, st>>>(*d, *a);
+    case FAM_SCALAR: {
+      const dim3 g = batch_grid(1, count, 132 * 2);
+      if (d->t_in0 == LIBXSMM_DATATYPE_F64) meltw_scalar_kernel<double, B><<<g, 1024, 0, st>>>(*d, ka, tl);
+      else meltw_scalar_kernel<float, B><<<g, 1024, 0, st>>>(*d, ka, tl);
       return launch_done("meltw_scalar");
+    }
     case FAM_TRANSFORM: case FAM_GS: {
       const long long work = (long long)(d->ldo > d->m ? d->ldo : d->m) * ((d->n + 3) / 4 * 4);
       long long grid = (work + 255) / 256; if (grid > 132 * 16) grid = 132 * 16; if (grid < 1) grid = 1;
       const int ts = xb_dev_typesize(d->t_in0);
+      const long long si = a->s_in0, so = a->s_out;
       if (variant == 1) {
         const long long tiles = (long long)((d->m + 63) / 64) * ((d->n + 63) / 64);
         if (tiles > 0x7fffffffll) return 1;
-        const unsigned int tg = (unsigned int)tiles;
-        if (ts == 8) meltw_transpose_tiled_kernel<unsigned long long><<<tg, 256, 0, st>>>((const unsigned long long*)a->in0, (unsigned long long*)a->out, d->m, d->n, d->ldi, d->ldo);
-        else if (ts == 4) meltw_transpose_tiled_kernel<unsigned int><<<tg, 256, 0, st>>>((const unsigned int*)a->in0, (unsigned int*)a->out, d->m, d->n, d->ldi, d->ldo);
-        else if (ts == 2) meltw_transpose_tiled_kernel<unsigned short><<<tg, 256, 0, st>>>((const unsigned short*)a->in0, (unsigned short*)a->out, d->m, d->n, d->ldi, d->ldo);
-        else meltw_transpose_tiled_kernel<unsigned char><<<tg, 256, 0, st>>>((const unsigned char*)a->in0, (unsigned char*)a->out, d->m, d->n, d->ldi, d->ldo);
+        const dim3 tg = batch_grid(tiles, count, 132 * 8);
+        if (ts == 8) meltw_transpose_tiled_kernel<unsigned long long, B><<<tg, 256, 0, st>>>((const unsigned long long*)a->in0, (unsigned long long*)a->out, d->m, d->n, d->ldi, d->ldo, count, si, so);
+        else if (ts == 4) meltw_transpose_tiled_kernel<unsigned int, B><<<tg, 256, 0, st>>>((const unsigned int*)a->in0, (unsigned int*)a->out, d->m, d->n, d->ldi, d->ldo, count, si, so);
+        else if (ts == 2) meltw_transpose_tiled_kernel<unsigned short, B><<<tg, 256, 0, st>>>((const unsigned short*)a->in0, (unsigned short*)a->out, d->m, d->n, d->ldi, d->ldo, count, si, so);
+        else meltw_transpose_tiled_kernel<unsigned char, B><<<tg, 256, 0, st>>>((const unsigned char*)a->in0, (unsigned char*)a->out, d->m, d->n, d->ldi, d->ldo, count, si, so);
         return launch_done("meltw_transpose");
       }
       if (variant == 3) {
         const long long items = (long long)((d->n + (ts == 2 ? 2 : 4) - 1) / (ts == 2 ? 2 : 4)) * (d->ldo / (16 / ts));
-        const unsigned int vg = (unsigned int)((items + 255) / 256);
-        if (ts == 2) meltw_vnni_pack_vec_kernel<unsigned short, 2><<<vg, 256, 0, st>>>((const unsigned short*)a->in0, (unsigned short*)a->out, d->m, d->n, d->ldi, d->ldo);
-        else meltw_vnni_pack_vec_kernel<unsigned char, 4><<<vg, 256, 0, st>>>((const unsigned char*)a->in0, (unsigned char*)a->out, d->m, d->n, d->ldi, d->ldo);
+        const dim3 vg = batch_grid((items + 255) / 256, count, 132 * 16);
+        if (ts == 2) meltw_vnni_pack_vec_kernel<unsigned short, 2, B><<<vg, 256, 0, st>>>((const unsigned short*)a->in0, (unsigned short*)a->out, d->m, d->n, d->ldi, d->ldo, count, si, so);
+        else meltw_vnni_pack_vec_kernel<unsigned char, 4, B><<<vg, 256, 0, st>>>((const unsigned char*)a->in0, (unsigned char*)a->out, d->m, d->n, d->ldi, d->ldo, count, si, so);
         return launch_done("meltw_vnni_pack_vec");
       }
       if (variant == 2) {
         const int V = (ts == 2) ? 2 : 4;
         const long long workp = (long long)((d->n + V - 1) / V) * ((d->ldo + 3) / 4);
         long long pg = (workp + 255) / 256; if (pg > 132 * 16) pg = 132 * 16;
-        if (ts == 2) meltw_vnni_pack_kernel<unsigned short, 2><<<(unsigned int)pg, 256, 0, st>>>((const unsigned short*)a->in0, (unsigned short*)a->out, d->m, d->n, d->ldi, d->ldo);
-        else meltw_vnni_pack_kernel<unsigned char, 4><<<(unsigned int)pg, 256, 0, st>>>((const unsigned char*)a->in0, (unsigned char*)a->out, d->m, d->n, d->ldi, d->ldo);
+        const dim3 g = batch_grid(pg, count, 132 * 16);
+        if (ts == 2) meltw_vnni_pack_kernel<unsigned short, 2, B><<<g, 256, 0, st>>>((const unsigned short*)a->in0, (unsigned short*)a->out, d->m, d->n, d->ldi, d->ldo, count, si, so);
+        else meltw_vnni_pack_kernel<unsigned char, 4, B><<<g, 256, 0, st>>>((const unsigned char*)a->in0, (unsigned char*)a->out, d->m, d->n, d->ldi, d->ldo, count, si, so);
         return launch_done("meltw_vnni_pack");
       }
       if (fam == FAM_TRANSFORM) {
-        if (ts == 8) meltw_transform_kernel<unsigned long long><<<(unsigned int)grid, 256, 0, st>>>(*d, *a);
-        else if (ts == 4) meltw_transform_kernel<unsigned int><<<(unsigned int)grid, 256, 0, st>>>(*d, *a);
-        else if (ts == 2) meltw_transform_kernel<unsigned short><<<(unsigned int)grid, 256, 0, st>>>(*d, *a);
-        else meltw_transform_kernel<unsigned char><<<(unsigned int)grid, 256, 0, st>>>(*d, *a);
+        const dim3 g = batch_grid(grid, count, 132 * 16);
+        if (ts == 8) meltw_transform_kernel<unsigned long long, B><<<g, 256, 0, st>>>(*d, ka, tl);
+        else if (ts == 4) meltw_transform_kernel<unsigned int, B><<<g, 256, 0, st>>>(*d, ka, tl);
+        else if (ts == 2) meltw_transform_kernel<unsigned short, B><<<g, 256, 0, st>>>(*d, ka, tl);
+        else meltw_transform_kernel<unsigned char, B><<<g, 256, 0, st>>>(*d, ka, tl);
       } else {
-        if (ts == 4) meltw_gs_kernel<unsigned int><<<(unsigned int)grid, 256, 0, st>>>(*d, *a);
-        else if (ts == 2) meltw_gs_kernel<unsigned short><<<(unsigned int)grid, 256, 0, st>>>(*d, *a);
-        else meltw_gs_kernel<unsigned char><<<(unsigned int)grid, 256, 0, st>>>(*d, *a);
+        if (ts == 4) meltw_gs_kernel<unsigned int><<<(unsigned int)grid, 256, 0, st>>>(*d, ka);
+        else if (ts == 2) meltw_gs_kernel<unsigned short><<<(unsigned int)grid, 256, 0, st>>>(*d, ka);
+        else meltw_gs_kernel<unsigned char><<<(unsigned int)grid, 256, 0, st>>>(*d, ka);
       }
       return launch_done("meltw_move");
     }
     case FAM_QUANT: {
       long long grid = ((long long)d->m * d->n + 255) / 256; if (grid > 132 * 16) grid = 132 * 16;
-      meltw_quant_kernel<<<(unsigned int)grid, 256, 0, st>>>(*d, *a);
+      meltw_quant_kernel<B><<<batch_grid(grid, count, 132 * 16), 256, 0, st>>>(*d, ka, tl);
       return launch_done("meltw_quant");
     }
     case FAM_MXQUANT: {
       const int blk = (d->t_out == LIBXSMM_DATATYPE_NVFP4X2) ? 16 : 32;
       const long long items = (long long)(d->m / blk) * d->n;
       if (items <= 0) return 0;
-      const unsigned int g = (unsigned int)((items + 127) / 128);
+      const dim3 g = batch_grid((items + 127) / 128, count, 132 * 16);
       const unsigned short* in = (const unsigned short*)a->in0; unsigned char* out = (unsigned char*)a->out; unsigned char* sc = (unsigned char*)a->out_aux;
-      if (d->t_out == LIBXSMM_DATATYPE_MXFP4X2) meltw_mxquant_kernel<32, 0><<<g, 128, 0, st>>>(in, out, sc, d->m, d->n, d->ldi, d->ldo);
-      else if (d->t_out == LIBXSMM_DATATYPE_NVFP4X2) meltw_mxquant_kernel<16, 1><<<g, 128, 0, st>>>(in, out, sc, d->m, d->n, d->ldi, d->ldo);
-      else meltw_mxquant_kernel<32, 2><<<g, 128, 0, st>>>(in, out, sc, d->m, d->n, d->ldi, d->ldo);
+      if (d->t_out == LIBXSMM_DATATYPE_MXFP4X2) meltw_mxquant_kernel<32, 0, B><<<g, 128, 0, st>>>(in, out, sc, d->m, d->n, d->ldi, d->ldo, count, a->s_in0, a->s_out, a->s_out_aux);
+      else if (d->t_out == LIBXSMM_DATATYPE_NVFP4X2) meltw_mxquant_kernel<16, 1, B><<<g, 128, 0, st>>>(in, out, sc, d->m, d->n, d->ldi, d->ldo, count, a->s_in0, a->s_out, a->s_out_aux);
+      else meltw_mxquant_kernel<32, 2, B><<<g, 128, 0, st>>>(in, out, sc, d->m, d->n, d->ldi, d->ldo, count, a->s_in0, a->s_out, a->s_out_aux);
       return launch_done("meltw_mxquant");
     }
     case FAM_DROPOUT: {
@@ -1055,14 +1157,16 @@ extern "C" int xb_meltw_launch(const xb_meltw_desc* d, const xb_meltw_args* a) {
         meltw_rng_kernel<<<1, 32, 0, st>>>((unsigned int*)a->rng, a->rnd, (long long)((d->m + 15) / 16) * d->n);
         if (launch_done("meltw_rng") != 0) return 1;
       }
-      meltw_dropout_kernel<<<(unsigned int)grid, 256, 0, st>>>(*d, *a);
+      meltw_dropout_kernel<B><<<batch_grid(grid, count, 132 * 8), 256, 0, st>>>(*d, ka, tl);
       return launch_done("meltw_dropout");
     }
     case FAM_SPLIT: {
       long long grid = ((long long)d->m * d->n + 255) / 256; if (grid > 132 * 16) grid = 132 * 16;
-      meltw_split_kernel<<<(unsigned int)grid, 256, 0, st>>>(*d, *a);
+      meltw_split_kernel<<<(unsigned int)grid, 256, 0, st>>>(*d, ka);
       return launch_done("meltw_split");
     }
     default: return 1;
   }
+  };
+  return (count > 1) ? run(std::true_type()) : run(std::false_type());
 }

@@ -205,11 +205,16 @@ typedef struct xb_meltw_args {
   void* rng;                 /* DROPOUT: 4 x 16 words of generator state (device copy, updated by the kernel) */
   float* rnd;                /* DROPOUT: scratch for the uniform numbers, 16 per group of rows */
   unsigned char* rnd8;       /* STOCHASTIC_ROUND to BF8: one random byte per element in the reference's visiting order (NULL: round to nearest) */
+  /* tile axis: `count` calls of the handle in one launch, call t with every pointer above (in0 .. out_aux) advanced by t times its
+   * byte stride; 0 or 1 is a single call. Generator state, scratch and the by-value fields are shared by the calls. */
+  long long count;
+  long long s_in0, s_in1, s_in2, s_in_aux, s_out, s_out_aux;
 } xb_meltw_args;
 void xb_invoke_meqn(const struct xb_slot* s, const void* param);
 void xb_meqn_release(void* work);
 int xb_meltw_supported(const xb_meltw_desc* d);                          /* pure host logic */
 int xb_meltw_launch(const xb_meltw_desc* d, const xb_meltw_args* a);
+int xb_meltw_batchable(const xb_meltw_desc* d);                         /* host_meltw.c: 0 if a call carries per-call state */
 int xb_sreg_launch(const xb_sparse_desc* d, const void* b, void* c, long long n_total);
 int xb_packed_sp_launch(const xb_sparse_desc* d, const void* a, const void* b, void* c, long long count,
                         long long stride_a, long long stride_b, long long stride_c);
