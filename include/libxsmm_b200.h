@@ -135,6 +135,23 @@ LIBXSMM_API int libxsmm_b200_meqn_batch_strided(libxsmm_meqn_function kernel, co
   const long long* input_strides, long long output_stride, long long output_aux_stride,
   const long long* ops_strides, long long count);
 
+/* ---- batched packed-sparse, packed-dense and BCSC calls ----------------------------------------
+ * count calls of one libxsmm_create_packed_spgemm_csr / _csc, libxsmm_create_packed_gemm / _ac_rm / _bc_rm or
+ * libxsmm_create_packed_spgemm_bcsc handle in one launch. Call t is kernel(param) with a.primary, b.primary (BCSC: the block
+ * values) and c.primary advanced by t times their stride (BYTES; 0 = one operand shared by every call). Everything else in *param
+ * is read once, from call 0, and shared: for BCSC the pattern (b.secondary colptr, b.tertiary rowidx, b.quaternary block-column
+ * count), which may be device-resident or host memory (then staged once). Returns 0; -1 for a NULL or foreign handle, count < 0,
+ * a NULL operand or pattern, a negative stride, a stride that is not a multiple of its operand's element size, or a C stride
+ * smaller than the bytes one call writes through C (outputs of consecutive calls would overlap); -4 if A, B or C is pageable host
+ * memory (device, managed or pinned only); LIBXSMM_B200_ERROR_NOT_BATCHABLE for fsspmdm handles
+ * (libxsmm_create_spgemm_csr_areg), whose single call already covers every column of B; the positive CUDA error if a launch fails.
+ * count == 0 does nothing. Honours libxsmm_b200_set_blocking. A BCSC batch takes the kernel libxsmm_b200_bcsc_variant names for
+ * its call 0 when its strides are multiples of 16 bytes; otherwise the exact-order kernel (libxsmm_b200_launch_count_backend
+ * tells which ran). */
+typedef struct libxsmm_b200_spgemm_strides { long long a, b, c; } libxsmm_b200_spgemm_strides;
+LIBXSMM_API int libxsmm_b200_spgemm_batch_strided(libxsmm_gemmfunction kernel, const libxsmm_gemm_param* param,
+  const libxsmm_b200_spgemm_strides* strides, long long count);
+
 #if defined(__cplusplus)
 }
 #endif

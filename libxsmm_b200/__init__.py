@@ -318,6 +318,13 @@ libxsmm_b200_meltw_batch_strided = _sig("libxsmm_b200_meltw_batch_strided", _I, 
 libxsmm_b200_meqn_batch_strided = _sig("libxsmm_b200_meqn_batch_strided", _I,
                                        [_P, C.POINTER(MeqnParam), C.POINTER(_LL), _LL, _LL, C.POINTER(_LL), _LL])
 
+
+class SpgemmStrides(C.Structure):
+    _fields_ = [(n, C.c_longlong) for n in ("a", "b", "c")]
+
+
+libxsmm_b200_spgemm_batch_strided = _sig("libxsmm_b200_spgemm_batch_strided", _I, [_P, C.POINTER(GemmParam), C.POINTER(SpgemmStrides), _LL])
+
 EXPORTED = [n for n in dir() if n.startswith("libxsmm_") and callable(globals()[n])]
 
 

@@ -14,6 +14,9 @@
 // B blocks ([bn][bk], k contiguous: the K-major operand) are copied into the canonical no-swizzle shared-memory layout
 // (8 x 16-byte core matrices), two buffers so that the copy of the next block overlaps the MMAs of the current one.
 // The pattern (colptr, rowidx) and the values arrive with the call and are read directly: no preparation kernel.
+// Call axis (a strided batch, xb_sparse_calls): the template flag B, as in bcsc_simt_kernel. B = false is the single call, its loop
+// over the calls folds away at compile time. B = true keeps the single call's grid of items in x and strides the calls through
+// blockIdx.y; every call walks the same (group, block-column) items with A, the block values and C at its own bases.
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -53,9 +56,9 @@ __device__ __forceinline__ void mma_rs(float (&d)[NC / 2], const uint32_t (&a)[4
 }
 
 // NC: columns per instruction, NCH: instructions side by side (NC * NCH >= bn)
-template <int NC, int NCH>
+template <int NC, int NCH, bool B>
 __global__ void __launch_bounds__(128, (NCH >= 4) ? 2 : 4)
-bcsc_wg_kernel(const BcscParams P) {
+bcsc_wg_kernel(const BcscParams P, const xb_sparse_calls tl) {
   extern __shared__ __align__(128) uint8_t smem_raw[];
   const int buf_bytes = NC * NCH * P.bk * 2;                 // the instructions read NC * NCH rows of a block
   uint8_t* sbuf[2] = {smem_raw, smem_raw + buf_bytes};
@@ -64,6 +67,11 @@ bcsc_wg_kernel(const BcscParams P) {
   const long long KW = P.K / 2;
   float acc[NCH][NC / 2];
   int buf = 0;
+#pragma unroll 1
+  for (long long t = B ? blockIdx.y : 0; t < (B ? tl.count : 1); t += B ? gridDim.y : 1) {
+  const uint32_t* const pa = B ? (const uint32_t*)((const char*)P.a + t * tl.s_a) : P.a;
+  const uint4* const pb = B ? (const uint4*)((const char*)P.b_vals + t * tl.s_b) : P.b_vals;
+  unsigned short* const pc = B ? (unsigned short*)((char*)P.c + t * tl.s_c) : P.c;
   for (long long item = blockIdx.x; item < P.items; item += gridDim.x) {
     const long long grp = item / P.nbc;
     const int j = (int)(item - grp * P.nbc);
@@ -73,7 +81,7 @@ bcsc_wg_kernel(const BcscParams P) {
     for (int h = 0; h < 2; ++h) {
       const long long R = grp * 64 + 16 * wq + (lane >> 2) + 8 * h, mb = R / P.M;
       avalid[h] = mb < P.m_blocks;
-      arow[h] = P.a + (avalid[h] ? mb * KW * P.M + (R - mb * P.M) : 0);
+      arow[h] = pa + (avalid[h] ? mb * KW * P.M + (R - mb * P.M) : 0);
     }
     const unsigned int z0 = P.colptr[j], z1 = P.colptr[j + 1];
     bool started = false;
@@ -83,7 +91,7 @@ bcsc_wg_kernel(const BcscParams P) {
       // every warp has passed its wait_group after the MMAs that read this buffer two blocks ago (or the previous item's
       // wait_group 0): only then may any warp overwrite it
       __syncthreads();
-      stage_block(sbuf[buf], P.b_vals + (size_t)z * (P.bn * P.bk / 8), P.bn, P.bk);
+      stage_block(sbuf[buf], pb + (size_t)z * (P.bn * P.bk / 8), P.bn, P.bk);
       xb_fence_proxy_async();
       __syncthreads();
       const long long kw0 = (long long)kb * (P.bk / 2);
@@ -120,11 +128,12 @@ bcsc_wg_kernel(const BcscParams P) {
         const int col = c * NC + c0 + 8 * (i >> 2) + (i & 1), h = (i >> 1) & 1;
         if (col >= P.bn || !avalid[h]) continue;
         const long long R = grp * 64 + r0 + 8 * h, mb = R / P.M;
-        char* p = reinterpret_cast<char*>(P.c + (mb * ncols + (long long)j * P.bn + col) * P.M + (R - mb * P.M));
+        char* p = reinterpret_cast<char*>(pc + (mb * ncols + (long long)j * P.bn + col) * P.M + (R - mb * P.M));
         if (P.beta0) xb_ep_store_one<XB_EP_BF16, true>(__float_as_uint(acc[c][i]), p, 0.0f);
         else xb_ep_store_one<XB_EP_BF16, false>(__float_as_uint(acc[c][i]), p, 0.0f);
       }
     }
+  }
   }
 }
 
@@ -137,12 +146,18 @@ int device_sms() {
 }
 
 // MaxDynamicSharedMemorySize is a per-device function attribute: set it once per (instantiation, device)
-template <int NC, int NCH>
-cudaError_t launch(long long grid, size_t smem, cudaStream_t stream, const BcscParams& P) {
+template <int NC, int NCH, bool B>
+cudaError_t launch_one(dim3 grid, size_t smem, cudaStream_t stream, const BcscParams& P, const xb_sparse_calls& tl) {
   static unsigned long long done = 0ull;
-  if (xb_rt_first_use_on_device(&done)) cudaFuncSetAttribute(bcsc_wg_kernel<NC, NCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * NC * NCH * 64 * 2);
-  bcsc_wg_kernel<NC, NCH><<<(unsigned int)grid, 128, smem, stream>>>(P);
+  if (xb_rt_first_use_on_device(&done)) cudaFuncSetAttribute(bcsc_wg_kernel<NC, NCH, B>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * NC * NCH * 64 * 2);
+  bcsc_wg_kernel<NC, NCH, B><<<grid, 128, smem, stream>>>(P, tl);
   return cudaGetLastError();
+}
+// a single call: one row of CTAs; a batch: up to 65,535 rows of calls, the rest looped over in the kernel
+template <int NC, int NCH>
+cudaError_t launch(long long grid, size_t smem, cudaStream_t stream, const BcscParams& P, const xb_sparse_calls& tl) {
+  if (tl.count > 1) return launch_one<NC, NCH, true>(dim3((unsigned int)grid, (unsigned int)(tl.count < 65535 ? tl.count : 65535)), smem, stream, P, tl);
+  return launch_one<NC, NCH, false>(dim3((unsigned int)grid), smem, stream, P, tl);
 }
 
 }  // namespace
@@ -163,13 +178,17 @@ extern "C" int xb_bcsc_tc_variant(const xb_sparse_desc* d, unsigned long long n_
   return 1;
 }
 
-// returns 0 if launched, <0 if this descriptor/problem is not served by the tensor-core kernel (caller falls back)
+// returns 0 if launched, <0 if this descriptor/problem is not served by the tensor-core kernel (caller falls back). The kernel reads
+// A, the block values and C in 16-byte units: the operands of every call, so in a batch (d->calls) also the strides, must be
+// 16-byte aligned, or the exact-order kernel runs.
 extern "C" int xb_bcsc_tc_launch(const xb_sparse_desc* d, void** work, const void* a, const void* b_vals, const unsigned int* colptr,
                                  const unsigned int* rowidx, unsigned long long n_blocks, unsigned int nnzb, void* c)
 {
+  const xb_sparse_calls tl = d->calls;
+  const unsigned long long strides = (tl.count > 1) ? (unsigned long long)(tl.s_a | tl.s_b | tl.s_c) : 0ull;
   (void)work; (void)nnzb;
   if (xb_bcsc_tc_variant(d, n_blocks) == 0) return -1;
-  if ((((uintptr_t)a | (uintptr_t)b_vals | (uintptr_t)c) & 15) != 0) return -1;
+  if ((((uintptr_t)a | (uintptr_t)b_vals | (uintptr_t)c | strides) & 15) != 0) return -1;
   BcscParams P; memset(&P, 0, sizeof(P));
   P.M = d->packed_width; P.K = d->k; P.bk = d->bk; P.bn = d->bn; P.nbc = (int)n_blocks;
   P.m_blocks = d->m; P.ngroups = (d->m * (long long)P.M + 63) / 64; P.items = P.ngroups * P.nbc;
@@ -181,11 +200,11 @@ extern "C" int xb_bcsc_tc_launch(const xb_sparse_desc* d, void** work, const voi
   cudaStream_t stream = (cudaStream_t)xb_rt_stream();
   cudaError_t e;
   switch (nt) {
-    case 16:  e = launch<16, 1>(grid, smem, stream, P); break;
-    case 32:  e = launch<32, 1>(grid, smem, stream, P); break;
-    case 64:  e = launch<64, 1>(grid, smem, stream, P); break;
-    case 128: e = launch<64, 2>(grid, smem, stream, P); break;
-    default:  e = launch<64, 4>(grid, smem, stream, P); break;
+    case 16:  e = launch<16, 1>(grid, smem, stream, P, tl); break;
+    case 32:  e = launch<32, 1>(grid, smem, stream, P, tl); break;
+    case 64:  e = launch<64, 1>(grid, smem, stream, P, tl); break;
+    case 128: e = launch<64, 2>(grid, smem, stream, P, tl); break;
+    default:  e = launch<64, 4>(grid, smem, stream, P, tl); break;
   }
   xb_rt_count_launch_backend(LIBXSMM_B200_BACKEND_TCGEN05);
   if (e != cudaSuccess) { xb_rt_note_error((int)e, "bcsc_tc"); return (int)e; }

@@ -223,16 +223,59 @@ static const void* xb_dev_in(const void* p, size_t bytes, int* staged) {
   else { void* d = xb_rt_scratch(bytes); if (d != NULL) { xb_rt_upload(d, p, bytes); *staged = 1; } return d; }
 }
 
+/* the bytes one call reads through A and B and writes through C. BCSC: B is the block values (nnzb blocks; 0 while the count is
+ * unknown on the host) and C covers n_blocks block-columns. Single calls stage by these extents, batches check their C stride
+ * against them. */
+static void xb_sparse_extents(const xb_sparse_desc* d, unsigned long long n_blocks, unsigned int nnzb, size_t* ab, size_t* bb, size_t* cb) {
+  const size_t ts = libxsmm_typesize((libxsmm_datatype)d->ta), tsc = libxsmm_typesize((libxsmm_datatype)d->tc);
+  const size_t P = (size_t)d->packed_width;
+  switch (d->kind) {
+    case XB_KIND_SREG:     /* a=NULL, b=B, c=C covering max_N columns (src/libxsmm_fsspmdm.c:491-515) */
+      *ab = 0; *bb = ((size_t)(d->k - 1) * d->ldb + d->max_n) * ts; *cb = ((size_t)(d->m - 1) * d->ldc + d->max_n) * ts; break;
+    case XB_KIND_SP_A_CSR: case XB_KIND_SP_B_CSR: case XB_KIND_SP_B_CSC: case XB_KIND_SP_C_CSC:
+      *ab = (d->kind == XB_KIND_SP_A_CSR) ? (size_t)d->nnz * ts
+          : (d->kind == XB_KIND_SP_C_CSC) ? (size_t)d->k * d->lda * P * ts   /* A is [K][lda][P] there */ : (size_t)d->m * d->lda * P * ts;
+      *bb = (d->kind == XB_KIND_SP_B_CSR || d->kind == XB_KIND_SP_B_CSC) ? (size_t)d->nnz * ts : (size_t)d->k * d->ldb * P * ts;
+      *cb = (d->kind == XB_KIND_SP_C_CSC) ? (size_t)d->nnz * ts /* one scalar per non-zero */ : (size_t)d->m * d->ldc * P * ts;
+      break;
+    case XB_KIND_PK_GEMM: case XB_KIND_PK_AC_RM: case XB_KIND_PK_BC_RM:
+      *ab = (d->kind == XB_KIND_PK_GEMM) ? (size_t)d->k * d->lda * P * ts : ((d->kind == XB_KIND_PK_AC_RM) ? (size_t)d->m * d->lda * P * ts : (size_t)d->m * d->lda * ts);
+      *bb = (d->kind == XB_KIND_PK_GEMM) ? (size_t)d->n * d->ldb * P * ts : ((d->kind == XB_KIND_PK_AC_RM) ? (size_t)d->k * d->ldb * ts : (size_t)d->k * d->ldb * P * ts);
+      *cb = ((d->kind == XB_KIND_PK_GEMM) ? (size_t)d->n : (size_t)d->m) * d->ldc * P * ts;
+      break;
+    case XB_KIND_BCSC:     /* slots: samples/xgemm_sparse/spmm_kernel.c:451-466 */
+      *ab = (size_t)d->m * d->k * P * ts; *bb = (size_t)nnzb * d->bk * d->bn * libxsmm_typesize((libxsmm_datatype)d->tb);
+      *cb = (size_t)d->m * n_blocks * d->bn * P * tsc;
+      break;
+    default: *ab = *bb = *cb = 0; break;
+  }
+}
+
+/* the BCSC pattern of a call: block-column count (b.quaternary, read on the host), colptr (b.secondary) and rowidx (b.tertiary);
+ * a host-readable pattern is staged and its block count read, a device-resident one passes as is with nnzb 0 (unknown).
+ * Returns 1 if there is nothing to run (no pattern or no block-columns). */
+static int xb_bcsc_pattern(const libxsmm_gemm_param* p, unsigned long long* nbc, unsigned int* nnzb, const void** cp, const void** ri, int* staged) {
+  const unsigned int* colptr_h = (const unsigned int*)p->b.secondary;
+  *nbc = (p->b.quaternary != NULL) ? *(const unsigned long long*)p->b.quaternary : 0ull;
+  *nnzb = 0;
+  if (*nbc == 0 || colptr_h == NULL) return 1;
+  if (xb_rt_ptr_kind(colptr_h) != 1) *nnzb = colptr_h[*nbc];   /* device-resident pattern: count stays on the device (0 = unknown) */
+  *cp = xb_dev_in(colptr_h, (size_t)(*nbc + 1) * sizeof(unsigned int), staged);
+  *ri = (*nnzb == 0) ? p->b.tertiary : xb_dev_in(p->b.tertiary, (size_t)*nnzb * sizeof(unsigned int), staged);
+  return 0;
+}
+
 void xb_invoke_sparse(const xb_slot* s, const libxsmm_gemm_param* p) {
   const xb_sparse_desc* d = &s->u.sp;
-  const size_t ts = libxsmm_typesize((libxsmm_datatype)d->ta), tsc = libxsmm_typesize((libxsmm_datatype)d->tc);
+  const size_t ts = libxsmm_typesize((libxsmm_datatype)d->ta);
   int staged = 0, rc = 0;
-  void* c_host = NULL; void* c_dev = NULL; size_t c_bytes = 0;
+  void* c_host = NULL; void* c_dev = NULL; size_t ab = 0, bb = 0, c_bytes = 0;
   size_t c_pitch = 0, c_width = 0, c_rows = 0;   /* non-zero: the staged C is a column block of a wider matrix (see XB_KIND_SREG) */
   switch (d->kind) {
-    case XB_KIND_SREG: {   /* a=NULL, b=B, c=C covering max_N columns (src/libxsmm_fsspmdm.c:491-515) */
-      const size_t bb = ((size_t)(d->k - 1) * d->ldb + d->max_n) * ts; c_bytes = ((size_t)(d->m - 1) * d->ldc + d->max_n) * ts;
-      const void* b = xb_dev_in(p->b.primary, bb, &staged);
+    case XB_KIND_SREG: {
+      const void* b;
+      xb_sparse_extents(d, 0, 0, &ab, &bb, &c_bytes);
+      b = xb_dev_in(p->b.primary, bb, &staged);
       c_dev = p->c.primary;
       if (xb_rt_ptr_kind(p->c.primary) == 0) {
         c_host = p->c.primary; c_dev = xb_rt_scratch(c_bytes); staged = 1;
@@ -245,43 +288,23 @@ void xb_invoke_sparse(const xb_slot* s, const libxsmm_gemm_param* p) {
       if (b == NULL || c_dev == NULL) { rc = 2; break; }
       rc = xb_sreg_launch(d, b, c_dev, d->max_n);
     } break;
-    case XB_KIND_SP_A_CSR: case XB_KIND_SP_B_CSR: case XB_KIND_SP_B_CSC: case XB_KIND_SP_C_CSC: {
-      const size_t P = (size_t)d->packed_width;
-      const size_t ab = (d->kind == XB_KIND_SP_A_CSR) ? (size_t)d->nnz * ts
-                      : (d->kind == XB_KIND_SP_C_CSC) ? (size_t)d->k * d->lda * P * ts   /* A is [K][lda][P] there */ : (size_t)d->m * d->lda * P * ts;
-      const size_t bb = (d->kind == XB_KIND_SP_B_CSR || d->kind == XB_KIND_SP_B_CSC) ? (size_t)d->nnz * ts : (size_t)d->k * d->ldb * P * ts;
-      const void *a, *b;
-      c_bytes = (d->kind == XB_KIND_SP_C_CSC) ? (size_t)d->nnz * ts /* one scalar per non-zero */ : (size_t)d->m * d->ldc * P * ts;
-      a = xb_dev_in(p->a.primary, ab, &staged); b = xb_dev_in(p->b.primary, bb, &staged);
-      c_dev = p->c.primary;
-      if (xb_rt_ptr_kind(p->c.primary) == 0) { c_host = p->c.primary; c_dev = xb_rt_scratch(c_bytes); if (c_dev) xb_rt_upload(c_dev, c_host, c_bytes); staged = 1; }
-      if (a == NULL || b == NULL || c_dev == NULL) { rc = 2; break; }
-      rc = xb_packed_sp_launch(d, a, b, c_dev, 1, 0, 0, 0);
-    } break;
+    case XB_KIND_SP_A_CSR: case XB_KIND_SP_B_CSR: case XB_KIND_SP_B_CSC: case XB_KIND_SP_C_CSC:
     case XB_KIND_PK_GEMM: case XB_KIND_PK_AC_RM: case XB_KIND_PK_BC_RM: {
-      const size_t P = (size_t)d->packed_width;
-      const size_t ab = (d->kind == XB_KIND_PK_GEMM) ? (size_t)d->k * d->lda * P * ts : ((d->kind == XB_KIND_PK_AC_RM) ? (size_t)d->m * d->lda * P * ts : (size_t)d->m * d->lda * ts);
-      const size_t bb = (d->kind == XB_KIND_PK_GEMM) ? (size_t)d->n * d->ldb * P * ts : ((d->kind == XB_KIND_PK_AC_RM) ? (size_t)d->k * d->ldb * ts : (size_t)d->k * d->ldb * P * ts);
       const void *a, *b;
-      c_bytes = ((d->kind == XB_KIND_PK_GEMM) ? (size_t)d->n : (size_t)d->m) * d->ldc * P * ts;
+      xb_sparse_extents(d, 0, 0, &ab, &bb, &c_bytes);
       a = xb_dev_in(p->a.primary, ab, &staged); b = xb_dev_in(p->b.primary, bb, &staged);
       c_dev = p->c.primary;
       if (xb_rt_ptr_kind(p->c.primary) == 0) { c_host = p->c.primary; c_dev = xb_rt_scratch(c_bytes); if (c_dev) xb_rt_upload(c_dev, c_host, c_bytes); staged = 1; }
       if (a == NULL || b == NULL || c_dev == NULL) { rc = 2; break; }
       rc = xb_packed_sp_launch(d, a, b, c_dev, 1, 0, 0, 0);
     } break;
-    case XB_KIND_BCSC: {   /* slots: samples/xgemm_sparse/spmm_kernel.c:451-466 */
-      const unsigned long long nbc = (p->b.quaternary != NULL) ? *(const unsigned long long*)p->b.quaternary : 0ull;
-      const unsigned int* colptr_h = (const unsigned int*)p->b.secondary;
-      unsigned int nnzb = 0;
-      const void *a, *bv, *cp, *ri;
-      if (nbc == 0 || colptr_h == NULL) break;
-      if (xb_rt_ptr_kind(colptr_h) != 1) nnzb = colptr_h[nbc];   /* device-resident pattern: count stays on the device (0 = unknown) */
-      c_bytes = (size_t)d->m * nbc * d->bn * d->packed_width * tsc;
-      a = xb_dev_in(p->a.primary, (size_t)d->m * d->k * d->packed_width * ts, &staged);
-      bv = (nnzb == 0) ? p->b.primary : xb_dev_in(p->b.primary, (size_t)nnzb * d->bk * d->bn * libxsmm_typesize((libxsmm_datatype)d->tb), &staged);
-      cp = xb_dev_in(colptr_h, (size_t)(nbc + 1) * sizeof(unsigned int), &staged);
-      ri = (nnzb == 0) ? p->b.tertiary : xb_dev_in(p->b.tertiary, (size_t)nnzb * sizeof(unsigned int), &staged);
+    case XB_KIND_BCSC: {
+      unsigned long long nbc; unsigned int nnzb;
+      const void *a, *bv, *cp = NULL, *ri = NULL;
+      if (xb_bcsc_pattern(p, &nbc, &nnzb, &cp, &ri, &staged)) break;
+      xb_sparse_extents(d, nbc, nnzb, &ab, &bb, &c_bytes);
+      a = xb_dev_in(p->a.primary, ab, &staged);
+      bv = (nnzb == 0) ? p->b.primary : xb_dev_in(p->b.primary, bb, &staged);
       c_dev = p->c.primary;
       if (xb_rt_ptr_kind(p->c.primary) == 0) { c_host = p->c.primary; c_dev = xb_rt_scratch(c_bytes); if (c_dev && !d->beta0) xb_rt_upload(c_dev, c_host, c_bytes); staged = 1; }
       if (a == NULL || bv == NULL || cp == NULL || ri == NULL || c_dev == NULL) { rc = 2; break; }
@@ -292,6 +315,52 @@ void xb_invoke_sparse(const xb_slot* s, const libxsmm_gemm_param* p) {
   if (rc != 0) { xb_rt_note_error(rc, "invoke_sparse"); xb_rt_scratch_reset(); return; }
   if (c_host != NULL) { if (c_rows != 0) xb_rt_memcpy2d_async(c_host, c_dev, c_pitch, c_width, c_rows); else xb_rt_memcpy_async(c_host, c_dev, c_bytes); }
   if (staged || xb_rt_blocking()) { xb_rt_sync(); xb_rt_scratch_reset(); }
+}
+
+/* ---- strided batch: `count` calls of one packed or BCSC handle in one launch ----------------------------------------------------
+ * Call t is kernel(param) with a/b/c.primary advanced by t times their byte strides; everything else in *param (the BCSC pattern
+ * and block-column count included) is read once, from call 0. Nothing is staged but a host-readable BCSC pattern, which every call
+ * shares: A, B and C must be device-accessible. fsspmdm handles are not batchable: one call already covers every column of B. */
+LIBXSMM_API int libxsmm_b200_spgemm_batch_strided(libxsmm_gemmfunction kernel, const libxsmm_gemm_param* param,
+                                                  const libxsmm_b200_spgemm_strides* strides, long long count)
+{
+  const xb_slot* s = xb_slot_of((const void*)kernel);
+  xb_sparse_desc d;
+  unsigned long long nbc = 0; unsigned int nnzb = 0;
+  const void *cp = NULL, *ri = NULL;
+  size_t ab, bb, cb, tsa, tsb, tsc;
+  int staged = 0, rc;
+  if (s == NULL || param == NULL || strides == NULL || count < 0) return -1;
+  switch (s->kind) {
+    case XB_KIND_SREG: return LIBXSMM_B200_ERROR_NOT_BATCHABLE;
+    case XB_KIND_SP_A_CSR: case XB_KIND_SP_B_CSR: case XB_KIND_SP_B_CSC: case XB_KIND_SP_C_CSC:
+    case XB_KIND_PK_GEMM: case XB_KIND_PK_AC_RM: case XB_KIND_PK_BC_RM: case XB_KIND_BCSC: break;
+    default: return -1;
+  }
+  d = s->u.sp;
+  tsa = libxsmm_typesize((libxsmm_datatype)d.ta); tsb = libxsmm_typesize((libxsmm_datatype)d.tb); tsc = libxsmm_typesize((libxsmm_datatype)d.tc);
+  /* a stride must keep every call's operand aligned to its elements */
+  if (strides->a < 0 || strides->b < 0 || strides->c < 0) return -1;
+  if (strides->a % (long long)tsa != 0 || strides->b % (long long)tsb != 0 || strides->c % (long long)tsc != 0) return -1;
+  if (count == 0) return 0;
+  if (param->a.primary == NULL || param->b.primary == NULL || param->c.primary == NULL) return -1;
+  if (d.kind == XB_KIND_BCSC && (param->b.secondary == NULL || param->b.tertiary == NULL || param->b.quaternary == NULL)) return -1;
+  if (xb_rt_ptr_kind(param->a.primary) == 0 || xb_rt_ptr_kind(param->b.primary) == 0 || xb_rt_ptr_kind(param->c.primary) == 0) return -4;
+  if (d.kind == XB_KIND_BCSC) {
+    if (xb_bcsc_pattern(param, &nbc, &nnzb, &cp, &ri, &staged)) return 0;     /* no block-columns: nothing to run, like a single call */
+    if (cp == NULL || ri == NULL) { xb_rt_scratch_reset(); return 2; }
+  }
+  xb_sparse_extents(&d, nbc, nnzb, &ab, &bb, &cb);
+  if (count > 1 && strides->c < (long long)cb) { if (staged) xb_rt_scratch_reset(); return -1; }   /* C of call t reaches into call t + 1 */
+  if (d.kind == XB_KIND_BCSC) {
+    d.calls.count = count; d.calls.s_a = strides->a; d.calls.s_b = strides->b; d.calls.s_c = strides->c;
+    rc = xb_bcsc_launch(&d, param->a.primary, param->b.primary, (const unsigned int*)cp, (const unsigned int*)ri, nbc, nnzb, param->c.primary);
+  } else {
+    rc = xb_packed_sp_launch(&d, param->a.primary, param->b.primary, param->c.primary, count, strides->a, strides->b, strides->c);
+  }
+  if (rc == 0 && (staged || xb_rt_blocking())) rc = xb_rt_sync();
+  if (staged) xb_rt_scratch_reset();
+  return rc;
 }
 
 /* ---- fsspmdm ------------------------------------------------------------------------------------------------ */

@@ -156,7 +156,9 @@ __global__ void __launch_bounds__(256) sreg_direct_kernel(const SregParams P) {
 }
 
 // ------------------------------------------------------------------------------------------------------
-// packed sparse: one CTA per batch item, threads over (n, p)
+// packed sparse: one CTA per batch item, threads over (n, p). The call axis (count, strides) of every packed kernel runs through
+// blockIdx.y: a single call launches its own grid in x with one row of CTAs, a batch stacks up to 65,535 rows of calls and loops
+// over the rest.
 struct PackedParams {
   int kind, M, N, K, P, lda, ldb, ldc, beta0, is_f64;
   const unsigned int* ptr; const unsigned int* idx;
@@ -167,7 +169,7 @@ struct PackedParams {
 template <typename T>
 __global__ void __launch_bounds__(256) packed_sp_kernel(const PackedParams Q) {
   const int P = Q.P;
-  for (long long item = blockIdx.x; item < Q.count; item += gridDim.x) {
+  for (long long item = blockIdx.y; item < Q.count; item += gridDim.y) {
     const T* A = (const T*)(Q.a + item * Q.stride_a); const T* B = (const T*)(Q.b + item * Q.stride_b);
     T* C = (T*)(Q.c + item * Q.stride_c);
     const int work = Q.M * Q.N * P;
@@ -255,6 +257,10 @@ __global__ void __launch_bounds__(256) packed_dense_kernel(const PackedParams Q)
 
 // ------------------------------------------------------------------------------------------------------
 // BCSC exact-order kernel. One CTA per (m_block, block-column); thread per (m, n_local) element.
+// Call axis (a strided batch, xb_sparse_calls): the template flag B. A single call launches B = false, whose loop over the calls is
+// the one iteration t = 0 and folds away at compile time, so its code is that of the kernel without the axis. A batch launches
+// B = true: blockIdx.x keeps the single call's split of the (m_block, block-column) items, blockIdx.y strides the calls, and call t
+// reads A and the block values and writes C at its bases advanced by t times their byte strides. The pattern is shared.
 struct BcscParams {
   int M, K, bk, bn, ta, tb, tc, beta0, trans_a, vnni_a, vnni_b_t;
   long long N;                  // total columns = n_blocks * bn
@@ -266,15 +272,21 @@ __device__ __forceinline__ float bcsc_load_f(const char* base, size_t idx, int t
   return (t == LIBXSMM_DATATYPE_F32) ? ((const float*)base)[idx] : xb_bf16_to_f32(((const unsigned short*)base)[idx]);
 }
 
-__global__ void __launch_bounds__(256) bcsc_simt_kernel(const BcscParams Q) {
+template <bool B>
+__global__ void __launch_bounds__(256) bcsc_simt_kernel(const BcscParams Q, const xb_sparse_calls tl) {
   const long long nbc = Q.N / Q.bn;
   const size_t tsa = xb_dev_typesize(Q.ta), tsc = xb_dev_typesize(Q.tc);
   const bool is_int = (Q.tc == LIBXSMM_DATATYPE_I32);
   const int v = (Q.ta == LIBXSMM_DATATYPE_BF16) ? 2 : ((Q.ta == LIBXSMM_DATATYPE_F32) ? 1 : 4);
+#pragma unroll 1
+  for (long long t = B ? blockIdx.y : 0; t < (B ? tl.count : 1); t += B ? gridDim.y : 1) {
+  const char* const a0 = B ? Q.a + t * tl.s_a : Q.a;
+  const char* const bvals = B ? Q.bvals + t * tl.s_b : Q.bvals;
+  char* const c0 = B ? Q.c + t * tl.s_c : Q.c;
   for (long long w = blockIdx.x; w < Q.m_blocks * nbc; w += gridDim.x) {
     const long long mb = w / nbc, jb = w % nbc;
-    const char* A = Q.a + (size_t)mb * Q.K * Q.M * tsa;
-    char* C = Q.c + (size_t)mb * Q.N * Q.M * tsc;
+    const char* A = a0 + (size_t)mb * Q.K * Q.M * tsa;
+    char* C = c0 + (size_t)mb * Q.N * Q.M * tsc;
     for (int e = threadIdx.x; e < Q.M * Q.bn; e += blockDim.x) {
       const int i = e % Q.M, nl = e / Q.M;
       const long long j = jb * Q.bn + nl;
@@ -297,12 +309,12 @@ __global__ void __launch_bounds__(256) bcsc_simt_kernel(const BcscParams Q) {
           if (Q.vnni_b_t) bi = (size_t)z * Q.bk * Q.bn + (size_t)(kk / v) * Q.bn * v + (size_t)nl * v + (kk % v);
           else bi = (size_t)z * Q.bk * Q.bn + (size_t)nl * Q.bk + kk;
           if (is_int) {
-            const unsigned char ar = ((const unsigned char*)A)[ai], br = ((const unsigned char*)Q.bvals)[bi];
+            const unsigned char ar = ((const unsigned char*)A)[ai], br = ((const unsigned char*)bvals)[bi];
             const int av = (Q.ta == LIBXSMM_DATATYPE_U8) ? (int)ar : (int)(signed char)ar;
             const int bv = (Q.tb == LIBXSMM_DATATYPE_U8) ? (int)br : (int)(signed char)br;
             iacc += av * bv;
           } else {
-            facc = __fadd_rn(facc, __fmul_rn(bcsc_load_f(A, ai, Q.ta), bcsc_load_f(Q.bvals, bi, Q.tb)));
+            facc = __fadd_rn(facc, __fmul_rn(bcsc_load_f(A, ai, Q.ta), bcsc_load_f(bvals, bi, Q.tb)));
           }
         }
       }
@@ -310,6 +322,7 @@ __global__ void __launch_bounds__(256) bcsc_simt_kernel(const BcscParams Q) {
       else if (Q.tc == LIBXSMM_DATATYPE_F32) ((float*)C)[ci] = facc;
       else ((unsigned short*)C)[ci] = xb_f32_to_bf16_rne(facc);
     }
+  }
   }
 }
 
@@ -426,7 +439,8 @@ extern "C" int xb_packed_sp_launch(const xb_sparse_desc* d, const void* a, const
     const dim3 g2(gx < 1024 ? gx : 1024, grid);
     if (Q.is_f64) packed_csparse_kernel<double><<<g2, 256, 0, stream>>>(Q); else packed_csparse_kernel<float><<<g2, 256, 0, stream>>>(Q);
   } else {
-    if (Q.is_f64) packed_sp_kernel<double><<<grid, 256, 0, stream>>>(Q); else packed_sp_kernel<float><<<grid, 256, 0, stream>>>(Q);
+    const dim3 g2(1, grid);
+    if (Q.is_f64) packed_sp_kernel<double><<<g2, 256, 0, stream>>>(Q); else packed_sp_kernel<float><<<g2, 256, 0, stream>>>(Q);
   }
   return check_launch("packed_sp");
 }
@@ -450,6 +464,12 @@ extern "C" int xb_bcsc_launch(xb_sparse_desc* d, const void* a, const void* b_va
   if (Q.m_blocks <= 0 || n_blocks == 0) return 0;
   const long long work = Q.m_blocks * (long long)n_blocks;
   const unsigned int grid = (unsigned int)(work < (1 << 20) ? work : (1 << 20));
-  bcsc_simt_kernel<<<grid, 256, 0, (cudaStream_t)xb_rt_stream()>>>(Q);
+  cudaStream_t stream = (cudaStream_t)xb_rt_stream();
+  if (d->calls.count > 1) {
+    const dim3 g2(grid, (unsigned int)(d->calls.count < 65535 ? d->calls.count : 65535));
+    bcsc_simt_kernel<true><<<g2, 256, 0, stream>>>(Q, d->calls);
+  } else {
+    bcsc_simt_kernel<false><<<grid, 256, 0, stream>>>(Q, d->calls);
+  }
   return check_launch("bcsc_simt", LIBXSMM_B200_BACKEND_SIMT);
 }

@@ -55,6 +55,10 @@ typedef struct xb_meltw_desc {
   int t_in0, t_in1, t_in2, t_out, t_comp;
 } xb_meltw_desc;
 
+/* call axis of a strided batch of sparse calls (libxsmm_b200_spgemm_batch_strided): `count` calls, call t with A, the B values and C
+ * advanced by t times their byte strides; 0 or 1 is a single call. The pattern and everything else are shared by the calls. */
+typedef struct xb_sparse_calls { long long count, s_a, s_b, s_c; } xb_sparse_calls;
+
 /* sparse kernels: pattern lives in device memory owned by the slot */
 typedef struct xb_sparse_desc {
   int kind;                           /* XB_KIND_SP_* / BCSC / SREG */
@@ -72,6 +76,9 @@ typedef struct xb_sparse_desc {
   /* BCSC: per-(device, stream) scratch owned by the handle (pattern cache, re-packed B); created on first call, never
    * touched by the descriptor's readers (bcsc_tc.cu: BcscState) */
   void* work;
+  /* BCSC: zero in a handle; a batch hands xb_bcsc_launch a copy of the descriptor with its call axis here, so the handle itself
+   * is never written and stays re-entrant */
+  xb_sparse_calls calls;
 } xb_sparse_desc;
 
 typedef struct xb_slot {
