@@ -1,6 +1,6 @@
 # libxsmm_b200 -- build of the C-ABI library (host C + sm_90a CUDA) and of the test oracles.
 #   make lib      -> libxsmm_b200/lib/libxsmm_b200.so   (the product)
-#   make oracle   -> oracle/liboracle.so, liboracle_mx.so, liboracle_dq.so (C restatement, test infrastructure)
+#   make oracle   -> oracle/liboracle.so, liboracle_mx.so, liboracle_dq.so, liboracle_lowbit.so (C restatement, test infrastructure)
 #   make ref      -> oracle/_ref/libxsmm_ref.so         (the unmodified reference, header-only build;
 #                                                        only where /root/reference exists)
 NVCC      ?= /usr/local/cuda/bin/nvcc
@@ -34,7 +34,7 @@ $(LIB): $(OBJS)
 	$(NVCC) -shared $(ARCH) -cudart static -o $@ $(OBJS) -lpthread -ldl
 	ln -sf libxsmm_b200.so libxsmm_b200/lib/libxsmm.so
 
-oracle: oracle/liboracle.so oracle/liboracle_mx.so oracle/liboracle_dq.so
+oracle: oracle/liboracle.so oracle/liboracle_mx.so oracle/liboracle_dq.so oracle/liboracle_lowbit.so
 oracle/liboracle.so: oracle/oracle.c oracle/oracle_meltw.c
 	$(CC) -O2 -std=gnu99 -fPIC -shared -ffp-contract=off -fopenmp -Iinclude -o $@ oracle/oracle.c oracle/oracle_meltw.c -lm
 # the MX fp8 GEMM restatement uses liboracle.so's conversions
@@ -43,13 +43,16 @@ oracle/liboracle_mx.so: oracle/oracle_mx.c oracle/liboracle.so
 # the dequantising GEMM restatement too
 oracle/liboracle_dq.so: oracle/oracle_dq.c oracle/liboracle.so
 	$(CC) -O2 -std=gnu99 -fPIC -shared -ffp-contract=off -o $@ oracle/oracle_dq.c -Loracle -loracle -Wl,-rpath,'$$ORIGIN' -lm
+# and the low-bit weight GEMM restatement (bf16 rounding)
+oracle/liboracle_lowbit.so: oracle/oracle_lowbit.c oracle/liboracle.so
+	$(CC) -O2 -std=gnu99 -fPIC -shared -ffp-contract=off -o $@ oracle/oracle_lowbit.c -Loracle -loracle -Wl,-rpath,'$$ORIGIN' -lm
 
-ref: oracle/_ref/libxsmm_ref.so oracle/_ref/libxsmm_ref_mx.so oracle/_ref/libxsmm_ref_dq.so
-oracle/_ref/libxsmm_ref.so oracle/_ref/libxsmm_ref_mx.so oracle/_ref/libxsmm_ref_dq.so: oracle/_ref/libxsmm_ref%.so: oracle/ref%_shim.c
+ref: oracle/_ref/libxsmm_ref.so oracle/_ref/libxsmm_ref_mx.so oracle/_ref/libxsmm_ref_dq.so oracle/_ref/libxsmm_ref_lowbit.so
+oracle/_ref/libxsmm_ref.so oracle/_ref/libxsmm_ref_mx.so oracle/_ref/libxsmm_ref_dq.so oracle/_ref/libxsmm_ref_lowbit.so: oracle/_ref/libxsmm_ref%.so: oracle/ref%_shim.c
 	@mkdir -p oracle/_ref
 	@if [ -d $(REFDIR)/include ]; then \
 	  $(CC) -O2 -fPIC -shared -fvisibility=hidden -Wl,-Bsymbolic -fopenmp -ffp-contract=off -I$(REFDIR)/include -I$(REFDIR)/src -o $@ $< -lm -lpthread -ldl; \
 	else echo "reference tree not present: keeping prebuilt $@"; fi
 
 clean:
-	rm -rf build $(LIB) oracle/liboracle.so oracle/liboracle_mx.so oracle/liboracle_dq.so
+	rm -rf build $(LIB) oracle/liboracle.so oracle/liboracle_mx.so oracle/liboracle_dq.so oracle/liboracle_lowbit.so

@@ -75,7 +75,8 @@ LIBXSMM_API int libxsmm_b200_memcpy(void* dst, const void* src, size_t size); /*
  * bit mask (libxsmm_dispatch_brgemm_ext), VNNI-packed C, MX handles (their block scales travel per call: use
  * libxsmm_b200_gemm_batch_strided_scaled), and for the strided forms int8 -> f32 (the scale travels in c.tertiary of a call) and
  * a dequantising A with row scales (I8 x BF16, I8 / I4 / U4 x F16: use libxsmm_b200_gemm_batch_strided_scaled or
- * libxsmm_b200_gemm_batch; BF8 x F16 has no scales and batches in every form); nothing is launched and C is left untouched */
+ * libxsmm_b200_gemm_batch; BF8 x F16 has no scales and batches in every form) or MXFP4 x I8 (block scales: the same two forms; I2 / I1 x
+ * I8 / U8 have no scales and batch in every form); nothing is launched and C is left untouched */
 #define LIBXSMM_B200_ERROR_NOT_BATCHABLE (-6)
 LIBXSMM_API int libxsmm_b200_gemm_batch_strided(libxsmm_gemmfunction kernel,
   const void* a, const void* b, void* c, long long stride_a, long long stride_b, long long stride_c,
@@ -90,6 +91,8 @@ LIBXSMM_API int libxsmm_b200_gemm_batch_strided_multi(libxsmm_gemmfunction kerne
  * BYTES. Also I8 x BF16 and I8 x F16 handles (dequantising A): the m row scales of tile t are scf_a + t*stride_scf_a (f32 next to
  * a bf16 B, f16 next to an f16 B); stride 0 shares one set of scales, as a batch over one quantised weight does; scf_b / scf_c are
  * not read; -2 for address / offset batch-reduce. An int4 A also needs zero points per tile: use libxsmm_b200_gemm_batch.
+ * Also MXFP4 x I8 handles: A's E8M0 block scales of tile t are scf_a + t*stride_scf_a ([k/32][lda] bytes per block), B's f32 block
+ * scales scf_b + t*stride_scf_b ([n][ldb/32] floats per block); scf_c is not read; -2 for address / offset batch-reduce.
  * Every operand must be device-accessible (-4 for pageable host memory); -1 for a handle without per-call scales.
  * An MXBF8 C is quantised from an f32 image in device scratch: the batch then runs in chunks of at most 64 MiB of image and the
  * call returns after the device has finished. */
@@ -99,9 +102,10 @@ LIBXSMM_API int libxsmm_b200_gemm_batch_strided_scaled(libxsmm_gemmfunction kern
   unsigned long long br_count, long long count);
 /* general form: one reference argument struct per tile (address/offset batch-reduce modes, scale
  * factors...). All matrix pointers must be device-accessible. A dequantising A reads each tile's a.tertiary (row scales) and,
- * for I4 / U4, a.quaternary (f16 zero points); -1 if one is missing. */
+ * for I4 / U4, a.quaternary (f16 zero points); MXFP4 x I8 each tile's a.tertiary and b.tertiary (block scales; address mode: arrays
+ * of br pointers); -1 if one is missing. */
 LIBXSMM_API int libxsmm_b200_gemm_batch(libxsmm_gemmfunction kernel, const libxsmm_gemm_param* params, long long count);
-/* prepared form of the above: resolve and upload once, replay many times (NULL for handles with per-call row scales) */
+/* prepared form of the above: resolve and upload once, replay many times (NULL for handles with per-call row or block scales) */
 typedef struct libxsmm_b200_gemm_plan libxsmm_b200_gemm_plan;
 LIBXSMM_API libxsmm_b200_gemm_plan* libxsmm_b200_gemm_plan_create(libxsmm_gemmfunction kernel,
   const libxsmm_gemm_param* params, long long count);

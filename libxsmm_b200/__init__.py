@@ -23,7 +23,7 @@ _DT = ("F64 F32 BF16 F16 BF8 HF8 I64 U64 I32 U32 I16 U16 I8 U8 MXBF8 MXHF8 MXBF6
        "MXFP4X2 NVFP4X2 I2X4 I1X8 BF32 IMPLICIT UNSUPPORTED").split()
 for _i, _n in enumerate(_DT):
     globals()["DATATYPE_" + _n] = _i
-TYPESIZE = {0: 8, 1: 4, 2: 2, 3: 2, 4: 1, 5: 1, 6: 8, 7: 8, 8: 4, 9: 4, 10: 2, 11: 2, 12: 1, 13: 1, 14: 1, 15: 1, 18: 1, 19: 1, 24: 4}
+TYPESIZE = {0: 8, 1: 4, 2: 2, 3: 2, 4: 1, 5: 1, 6: 8, 7: 8, 8: 4, 9: 4, 10: 2, 11: 2, 12: 1, 13: 1, 14: 1, 15: 1, 18: 1, 19: 1, 20: 1, 22: 1, 23: 1, 24: 4}
 
 GEMM_FLAG_NONE = 0
 GEMM_FLAG_TRANS_A = 1
@@ -346,7 +346,8 @@ def call_gemm(kernel, a, b, c, br_count=None, a_aux=None, b_aux=None, scf=None, 
               a_scales=None, b_scales=None, c_scales=None, a_zero_points=None):
     """Invoke a GEMM-family handle like the reference drivers do (fill libxsmm_gemm_param, call).
     a_scales / b_scales / c_scales: the E8M0 block scales of an MX handle (a/b/c.tertiary); a_scales is also the m row scales of a
-    dequantising A (I8 x BF16: f32, I8 / I4 / U4 x F16: f16), and a_zero_points the m f16 zero points of an int4 A (a.quaternary)."""
+    dequantising A (I8 x BF16: f32, I8 / I4 / U4 x F16: f16), and a_zero_points the m f16 zero points of an int4 A (a.quaternary);
+    for MXFP4 x I8, a_scales / b_scales are A's E8M0 and B's f32 block scales."""
     p = GemmParam()
     keep = []
     if br_count is not None:

@@ -22,12 +22,15 @@
 
 namespace {
 
-enum { P_F64 = 0, P_F32, P_I16, P_I8_I32, P_I8_F32, P_F16_F16, P_F16_F32, P_BF16_F32, P_BF16_BF16, P_I4_I32, P_BITMAP, P_FP8, P_MX8, P_DQ, P_NONE };
+enum { P_F64 = 0, P_F32, P_I16, P_I8_I32, P_I8_F32, P_F16_F16, P_F16_F32, P_BF16_F32, P_BF16_BF16, P_I4_I32, P_BITMAP, P_FP8, P_MX8, P_DQ, P_NONE, P_LOWBIT };
 
 __host__ __device__ inline int xb_path_of(const xb_gemm_desc& d) {
   const int a = d.ta, b = d.tb, c = d.tc, comp = d.tcomp;
   const bool a8 = (a == LIBXSMM_DATATYPE_I8 || a == LIBXSMM_DATATYPE_U8);
   const bool b8 = (b == LIBXSMM_DATATYPE_I8 || b == LIBXSMM_DATATYPE_U8);
+  if (xb_lowbit_form(&d) != XB_LB_NONE) {   // I2 / I1 / MXFP4 A x 8-bit B (reference :1009-1272); the layout rules live in host_core.c
+    return (d.fuse_colbias == 0 && d.cp_op == 0 && (d.flags & LIBXSMM_GEMM_FLAG_DECOMPRESS_A_VIA_BITMASK) == 0) ? P_LOWBIT : P_NONE;
+  }
   if (a == LIBXSMM_DATATYPE_MXBF8 || a == LIBXSMM_DATATYPE_MXHF8) {   // MX fp8 (reference :2620-2679); the layout rules live in host_core.c
     const bool cok = (c == LIBXSMM_DATATYPE_F32) || (c == LIBXSMM_DATATYPE_MXBF8 && a == LIBXSMM_DATATYPE_MXBF8);
     return (b == a && comp == LIBXSMM_DATATYPE_F32 && cok && (d.br_type == 0 || d.br_type == 3) && d.fuse_colbias == 0 && d.cp_op == 0) ? P_MX8 : P_NONE;
@@ -787,6 +790,167 @@ cudaError_t launch_i8(const xb_gemm_launch& L, int path, int wpt, int words_per_
 #undef XB_I8_CASE
   return cudaGetLastError();
 }
+
+
+// ---- low-bit A x 8-bit B: ternary I2X4 / binary I1X8 x I8 / U8 -> I32, MXFP4X2 x I8 -> F32 / BF16 (reference :1009-1272) -------
+// Every product is a small integer times an 8-bit one: A is expanded to four int8 per word in registers and multiplied by four k of
+// B with dp4a (B unsigned for a U8 B). Integer sums wrap modulo 2^32 like the reference's int += and are exact in any order, so I2 / I1
+// need not follow the reference's loop order. MXFP4 keeps it where it matters: one exact int32 sum t per (element, r, 32-k block),
+// then acc += (t * sa) * sb over (r, block) from 0, and C = (beta0 ? 0 : C) + acc (F32) or bf16_rne(bf16(C or 0) + acc) (BF16).
+// A layouts (bytes; s = k/4, g = k/8, q = k%4):
+//   I2X4   A[s*lda + (i % (m/4))*4 + q], the 2-bit code of row i in bit pair i / (m/4); codes 0, 1, 2, 3 -> 0, +1, -1, -1 (:19-57)
+//   I1X8   A[s*lda/2 + i/2], bit q of the low nibble (even i) or of the high nibble (odd i); clear -> +1, set -> -1
+//   MXFP4  A[g*lda*4 + i*4 + q], low nibble k = 8g+q, high nibble k = 8g+q+4, widened by the integer table of :67 (not e2m1)
+// B is [n][ldb] bytes. MXFP4 scales: A's E8M0 bytes [k/32][lda] widened as s << 23, B's f32 [n][ldb/32]; block r of a batch-reduce
+// moves them as :200-236 does (address: arrays of br pointers; offset: + offs_a*2/32 bytes and + offs_b/32 floats; stride likewise).
+// One CTA per tile. A thread owns one row and LB_E consecutive columns, so each A word is expanded once and used LB_E times. B goes
+// through shared memory in panels of LB_NB columns x LB_KC k: the CTA reads B once per pass over its rows.
+constexpr int LB_E = 16, LB_KC = 128, LB_NB = 256, LB_THREADS = 256, LB_SW = LB_KC / 4 + 1;   // LB_SW: panel row stride in words
+
+__device__ __forceinline__ unsigned int lb_ld4(const unsigned char* p, bool aligned) {
+  if (aligned) return *reinterpret_cast<const unsigned int*>(p);
+  return (unsigned int)p[0] | ((unsigned int)p[1] << 8) | ((unsigned int)p[2] << 16) | ((unsigned int)p[3] << 24);
+}
+// byte q of w holds a 2-bit code in its low bits -> int8 0, +1, -1, -1 for codes 0, 1, 2, 3
+__device__ __forceinline__ unsigned int lb_expand_i2(unsigned int w) {
+  return (((w >> 1) & 0x01010101u) * 0xffu) | (w & 0x01010101u);
+}
+// bit q of x -> int8 +1 (clear) or -1 (set) in byte q
+__device__ __forceinline__ unsigned int lb_expand_i1(unsigned int x) {
+  const unsigned int w = (x & 1u) | ((x & 2u) << 7) | ((x & 4u) << 14) | ((x & 8u) << 21);
+  return 0x01010101u | (w * 0xfeu);
+}
+// byte q of w holds an fp4 code in its low nibble -> int8 of {0, 11, 21, 32, 42, 64, 85, 127}, negated when bit 3 is set
+__device__ __forceinline__ unsigned int lb_expand_fp4(unsigned int w) {
+  unsigned int sel = w & 0x07070707u;
+  sel = (sel | (sel >> 4)) & 0x00ff00ffu;
+  sel = (sel | (sel >> 8)) & 0x0000ffffu;                        // one prmt selector nibble per byte
+  const unsigned int mag = __byte_perm(0x20150b00u, 0x7f55402au, sel);
+  const unsigned int neg = ((w >> 3) & 0x01010101u) * 0xffu;
+  return (__vneg4(mag) & neg) | (mag & ~neg);
+}
+
+// MXFP4 scale bases of tile t; kept out of resolve_tile like resolve_scales
+__device__ inline void lb_scales(const xb_gemm_launch& L, long long t, const unsigned char*& as, const float*& bs) {
+  if (L.recs != nullptr) { as = (const unsigned char*)L.recs[t].a_s; bs = (const float*)L.recs[t].b_s; return; }
+  as = (const unsigned char*)L.one.a_s; bs = (const float*)L.one.b_s;
+  if (!(L.a == nullptr && L.c == nullptr)) { as += t * L.tile_stride_as; bs = (const float*)((const char*)bs + t * L.tile_stride_bs); }
+}
+
+template <int FORM, bool UB>
+__global__ void __launch_bounds__(LB_THREADS) gemm_lowbit_kernel(const xb_gemm_launch L) {
+  __shared__ unsigned int sb[LB_NB * LB_SW];
+  const xb_gemm_desc& d = L.d;
+  const int m = d.m, n = d.n, k = d.k, m4 = d.m / 4;
+  const long long lda = d.lda, ldb = d.ldb, ldc = d.ldc;
+  const bool beta0 = (d.flags & LIBXSMM_GEMM_FLAG_BETA_0) != 0;
+  for (long long t = blockIdx.x; t < L.count; t += gridDim.x) {
+    TileCtx x; resolve_tile(L, t, x);
+    const unsigned char* as = nullptr; const float* bs = nullptr;
+    if (FORM == XB_LB_MXFP4) lb_scales(L, t, as, bs);
+    for (int j0 = 0; j0 < n; j0 += LB_NB) {
+      const int nb = (n - j0 < LB_NB) ? n - j0 : LB_NB;
+      const int items = m * ((nb + LB_E - 1) / LB_E);
+      for (int w0 = 0; w0 < items; w0 += LB_THREADS) {
+        const int w = w0 + (int)threadIdx.x;
+        const bool live = w < items;
+        const int i = live ? w % m : 0, jg = live ? (w / m) * LB_E : 0;   // row; first column of the group within the panel
+        unsigned int acc[LB_E];                                          // I2 / I1: the sums; MXFP4: the block sums
+        float facc[LB_E];
+#pragma unroll
+        for (int p = 0; p < LB_E; ++p) { acc[p] = 0u; facc[p] = 0.0f; }
+        for (unsigned long long r = 0; r < x.br; ++r) {
+          const char *pa, *pb; br_ptrs(d, x, r, 1, 1, pa, pb);
+          const unsigned char* ua = (const unsigned char*)pa;
+          const unsigned char* psa = nullptr; const float* psb = nullptr;
+          if (FORM == XB_LB_MXFP4) {
+            switch (d.br_type) {
+              case 1: psa = ((const unsigned char* const*)as)[r]; psb = ((const float* const*)bs)[r]; break;
+              case 2: psa = as + (x.a_offs[r] * 2) / 32; psb = bs + x.b_offs[r] / 32; break;
+              case 3: psa = as + ((d.br_stride_a * 2) / 32) * (long long)r; psb = bs + (d.br_stride_b / 32) * (long long)r; break;
+              default: psa = as; psb = bs;
+            }
+          }
+          const bool b_al = (((uintptr_t)pb | (uintptr_t)ldb) & 3) == 0;
+          const bool a_al = (FORM == XB_LB_MXFP4) ? (((uintptr_t)ua & 3) == 0) : ((((uintptr_t)ua | (uintptr_t)lda) & 3) == 0);
+          for (int k0 = 0; k0 < k; k0 += LB_KC) {
+            const int kw = ((k - k0 < LB_KC) ? k - k0 : LB_KC) / 4;       // words of k in this panel
+            __syncthreads();                                              // the previous panel is consumed
+            for (int e = threadIdx.x; e < nb * kw; e += LB_THREADS) {
+              const int jj = e / kw, q = e - jj * kw;
+              sb[jj * LB_SW + q] = lb_ld4((const unsigned char*)pb + (long long)(j0 + jj) * ldb + k0 + 4 * q, b_al);
+            }
+            __syncthreads();
+            if (!live) continue;
+            const unsigned int* sbj = sb + jg * LB_SW;                    // columns past nb read stale words that are never stored
+            if (FORM == XB_LB_MXFP4) {
+              for (int bl = 0; bl < kw / 8; ++bl) {
+                const long long sblk = k0 / 32 + bl;
+#pragma unroll
+                for (int p = 0; p < LB_E; ++p) acc[p] = 0u;
+#pragma unroll
+                for (int g8 = 0; g8 < 4; ++g8) {
+                  const unsigned int word = lb_ld4(ua + (sblk * 4 + g8) * lda * 4 + (long long)i * 4, a_al);
+                  const unsigned int lo = lb_expand_fp4(word & 0x0f0f0f0fu), hi = lb_expand_fp4((word >> 4) & 0x0f0f0f0fu);
+                  const int qw = bl * 8 + g8 * 2;
+#pragma unroll
+                  for (int p = 0; p < LB_E; ++p) {
+                    acc[p] = dp4a_x<false, false>(lo, sbj[p * LB_SW + qw], acc[p]);
+                    acc[p] = dp4a_x<false, false>(hi, sbj[p * LB_SW + qw + 1], acc[p]);
+                  }
+                }
+                const float sa = mx_scale(psa[sblk * lda + i]);
+#pragma unroll
+                for (int p = 0; p < LB_E; ++p) {
+                  const int j = j0 + jg + p;
+                  if (j < n) facc[p] = __fadd_rn(facc[p], __fmul_rn(__fmul_rn((float)(int)acc[p], sa), psb[(long long)j * (ldb / 32) + sblk]));
+                }
+              }
+            } else {
+              for (int q = 0; q < kw; ++q) {
+                const long long s = k0 / 4 + q;
+                unsigned int av;
+                if (FORM == XB_LB_I2) av = lb_expand_i2((lb_ld4(ua + s * lda + (long long)(i % m4) * 4, a_al) >> (2 * (i / m4))) & 0x03030303u);
+                else av = lb_expand_i1((unsigned int)(ua[(s * lda) / 2 + i / 2] >> (4 * (i & 1))) & 0xfu);
+#pragma unroll
+                for (int p = 0; p < LB_E; ++p) acc[p] = dp4a_x<false, UB>(av, sbj[p * LB_SW + q], acc[p]);
+              }
+            }
+          }
+        }
+        if (!live) continue;
+#pragma unroll
+        for (int p = 0; p < LB_E; ++p) {
+          const int j = j0 + jg + p;
+          if (j >= n) break;
+          const long long ci = (long long)j * ldc + i;
+          if (FORM != XB_LB_MXFP4) {
+            unsigned int v = acc[p];
+            if (!beta0) v += (unsigned int)reinterpret_cast<const int*>(x.c)[ci];
+            reinterpret_cast<int*>(x.c)[ci] = (int)v;
+          } else if (d.tc == LIBXSMM_DATATYPE_F32) {
+            float* c = reinterpret_cast<float*>(x.c) + ci;
+            *c = __fadd_rn(beta0 ? 0.0f : *c, facc[p]);
+          } else {
+            unsigned short* c = reinterpret_cast<unsigned short*>(x.c) + ci;
+            *c = xb_f32_to_bf16_rne(__fadd_rn(beta0 ? 0.0f : xb_bf16_to_f32(*c), facc[p]));
+          }
+        }
+      }
+    }
+  }
+}
+
+cudaError_t launch_lowbit(const xb_gemm_launch& L, unsigned int grid, cudaStream_t st) {
+  const int form = xb_lowbit_form(&L.d);
+  const bool ub = (L.d.tb == LIBXSMM_DATATYPE_U8);
+  if (form == XB_LB_I2 && ub) gemm_lowbit_kernel<XB_LB_I2, true><<<grid, LB_THREADS, 0, st>>>(L);
+  else if (form == XB_LB_I2) gemm_lowbit_kernel<XB_LB_I2, false><<<grid, LB_THREADS, 0, st>>>(L);
+  else if (form == XB_LB_I1 && ub) gemm_lowbit_kernel<XB_LB_I1, true><<<grid, LB_THREADS, 0, st>>>(L);
+  else if (form == XB_LB_I1) gemm_lowbit_kernel<XB_LB_I1, false><<<grid, LB_THREADS, 0, st>>>(L);
+  else gemm_lowbit_kernel<XB_LB_MXFP4, false><<<grid, LB_THREADS, 0, st>>>(L);
+  return cudaGetLastError();
+}
 }  // namespace
 
 extern "C" int xb_gemm_simt_supported(const xb_gemm_desc* d) {
@@ -839,6 +1003,15 @@ extern "C" int xb_gemm_simt_launch(const xb_gemm_launch* L) {
     xb_rt_count_launch_backend(LIBXSMM_B200_BACKEND_SIMT);
     const cudaError_t qe = cudaGetLastError();
     if (qe != cudaSuccess) { xb_rt_note_error((int)qe, "gemm_dq"); return (int)qe; }
+    return 0;
+  }
+  if (path == P_LOWBIT) {
+    if (xb_lowbit_form(&L->d) == XB_LB_MXFP4 && L->recs == nullptr && (L->one.a_s == nullptr || L->one.b_s == nullptr)) {
+      xb_rt_note_error(1, "MXFP4 x I8: block scales missing (a.tertiary, b.tertiary)"); return 1;
+    }
+    const cudaError_t le = launch_lowbit(*L, (unsigned int)(L->count < (1 << 20) ? L->count : (1 << 20)), (cudaStream_t)xb_rt_stream());
+    xb_rt_count_launch_backend(LIBXSMM_B200_BACKEND_SIMT);
+    if (le != cudaSuccess) { xb_rt_note_error((int)le, "gemm_lowbit"); return (int)le; }
     return 0;
   }
   if (path == P_I4_I32 && L->one.a_q == nullptr && L->recs == nullptr) { xb_rt_note_error(1, "int4 A: zero points missing (a.quaternary)"); return 1; }

@@ -304,6 +304,33 @@ static int xb_dq_desc_ok(const xb_gemm_desc* d, int ext) {
   return 1;
 }
 
+/* a 2-bit or 1-bit A, or an MXFP4 A next to an 8-bit B: the low-bit weight tuples and their mis-typed neighbours (none of which
+ * dispatched before) */
+static int xb_is_lowbit_family(const xb_gemm_desc* d) {
+  return d->ta == LIBXSMM_DATATYPE_I2X4 || d->ta == LIBXSMM_DATATYPE_I1X8
+      || (d->ta == LIBXSMM_DATATYPE_MXFP4X2 && (d->tb == LIBXSMM_DATATYPE_I8 || d->tb == LIBXSMM_DATATYPE_U8));
+}
+
+/* low-bit A (xb_lowbit_form; reference src/generator_gemm_reference_impl.c:1009-1272, set-up :457-490, :560-620): 1 if the reference
+ * defines a result for the descriptor in the layout the flags ask for. As for xb_dq_desc_ok, a flag the reference would ignore is
+ * declined rather than obeyed. */
+static int xb_lowbit_desc_ok(const xb_gemm_desc* d, int ext) {
+  const int form = xb_lowbit_form(d);
+  const unsigned int vnni_intlv = LIBXSMM_GEMM_FLAG_VNNI_A | LIBXSMM_GEMM_FLAG_INTLV_A_FORMAT;
+  if (ext || form == XB_LB_NONE) return 0;                 /* no fused form; MXFP4 x U8 (see xb_lowbit_form), other comp / C types */
+  /* every branch reads A in its packed layout, B as [n][ldb] and C flat; bitmap A is the sparse branch (:857-948) */
+  if ((d->flags & (LIBXSMM_GEMM_FLAG_TRANS_A | LIBXSMM_GEMM_FLAG_TRANS_B | LIBXSMM_GEMM_FLAG_VNNI_B | LIBXSMM_GEMM_FLAG_VNNI_C
+                   | LIBXSMM_GEMM_FLAG_DECOMPRESS_A_VIA_BITMASK)) != 0) return 0;
+  if (d->ldb < d->k || d->lda < d->m) return 0;
+  if (form == XB_LB_I2) {   /* :482; rows past 4*(m/4) and k past 4*(k/4) would be left out */
+    return (d->flags & vnni_intlv) == vnni_intlv && (d->m % 4) == 0 && (d->k % 4) == 0;
+  }
+  if (form == XB_LB_I1) {   /* :486 ignores INTLV_A_FORMAT; rows come in pairs (:1204) and k in fours (:1211) */
+    return (d->flags & vnni_intlv) == LIBXSMM_GEMM_FLAG_VNNI_A && (d->m % 2) == 0 && (d->k % 4) == 0 && (d->lda % 2) == 0;
+  }
+  return (d->flags & vnni_intlv) == vnni_intlv && (d->k % 32) == 0;   /* MXFP4: :467, 32-k scale blocks */
+}
+
 static int xb_make_gemm_desc(xb_gemm_desc* d, const libxsmm_gemm_shape* shape, unsigned int flags, unsigned int prefetch,
                              const libxsmm_gemm_batch_reduce_config* br, int ext)
 {
@@ -331,6 +358,11 @@ static int xb_make_gemm_desc(xb_gemm_desc* d, const libxsmm_gemm_shape* shape, u
   }
   if (xb_is_dq_family(d)) {   /* dequantising A: its own layout rules, exact-order kernel only */
     if (!xb_dq_desc_ok(d, ext) || !xb_gemm_simt_supported(d)) return 0;
+    d->backend = LIBXSMM_B200_BACKEND_SIMT;
+    return 1;
+  }
+  if (xb_is_lowbit_family(d)) {   /* low-bit A x 8-bit B: its own layout rules, dp4a kernel on CUDA cores */
+    if (!xb_lowbit_desc_ok(d, ext) || !xb_gemm_simt_supported(d)) return 0;
     d->backend = LIBXSMM_B200_BACKEND_SIMT;
     return 1;
   }
@@ -434,6 +466,12 @@ static size_t xb_extent_a(const xb_gemm_desc* d) {   /* elements touched in one 
     if ((d->flags & LIBXSMM_GEMM_FLAG_VNNI_A) != 0) return (size_t)(d->k / 2 - 1) * d->lda * 2 + (size_t)d->m * 2;
     return (size_t)(d->k - 1) * d->lda + d->m;
   }
+  switch (xb_lowbit_form(d)) {                        /* bytes: I2 [k/4][lda], I1 [k/4][lda/2], MXFP4 [k/8][lda][4] */
+    case XB_LB_I2: return (size_t)(d->k / 4 - 1) * d->lda + (size_t)d->m;
+    case XB_LB_I1: return (size_t)(d->k / 4 - 1) * (d->lda / 2) + (size_t)(d->m / 2);
+    case XB_LB_MXFP4: return (size_t)(d->k / 8 - 1) * d->lda * 4 + (size_t)d->m * 4;
+    default: break;
+  }
   if (d->ta == LIBXSMM_DATATYPE_I4X2 || d->ta == LIBXSMM_DATATYPE_U4X2) return (size_t)(d->k / 8 - 1) * d->lda * 4 + (size_t)d->m * 4;   /* bytes: 8 k per 4 bytes */
   if (xb_is_mx8(d->ta)) return (size_t)(d->k / 4 - 1) * d->lda * 4 + (size_t)d->m * 4;                                                 /* VNNI4 */
   const int trans_a = (d->flags & LIBXSMM_GEMM_FLAG_TRANS_A) != 0, vnni_a = (d->flags & LIBXSMM_GEMM_FLAG_VNNI_A) != 0;
@@ -474,6 +512,23 @@ static const void* xb_stage_in(const void* p, size_t bytes, int* staged) {
     *staged = 1;
     return dptr;
   }
+}
+
+/* an address-mode array of br pointers to side data of `bytes` bytes each (MXFP4 block scales): a device array is used as given,
+ * a host-readable one is copied with each pointer made device-usable */
+static const void* xb_stage_ptr_array(const void* arr, unsigned long long br, size_t bytes, int* staged) {
+  const size_t nbytes = (size_t)(br ? br : 1) * sizeof(void*);
+  const void** h; void* dev; unsigned long long r;
+  if (arr == NULL || xb_rt_ptr_kind(arr) == 1) return arr;
+  h = (const void**)calloc(1, nbytes);
+  dev = xb_rt_scratch(nbytes);
+  if (h == NULL || dev == NULL) { free(h); return NULL; }
+  for (r = 0; r < br; ++r) h[r] = xb_stage_in(((const void* const*)arr)[r], bytes, staged);
+  xb_rt_upload(dev, h, nbytes);
+  xb_rt_sync();                      /* h is pageable: make sure the upload consumed it */
+  free(h);
+  *staged = 1;
+  return dev;
 }
 
 static int xb_run_gemm_launch(const xb_gemm_launch* L) {
@@ -545,6 +600,24 @@ static void xb_invoke_gemm(const xb_slot* s, const libxsmm_gemm_param* p) {
                                                                           * int4: a.quaternary, m f16 zero points. One set for every r. */
     L.one.a_s = xb_stage_in(p->a.tertiary, (size_t)d->m * (xb_dq_form(d) == XB_DQ_I8_BF16 ? 4 : 2), &staged);
     if (xb_dq_form(d) == XB_DQ_I4_F16) L.one.a_q = xb_stage_in(p->a.quaternary, (size_t)d->m * 2, &staged);
+  } else if (xb_lowbit_form(d) == XB_LB_MXFP4) {   /* a.tertiary: E8M0 bytes [k/32][lda]; b.tertiary: f32 [n][ldb/32]; block r's as in xb_gemm_simt */
+    const size_t ea = (size_t)(d->k / 32 - 1) * d->lda + (size_t)d->m, eb = ((size_t)(d->n - 1) * (size_t)(d->ldb / 32) + (size_t)(d->k / 32)) * 4;
+    if (d->br_type == 1) {
+      L.one.a_s = xb_stage_ptr_array(p->a.tertiary, br, ea, &staged);
+      L.one.b_s = xb_stage_ptr_array(p->b.tertiary, br, eb, &staged);
+    } else {
+      size_t span_sa = ea, span_sb = eb;
+      unsigned long long r;
+      if (d->br_type == 3 && br > 0) { span_sa += (size_t)(br - 1) * (size_t)((d->br_stride_a * 2) / 32); span_sb += (size_t)(br - 1) * (size_t)(d->br_stride_b / 32) * 4; }
+      if (d->br_type == 2) for (r = 0; r < br; ++r) {
+        const long long oa = (((const long long*)p->a.secondary)[r] * 2) / 32, ob = ((const long long*)p->b.secondary)[r] / 32;
+        if (oa > 0 && ea + (size_t)oa > span_sa) span_sa = ea + (size_t)oa;
+        if (ob > 0 && eb + (size_t)ob * 4 > span_sb) span_sb = eb + (size_t)ob * 4;
+      }
+      L.one.a_s = xb_stage_in(p->a.tertiary, span_sa, &staged);
+      L.one.b_s = xb_stage_in(p->b.tertiary, span_sb, &staged);
+    }
+    if (L.one.a_s == NULL || L.one.b_s == NULL) { xb_rt_note_error(2, "invoke_gemm: MXFP4 x I8 needs block scales in a.tertiary and b.tertiary"); xb_rt_scratch_reset(); return; }
   } else if (d->ta == LIBXSMM_DATATYPE_I4X2 || d->ta == LIBXSMM_DATATYPE_U4X2) {   /* a.quaternary: one zero-point byte per row (and per reduce step) */
     const size_t zb = (size_t)d->m + ((d->br_type == 3 && br > 0) ? (size_t)(br - 1) * (size_t)((d->br_stride_a * 2) / d->k) : 0);
     L.one.a_q = xb_stage_in(p->a.quaternary, zb, &staged);
@@ -692,12 +765,15 @@ static const xb_slot* xb_gemm_slot(const void* kernel) {
  * call only, the strided forms have no argument struct for the int8 -> f32 scale (c.tertiary), and no form but the scaled one carries
  * the MX block scales. The row scales of a dequantising A travel in the per-tile form and the scaled one (see xb_dq_scaled). */
 static int xb_dq_scaled(const xb_gemm_desc* d) { return xb_dq_form(d) != XB_DQ_NONE && xb_dq_form(d) != XB_DQ_BF8_F16; }
+/* MXFP4 x I8: A's and B's block scales (a.tertiary, b.tertiary) are per-call operands like the dequantising row scales; the I2 / I1
+ * forms carry none and batch in every form */
+static int xb_per_call_scales(const xb_gemm_desc* d) { return xb_dq_scaled(d) || xb_lowbit_form(d) == XB_LB_MXFP4; }
 
 static int xb_batch_refused(const xb_gemm_desc* d, int strided) {
   const int i8 = (d->ta == LIBXSMM_DATATYPE_I8 || d->ta == LIBXSMM_DATATYPE_U8);
   if (d->fuse_colbias != 0 || (d->flags & LIBXSMM_GEMM_FLAG_VNNI_C) != 0) return 1;
   if (xb_is_mx8(d->ta)) return 1;      /* MX block scales travel per call: libxsmm_b200_gemm_batch_strided_scaled */
-  if (strided && xb_dq_scaled(d)) return 1;   /* row scales: libxsmm_b200_gemm_batch_strided_scaled or libxsmm_b200_gemm_batch */
+  if (strided && xb_per_call_scales(d)) return 1;   /* row / block scales: libxsmm_b200_gemm_batch_strided_scaled or libxsmm_b200_gemm_batch */
   if (d->cp_op == LIBXSMM_MELTW_TYPE_UNARY_RELU && (d->cp_flags & LIBXSMM_MELTW_FLAG_UNARY_BITMASK_2BYTEMULT) != 0) return 1;
   return (strided && i8 && d->tc == LIBXSMM_DATATYPE_F32) ? 1 : 0;
 }
@@ -750,8 +826,21 @@ LIBXSMM_API int libxsmm_b200_gemm_batch_strided_scaled(libxsmm_gemmfunction kern
   if (s == NULL || count < 0 || s->kind != XB_KIND_GEMM) return -1;
   /* only MX handles and int8 dequantising ones take per-call scales here; int4 needs zero points as well: libxsmm_b200_gemm_batch */
   dq = xb_dq_form(&s->u.gemm);
-  if (!xb_is_mx8(s->u.gemm.ta) && dq != XB_DQ_I8_BF16 && dq != XB_DQ_I8_F16) return -1;
+  if (!xb_is_mx8(s->u.gemm.ta) && dq != XB_DQ_I8_BF16 && dq != XB_DQ_I8_F16 && xb_lowbit_form(&s->u.gemm) != XB_LB_MXFP4) return -1;
   if (count == 0) return 0;
+  if (xb_lowbit_form(&s->u.gemm) == XB_LB_MXFP4) {   /* block scales of tile t: scf_a + t*stride_scf_a (E8M0), scf_b + t*stride_scf_b (f32) */
+    if (a == NULL || b == NULL || c == NULL || scf_a == NULL || scf_b == NULL) return -1;
+    if (s->u.gemm.br_type == 1 || s->u.gemm.br_type == 2) return -2;   /* per-tile arrays: libxsmm_b200_gemm_batch */
+    if (xb_rt_ptr_kind(a) == 0 || xb_rt_ptr_kind(b) == 0 || xb_rt_ptr_kind(c) == 0 || xb_rt_ptr_kind(scf_a) == 0 || xb_rt_ptr_kind(scf_b) == 0) return -4;
+    memset(&L, 0, sizeof(L));
+    L.d = s->u.gemm; L.count = count; L.a = a; L.b = b; L.c = c;
+    L.tile_stride_a = stride_a; L.tile_stride_b = stride_b; L.tile_stride_c = stride_c;
+    L.one.a_s = scf_a; L.one.b_s = scf_b; L.tile_stride_as = stride_scf_a; L.tile_stride_bs = stride_scf_b;
+    L.br = (s->u.gemm.br_type == 0) ? 1ull : br_count;
+    rc = xb_run_gemm_launch(&L);
+    if (rc == 0 && xb_rt_blocking()) rc = xb_rt_sync();
+    return rc;
+  }
   if (dq != XB_DQ_NONE) {   /* row scales of tile t: scf_a + t*stride_scf_a (stride 0: shared weights' scales) */
     if (a == NULL || b == NULL || c == NULL || scf_a == NULL) return -1;
     if (s->u.gemm.br_type == 1 || s->u.gemm.br_type == 2) return -2;   /* per-tile arrays: libxsmm_b200_gemm_batch */
@@ -1005,10 +1094,15 @@ static libxsmm_b200_gemm_plan* xb_plan_make(const xb_slot* s, const libxsmm_gemm
   xb_gemm_rec* recs;
   char* arrays = NULL; size_t arrays_bytes = 0, off = 0;
   long long t;
+  int mx_arrays;
   if (s == NULL || params == NULL || count <= 0 || xb_batch_refused(&s->u.gemm, 0)) return NULL;
-  if (xb_dq_scaled(&s->u.gemm)) {   /* every tile brings its row scales (a.tertiary) and, for int4, zero points (a.quaternary) */
+  mx_arrays = (xb_lowbit_form(&s->u.gemm) == XB_LB_MXFP4);
+  if (xb_per_call_scales(&s->u.gemm)) {   /* every tile brings its row scales (a.tertiary) and, for int4, zero points (a.quaternary);
+                                           * MXFP4 x I8 its block scales (a.tertiary, b.tertiary) */
+    const int mxfp4 = (xb_lowbit_form(&s->u.gemm) == XB_LB_MXFP4);
     for (t = 0; t < count; ++t) {
-      if (params[t].a.tertiary == NULL || (xb_dq_form(&s->u.gemm) == XB_DQ_I4_F16 && params[t].a.quaternary == NULL)) return NULL;
+      if (params[t].a.tertiary == NULL || (xb_dq_form(&s->u.gemm) == XB_DQ_I4_F16 && params[t].a.quaternary == NULL)
+       || (mxfp4 && params[t].b.tertiary == NULL)) return NULL;
     }
   }
   plan = (libxsmm_b200_gemm_plan*)calloc(1, sizeof(*plan));
@@ -1020,6 +1114,10 @@ static libxsmm_b200_gemm_plan* xb_plan_make(const xb_slot* s, const libxsmm_gemm
     for (t = 0; t < count; ++t) {
       const unsigned long long br = *(const unsigned long long*)params[t].op.tertiary;
       if (xb_rt_ptr_kind(params[t].a.primary) != 1 || s->u.gemm.br_type == 2) arrays_bytes += 2 * (size_t)br * 8;
+      if (s->u.gemm.br_type == 1 && mx_arrays) {   /* MXFP4: the scale pointer arrays, copied alike */
+        if (xb_rt_ptr_kind(params[t].a.tertiary) != 1) arrays_bytes += (size_t)br * 8;
+        if (xb_rt_ptr_kind(params[t].b.tertiary) != 1) arrays_bytes += (size_t)br * 8;
+      }
     }
     if (arrays_bytes) {
       arrays = (char*)malloc(arrays_bytes);
@@ -1039,6 +1137,15 @@ static libxsmm_b200_gemm_plan* xb_plan_make(const xb_slot* s, const libxsmm_gemm
       memcpy(arrays + off, p->a.secondary, (size_t)r->br * 8); r->a_aux = (char*)plan->d_arrays + off; off += (size_t)r->br * 8;
       memcpy(arrays + off, p->b.secondary, (size_t)r->br * 8); r->b_aux = (char*)plan->d_arrays + off; off += (size_t)r->br * 8;
     }
+    if (mx_arrays) {   /* MXFP4 x I8: block scales; address mode: arrays of br pointers */
+      r->a_s = p->a.tertiary; r->b_s = p->b.tertiary;
+      if (s->u.gemm.br_type == 1 && xb_rt_ptr_kind(p->a.tertiary) != 1) {
+        memcpy(arrays + off, p->a.tertiary, (size_t)r->br * 8); r->a_s = (char*)plan->d_arrays + off; off += (size_t)r->br * 8;
+      }
+      if (s->u.gemm.br_type == 1 && xb_rt_ptr_kind(p->b.tertiary) != 1) {
+        memcpy(arrays + off, p->b.tertiary, (size_t)r->br * 8); r->b_s = (char*)plan->d_arrays + off; off += (size_t)r->br * 8;
+      }
+    }
     if (s->u.gemm.tc == LIBXSMM_DATATYPE_F32 && (s->u.gemm.ta == LIBXSMM_DATATYPE_I8 || s->u.gemm.ta == LIBXSMM_DATATYPE_U8)
         && p->c.tertiary != NULL) r->scf = *(const float*)p->c.tertiary;
     if (xb_dq_scaled(&s->u.gemm)) { r->a_s = p->a.tertiary; r->a_q = p->a.quaternary; }
@@ -1052,12 +1159,13 @@ static libxsmm_b200_gemm_plan* xb_plan_make(const xb_slot* s, const libxsmm_gemm
   return plan;
 }
 
-/* a plan is prepared once and replayed: the row scales of a dequantising A are per-call operands, so such a handle gets no plan */
+/* a plan is prepared once and replayed: the row scales of a dequantising A and the block scales of MXFP4 x I8 are per-call
+ * operands, so such a handle gets no plan */
 LIBXSMM_API libxsmm_b200_gemm_plan* libxsmm_b200_gemm_plan_create(libxsmm_gemmfunction kernel,
   const libxsmm_gemm_param* params, long long count)
 {
   const xb_slot* s = xb_gemm_slot((const void*)kernel);
-  if (s == NULL || xb_dq_scaled(&s->u.gemm)) return NULL;
+  if (s == NULL || xb_per_call_scales(&s->u.gemm)) return NULL;
   return xb_plan_make(s, params, count);
 }
 

@@ -103,7 +103,8 @@ typedef struct xb_gemm_rec {
   float scf;            /* I8 x I8 -> F32 scalar scale */
   int pad_;
   /* MXBF8 / MXHF8: E8M0 block scales, one byte per (row, 32 k); a.tertiary [br][k/32][lda], b.tertiary [br][k/32][ldb],
-   * and for an MXBF8 C c.tertiary [n][ldc/32]. Dequantising A (xb_dq_form): a_s holds the m row scales of a.tertiary. */
+   * and for an MXBF8 C c.tertiary [n][ldc/32]. Dequantising A (xb_dq_form): a_s holds the m row scales of a.tertiary. MXFP4 x I8
+   * (xb_lowbit_form): a_s the E8M0 bytes of a.tertiary, b_s the f32 scales of b.tertiary (address mode: device arrays of br pointers). */
   const void* a_s; const void* b_s; void* c_s;
 } xb_gemm_rec;
 
@@ -125,6 +126,24 @@ static inline int xb_dq_form(const xb_gemm_desc* d) {
   if (d->ta == LIBXSMM_DATATYPE_I4X2 || d->ta == LIBXSMM_DATATYPE_U4X2) return XB_DQ_I4_F16;             /* :1793-1880 */
   if (d->ta == LIBXSMM_DATATYPE_BF8) return XB_DQ_BF8_F16;                                               /* :1731-1792 */
   return XB_DQ_NONE;
+}
+
+/* low-bit weights x 8-bit activations with an int32 comp (reference src/generator_gemm_reference_impl.c:1009-1272): ternary I2X4 and
+ * binary I1X8 A next to an I8 or U8 B -> I32, and MXFP4X2 A (E8M0 block scales in a.tertiary) next to an I8 B (f32 block scales in
+ * b.tertiary) -> F32 or BF16. The form of a descriptor by its types, or 0. MXFP4 x U8 is not a form: the reference reads those bytes
+ * as signed char (:1011) under a B type it calls unsigned, so dispatch declines it. */
+enum { XB_LB_NONE = 0, XB_LB_I2, XB_LB_I1, XB_LB_MXFP4 };
+#if defined(__CUDACC__)
+__host__ __device__
+#endif
+static inline int xb_lowbit_form(const xb_gemm_desc* d) {
+  const int b8 = (d->tb == LIBXSMM_DATATYPE_I8 || d->tb == LIBXSMM_DATATYPE_U8);
+  if (d->tcomp != LIBXSMM_DATATYPE_I32) return XB_LB_NONE;
+  if (d->ta == LIBXSMM_DATATYPE_I2X4 && b8 && d->tc == LIBXSMM_DATATYPE_I32) return XB_LB_I2;                  /* :1089-1198 */
+  if (d->ta == LIBXSMM_DATATYPE_I1X8 && b8 && d->tc == LIBXSMM_DATATYPE_I32) return XB_LB_I1;                  /* :1199-1272 */
+  if (d->ta == LIBXSMM_DATATYPE_MXFP4X2 && d->tb == LIBXSMM_DATATYPE_I8
+      && (d->tc == LIBXSMM_DATATYPE_F32 || d->tc == LIBXSMM_DATATYPE_BF16)) return XB_LB_MXFP4;                    /* :1009-1088 */
+  return XB_LB_NONE;
 }
 
 /* launch description handed to the CUDA side */
