@@ -71,12 +71,21 @@ LIBXSMM_API int libxsmm_b200_memcpy(void* dst, const void* src, size_t size); /*
  *   A + t*stride_a, B + t*stride_b, C + t*stride_c          (strides in BYTES)
  * and, inside a tile, the handle's own batch-reduce addressing (stride mode: the dispatch-time
  * br_stride hints; br_count as given). Returns 0 on success. */
-/* returned by every batch form (and a NULL plan) for a handle a batch cannot run like a single call: a fused column bias or ReLU
- * bit mask (libxsmm_dispatch_brgemm_ext), VNNI-packed C, MX handles (their block scales travel per call: use
- * libxsmm_b200_gemm_batch_strided_scaled), and for the strided forms int8 -> f32 (the scale travels in c.tertiary of a call) and
- * a dequantising A with row scales (I8 x BF16, I8 / I4 / U4 x F16: use libxsmm_b200_gemm_batch_strided_scaled or
- * libxsmm_b200_gemm_batch; BF8 x F16 has no scales and batches in every form) or MXFP4 x I8 (block scales: the same two forms; I2 / I1 x
- * I8 / U8 have no scales and batch in every form); nothing is launched and C is left untouched */
+/* Side operands: besides A, B and C, a call of some handles reads
+ *   scales:      a.tertiary, b.tertiary, c.tertiary -- MXBF8 / MXHF8: E8M0 block scales of A and B, and of an MXBF8 C;
+ *                I8 x BF16, I8 / I4 / U4 x F16 (dequantising A): A's m row scales; MXFP4 x I8: A's E8M0 and B's f32 block scales
+ *   zero points: a.quaternary -- I4 / U4 x F16 (f16, one per row) and I4 / U4 x I8 / U8 -> I32 (one byte per row and reduce step)
+ * BF8 x F16 and I2 / I1 x I8 / U8 have none. Batch rules:
+ *   - libxsmm_b200_gemm_batch_strided and _multi take no side operands: such a handle is not batchable there.
+ *   - libxsmm_b200_gemm_batch_strided_scaled takes the scales of handles without zero points: scf_a, scf_b and scf_c stand for
+ *     a.tertiary, b.tertiary and c.tertiary of tile 0, and tile t's are scf_x + t*stride_scf_x (BYTES; stride 0 shares one set, as
+ *     a batch over one quantised weight does). It needs exactly the pointers the handle's scales name and reads no other.
+ *   - libxsmm_b200_gemm_batch reads each tile's side operands from its argument struct, MX handles excepted (not batchable).
+ *   - a plan (libxsmm_b200_gemm_plan_create) is NULL for a handle with side operands: they are per-call operands.
+ * LIBXSMM_B200_ERROR_NOT_BATCHABLE is returned by every batch form (and a NULL plan) for a handle a batch cannot run like a single
+ * call: a fused column bias or ReLU bit mask (libxsmm_dispatch_brgemm_ext), VNNI-packed C, side operands where the form takes none
+ * (see above), and for the strided forms int8 -> f32 (the scale travels in c.tertiary of a call); nothing is launched and C is left
+ * untouched */
 #define LIBXSMM_B200_ERROR_NOT_BATCHABLE (-6)
 LIBXSMM_API int libxsmm_b200_gemm_batch_strided(libxsmm_gemmfunction kernel,
   const void* a, const void* b, void* c, long long stride_a, long long stride_b, long long stride_c,
@@ -86,26 +95,19 @@ LIBXSMM_API int libxsmm_b200_gemm_batch_strided(libxsmm_gemmfunction kernel,
 LIBXSMM_API int libxsmm_b200_gemm_batch_strided_multi(libxsmm_gemmfunction kernel,
   const void* a, const void* b, void* c, long long stride_a, long long stride_b, long long stride_c,
   unsigned long long br_count, long long count, int ndevices);
-/* MX GEMM (MXBF8 / MXHF8 handles) over a strided batch: the E8M0 block scales of tile t are scf_a + t*stride_scf_a (a.tertiary
- * of a single call), scf_b + t*stride_scf_b (b.tertiary) and, for an MXBF8 C, scf_c + t*stride_scf_c (c.tertiary); strides in
- * BYTES. Also I8 x BF16 and I8 x F16 handles (dequantising A): the m row scales of tile t are scf_a + t*stride_scf_a (f32 next to
- * a bf16 B, f16 next to an f16 B); stride 0 shares one set of scales, as a batch over one quantised weight does; scf_b / scf_c are
- * not read; -2 for address / offset batch-reduce. An int4 A also needs zero points per tile: use libxsmm_b200_gemm_batch.
- * Also MXFP4 x I8 handles: A's E8M0 block scales of tile t are scf_a + t*stride_scf_a ([k/32][lda] bytes per block), B's f32 block
- * scales scf_b + t*stride_scf_b ([n][ldb/32] floats per block); scf_c is not read; -2 for address / offset batch-reduce.
- * Every operand must be device-accessible (-4 for pageable host memory); -1 for a handle without per-call scales.
- * An MXBF8 C is quantised from an f32 image in device scratch: the batch then runs in chunks of at most 64 MiB of image and the
- * call returns after the device has finished. */
+/* the strided batch of a handle with scales (see "Side operands" above). -1 for a handle without scales or with zero points, or a
+ * NULL operand or scale pointer the handle needs; -2 for address / offset batch-reduce (per-tile arrays: libxsmm_b200_gemm_batch);
+ * -4 if an operand or scale is pageable host memory (device-accessible only). An MXBF8 C is quantised from an f32 image in device
+ * scratch: the batch then runs in chunks of at most 64 MiB of image and the call returns after the device has finished. */
 LIBXSMM_API int libxsmm_b200_gemm_batch_strided_scaled(libxsmm_gemmfunction kernel,
   const void* a, const void* b, void* c, long long stride_a, long long stride_b, long long stride_c,
   const void* scf_a, const void* scf_b, void* scf_c, long long stride_scf_a, long long stride_scf_b, long long stride_scf_c,
   unsigned long long br_count, long long count);
 /* general form: one reference argument struct per tile (address/offset batch-reduce modes, scale
- * factors...). All matrix pointers must be device-accessible. A dequantising A reads each tile's a.tertiary (row scales) and,
- * for I4 / U4, a.quaternary (f16 zero points); MXFP4 x I8 each tile's a.tertiary and b.tertiary (block scales; address mode: arrays
- * of br pointers); -1 if one is missing. */
+ * factors, side operands; MXFP4 x I8 in address mode: arrays of br scale pointers). All matrix pointers must be device-accessible.
+ * -1 if a tile lacks a side operand of the handle. */
 LIBXSMM_API int libxsmm_b200_gemm_batch(libxsmm_gemmfunction kernel, const libxsmm_gemm_param* params, long long count);
-/* prepared form of the above: resolve and upload once, replay many times (NULL for handles with per-call row or block scales) */
+/* prepared form of the above: resolve and upload once, replay many times (NULL for handles with side operands) */
 typedef struct libxsmm_b200_gemm_plan libxsmm_b200_gemm_plan;
 LIBXSMM_API libxsmm_b200_gemm_plan* libxsmm_b200_gemm_plan_create(libxsmm_gemmfunction kernel,
   const libxsmm_gemm_param* params, long long count);

@@ -78,31 +78,17 @@ struct TileCtx {
   float scf;
   const void* colbias; unsigned char* relu_mask;          // fused form (libxsmm_dispatch_brgemm_ext)
   const unsigned char* a_q;                                // int4: zero points; bitmap-compressed A: the bitmap
-  const unsigned char* a_s; const unsigned char* b_s; unsigned char* c_s;   // MX fp8: E8M0 block scales
+  const unsigned char* a_s; const unsigned char* b_s; unsigned char* c_s;   // scales of A, B and C (xb_gemm_sides)
 };
 
 __device__ inline void resolve_tile(const xb_gemm_launch& L, long long t, TileCtx& x) {
-  xb_gemm_rec r;
-  if (L.recs != nullptr) r = L.recs[t];
-  else if (L.a == nullptr && L.c == nullptr) r = L.one;
-  else {
-    r.a = (const char*)L.a + t * L.tile_stride_a; r.b = (const char*)L.b + t * L.tile_stride_b;
-    r.c = (char*)L.c + t * L.tile_stride_c; r.a_aux = nullptr; r.b_aux = nullptr; r.br = L.br; r.scf = L.one.scf;
-    r.d = L.one.d; r.c_aux = nullptr;                      // a shared bias column; masks only exist per call
-    r.a_q = L.one.a_q;
-    if (L.d.br_type == 2) { r.a_aux = L.one.a_aux; r.b_aux = L.one.b_aux; }
-  }
+  const xb_gemm_rec r = xb_gemm_tile(&L, t);
   x.a0 = (const char*)r.a; x.b0 = (const char*)r.b; x.c = (char*)r.c;
   x.a_addr = (const void* const*)r.a; x.b_addr = (const void* const*)r.b;
   x.a_offs = (const long long*)r.a_aux; x.b_offs = (const long long*)r.b_aux;
   x.br = (L.d.br_type == 0) ? 1ull : r.br; x.scf = r.scf;
   x.colbias = r.d; x.relu_mask = (unsigned char*)r.c_aux; x.a_q = (const unsigned char*)r.a_q;
-}
-
-// MX fp8 block scales of tile t; kept out of resolve_tile, whose other callers would carry the extra registers
-__device__ inline void resolve_scales(const xb_gemm_launch& L, long long t, TileCtx& x) {
-  x.a_s = (const unsigned char*)L.one.a_s; x.b_s = (const unsigned char*)L.one.b_s; x.c_s = (unsigned char*)L.one.c_s;
-  if (!(L.a == nullptr && L.c == nullptr)) { x.a_s += t * L.tile_stride_as; x.b_s += t * L.tile_stride_bs; if (x.c_s != nullptr) x.c_s += t * L.tile_stride_cs; }
+  x.a_s = (const unsigned char*)r.a_s; x.b_s = (const unsigned char*)r.b_s; x.c_s = (unsigned char*)r.c_s;
 }
 
 // base pointers of the r-th batch-reduce operand pair; mirrors libxsmm_calculate_brgemm_offsets
@@ -501,7 +487,7 @@ __global__ void __launch_bounds__(256) gemm_mx8_kernel(const xb_gemm_launch L, f
   const long long ldc = d.ldc;
   const bool beta0 = (d.flags & LIBXSMM_GEMM_FLAG_BETA_0) != 0;
   for (long long t = blockIdx.x; t < L.count; t += gridDim.x) {
-    TileCtx x; resolve_tile(L, t, x); resolve_scales(L, t, x);
+    TileCtx x; resolve_tile(L, t, x);
     for (int e = threadIdx.x; e < m * n; e += blockDim.x) {
       const int i = e % m, j = e / m;
       const float acc = dot_mx8(d, x, i, j);
@@ -531,7 +517,7 @@ __global__ void __launch_bounds__(128) gemm_mx8_quant_kernel(const xb_gemm_launc
   if (e >= L.count * per_tile) return;
   const long long t = e / per_tile;
   const int j = (int)((e % per_tile) / bm), b = (int)(e % bm);
-  TileCtx x; resolve_tile(L, t, x); resolve_scales(L, t, x);
+  TileCtx x; resolve_tile(L, t, x);
   const float* src = img + (t * n + j) * (long long)m + b * 32;
   float v[32], amax = 0.0f;
 #pragma unroll
@@ -565,13 +551,6 @@ __global__ void __launch_bounds__(128) gemm_mx8_quant_kernel(const xb_gemm_launc
 // I8 / I4 A and an F16 B, where the old value is first rounded to f16 (:1871-1876, :2016-2021).
 __device__ __forceinline__ float dq_f16r(float v) { return xb_f16_to_f32(xb_f32_to_f16(v)); }
 
-// row scales of tile t; kept out of resolve_tile like resolve_scales (the zero points travel in TileCtx::a_q)
-__device__ inline const void* dq_scales(const xb_gemm_launch& L, long long t) {
-  if (L.recs != nullptr) return L.recs[t].a_s;
-  if (L.a == nullptr && L.c == nullptr) return L.one.a_s;
-  return (const char*)L.one.a_s + t * L.tile_stride_as;
-}
-
 __global__ void __launch_bounds__(256) gemm_dq_kernel(const xb_gemm_launch L) {
   const xb_gemm_desc& d = L.d;
   const int form = xb_dq_form(&d);
@@ -583,13 +562,12 @@ __global__ void __launch_bounds__(256) gemm_dq_kernel(const xb_gemm_launch L) {
   const int kb = (i4 || (form == XB_DQ_BF8_F16 && (d.flags & LIBXSMM_GEMM_FLAG_VNNI_A) != 0)) ? 2 : 1;
   for (long long t = blockIdx.x; t < L.count; t += gridDim.x) {
     TileCtx x; resolve_tile(L, t, x);
-    const void* scl = dq_scales(L, t);
     for (int e = threadIdx.x; e < m * n; e += blockDim.x) {
       const int i = e % m, j = e / m;
       const long long ci = (long long)j * ldc + i;
       float sc = 1.0f, zp = 0.0f;
-      if (b16) sc = reinterpret_cast<const float*>(scl)[i];
-      else if (form != XB_DQ_BF8_F16) sc = xb_f16_to_f32(reinterpret_cast<const unsigned short*>(scl)[i]);
+      if (b16) sc = reinterpret_cast<const float*>(x.a_s)[i];
+      else if (form != XB_DQ_BF8_F16) sc = xb_f16_to_f32(reinterpret_cast<const unsigned short*>(x.a_s)[i]);
       if (i4) zp = xb_f16_to_f32(reinterpret_cast<const unsigned short*>(x.a_q)[i]);
       float acc = 0.0f;
       for (unsigned long long r = 0; r < x.br; ++r) {
@@ -779,7 +757,7 @@ bool i8_fast_ok(const xb_gemm_launch& L, int path) {
 }
 
 template <int TM, int TN>
-cudaError_t launch_i8(const xb_gemm_launch& L, int path, int wpt, int words_per_group, size_t smem, unsigned int grid, cudaStream_t st) {
+void launch_i8(const xb_gemm_launch& L, int path, int wpt, int words_per_group, size_t smem, unsigned int grid, cudaStream_t st) {
   const bool ua = (L.d.ta == LIBXSMM_DATATYPE_U8), ub = (L.d.tb == LIBXSMM_DATATYPE_U8);
   const int to_f32 = (path == P_I8_F32);
 #define XB_I8_CASE(A, B) do { \
@@ -788,7 +766,6 @@ cudaError_t launch_i8(const xb_gemm_launch& L, int path, int wpt, int words_per_
     gemm_i8_kernel<TM, TN, A, B><<<grid, I8_WARPS * 32, smem, st>>>(L, to_f32, wpt, words_per_group); } while (0)
   if (ua && ub) XB_I8_CASE(true, true); else if (ua) XB_I8_CASE(true, false); else if (ub) XB_I8_CASE(false, true); else XB_I8_CASE(false, false);
 #undef XB_I8_CASE
-  return cudaGetLastError();
 }
 
 
@@ -830,13 +807,6 @@ __device__ __forceinline__ unsigned int lb_expand_fp4(unsigned int w) {
   return (__vneg4(mag) & neg) | (mag & ~neg);
 }
 
-// MXFP4 scale bases of tile t; kept out of resolve_tile like resolve_scales
-__device__ inline void lb_scales(const xb_gemm_launch& L, long long t, const unsigned char*& as, const float*& bs) {
-  if (L.recs != nullptr) { as = (const unsigned char*)L.recs[t].a_s; bs = (const float*)L.recs[t].b_s; return; }
-  as = (const unsigned char*)L.one.a_s; bs = (const float*)L.one.b_s;
-  if (!(L.a == nullptr && L.c == nullptr)) { as += t * L.tile_stride_as; bs = (const float*)((const char*)bs + t * L.tile_stride_bs); }
-}
-
 template <int FORM, bool UB>
 __global__ void __launch_bounds__(LB_THREADS) gemm_lowbit_kernel(const xb_gemm_launch L) {
   __shared__ unsigned int sb[LB_NB * LB_SW];
@@ -846,8 +816,7 @@ __global__ void __launch_bounds__(LB_THREADS) gemm_lowbit_kernel(const xb_gemm_l
   const bool beta0 = (d.flags & LIBXSMM_GEMM_FLAG_BETA_0) != 0;
   for (long long t = blockIdx.x; t < L.count; t += gridDim.x) {
     TileCtx x; resolve_tile(L, t, x);
-    const unsigned char* as = nullptr; const float* bs = nullptr;
-    if (FORM == XB_LB_MXFP4) lb_scales(L, t, as, bs);
+    const unsigned char* as = x.a_s; const float* bs = (const float*)x.b_s;   // MXFP4 block scales (address mode: arrays of br pointers)
     for (int j0 = 0; j0 < n; j0 += LB_NB) {
       const int nb = (n - j0 < LB_NB) ? n - j0 : LB_NB;
       const int items = m * ((nb + LB_E - 1) / LB_E);
@@ -941,7 +910,7 @@ __global__ void __launch_bounds__(LB_THREADS) gemm_lowbit_kernel(const xb_gemm_l
   }
 }
 
-cudaError_t launch_lowbit(const xb_gemm_launch& L, unsigned int grid, cudaStream_t st) {
+void launch_lowbit(const xb_gemm_launch& L, unsigned int grid, cudaStream_t st) {
   const int form = xb_lowbit_form(&L.d);
   const bool ub = (L.d.tb == LIBXSMM_DATATYPE_U8);
   if (form == XB_LB_I2 && ub) gemm_lowbit_kernel<XB_LB_I2, true><<<grid, LB_THREADS, 0, st>>>(L);
@@ -949,7 +918,14 @@ cudaError_t launch_lowbit(const xb_gemm_launch& L, unsigned int grid, cudaStream
   else if (form == XB_LB_I1 && ub) gemm_lowbit_kernel<XB_LB_I1, true><<<grid, LB_THREADS, 0, st>>>(L);
   else if (form == XB_LB_I1) gemm_lowbit_kernel<XB_LB_I1, false><<<grid, LB_THREADS, 0, st>>>(L);
   else gemm_lowbit_kernel<XB_LB_MXFP4, false><<<grid, LB_THREADS, 0, st>>>(L);
-  return cudaGetLastError();
+}
+
+// after a launch: counts it and notes a launch error
+int launched(const char* what) {
+  xb_rt_count_launch_backend(LIBXSMM_B200_BACKEND_SIMT);
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) { xb_rt_note_error((int)e, what); return (int)e; }
+  return 0;
 }
 }  // namespace
 
@@ -966,62 +942,39 @@ extern "C" int xb_gemm_simt_launch(const xb_gemm_launch* L) {
   const int path = xb_path_of(L->d);
   if (path == P_NONE) return 1;
   if (L->count <= 0) return 0;
+  if (L->recs == nullptr && xb_gemm_rec_lacks(&L->one, xb_gemm_sides(&L->d))) {
+    xb_rt_note_error(1, "GEMM: side operand missing (scales in a/b/c.tertiary, zero points in a.quaternary)"); return 1;
+  }
+  cudaStream_t st = (cudaStream_t)xb_rt_stream();
+  const unsigned int grid = (unsigned int)(L->count < (1 << 20) ? L->count : (1 << 20));   // one CTA per tile, grid-stride beyond
   if (path == P_BITMAP) {
     if (L->count != 1 || L->recs != nullptr || L->one.a_q == nullptr) { xb_rt_note_error(1, "bitmap-compressed A: single calls only"); return 1; }
     unsigned int* prefix = (unsigned int*)xb_rt_scratch((size_t)(((long long)L->d.m * L->d.k + 31) / 32) * 4 + 16);
     if (prefix == nullptr) return 2;
-    gemm_bitmap_kernel<<<1, 1024, 0, (cudaStream_t)xb_rt_stream()>>>(*L, prefix);
-    xb_rt_count_launch_backend(LIBXSMM_B200_BACKEND_SIMT);
-    const cudaError_t be = cudaGetLastError();
-    if (be != cudaSuccess) { xb_rt_note_error((int)be, "gemm_bitmap"); return (int)be; }
-    return 0;
+    gemm_bitmap_kernel<<<1, 1024, 0, st>>>(*L, prefix);
+    return launched("gemm_bitmap");
   }
   if (path == P_MX8) {
-    if (L->recs != nullptr || L->one.a_s == nullptr || L->one.b_s == nullptr || (L->d.tc == LIBXSMM_DATATYPE_MXBF8 && L->one.c_s == nullptr)) {
-      xb_rt_note_error(1, "MX fp8: block scales missing (a/b.tertiary, c.tertiary for an MXBF8 C)"); return 1;
-    }
     float* img = nullptr;                        // MXBF8 C: f32 image in the caller's scratch arena (reset after the sync)
     if (L->d.tc == LIBXSMM_DATATYPE_MXBF8 && nullptr == (img = (float*)xb_rt_scratch((size_t)L->count * L->d.m * L->d.n * 4))) return 2;
-    cudaStream_t st = (cudaStream_t)xb_rt_stream();
-    gemm_mx8_kernel<<<(unsigned int)(L->count < (1 << 20) ? L->count : (1 << 20)), 256, 0, st>>>(*L, img);
-    xb_rt_count_launch_backend(LIBXSMM_B200_BACKEND_SIMT);
-    if (img != nullptr) {
-      const long long blocks = L->count * L->d.n * (L->d.m / 32);
-      gemm_mx8_quant_kernel<<<(unsigned int)((blocks + 127) / 128), 128, 0, st>>>(*L, img);
-      xb_rt_count_launch_backend(LIBXSMM_B200_BACKEND_SIMT);
-    }
-    const cudaError_t me = cudaGetLastError();
-    if (me != cudaSuccess) { xb_rt_note_error((int)me, "gemm_mx8"); return (int)me; }
-    return 0;
+    gemm_mx8_kernel<<<grid, 256, 0, st>>>(*L, img);
+    const int rc = launched("gemm_mx8");
+    if (rc != 0 || img == nullptr) return rc;
+    const long long blocks = L->count * L->d.n * (L->d.m / 32);
+    gemm_mx8_quant_kernel<<<(unsigned int)((blocks + 127) / 128), 128, 0, st>>>(*L, img);
+    return launched("gemm_mx8_quant");
   }
   if (path == P_DQ) {
-    const int form = xb_dq_form(&L->d);
-    if (L->recs == nullptr && ((form != XB_DQ_BF8_F16 && L->one.a_s == nullptr) || (form == XB_DQ_I4_F16 && L->one.a_q == nullptr))) {
-      xb_rt_note_error(1, "dequantising A: row scales (a.tertiary) or int4 zero points (a.quaternary) missing"); return 1;
-    }
-    gemm_dq_kernel<<<(unsigned int)(L->count < (1 << 20) ? L->count : (1 << 20)), 256, 0, (cudaStream_t)xb_rt_stream()>>>(*L);
-    xb_rt_count_launch_backend(LIBXSMM_B200_BACKEND_SIMT);
-    const cudaError_t qe = cudaGetLastError();
-    if (qe != cudaSuccess) { xb_rt_note_error((int)qe, "gemm_dq"); return (int)qe; }
-    return 0;
+    gemm_dq_kernel<<<grid, 256, 0, st>>>(*L);
+    return launched("gemm_dq");
   }
   if (path == P_LOWBIT) {
-    if (xb_lowbit_form(&L->d) == XB_LB_MXFP4 && L->recs == nullptr && (L->one.a_s == nullptr || L->one.b_s == nullptr)) {
-      xb_rt_note_error(1, "MXFP4 x I8: block scales missing (a.tertiary, b.tertiary)"); return 1;
-    }
-    const cudaError_t le = launch_lowbit(*L, (unsigned int)(L->count < (1 << 20) ? L->count : (1 << 20)), (cudaStream_t)xb_rt_stream());
-    xb_rt_count_launch_backend(LIBXSMM_B200_BACKEND_SIMT);
-    if (le != cudaSuccess) { xb_rt_note_error((int)le, "gemm_lowbit"); return (int)le; }
-    return 0;
+    launch_lowbit(*L, grid, st);
+    return launched("gemm_lowbit");
   }
-  if (path == P_I4_I32 && L->one.a_q == nullptr && L->recs == nullptr) { xb_rt_note_error(1, "int4 A: zero points missing (a.quaternary)"); return 1; }
   if (L->d.fuse_colbias != 0 || L->d.cp_op != 0) {
-    const long long fgrid = L->count < (1 << 20) ? L->count : (1 << 20);
-    gemm_simt_fused_kernel<<<(unsigned int)fgrid, 256, 0, (cudaStream_t)xb_rt_stream()>>>(*L, path);
-    xb_rt_count_launch_backend(LIBXSMM_B200_BACKEND_SIMT);
-    const cudaError_t fe = cudaGetLastError();
-    if (fe != cudaSuccess) { xb_rt_note_error((int)fe, "gemm_simt_fused"); return (int)fe; }
-    return 0;
+    gemm_simt_fused_kernel<<<grid, 256, 0, st>>>(*L, path);
+    return launched("gemm_simt_fused");
   }
   if (i8_fast_ok(*L, path) && getenv("LIBXSMM_B200_I8_EXACT_ORDER") == nullptr) {
     const int small = (L->d.m < L->d.n) ? L->d.m : L->d.n;
@@ -1038,22 +991,14 @@ extern "C" int xb_gemm_simt_launch(const xb_gemm_launch* L) {
       if (sms == 0) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); if (sms <= 0) sms = 132; }
       const long long ctas_needed = (L->count + groups - 1) / groups;
       long long per_sm = (long long)((220 * 1024) / (smem + 1024)); if (per_sm < 1) per_sm = 1; if (per_sm > 2) per_sm = 2;   // 64 registers x 512 threads: two CTAs per SM
-      long long grid = (long long)sms * per_sm;
-      if (grid > ctas_needed) grid = ctas_needed;
-      cudaStream_t st = (cudaStream_t)xb_rt_stream();
-      cudaError_t e;
-      if (tm == 4) e = launch_i8<4, 8>(*L, path, wpt, words, smem, (unsigned int)grid, st);
-      else if (tm == 2) e = launch_i8<2, 4>(*L, path, wpt, words, smem, (unsigned int)grid, st);
-      else e = launch_i8<1, 2>(*L, path, wpt, words, smem, (unsigned int)grid, st);
-      xb_rt_count_launch_backend(LIBXSMM_B200_BACKEND_SIMT);
-      if (e != cudaSuccess) { xb_rt_note_error((int)e, "gemm_i8"); return (int)e; }
-      return 0;
+      long long i8_grid = (long long)sms * per_sm;
+      if (i8_grid > ctas_needed) i8_grid = ctas_needed;
+      if (tm == 4) launch_i8<4, 8>(*L, path, wpt, words, smem, (unsigned int)i8_grid, st);
+      else if (tm == 2) launch_i8<2, 4>(*L, path, wpt, words, smem, (unsigned int)i8_grid, st);
+      else launch_i8<1, 2>(*L, path, wpt, words, smem, (unsigned int)i8_grid, st);
+      return launched("gemm_i8");
     }
   }
-  const long long grid = L->count < (1 << 20) ? L->count : (1 << 20);
-  gemm_simt_kernel<<<(unsigned int)grid, 256, 0, (cudaStream_t)xb_rt_stream()>>>(*L, path);
-  xb_rt_count_launch_backend(LIBXSMM_B200_BACKEND_SIMT);
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) { xb_rt_note_error((int)e, "gemm_simt"); return (int)e; }
-  return 0;
+  gemm_simt_kernel<<<grid, 256, 0, st>>>(*L, path);
+  return launched("gemm_simt");
 }

@@ -531,6 +531,47 @@ static const void* xb_stage_ptr_array(const void* arr, unsigned long long br, si
   return dev;
 }
 
+/* stages the side operands xb_gemm_sides names for one call of br blocks into one->a_s, b_s, c_s and a_q (NULL where the call has none):
+ * the only code that knows their byte extents. An MXBF8 C's scales are written by the kernel: a pageable c.tertiary gets a device block
+ * that xb_invoke_gemm copies back. */
+static void xb_stage_sides(const xb_gemm_desc* d, const libxsmm_gemm_param* p, unsigned long long br, xb_gemm_rec* one, int* staged) {
+  const int sides = xb_gemm_sides(d);
+  if (sides == 0) return;
+  if (xb_dq_form(d) != XB_DQ_NONE) {   /* a.tertiary: m row scales (f32 next to a bf16 B, else f16); int4: a.quaternary, m f16 zero points.
+                                        * One set for every r. */
+    one->a_s = xb_stage_in(p->a.tertiary, (size_t)d->m * (xb_dq_form(d) == XB_DQ_I8_BF16 ? 4 : 2), staged);
+    if (sides & XB_SIDE_A_Q) one->a_q = xb_stage_in(p->a.quaternary, (size_t)d->m * 2, staged);
+  } else if (xb_lowbit_form(d) == XB_LB_MXFP4) {   /* a.tertiary: E8M0 bytes [k/32][lda]; b.tertiary: f32 [n][ldb/32]; block r's as in xb_gemm_simt */
+    const size_t ea = (size_t)(d->k / 32 - 1) * d->lda + (size_t)d->m, eb = ((size_t)(d->n - 1) * (size_t)(d->ldb / 32) + (size_t)(d->k / 32)) * 4;
+    if (d->br_type == 1) {
+      one->a_s = xb_stage_ptr_array(p->a.tertiary, br, ea, staged);
+      one->b_s = xb_stage_ptr_array(p->b.tertiary, br, eb, staged);
+    } else {
+      size_t span_sa = ea, span_sb = eb;
+      unsigned long long r;
+      if (d->br_type == 3 && br > 0) { span_sa += (size_t)(br - 1) * (size_t)((d->br_stride_a * 2) / 32); span_sb += (size_t)(br - 1) * (size_t)(d->br_stride_b / 32) * 4; }
+      if (d->br_type == 2) for (r = 0; r < br; ++r) {
+        const long long oa = (((const long long*)p->a.secondary)[r] * 2) / 32, ob = ((const long long*)p->b.secondary)[r] / 32;
+        if (oa > 0 && ea + (size_t)oa > span_sa) span_sa = ea + (size_t)oa;
+        if (ob > 0 && eb + (size_t)ob * 4 > span_sb) span_sb = eb + (size_t)ob * 4;
+      }
+      one->a_s = xb_stage_in(p->a.tertiary, span_sa, staged);
+      one->b_s = xb_stage_in(p->b.tertiary, span_sb, staged);
+    }
+  } else if (sides == XB_SIDE_A_Q) {   /* int4 A x 8-bit B: a.quaternary, one zero-point byte per row (and per reduce step) */
+    const size_t zb = (size_t)d->m + ((d->br_type == 3 && br > 0) ? (size_t)(br - 1) * (size_t)((d->br_stride_a * 2) / d->k) : 0);
+    one->a_q = xb_stage_in(p->a.quaternary, zb, staged);
+  } else {   /* MX fp8, E8M0 block scales: a.tertiary [br][k/32][lda], b.tertiary [br][k/32][ldb] and, for an MXBF8 C, c.tertiary [n][ldc/32] */
+    one->a_s = xb_stage_in(p->a.tertiary, xb_extent_mx_scales(d, br, d->lda, d->m), staged);
+    one->b_s = xb_stage_in(p->b.tertiary, xb_extent_mx_scales(d, br, d->ldb, d->n), staged);
+    if (sides & XB_SIDE_C_S) {
+      *staged = 1;                     /* the f32 image lives in the scratch arena until the caller's sync */
+      one->c_s = (p->c.tertiary != NULL && xb_rt_ptr_kind(p->c.tertiary) == 0) ? xb_rt_scratch((size_t)(d->n - 1) * (d->ldc / 32) + (size_t)(d->m / 32))
+                                                                               : p->c.tertiary;
+    }
+  }
+}
+
 static int xb_run_gemm_launch(const xb_gemm_launch* L) {
   if (L->d.backend != LIBXSMM_B200_BACKEND_TCGEN05) return xb_gemm_simt_launch(L);
   return xb_gemm_ts_supported(&L->d) ? xb_gemm_ts_launch(L) : xb_gemm_tc_launch(L);
@@ -544,7 +585,8 @@ static void xb_invoke_gemm(const xb_slot* s, const libxsmm_gemm_param* p) {
   const size_t ext_a = xb_extent_a(d) * tsa, ext_b = xb_extent_b(d) * tsb, ext_c = (vnni_c ? (size_t)d->n * d->ldc : ((size_t)(d->n - 1) * d->ldc + d->m)) * tsc;
   const unsigned long long br = (d->br_type != 0 && p->op.tertiary != NULL) ? *(const unsigned long long*)p->op.tertiary : 1ull;
   xb_gemm_launch L;
-  xb_copyback cb, cb_mask; int staged = 0, need_cb = 0, need_cb_mask = 0, need_cb_scf = 0;
+  const int sides = xb_gemm_sides(d);
+  xb_copyback cb, cb_mask; int staged = 0, need_cb = 0, need_cb_mask = 0;
   memset(&L, 0, sizeof(L)); memset(&cb, 0, sizeof(cb)); memset(&cb_mask, 0, sizeof(cb_mask));
   L.d = *d; L.count = 1;
   L.one.br = br;
@@ -596,32 +638,9 @@ static void xb_invoke_gemm(const xb_slot* s, const libxsmm_gemm_param* p) {
     L.one.a = xb_stage_in(p->a.primary, span_a ? span_a : 1, &staged);
     L.one.b = xb_stage_in(p->b.primary, span_b, &staged);
   }
-  if (xb_dq_form(d) != XB_DQ_NONE && xb_dq_form(d) != XB_DQ_BF8_F16) {   /* a.tertiary: m row scales (f32 next to a bf16 B, else f16);
-                                                                          * int4: a.quaternary, m f16 zero points. One set for every r. */
-    L.one.a_s = xb_stage_in(p->a.tertiary, (size_t)d->m * (xb_dq_form(d) == XB_DQ_I8_BF16 ? 4 : 2), &staged);
-    if (xb_dq_form(d) == XB_DQ_I4_F16) L.one.a_q = xb_stage_in(p->a.quaternary, (size_t)d->m * 2, &staged);
-  } else if (xb_lowbit_form(d) == XB_LB_MXFP4) {   /* a.tertiary: E8M0 bytes [k/32][lda]; b.tertiary: f32 [n][ldb/32]; block r's as in xb_gemm_simt */
-    const size_t ea = (size_t)(d->k / 32 - 1) * d->lda + (size_t)d->m, eb = ((size_t)(d->n - 1) * (size_t)(d->ldb / 32) + (size_t)(d->k / 32)) * 4;
-    if (d->br_type == 1) {
-      L.one.a_s = xb_stage_ptr_array(p->a.tertiary, br, ea, &staged);
-      L.one.b_s = xb_stage_ptr_array(p->b.tertiary, br, eb, &staged);
-    } else {
-      size_t span_sa = ea, span_sb = eb;
-      unsigned long long r;
-      if (d->br_type == 3 && br > 0) { span_sa += (size_t)(br - 1) * (size_t)((d->br_stride_a * 2) / 32); span_sb += (size_t)(br - 1) * (size_t)(d->br_stride_b / 32) * 4; }
-      if (d->br_type == 2) for (r = 0; r < br; ++r) {
-        const long long oa = (((const long long*)p->a.secondary)[r] * 2) / 32, ob = ((const long long*)p->b.secondary)[r] / 32;
-        if (oa > 0 && ea + (size_t)oa > span_sa) span_sa = ea + (size_t)oa;
-        if (ob > 0 && eb + (size_t)ob * 4 > span_sb) span_sb = eb + (size_t)ob * 4;
-      }
-      L.one.a_s = xb_stage_in(p->a.tertiary, span_sa, &staged);
-      L.one.b_s = xb_stage_in(p->b.tertiary, span_sb, &staged);
-    }
-    if (L.one.a_s == NULL || L.one.b_s == NULL) { xb_rt_note_error(2, "invoke_gemm: MXFP4 x I8 needs block scales in a.tertiary and b.tertiary"); xb_rt_scratch_reset(); return; }
-  } else if (d->ta == LIBXSMM_DATATYPE_I4X2 || d->ta == LIBXSMM_DATATYPE_U4X2) {   /* a.quaternary: one zero-point byte per row (and per reduce step) */
-    const size_t zb = (size_t)d->m + ((d->br_type == 3 && br > 0) ? (size_t)(br - 1) * (size_t)((d->br_stride_a * 2) / d->k) : 0);
-    L.one.a_q = xb_stage_in(p->a.quaternary, zb, &staged);
-    if (L.one.a_q == NULL) { xb_rt_note_error(2, "invoke_gemm: int4 A needs zero points in a.quaternary"); xb_rt_scratch_reset(); return; }
+  xb_stage_sides(d, p, br, &L.one, &staged);
+  if (xb_gemm_rec_lacks(&L.one, sides)) {
+    xb_rt_note_error(1, "invoke_gemm: side operand missing (scales in a/b/c.tertiary, zero points in a.quaternary)"); xb_rt_scratch_reset(); return;
   }
   /* C: staged copy is seeded from the host whenever old contents can survive (beta=1 or ldc>m) */
   if (p->c.primary != NULL && xb_rt_ptr_kind(p->c.primary) == 0) {
@@ -633,18 +652,6 @@ static void xb_invoke_gemm(const xb_slot* s, const libxsmm_gemm_param* p) {
   } else L.one.c = p->c.primary;
   if (d->tc == LIBXSMM_DATATYPE_F32 && (d->ta == LIBXSMM_DATATYPE_I8 || d->ta == LIBXSMM_DATATYPE_U8) && p->c.tertiary != NULL) {
     L.one.scf = *(const float*)p->c.tertiary;
-  }
-  if (xb_is_mx8(d->ta)) {   /* E8M0 block scales: a.tertiary, b.tertiary and, for an MXBF8 C, c.tertiary [n][ldc/32] */
-    L.one.a_s = xb_stage_in(p->a.tertiary, xb_extent_mx_scales(d, br, d->lda, d->m), &staged);
-    L.one.b_s = xb_stage_in(p->b.tertiary, xb_extent_mx_scales(d, br, d->ldb, d->n), &staged);
-    if (d->tc == LIBXSMM_DATATYPE_MXBF8) {
-      staged = 1;                      /* the f32 image lives in the scratch arena until the sync below */
-      if (p->c.tertiary != NULL && xb_rt_ptr_kind(p->c.tertiary) == 0) {
-        L.one.c_s = xb_rt_scratch((size_t)(d->n - 1) * (d->ldc / 32) + (size_t)(d->m / 32));
-        if (L.one.c_s == NULL) { xb_rt_scratch_reset(); return; }
-        need_cb_scf = 1;
-      } else L.one.c_s = p->c.tertiary;
-    }
   }
   if (s->kind == XB_KIND_GEMM_EXT && (d->fuse_colbias != 0 || d->cp_op != 0)) {   /* d.primary: bias column; c.secondary: ReLU bitmask */
     const libxsmm_gemm_ext_param* pe = (const libxsmm_gemm_ext_param*)p;
@@ -683,7 +690,7 @@ static void xb_invoke_gemm(const xb_slot* s, const libxsmm_gemm_param* p) {
     else xb_rt_memcpy2d_async(cb.host, cb.dev, (size_t)d->ldc * tsc, (size_t)d->m * tsc, (size_t)d->n);
   }
   if (need_cb_mask) xb_rt_memcpy_async(cb_mask.host, cb_mask.dev, cb_mask.bytes);
-  if (need_cb_scf) xb_rt_memcpy2d_async(p->c.tertiary, L.one.c_s, (size_t)(d->ldc / 32), (size_t)(d->m / 32), (size_t)d->n);   /* the m/32 scale bytes of each column */
+  if ((sides & XB_SIDE_C_S) && L.one.c_s != p->c.tertiary) xb_rt_memcpy2d_async(p->c.tertiary, L.one.c_s, (size_t)(d->ldc / 32), (size_t)(d->m / 32), (size_t)d->n);   /* the m/32 scale bytes of each column */
   if (staged || xb_rt_blocking()) { xb_rt_sync(); xb_rt_scratch_reset(); }
 }
 
@@ -762,18 +769,12 @@ static const xb_slot* xb_gemm_slot(const void* kernel) {
 
 /* 1 if a batch entry point cannot run this handle as a single call would: a fused handle's bias column and ReLU bit mask are
  * per-call operands (libxsmm_gemm_ext_param) that no batch form carries, VNNI-packed C is re-packed by a pass after a single
- * call only, the strided forms have no argument struct for the int8 -> f32 scale (c.tertiary), and no form but the scaled one carries
- * the MX block scales. The row scales of a dequantising A travel in the per-tile form and the scaled one (see xb_dq_scaled). */
-static int xb_dq_scaled(const xb_gemm_desc* d) { return xb_dq_form(d) != XB_DQ_NONE && xb_dq_form(d) != XB_DQ_BF8_F16; }
-/* MXFP4 x I8: A's and B's block scales (a.tertiary, b.tertiary) are per-call operands like the dequantising row scales; the I2 / I1
- * forms carry none and batch in every form */
-static int xb_per_call_scales(const xb_gemm_desc* d) { return xb_dq_scaled(d) || xb_lowbit_form(d) == XB_LB_MXFP4; }
-
+ * call only, the strided forms have no argument struct for the int8 -> f32 scale (c.tertiary) or for side operands
+ * (xb_gemm_sides: libxsmm_b200_gemm_batch_strided_scaled takes scales), and the per-tile records carry no MX fp8 block scales. */
 static int xb_batch_refused(const xb_gemm_desc* d, int strided) {
   const int i8 = (d->ta == LIBXSMM_DATATYPE_I8 || d->ta == LIBXSMM_DATATYPE_U8);
   if (d->fuse_colbias != 0 || (d->flags & LIBXSMM_GEMM_FLAG_VNNI_C) != 0) return 1;
-  if (xb_is_mx8(d->ta)) return 1;      /* MX block scales travel per call: libxsmm_b200_gemm_batch_strided_scaled */
-  if (strided && xb_per_call_scales(d)) return 1;   /* row / block scales: libxsmm_b200_gemm_batch_strided_scaled or libxsmm_b200_gemm_batch */
+  if (strided ? xb_gemm_sides(d) != 0 : xb_is_mx8(d->ta)) return 1;
   if (d->cp_op == LIBXSMM_MELTW_TYPE_UNARY_RELU && (d->cp_flags & LIBXSMM_MELTW_FLAG_UNARY_BITMASK_2BYTEMULT) != 0) return 1;
   return (strided && i8 && d->tc == LIBXSMM_DATATYPE_F32) ? 1 : 0;
 }
@@ -822,51 +823,25 @@ LIBXSMM_API int libxsmm_b200_gemm_batch_strided_scaled(libxsmm_gemmfunction kern
 {
   const xb_slot* s = xb_gemm_slot((const void*)kernel);
   xb_gemm_launch L;
-  int rc, dq;
+  int rc, sides;
   if (s == NULL || count < 0 || s->kind != XB_KIND_GEMM) return -1;
-  /* only MX handles and int8 dequantising ones take per-call scales here; int4 needs zero points as well: libxsmm_b200_gemm_batch */
-  dq = xb_dq_form(&s->u.gemm);
-  if (!xb_is_mx8(s->u.gemm.ta) && dq != XB_DQ_I8_BF16 && dq != XB_DQ_I8_F16 && xb_lowbit_form(&s->u.gemm) != XB_LB_MXFP4) return -1;
+  /* handles with scales and no zero points (those need libxsmm_b200_gemm_batch); tile t's are scf_x + t*stride_scf_x */
+  sides = xb_gemm_sides(&s->u.gemm);
+  if (sides == 0 || (sides & XB_SIDE_A_Q) != 0) return -1;
   if (count == 0) return 0;
-  if (xb_lowbit_form(&s->u.gemm) == XB_LB_MXFP4) {   /* block scales of tile t: scf_a + t*stride_scf_a (E8M0), scf_b + t*stride_scf_b (f32) */
-    if (a == NULL || b == NULL || c == NULL || scf_a == NULL || scf_b == NULL) return -1;
-    if (s->u.gemm.br_type == 1 || s->u.gemm.br_type == 2) return -2;   /* per-tile arrays: libxsmm_b200_gemm_batch */
-    if (xb_rt_ptr_kind(a) == 0 || xb_rt_ptr_kind(b) == 0 || xb_rt_ptr_kind(c) == 0 || xb_rt_ptr_kind(scf_a) == 0 || xb_rt_ptr_kind(scf_b) == 0) return -4;
-    memset(&L, 0, sizeof(L));
-    L.d = s->u.gemm; L.count = count; L.a = a; L.b = b; L.c = c;
-    L.tile_stride_a = stride_a; L.tile_stride_b = stride_b; L.tile_stride_c = stride_c;
-    L.one.a_s = scf_a; L.one.b_s = scf_b; L.tile_stride_as = stride_scf_a; L.tile_stride_bs = stride_scf_b;
-    L.br = (s->u.gemm.br_type == 0) ? 1ull : br_count;
-    rc = xb_run_gemm_launch(&L);
-    if (rc == 0 && xb_rt_blocking()) rc = xb_rt_sync();
-    return rc;
-  }
-  if (dq != XB_DQ_NONE) {   /* row scales of tile t: scf_a + t*stride_scf_a (stride 0: shared weights' scales) */
-    if (a == NULL || b == NULL || c == NULL || scf_a == NULL) return -1;
-    if (s->u.gemm.br_type == 1 || s->u.gemm.br_type == 2) return -2;   /* per-tile arrays: libxsmm_b200_gemm_batch */
-    if (xb_rt_ptr_kind(a) == 0 || xb_rt_ptr_kind(b) == 0 || xb_rt_ptr_kind(c) == 0 || xb_rt_ptr_kind(scf_a) == 0) return -4;
-    memset(&L, 0, sizeof(L));
-    L.d = s->u.gemm; L.count = count; L.a = a; L.b = b; L.c = c;
-    L.tile_stride_a = stride_a; L.tile_stride_b = stride_b; L.tile_stride_c = stride_c;
-    L.one.a_s = scf_a; L.tile_stride_as = stride_scf_a;
-    L.br = (s->u.gemm.br_type == 0) ? 1ull : br_count;
-    rc = xb_run_gemm_launch(&L);
-    if (rc == 0 && xb_rt_blocking()) rc = xb_rt_sync();
-    return rc;
-  }
-  {
-    const int mx_c = (s->u.gemm.tc == LIBXSMM_DATATYPE_MXBF8);
-    if (a == NULL || b == NULL || c == NULL || scf_a == NULL || scf_b == NULL || (mx_c && scf_c == NULL)) return -1;
-    if (xb_rt_ptr_kind(a) == 0 || xb_rt_ptr_kind(b) == 0 || xb_rt_ptr_kind(c) == 0 || xb_rt_ptr_kind(scf_a) == 0
-     || xb_rt_ptr_kind(scf_b) == 0 || (mx_c && xb_rt_ptr_kind(scf_c) == 0)) return -4;               /* device-accessible operands only */
-  }
   memset(&L, 0, sizeof(L));
   L.d = s->u.gemm;
   L.tile_stride_a = stride_a; L.tile_stride_b = stride_b; L.tile_stride_c = stride_c;
-  L.tile_stride_as = stride_scf_a; L.tile_stride_bs = stride_scf_b; L.tile_stride_cs = stride_scf_c;
-  L.br = (s->u.gemm.br_type == 0) ? 1ull : br_count;
-  if (L.d.tc != LIBXSMM_DATATYPE_MXBF8) {
-    L.count = count; L.a = a; L.b = b; L.c = c; L.one.a_s = scf_a; L.one.b_s = scf_b;
+  L.br = (L.d.br_type == 0) ? 1ull : br_count;
+  if (sides & XB_SIDE_A_S) { L.one.a_s = scf_a; L.tile_stride_as = stride_scf_a; }
+  if (sides & XB_SIDE_B_S) { L.one.b_s = scf_b; L.tile_stride_bs = stride_scf_b; }
+  if (sides & XB_SIDE_C_S) { L.one.c_s = scf_c; L.tile_stride_cs = stride_scf_c; }
+  if (a == NULL || b == NULL || c == NULL || xb_gemm_rec_lacks(&L.one, sides)) return -1;
+  if (L.d.br_type == 1 || L.d.br_type == 2) return -2;   /* per-tile arrays: libxsmm_b200_gemm_batch */
+  if (xb_rt_ptr_kind(a) == 0 || xb_rt_ptr_kind(b) == 0 || xb_rt_ptr_kind(c) == 0 || (L.one.a_s != NULL && xb_rt_ptr_kind(L.one.a_s) == 0)
+   || (L.one.b_s != NULL && xb_rt_ptr_kind(L.one.b_s) == 0) || (L.one.c_s != NULL && xb_rt_ptr_kind(L.one.c_s) == 0)) return -4;   /* device-accessible operands only */
+  if ((sides & XB_SIDE_C_S) == 0) {
+    L.count = count; L.a = a; L.b = b; L.c = c;
     rc = xb_run_gemm_launch(&L);
     if (rc == 0 && xb_rt_blocking()) rc = xb_rt_sync();
     return rc;
@@ -1088,22 +1063,29 @@ static int xb_plan_try_pool(libxsmm_b200_gemm_plan* plan, const xb_slot* s, cons
   return 1;
 }
 
+/* the side operands `sides` names in one call's argument struct, into the record fields the kernels read */
+static void xb_param_sides(xb_gemm_rec* r, const libxsmm_gemm_param* p, int sides) {
+  if (sides & XB_SIDE_A_S) r->a_s = p->a.tertiary;
+  if (sides & XB_SIDE_B_S) r->b_s = p->b.tertiary;
+  if (sides & XB_SIDE_C_S) r->c_s = p->c.tertiary;
+  if (sides & XB_SIDE_A_Q) r->a_q = p->a.quaternary;
+}
+
 /* the per-tile records of a batch: libxsmm_b200_gemm_batch and libxsmm_b200_gemm_plan_create */
 static libxsmm_b200_gemm_plan* xb_plan_make(const xb_slot* s, const libxsmm_gemm_param* params, long long count) {
   libxsmm_b200_gemm_plan* plan;
   xb_gemm_rec* recs;
   char* arrays = NULL; size_t arrays_bytes = 0, off = 0;
   long long t;
-  int mx_arrays;
+  int mx_arrays, sides;
   if (s == NULL || params == NULL || count <= 0 || xb_batch_refused(&s->u.gemm, 0)) return NULL;
   mx_arrays = (xb_lowbit_form(&s->u.gemm) == XB_LB_MXFP4);
-  if (xb_per_call_scales(&s->u.gemm)) {   /* every tile brings its row scales (a.tertiary) and, for int4, zero points (a.quaternary);
-                                           * MXFP4 x I8 its block scales (a.tertiary, b.tertiary) */
-    const int mxfp4 = (xb_lowbit_form(&s->u.gemm) == XB_LB_MXFP4);
-    for (t = 0; t < count; ++t) {
-      if (params[t].a.tertiary == NULL || (xb_dq_form(&s->u.gemm) == XB_DQ_I4_F16 && params[t].a.quaternary == NULL)
-       || (mxfp4 && params[t].b.tertiary == NULL)) return NULL;
-    }
+  sides = xb_gemm_sides(&s->u.gemm);
+  for (t = 0; t < count && sides != 0; ++t) {   /* every tile brings each side operand of the handle */
+    xb_gemm_rec r;
+    memset(&r, 0, sizeof(r));
+    xb_param_sides(&r, &params[t], sides);
+    if (xb_gemm_rec_lacks(&r, sides)) return NULL;
   }
   plan = (libxsmm_b200_gemm_plan*)calloc(1, sizeof(*plan));
   if (plan != NULL && xb_plan_try_pool(plan, s, params, count)) return plan;
@@ -1137,8 +1119,8 @@ static libxsmm_b200_gemm_plan* xb_plan_make(const xb_slot* s, const libxsmm_gemm
       memcpy(arrays + off, p->a.secondary, (size_t)r->br * 8); r->a_aux = (char*)plan->d_arrays + off; off += (size_t)r->br * 8;
       memcpy(arrays + off, p->b.secondary, (size_t)r->br * 8); r->b_aux = (char*)plan->d_arrays + off; off += (size_t)r->br * 8;
     }
-    if (mx_arrays) {   /* MXFP4 x I8: block scales; address mode: arrays of br pointers */
-      r->a_s = p->a.tertiary; r->b_s = p->b.tertiary;
+    xb_param_sides(r, p, sides);
+    if (mx_arrays) {   /* MXFP4 x I8 block scales, address mode: arrays of br pointers */
       if (s->u.gemm.br_type == 1 && xb_rt_ptr_kind(p->a.tertiary) != 1) {
         memcpy(arrays + off, p->a.tertiary, (size_t)r->br * 8); r->a_s = (char*)plan->d_arrays + off; off += (size_t)r->br * 8;
       }
@@ -1148,7 +1130,6 @@ static libxsmm_b200_gemm_plan* xb_plan_make(const xb_slot* s, const libxsmm_gemm
     }
     if (s->u.gemm.tc == LIBXSMM_DATATYPE_F32 && (s->u.gemm.ta == LIBXSMM_DATATYPE_I8 || s->u.gemm.ta == LIBXSMM_DATATYPE_U8)
         && p->c.tertiary != NULL) r->scf = *(const float*)p->c.tertiary;
-    if (xb_dq_scaled(&s->u.gemm)) { r->a_s = p->a.tertiary; r->a_q = p->a.quaternary; }
   }
   plan->d_recs = (xb_gemm_rec*)xb_rt_device_malloc((size_t)count * sizeof(xb_gemm_rec));
   if (plan->d_recs == NULL) { free(arrays); free(recs); xb_rt_device_free(plan->d_arrays); free(plan); return NULL; }
@@ -1159,13 +1140,12 @@ static libxsmm_b200_gemm_plan* xb_plan_make(const xb_slot* s, const libxsmm_gemm
   return plan;
 }
 
-/* a plan is prepared once and replayed: the row scales of a dequantising A and the block scales of MXFP4 x I8 are per-call
- * operands, so such a handle gets no plan */
+/* a plan is prepared once and replayed: side operands (xb_gemm_sides) are per-call operands, so such a handle gets no plan */
 LIBXSMM_API libxsmm_b200_gemm_plan* libxsmm_b200_gemm_plan_create(libxsmm_gemmfunction kernel,
   const libxsmm_gemm_param* params, long long count)
 {
   const xb_slot* s = xb_gemm_slot((const void*)kernel);
-  if (s == NULL || xb_per_call_scales(&s->u.gemm)) return NULL;
+  if (s == NULL || xb_gemm_sides(&s->u.gemm) != 0) return NULL;
   return xb_plan_make(s, params, count);
 }
 
@@ -1199,7 +1179,7 @@ LIBXSMM_API int libxsmm_b200_gemm_batch(libxsmm_gemmfunction kernel, const libxs
   int rc;
   if (s != NULL && xb_batch_refused(&s->u.gemm, 0)) return LIBXSMM_B200_ERROR_NOT_BATCHABLE;
   if (count == 0) return 0;
-  plan = xb_plan_make(s, params, count);   /* unlike a plan, one batch call also carries dequantising A's row scales */
+  plan = xb_plan_make(s, params, count);   /* unlike a plan, one batch call also carries each tile's side operands */
   if (plan == NULL) return -1;
   rc = libxsmm_b200_gemm_plan_run(plan);
   if (rc == 0 && !xb_rt_blocking()) rc = xb_rt_sync();   /* the plan's arrays must outlive the launch */

@@ -146,6 +146,36 @@ static inline int xb_lowbit_form(const xb_gemm_desc* d) {
   return XB_LB_NONE;
 }
 
+/* side operands: what a call of a GEMM descriptor reads next to A, B and C, one bit each. A's scales (a.tertiary) are the row scales of
+ * a dequantising A or the E8M0 block scales of MX fp8 / MXFP4 A; B's (b.tertiary) the block scales of MX fp8 / MXFP4 x I8; C's
+ * (c.tertiary) those of an MXBF8 C; A's zero points (a.quaternary) those of an int4 A. In a record: a_s, b_s, c_s and a_q. */
+enum { XB_SIDE_A_S = 1, XB_SIDE_B_S = 2, XB_SIDE_C_S = 4, XB_SIDE_A_Q = 8 };
+#if defined(__CUDACC__)
+__host__ __device__
+#endif
+static inline int xb_gemm_sides(const xb_gemm_desc* d) {
+  const int dq = xb_dq_form(d);
+  if (d->ta == LIBXSMM_DATATYPE_MXBF8 || d->ta == LIBXSMM_DATATYPE_MXHF8) {
+    return XB_SIDE_A_S | XB_SIDE_B_S | (d->tc == LIBXSMM_DATATYPE_MXBF8 ? XB_SIDE_C_S : 0);
+  }
+  if (dq == XB_DQ_I8_BF16 || dq == XB_DQ_I8_F16) return XB_SIDE_A_S;
+  if (dq == XB_DQ_I4_F16) return XB_SIDE_A_S | XB_SIDE_A_Q;
+  if (xb_lowbit_form(d) == XB_LB_MXFP4) return XB_SIDE_A_S | XB_SIDE_B_S;
+  if ((d->ta == LIBXSMM_DATATYPE_I4X2 || d->ta == LIBXSMM_DATATYPE_U4X2) && (d->tb == LIBXSMM_DATATYPE_I8 || d->tb == LIBXSMM_DATATYPE_U8)) {
+    return XB_SIDE_A_Q;
+  }
+  return 0;
+}
+
+/* 1 if a side operand of `sides` is NULL in r */
+#if defined(__CUDACC__)
+__host__ __device__
+#endif
+static inline int xb_gemm_rec_lacks(const xb_gemm_rec* r, int sides) {
+  return ((sides & XB_SIDE_A_S) && r->a_s == NULL) || ((sides & XB_SIDE_B_S) && r->b_s == NULL)
+      || ((sides & XB_SIDE_C_S) && r->c_s == NULL) || ((sides & XB_SIDE_A_Q) && r->a_q == NULL);
+}
+
 /* launch description handed to the CUDA side */
 typedef struct xb_gemm_launch {
   xb_gemm_desc d;
@@ -159,6 +189,26 @@ typedef struct xb_gemm_launch {
   const xb_gemm_rec* recs;
   xb_gemm_rec one;      /* count==1 && !recs: passed by value */
 } xb_gemm_launch;
+
+/* the complete record of tile t: the per-tile record, the single call, or a strided batch's bases advanced by t tile strides (a side
+ * operand the launch lacks is NULL with a tile stride of 0). A strided batch shares `one`'s scale factor, bias column and zero
+ * points, has offset arrays in offset mode only and no masks. */
+#if defined(__CUDACC__)
+__host__ __device__
+#endif
+static inline xb_gemm_rec xb_gemm_tile(const xb_gemm_launch* L, long long t) {
+  xb_gemm_rec r;
+  if (L->recs != NULL) r = L->recs[t];
+  else if (L->a == NULL && L->c == NULL) r = L->one;
+  else {
+    r.a = (const char*)L->a + t * L->tile_stride_a; r.b = (const char*)L->b + t * L->tile_stride_b; r.c = (char*)L->c + t * L->tile_stride_c;
+    r.a_aux = NULL; r.b_aux = NULL; r.br = L->br; r.scf = L->one.scf; r.d = L->one.d; r.c_aux = NULL; r.a_q = L->one.a_q;
+    if (L->d.br_type == 2) { r.a_aux = L->one.a_aux; r.b_aux = L->one.b_aux; }
+    r.a_s = (const char*)L->one.a_s + t * L->tile_stride_as; r.b_s = (const char*)L->one.b_s + t * L->tile_stride_bs;
+    r.c_s = (L->one.c_s != NULL) ? (char*)L->one.c_s + t * L->tile_stride_cs : NULL;
+  }
+  return r;
+}
 
 /* ---- CUDA runtime layer (runtime.cu) ----------------------------------------------------------- */
 int xb_rt_device_count(void);

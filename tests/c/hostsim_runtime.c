@@ -114,13 +114,7 @@ static int sim_gemm_tile(const xb_gemm_desc* d, const xb_gemm_rec* r) {
 int xb_gemm_simt_supported(const xb_gemm_desc* d) { return d->m > 0 && d->n > 0 && d->k > 0; }
 int xb_gemm_simt_launch(const xb_gemm_launch* L) {
   long long t; int rc = 0;
-  if (L->recs != NULL) { for (t = 0; t < L->count && rc == 0; ++t) rc = sim_gemm_tile(&L->d, &L->recs[t]); }
-  else if (L->count == 1 && L->a == NULL) rc = sim_gemm_tile(&L->d, &L->one);
-  else for (t = 0; t < L->count && rc == 0; ++t) {
-    xb_gemm_rec r; memset(&r, 0, sizeof(r));
-    r.a = (const char*)L->a + t * L->tile_stride_a; r.b = (const char*)L->b + t * L->tile_stride_b; r.c = (char*)L->c + t * L->tile_stride_c; r.br = L->br;
-    rc = sim_gemm_tile(&L->d, &r);
-  }
+  for (t = 0; t < L->count && rc == 0; ++t) { const xb_gemm_rec r = xb_gemm_tile(L, t); rc = sim_gemm_tile(&L->d, &r); }
   if (rc != 0) fprintf(stderr, "hostsim: the oracle refused a GEMM tile (rc %d)\n", rc);
   return rc;
 }

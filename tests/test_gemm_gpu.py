@@ -253,6 +253,16 @@ def test_int4_gemm_with_zero_points_bit_exact():
                     X.GEMMFUNCTION(kern)(C.byref(p)); X.check()
                     got = host(d_c, np.int32) if resident else hc
                     assert np.array_equal(got, want), (dims, br_type, beta0, resident)
+                if br_type:   # per-tile batch: each record carries its own tile's zero points (a.quaternary)
+                    zpt2 = ((zpt + 7) % 16).astype(np.uint8); want2 = c0.copy()
+                    assert oracle["gemm_i4"](iarr(*dims), flags, br_type, blk_a, blk_b, br, a.ctypes.data, b.ctypes.data, want2.ctypes.data, zpt2.ctypes.data) == 0
+                    d_a, d_b, d_zs, d_cs = dev(a), dev(b), (dev(zpt), dev(zpt2)), (dev(c0), dev(c0))
+                    params = (X.GemmParam * 2)(); brv = C.c_ulonglong(br)
+                    for t in range(2):
+                        params[t].op.tertiary = C.addressof(brv)
+                        params[t].a.primary, params[t].b.primary, params[t].c.primary, params[t].a.quaternary = d_a.data_ptr(), d_b.data_ptr(), d_cs[t].data_ptr(), d_zs[t].data_ptr()
+                    assert X.libxsmm_b200_gemm_batch(kern, params, 2) == 0; X.check()
+                    assert np.array_equal(host(d_cs[0], np.int32), want) and np.array_equal(host(d_cs[1], np.int32), want2), (dims, beta0, "batch")
     # what the reference cannot build answers NULL here too: no zero-point layout for address mode in this kernel, k % 8 != 0
     sh = X.libxsmm_create_gemm_shape(16, 16, 12, 16, 12, 16, I4X2, gen.U8, gen.I32, gen.I32)
     assert not X.libxsmm_dispatch_gemm(sh, cases.FLAG_VNNI_A | FLAG_INTLV_A | FLAG_COL_VEC_ZPT, 0)

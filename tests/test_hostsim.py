@@ -402,3 +402,57 @@ def test_batch_entry_points_refuse_handles_they_cannot_run_like_a_single_call(si
                 X.GEMMFUNCTION(fn)(C.byref(p))
             assert np.array_equal(c, want)
             assert not np.array_equal(c, c0)
+
+
+def test_int4_zero_points_travel_per_tile_in_the_batch_form(sim):
+    """An I4X2 x U8 -> I32 handle reads zero points from a.quaternary, one byte per row and reduce step. libxsmm_b200_gemm_batch carries
+    each tile's pointer into its record, so the batch gives what one call per tile gives; a tile without zero points is refused (-1) before
+    anything runs. The strided forms have no place for them (LIBXSMM_B200_ERROR_NOT_BATCHABLE) and a plan, which is replayed, gets none."""
+    from test_oracle_vs_ref import FLAG_INTLV_A, FLAG_MXK_ZPT, I4X2, int4_case
+    lib = sim.lib
+    I, U, P, LL, ULL, UB = C.c_int, C.c_uint, C.c_void_p, C.c_longlong, C.c_ulonglong, C.c_ubyte
+    for name, res, args in (("libxsmm_create_gemm_shape", X.GemmShape, [I] * 10), ("libxsmm_create_gemm_batch_reduce_config", X.BatchReduceConfig, [I, I, I, UB]),
+                            ("libxsmm_dispatch_brgemm", P, [X.GemmShape, U, U, X.BatchReduceConfig]),
+                            ("libxsmm_b200_gemm_batch_strided", I, [P, P, P, P, LL, LL, LL, ULL, LL]),
+                            ("libxsmm_b200_gemm_batch_strided_multi", I, [P, P, P, P, LL, LL, LL, ULL, LL, I]),
+                            ("libxsmm_b200_gemm_batch", I, [P, C.POINTER(X.GemmParam), LL]), ("libxsmm_b200_gemm_plan_create", P, [P, C.POINTER(X.GemmParam), LL]),
+                            ("libxsmm_b200_launch_count", ULL, [])):
+        fn = getattr(lib, name); fn.restype = res; fn.argtypes = args
+    NOT_BATCHABLE = -6          # include/libxsmm_b200.h
+    rng = np.random.default_rng(13)
+    count, br = 3, 4
+    tiles = [int4_case(rng, 13, 6, 16, br, 3) for _ in range(count)]
+    dims, _, _, _, _, blk_a, blk_b = tiles[0]
+    fn = lib.libxsmm_dispatch_brgemm(lib.libxsmm_create_gemm_shape(*dims, I4X2, gen.U8, gen.I32, gen.I32), X.GEMM_FLAG_VNNI_A | FLAG_INTLV_A | FLAG_MXK_ZPT, 0,
+                                     lib.libxsmm_create_gemm_batch_reduce_config(X.GEMM_BATCH_REDUCE_STRIDE, blk_a, blk_b, 0))
+    assert fn
+    brv = C.c_ulonglong(br)
+    c = [t[4].copy() for t in tiles]
+    params = (X.GemmParam * count)()
+    for t, (_, a, b, zpt, _, _, _) in enumerate(tiles):
+        params[t].op.tertiary = C.addressof(brv)
+        params[t].a.primary, params[t].b.primary, params[t].c.primary, params[t].a.quaternary = a.ctypes.data, b.ctypes.data, c[t].ctypes.data, zpt.ctypes.data
+    # a tile without zero points: nothing runs
+    params[1].a.quaternary = None
+    n0 = lib.libxsmm_b200_launch_count()
+    assert lib.libxsmm_b200_gemm_batch(fn, params, count) == -1
+    assert lib.libxsmm_b200_launch_count() == n0
+    assert all(np.array_equal(c[t], tiles[t][4]) for t in range(count))
+    params[1].a.quaternary = tiles[1][3].ctypes.data
+    # strided forms and plans
+    a0, b0, c0 = tiles[0][1], tiles[0][2], c[0]
+    assert lib.libxsmm_b200_gemm_batch_strided(fn, a0.ctypes.data, b0.ctypes.data, c0.ctypes.data, 0, 0, 0, br, count) == NOT_BATCHABLE
+    assert lib.libxsmm_b200_gemm_batch_strided_multi(fn, a0.ctypes.data, b0.ctypes.data, c0.ctypes.data, 0, 0, 0, br, count, 1) == NOT_BATCHABLE
+    assert not lib.libxsmm_b200_gemm_plan_create(fn, params, count)
+    assert lib.libxsmm_b200_launch_count() == n0
+    assert all(np.array_equal(c[t], tiles[t][4]) for t in range(count))
+    # the batch equals one call per tile
+    assert lib.libxsmm_b200_gemm_batch(fn, params, count) == 0
+    assert lib.libxsmm_b200_launch_count() == n0 + count
+    for t, (_, a, b, zpt, c_init, _, _) in enumerate(tiles):
+        want = c_init.copy()
+        p = X.GemmParam(); p.op.tertiary = C.addressof(brv)
+        p.a.primary, p.b.primary, p.c.primary, p.a.quaternary = a.ctypes.data, b.ctypes.data, want.ctypes.data, zpt.ctypes.data
+        X.GEMMFUNCTION(fn)(C.byref(p))
+        assert np.array_equal(c[t], want), t
+        assert not np.array_equal(want, c_init), t
