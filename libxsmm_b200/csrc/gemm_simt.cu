@@ -22,54 +22,6 @@
 
 namespace {
 
-enum { P_F64 = 0, P_F32, P_I16, P_I8_I32, P_I8_F32, P_F16_F16, P_F16_F32, P_BF16_F32, P_BF16_BF16, P_I4_I32, P_BITMAP, P_FP8, P_MX8, P_DQ, P_NONE, P_LOWBIT };
-
-__host__ __device__ inline int xb_path_of(const xb_gemm_desc& d) {
-  const int a = d.ta, b = d.tb, c = d.tc, comp = d.tcomp;
-  const bool a8 = (a == LIBXSMM_DATATYPE_I8 || a == LIBXSMM_DATATYPE_U8);
-  const bool b8 = (b == LIBXSMM_DATATYPE_I8 || b == LIBXSMM_DATATYPE_U8);
-  if (xb_lowbit_form(&d) != XB_LB_NONE) {   // I2 / I1 / MXFP4 A x 8-bit B (reference :1009-1272); the layout rules live in host_core.c
-    return (d.fuse_colbias == 0 && d.cp_op == 0 && (d.flags & LIBXSMM_GEMM_FLAG_DECOMPRESS_A_VIA_BITMASK) == 0) ? P_LOWBIT : P_NONE;
-  }
-  if (a == LIBXSMM_DATATYPE_MXBF8 || a == LIBXSMM_DATATYPE_MXHF8) {   // MX fp8 (reference :2620-2679); the layout rules live in host_core.c
-    const bool cok = (c == LIBXSMM_DATATYPE_F32) || (c == LIBXSMM_DATATYPE_MXBF8 && a == LIBXSMM_DATATYPE_MXBF8);
-    return (b == a && comp == LIBXSMM_DATATYPE_F32 && cok && (d.br_type == 0 || d.br_type == 3) && d.fuse_colbias == 0 && d.cp_op == 0) ? P_MX8 : P_NONE;
-  }
-  if (xb_dq_form(&d) != XB_DQ_NONE) {   // dequantising A (reference :1684-2024); the layout rules live in host_core.c
-    return (d.fuse_colbias == 0 && d.cp_op == 0 && (d.flags & LIBXSMM_GEMM_FLAG_DECOMPRESS_A_VIA_BITMASK) == 0) ? P_DQ : P_NONE;
-  }
-  if ((d.flags & LIBXSMM_GEMM_FLAG_DECOMPRESS_A_VIA_BITMASK) != 0) {   // bitmap-compressed A (reference :857-948): float operands, no batch reduce
-    const bool fa = (a == LIBXSMM_DATATYPE_F32 || a == LIBXSMM_DATATYPE_BF16 || a == LIBXSMM_DATATYPE_F16);
-    const bool fb = (b == LIBXSMM_DATATYPE_F32 || b == LIBXSMM_DATATYPE_BF16 || b == LIBXSMM_DATATYPE_F16);
-    const bool fc = (c == LIBXSMM_DATATYPE_F32 || c == LIBXSMM_DATATYPE_BF16 || c == LIBXSMM_DATATYPE_F16);
-    const int kb = (a == LIBXSMM_DATATYPE_F32) ? 1 : ((b == LIBXSMM_DATATYPE_F32) ? 1 : 2);
-    return (fa && fb && fc && d.br_type == 0 && (d.k % kb) == 0 && d.fuse_colbias == 0 && d.cp_op == 0) ? P_BITMAP : P_NONE;
-  }
-  if (a == LIBXSMM_DATATYPE_I4X2 || a == LIBXSMM_DATATYPE_U4X2) {       // 4-bit A with zero points x 8-bit B -> I32 (reference :1273-1321)
-    const unsigned int need = LIBXSMM_GEMM_FLAG_VNNI_A | LIBXSMM_GEMM_FLAG_INTLV_A_FORMAT;
-    return ((d.flags & need) == need && b8 && c == LIBXSMM_DATATYPE_I32 && comp == LIBXSMM_DATATYPE_I32 && (d.k % 8) == 0
-            && (d.br_type == 0 || d.br_type == 3)) ? P_I4_I32 : P_NONE;
-  }
-  if (a == LIBXSMM_DATATYPE_F64 && b == a && c == a && comp == a) return P_F64;
-  if ((a == LIBXSMM_DATATYPE_F32 || a == LIBXSMM_DATATYPE_BF32) && (b == LIBXSMM_DATATYPE_F32 || b == LIBXSMM_DATATYPE_BF32)
-      && c == LIBXSMM_DATATYPE_F32 && comp == LIBXSMM_DATATYPE_F32) return P_F32;
-  if (a == LIBXSMM_DATATYPE_I16 && b == a && c == LIBXSMM_DATATYPE_I32 && comp == LIBXSMM_DATATYPE_I32) return P_I16;
-  if (a8 && b8 && c == LIBXSMM_DATATYPE_I32 && comp == LIBXSMM_DATATYPE_I32) return P_I8_I32;
-  if (a8 && b8 && c == LIBXSMM_DATATYPE_F32 && comp == LIBXSMM_DATATYPE_I32) return P_I8_F32;
-  const bool f16comp = (comp == LIBXSMM_DATATYPE_F16 || comp == LIBXSMM_DATATYPE_F32 || comp == LIBXSMM_DATATYPE_IMPLICIT);
-  if (a == LIBXSMM_DATATYPE_F16 && b == a && c == LIBXSMM_DATATYPE_F16 && f16comp) return P_F16_F16;
-  if (a == LIBXSMM_DATATYPE_F16 && b == a && c == LIBXSMM_DATATYPE_F32 && f16comp) return P_F16_F32;
-  if (a == LIBXSMM_DATATYPE_BF16 && b == a && c == LIBXSMM_DATATYPE_F32 && comp == LIBXSMM_DATATYPE_F32) return P_BF16_F32;
-  if (a == LIBXSMM_DATATYPE_BF16 && b == a && c == LIBXSMM_DATATYPE_BF16 && comp == LIBXSMM_DATATYPE_F32) return P_BF16_BF16;
-  // 8-bit float A (reference :2171-2366 with a bf16 B, :2420-2630 with B and C of A's type or f32): f32 accumulate, one rounding
-  if ((a == LIBXSMM_DATATYPE_BF8 || a == LIBXSMM_DATATYPE_HF8) && comp == LIBXSMM_DATATYPE_F32 && d.fuse_colbias == 0 && d.cp_op == 0
-      && (d.flags & (LIBXSMM_GEMM_FLAG_VNNI_C | LIBXSMM_GEMM_FLAG_VNNI_B)) == 0) {
-    if (b == a && (c == LIBXSMM_DATATYPE_F32 || c == a)) return P_FP8;
-    if (b == LIBXSMM_DATATYPE_BF16 && (c == LIBXSMM_DATATYPE_F32 || c == LIBXSMM_DATATYPE_BF16)) return P_FP8;
-  }
-  return P_NONE;
-}
-
 struct TileCtx {
   const char* a0; const char* b0; char* c;       // tile bases
   const void* const* a_addr; const void* const* b_addr;   // address mode
@@ -245,7 +197,7 @@ __global__ void __launch_bounds__(256) gemm_simt_fused_kernel(const xb_gemm_laun
         switch (path) {
           case P_F32: acc = dot_f32(d, g, x, i, j, beta0_eff ? 0.0f : seed); break;
           case P_I8_F32:
-            __builtin_assume(d.tc == LIBXSMM_DATATYPE_F32);   // xb_path_of: P_I8_F32 has an f32 C, so dot_i8 reads VNNI4
+            __builtin_assume(d.tc == LIBXSMM_DATATYPE_F32);   // xb_gemm_path: P_I8_F32 has an f32 C, so dot_i8 reads VNNI4
             acc = __fmul_rn((float)(int)dot_i8(d, g, x, i, j, 0u), x.scf);
             if (!beta0_eff) acc = __fadd_rn(acc, seed);
             break;
@@ -929,18 +881,9 @@ int launched(const char* what) {
 }
 }  // namespace
 
-extern "C" int xb_gemm_simt_supported(const xb_gemm_desc* d) {
-  const int path = xb_path_of(*d);
-  if (path == P_NONE) return 0;
-  if (d->fuse_colbias != 0 || d->cp_op != 0) {   // fused form: float C only (the reference's f32 image of C)
-    return path == P_F32 || path == P_I8_F32 || path == P_F16_F16 || path == P_F16_F32 || path == P_BF16_F32 || path == P_BF16_BF16;
-  }
-  return 1;
-}
-
 extern "C" int xb_gemm_simt_launch(const xb_gemm_launch* L) {
-  const int path = xb_path_of(L->d);
-  if (path == P_NONE) return 1;
+  const int path = L->d.path;
+  if (path == XB_PATH_NONE) return 1;
   if (L->count <= 0) return 0;
   if (L->recs == nullptr && xb_gemm_rec_lacks(&L->one, xb_gemm_sides(&L->d))) {
     xb_rt_note_error(1, "GEMM: side operand missing (scales in a/b/c.tertiary, zero points in a.quaternary)"); return 1;

@@ -29,8 +29,6 @@ static int g_force_simt = 0;
 static int g_reg[XB_REG_CAP];      /* 0: empty, else slot+1 */
 static size_t g_reg_size = 0;
 
-extern int xb_gemm_simt_supported(const xb_gemm_desc* d);
-
 static unsigned int xb_hash(const void* data, size_t n, unsigned int seed) {
   const unsigned char* p = (const unsigned char*)data;
   unsigned int h = 2166136261u ^ seed;
@@ -256,79 +254,117 @@ static int xb_tilecfg_inconsistent(unsigned int flags) {
   return nr != ns;
 }
 
-static int xb_is_mx8(int t) { return t == LIBXSMM_DATATYPE_MXBF8 || t == LIBXSMM_DATATYPE_MXHF8; }
-
-/* MXBF8 x MXBF8 and MXHF8 x MXHF8 with E8M0 block scales (reference src/generator_gemm_reference_impl.c:2620-2679); 1 if the
- * reference kernel defines a result for the descriptor. Every other MX tuple (MXHF8 -> MXHF8, mixed, MX6, MX4) matches no branch. */
-static int xb_mx8_desc_ok(const xb_gemm_desc* d, int ext) {
-  const unsigned int need = LIBXSMM_GEMM_FLAG_VNNI_A | LIBXSMM_GEMM_FLAG_VNNI_B | LIBXSMM_GEMM_FLAG_TRANS_B;
-  const int mx_c = (d->tc == LIBXSMM_DATATYPE_MXBF8);
-  if (ext) return 0;                                                           /* fused MX does not exist */
-  if (!xb_is_mx8(d->ta) || d->tb != d->ta || d->tcomp != LIBXSMM_DATATYPE_F32) return 0;
-  if (!(d->tc == LIBXSMM_DATATYPE_F32 || (mx_c && d->ta == LIBXSMM_DATATYPE_MXBF8))) return 0;
-  if ((d->flags & need) != need || (d->flags & LIBXSMM_GEMM_FLAG_TRANS_A) != 0) return 0;   /* the reference prints an error and leaves C (:2632-2635) */
-  if ((d->flags & (LIBXSMM_GEMM_FLAG_VNNI_C | LIBXSMM_GEMM_FLAG_DECOMPRESS_A_VIA_BITMASK)) != 0) return 0;                   /* not served for MX */
-  if ((d->k % 32) != 0 || d->lda < d->m || d->ldb < d->n) return 0;
-  /* block r is read at r*lda*k and r*ldb*k whatever the batch-reduce type says (:2646-2655): stride mode only where the hints agree;
-   * address and offset mode would read the pointer / offset arrays as data, which defines no result */
-  if (d->br_type == 1 || d->br_type == 2) return 0;
-  if (d->br_type == 3 && (d->br_stride_a != (long long)d->lda * d->k || d->br_stride_b != (long long)d->ldb * d->k)) return 0;
-  /* MXBF8 C: the reference accumulates into an uninitialised image unless beta = 0, and quantises whole 32-row blocks (:757-) */
-  if (mx_c && ((d->flags & LIBXSMM_GEMM_FLAG_BETA_0) == 0 || (d->m % 32) != 0 || (d->ldc % 32) != 0)) return 0;
-  return 1;
+/* A's layout (gemm_simt.cu gives the formulas): the VNNI factor its k is packed by (1: not packed) and, in *trans, whether TRANS_A
+ * is honoured. F64 / F32 / BF32 A are read flat whatever VNNI_A says; an int8 A next to an f32 C is always VNNI4; an 8-bit float A
+ * is VNNI4, or VNNI2 next to a bf16 B. The narrow forms (MX fp8, dequantising, low-bit) read A in layouts of their own. */
+static int xb_layout_a(const xb_gemm_desc* d, int* trans) {
+  const int ta = d->ta, is8 = (ta == LIBXSMM_DATATYPE_I8 || ta == LIBXSMM_DATATYPE_U8), is_f8 = (ta == LIBXSMM_DATATYPE_BF8 || ta == LIBXSMM_DATATYPE_HF8);
+  const int flat = (ta == LIBXSMM_DATATYPE_F64 || ta == LIBXSMM_DATATYPE_F32 || ta == LIBXSMM_DATATYPE_BF32);
+  *trans = (d->flags & LIBXSMM_GEMM_FLAG_TRANS_A) != 0 && (flat || ta == LIBXSMM_DATATYPE_BF16 || is_f8);
+  if ((d->flags & LIBXSMM_GEMM_FLAG_VNNI_A) != 0 ? flat : !(is8 && d->tc == LIBXSMM_DATATYPE_F32)) return 1;
+  return (is8 || (is_f8 && d->tb != LIBXSMM_DATATYPE_BF16)) ? 4 : 2;
 }
 
-/* a narrow A next to a 16-bit float B: the dequantising tuples and their unsigned / mis-typed neighbours (none of which dispatched before) */
-static int xb_is_dq_family(const xb_gemm_desc* d) {
-  const int a = d->ta, b = d->tb;
-  return ((a == LIBXSMM_DATATYPE_I8 || a == LIBXSMM_DATATYPE_U8 || a == LIBXSMM_DATATYPE_I4X2 || a == LIBXSMM_DATATYPE_U4X2)
-          && (b == LIBXSMM_DATATYPE_BF16 || b == LIBXSMM_DATATYPE_F16)) || (a == LIBXSMM_DATATYPE_BF8 && b == LIBXSMM_DATATYPE_F16);
+/* B's layout: the VNNI factor of its transposed, packed form (1: not packed) and, in *trans, whether TRANS_B is honoured. A bf16
+ * B under TRANS_B and VNNI_B is VNNI2-T, an MX fp8 B VNNI4-T. */
+static int xb_layout_b(const xb_gemm_desc* d, int* trans) {
+  const int tb = d->tb, mx = (tb == LIBXSMM_DATATYPE_MXBF8 || tb == LIBXSMM_DATATYPE_MXHF8);
+  *trans = (d->flags & LIBXSMM_GEMM_FLAG_TRANS_B) != 0 && (mx || tb == LIBXSMM_DATATYPE_F64 || tb == LIBXSMM_DATATYPE_F32 || tb == LIBXSMM_DATATYPE_BF32
+                                                           || tb == LIBXSMM_DATATYPE_BF16 || tb == LIBXSMM_DATATYPE_F16 || tb == LIBXSMM_DATATYPE_BF8 || tb == LIBXSMM_DATATYPE_HF8);
+  if (mx) return 4;
+  return (*trans && (d->flags & LIBXSMM_GEMM_FLAG_VNNI_B) != 0 && tb == LIBXSMM_DATATYPE_BF16) ? 2 : 1;
 }
 
-/* dequantising A (xb_dq_form; reference src/generator_gemm_reference_impl.c:1684-2024, operand slots :551-630): 1 if the reference
- * defines a result for the descriptor in the layout the flags ask for. A flag the reference would ignore rather than obey is declined,
- * so that no caller gets a layout other than the one asked for. */
-static int xb_dq_desc_ok(const xb_gemm_desc* d, int ext) {
-  const int form = xb_dq_form(d);
-  const int trans_b = (d->flags & LIBXSMM_GEMM_FLAG_TRANS_B) != 0, vnni_a = (d->flags & LIBXSMM_GEMM_FLAG_VNNI_A) != 0;
-  if (ext || form == XB_DQ_NONE) return 0;                 /* no fused form; U8 A (see xb_dq_form), other comp / C types */
-  /* no branch reads A transposed or B / C VNNI-packed; bitmap A is the sparse branch (:857-948); INTLV_A_FORMAT makes int4 the
-   * int8-B form (:472-480) */
-  if ((d->flags & (LIBXSMM_GEMM_FLAG_TRANS_A | LIBXSMM_GEMM_FLAG_VNNI_B | LIBXSMM_GEMM_FLAG_VNNI_C | LIBXSMM_GEMM_FLAG_DECOMPRESS_A_VIA_BITMASK
-                   | LIBXSMM_GEMM_FLAG_INTLV_A_FORMAT)) != 0) return 0;
-  if (form == XB_DQ_I8_BF16 && trans_b) return 0;          /* B is read [n][ldb] whatever the flag says (:1709) */
-  if ((form == XB_DQ_I8_BF16 || form == XB_DQ_I8_F16) && vnni_a) return 0;   /* A is read flat (l_k_block = 1, :1691, :1891, :1963) */
-  if (form == XB_DQ_I4_F16 && !vnni_a) return 0;           /* int4 x f16 is the VNNI_A form only (:472) */
-  if ((form == XB_DQ_I4_F16 || (form == XB_DQ_BF8_F16 && vnni_a)) && (d->k % 2) != 0) return 0;   /* k in pairs: an odd k would drop the last */
-  if (d->lda < d->m || d->ldb < (trans_b ? d->n : d->k)) return 0;
-  return 1;
-}
-
-/* a 2-bit or 1-bit A, or an MXFP4 A next to an 8-bit B: the low-bit weight tuples and their mis-typed neighbours (none of which
- * dispatched before) */
-static int xb_is_lowbit_family(const xb_gemm_desc* d) {
-  return d->ta == LIBXSMM_DATATYPE_I2X4 || d->ta == LIBXSMM_DATATYPE_I1X8
-      || (d->ta == LIBXSMM_DATATYPE_MXFP4X2 && (d->tb == LIBXSMM_DATATYPE_I8 || d->tb == LIBXSMM_DATATYPE_U8));
-}
-
-/* low-bit A (xb_lowbit_form; reference src/generator_gemm_reference_impl.c:1009-1272, set-up :457-490, :560-620): 1 if the reference
- * defines a result for the descriptor in the layout the flags ask for. As for xb_dq_desc_ok, a flag the reference would ignore is
- * declined rather than obeyed. */
-static int xb_lowbit_desc_ok(const xb_gemm_desc* d, int ext) {
-  const int form = xb_lowbit_form(d);
-  const unsigned int vnni_intlv = LIBXSMM_GEMM_FLAG_VNNI_A | LIBXSMM_GEMM_FLAG_INTLV_A_FORMAT;
-  if (ext || form == XB_LB_NONE) return 0;                 /* no fused form; MXFP4 x U8 (see xb_lowbit_form), other comp / C types */
-  /* every branch reads A in its packed layout, B as [n][ldb] and C flat; bitmap A is the sparse branch (:857-948) */
-  if ((d->flags & (LIBXSMM_GEMM_FLAG_TRANS_A | LIBXSMM_GEMM_FLAG_TRANS_B | LIBXSMM_GEMM_FLAG_VNNI_B | LIBXSMM_GEMM_FLAG_VNNI_C
-                   | LIBXSMM_GEMM_FLAG_DECOMPRESS_A_VIA_BITMASK)) != 0) return 0;
-  if (d->ldb < d->k || d->lda < d->m) return 0;
-  if (form == XB_LB_I2) {   /* :482; rows past 4*(m/4) and k past 4*(k/4) would be left out */
-    return (d->flags & vnni_intlv) == vnni_intlv && (d->m % 4) == 0 && (d->k % 4) == 0;
+/* The exact-order path that serves a GEMM descriptor, or XB_PATH_NONE: the one rule for which type tuples, flags, leading dimensions,
+ * divisibilities, batch-reduce modes and fusions dispatch. Line numbers cite the reference's src/generator_gemm_reference_impl.c.
+ * The narrow A forms (MX fp8, dequantising, low-bit) exist for the plain ABI only and decline every flag the reference would ignore
+ * rather than obey, so that no caller gets a layout other than the one asked for. */
+int xb_gemm_path(const xb_gemm_desc* d) {
+  const unsigned int f = d->flags;
+  const int ta = d->ta, tb = d->tb, tc = d->tc, comp = d->tcomp;
+  const int ext = (f & LIBXSMM_GEMM_FLAG_USE_XGEMM_EXT_ABI) != 0, vnni_a = (f & LIBXSMM_GEMM_FLAG_VNNI_A) != 0;
+  const int a8 = (ta == LIBXSMM_DATATYPE_I8 || ta == LIBXSMM_DATATYPE_U8), b8 = (tb == LIBXSMM_DATATYPE_I8 || tb == LIBXSMM_DATATYPE_U8);
+  const int a4 = (ta == LIBXSMM_DATATYPE_I4X2 || ta == LIBXSMM_DATATYPE_U4X2), b16 = (tb == LIBXSMM_DATATYPE_BF16 || tb == LIBXSMM_DATATYPE_F16);
+  const int a_f8 = (ta == LIBXSMM_DATATYPE_BF8 || ta == LIBXSMM_DATATYPE_HF8), a_mx = (ta == LIBXSMM_DATATYPE_MXBF8 || ta == LIBXSMM_DATATYPE_MXHF8);
+  int trans_a, trans_b, path = XB_PATH_NONE;
+  const int va = xb_layout_a(d, &trans_a);
+  xb_layout_b(d, &trans_b);
+  if (d->lda < (trans_a ? d->k : d->m) || d->ldb < (trans_b ? d->n : d->k)) return XB_PATH_NONE;
+  if (a_mx || tb == LIBXSMM_DATATYPE_MXBF8 || tb == LIBXSMM_DATATYPE_MXHF8 || tc == LIBXSMM_DATATYPE_MXBF8 || tc == LIBXSMM_DATATYPE_MXHF8) {
+    /* MXBF8 x MXBF8 and MXHF8 x MXHF8 with E8M0 block scales (:2620-2679); every other MX tuple matches no branch. The reference
+     * prints an error and leaves C without VNNI_A, VNNI_B and TRANS_B (:2632-2635). */
+    const unsigned int need = LIBXSMM_GEMM_FLAG_VNNI_A | LIBXSMM_GEMM_FLAG_VNNI_B | LIBXSMM_GEMM_FLAG_TRANS_B;
+    const int mx_c = (tc == LIBXSMM_DATATYPE_MXBF8);
+    if (ext || !a_mx || tb != ta || comp != LIBXSMM_DATATYPE_F32 || !(tc == LIBXSMM_DATATYPE_F32 || (mx_c && ta == LIBXSMM_DATATYPE_MXBF8))) return XB_PATH_NONE;
+    if ((f & (need | LIBXSMM_GEMM_FLAG_TRANS_A | LIBXSMM_GEMM_FLAG_VNNI_C | LIBXSMM_GEMM_FLAG_DECOMPRESS_A_VIA_BITMASK)) != need || (d->k % 32) != 0) return XB_PATH_NONE;
+    /* block r is read at r*lda*k and r*ldb*k whatever the batch-reduce type says (:2646-2655): stride mode only where the hints agree;
+     * address and offset mode would read the pointer / offset arrays as data, which defines no result */
+    if (d->br_type == 1 || d->br_type == 2) return XB_PATH_NONE;
+    if (d->br_type == 3 && (d->br_stride_a != (long long)d->lda * d->k || d->br_stride_b != (long long)d->ldb * d->k)) return XB_PATH_NONE;
+    /* MXBF8 C: the reference accumulates into an uninitialised image unless beta = 0, and quantises whole 32-row blocks (:757-) */
+    if (mx_c && ((f & LIBXSMM_GEMM_FLAG_BETA_0) == 0 || (d->m % 32) != 0 || (d->ldc % 32) != 0)) return XB_PATH_NONE;
+    return P_MX8;
   }
-  if (form == XB_LB_I1) {   /* :486 ignores INTLV_A_FORMAT; rows come in pairs (:1204) and k in fours (:1211) */
-    return (d->flags & vnni_intlv) == LIBXSMM_GEMM_FLAG_VNNI_A && (d->m % 2) == 0 && (d->k % 4) == 0 && (d->lda % 2) == 0;
+  if (((a8 || a4) && b16) || (ta == LIBXSMM_DATATYPE_BF8 && tb == LIBXSMM_DATATYPE_F16)) {
+    /* dequantising A (xb_dq_form, :1684-2024), and its unsigned / mis-typed neighbours. No branch reads A transposed or B / C
+     * VNNI-packed; bitmap A is the sparse branch (:857-948); INTLV_A_FORMAT makes int4 the int8-B form (:472-480). */
+    const int form = xb_dq_form(d);
+    if (ext || form == XB_DQ_NONE || (f & (LIBXSMM_GEMM_FLAG_TRANS_A | LIBXSMM_GEMM_FLAG_VNNI_B | LIBXSMM_GEMM_FLAG_VNNI_C
+                                           | LIBXSMM_GEMM_FLAG_DECOMPRESS_A_VIA_BITMASK | LIBXSMM_GEMM_FLAG_INTLV_A_FORMAT)) != 0) return XB_PATH_NONE;
+    if (form == XB_DQ_I8_BF16 && trans_b) return XB_PATH_NONE;                                   /* B is read [n][ldb] whatever the flag says (:1709) */
+    if ((form == XB_DQ_I8_BF16 || form == XB_DQ_I8_F16) && vnni_a) return XB_PATH_NONE;          /* A is read flat (l_k_block = 1, :1691, :1891, :1963) */
+    if (form == XB_DQ_I4_F16 && !vnni_a) return XB_PATH_NONE;                                    /* int4 x f16 is the VNNI_A form only (:472) */
+    if ((form == XB_DQ_I4_F16 || (form == XB_DQ_BF8_F16 && vnni_a)) && (d->k % 2) != 0) return XB_PATH_NONE;   /* k in pairs: an odd k would drop the last */
+    return P_DQ;
   }
-  return (d->flags & vnni_intlv) == vnni_intlv && (d->k % 32) == 0;   /* MXFP4: :467, 32-k scale blocks */
+  if (ta == LIBXSMM_DATATYPE_I2X4 || ta == LIBXSMM_DATATYPE_I1X8 || (ta == LIBXSMM_DATATYPE_MXFP4X2 && b8)) {
+    /* low-bit A (xb_lowbit_form, :1009-1272, set-up :457-490, :560-620), and its mis-typed neighbours. Every branch reads A in its
+     * packed layout, B as [n][ldb] and C flat; bitmap A is the sparse branch (:857-948). */
+    const int form = xb_lowbit_form(d);
+    const unsigned int packed = f & (LIBXSMM_GEMM_FLAG_VNNI_A | LIBXSMM_GEMM_FLAG_INTLV_A_FORMAT);
+    if (ext || form == XB_LB_NONE || (f & (LIBXSMM_GEMM_FLAG_TRANS_A | LIBXSMM_GEMM_FLAG_TRANS_B | LIBXSMM_GEMM_FLAG_VNNI_B | LIBXSMM_GEMM_FLAG_VNNI_C
+                                           | LIBXSMM_GEMM_FLAG_DECOMPRESS_A_VIA_BITMASK)) != 0) return XB_PATH_NONE;
+    switch (form) {
+      case XB_LB_I2:   /* :482; rows past 4*(m/4) and k past 4*(k/4) would be left out */
+        return (packed == (LIBXSMM_GEMM_FLAG_VNNI_A | LIBXSMM_GEMM_FLAG_INTLV_A_FORMAT) && (d->m % 4) == 0 && (d->k % 4) == 0) ? P_LOWBIT : XB_PATH_NONE;
+      case XB_LB_I1:   /* :486 ignores INTLV_A_FORMAT; rows come in pairs (:1204) and k in fours (:1211) */
+        return (packed == LIBXSMM_GEMM_FLAG_VNNI_A && (d->m % 2) == 0 && (d->k % 4) == 0 && (d->lda % 2) == 0) ? P_LOWBIT : XB_PATH_NONE;
+      default:         /* MXFP4: :467, 32-k scale blocks */
+        return (packed == (LIBXSMM_GEMM_FLAG_VNNI_A | LIBXSMM_GEMM_FLAG_INTLV_A_FORMAT) && (d->k % 32) == 0) ? P_LOWBIT : XB_PATH_NONE;
+    }
+  }
+  /* every other A: the layout of xb_layout_a / xb_layout_b, a 16-bit C in column pairs under VNNI_C */
+  if ((a_f8 && vnni_a && trans_a) || (d->k % va) != 0) return XB_PATH_NONE;
+  if ((f & LIBXSMM_GEMM_FLAG_VNNI_C) != 0 && ((d->n % 2) != 0 || libxsmm_typesize((libxsmm_datatype)tc) != 2)) return XB_PATH_NONE;
+  if ((f & LIBXSMM_GEMM_FLAG_DECOMPRESS_A_VIA_BITMASK) != 0) {   /* bitmap-compressed A (:857-948): float operands, no batch reduce */
+    const int fa = (ta == LIBXSMM_DATATYPE_F32 || ta == LIBXSMM_DATATYPE_BF16 || ta == LIBXSMM_DATATYPE_F16);
+    const int fb = (tb == LIBXSMM_DATATYPE_F32 || tb == LIBXSMM_DATATYPE_BF16 || tb == LIBXSMM_DATATYPE_F16);
+    const int fc = (tc == LIBXSMM_DATATYPE_F32 || tc == LIBXSMM_DATATYPE_BF16 || tc == LIBXSMM_DATATYPE_F16);
+    const int kb = (ta == LIBXSMM_DATATYPE_F32 || tb == LIBXSMM_DATATYPE_F32) ? 1 : 2;
+    if (fa && fb && fc && d->br_type == 0 && (d->k % kb) == 0) path = P_BITMAP;
+  } else if (a4) {   /* 4-bit A with zero points x 8-bit B -> I32 (:1273-1321) */
+    const unsigned int need = LIBXSMM_GEMM_FLAG_VNNI_A | LIBXSMM_GEMM_FLAG_INTLV_A_FORMAT;
+    if ((f & need) == need && b8 && tc == LIBXSMM_DATATYPE_I32 && comp == LIBXSMM_DATATYPE_I32 && (d->k % 8) == 0 && (d->br_type == 0 || d->br_type == 3)) path = P_I4_I32;
+  } else {
+    const int f16comp = (comp == LIBXSMM_DATATYPE_F16 || comp == LIBXSMM_DATATYPE_F32 || comp == LIBXSMM_DATATYPE_IMPLICIT);
+    if (ta == LIBXSMM_DATATYPE_F64 && tb == ta && tc == ta && comp == ta) path = P_F64;
+    else if ((ta == LIBXSMM_DATATYPE_F32 || ta == LIBXSMM_DATATYPE_BF32) && (tb == LIBXSMM_DATATYPE_F32 || tb == LIBXSMM_DATATYPE_BF32)
+             && tc == LIBXSMM_DATATYPE_F32 && comp == LIBXSMM_DATATYPE_F32) path = P_F32;
+    else if (ta == LIBXSMM_DATATYPE_I16 && tb == ta && tc == LIBXSMM_DATATYPE_I32 && comp == LIBXSMM_DATATYPE_I32) path = P_I16;
+    else if (a8 && b8 && tc == LIBXSMM_DATATYPE_I32 && comp == LIBXSMM_DATATYPE_I32) path = P_I8_I32;
+    else if (a8 && b8 && tc == LIBXSMM_DATATYPE_F32 && comp == LIBXSMM_DATATYPE_I32) path = P_I8_F32;
+    else if (ta == LIBXSMM_DATATYPE_F16 && tb == ta && tc == LIBXSMM_DATATYPE_F16 && f16comp) path = P_F16_F16;
+    else if (ta == LIBXSMM_DATATYPE_F16 && tb == ta && tc == LIBXSMM_DATATYPE_F32 && f16comp) path = P_F16_F32;
+    else if (ta == LIBXSMM_DATATYPE_BF16 && tb == ta && tc == LIBXSMM_DATATYPE_F32 && comp == LIBXSMM_DATATYPE_F32) path = P_BF16_F32;
+    else if (ta == LIBXSMM_DATATYPE_BF16 && tb == ta && tc == LIBXSMM_DATATYPE_BF16 && comp == LIBXSMM_DATATYPE_F32) path = P_BF16_BF16;
+    /* 8-bit float A (:2171-2366 with a bf16 B, :2420-2630 with B and C of A's type or f32): f32 accumulate, one rounding */
+    else if (a_f8 && comp == LIBXSMM_DATATYPE_F32 && (f & (LIBXSMM_GEMM_FLAG_VNNI_B | LIBXSMM_GEMM_FLAG_VNNI_C)) == 0
+             && ((tb == ta && (tc == LIBXSMM_DATATYPE_F32 || tc == ta)) || (tb == LIBXSMM_DATATYPE_BF16 && (tc == LIBXSMM_DATATYPE_F32 || tc == LIBXSMM_DATATYPE_BF16)))) path = P_FP8;
+  }
+  if (d->fuse_colbias != 0 || d->cp_op != 0) {   /* fused form: float C only (the reference's f32 image of C) */
+    return (path == P_F32 || path == P_I8_F32 || path == P_F16_F16 || path == P_F16_F32 || path == P_BF16_F32 || path == P_BF16_BF16) ? path : XB_PATH_NONE;
+  }
+  return path;
 }
 
 static int xb_make_gemm_desc(xb_gemm_desc* d, const libxsmm_gemm_shape* shape, unsigned int flags, unsigned int prefetch,
@@ -339,7 +375,9 @@ static int xb_make_gemm_desc(xb_gemm_desc* d, const libxsmm_gemm_shape* shape, u
   if (shape->lda <= 0 || shape->ldb <= 0 || shape->ldc < shape->m) return 0;
   d->m = shape->m; d->n = shape->n; d->k = shape->k; d->lda = shape->lda; d->ldb = shape->ldb; d->ldc = shape->ldc;
   d->ta = (int)shape->a_in_type; d->tb = (int)shape->b_in_type; d->tc = (int)shape->out_type; d->tcomp = (int)shape->comp_type;
-  d->flags = flags | (ext ? LIBXSMM_GEMM_FLAG_USE_XGEMM_EXT_ABI : LIBXSMM_GEMM_FLAG_USE_XGEMM_ABI);
+  /* the ABI flag says which dispatcher made the handle, whatever the caller passed */
+  d->flags = (flags & ~(unsigned int)(LIBXSMM_GEMM_FLAG_USE_XGEMM_ABI | LIBXSMM_GEMM_FLAG_USE_XGEMM_EXT_ABI))
+           | (ext ? LIBXSMM_GEMM_FLAG_USE_XGEMM_EXT_ABI : LIBXSMM_GEMM_FLAG_USE_XGEMM_ABI);
   d->prefetch = (int)prefetch;
   if (br != NULL) {
     switch ((int)br->br_type) {
@@ -351,39 +389,8 @@ static int xb_make_gemm_desc(xb_gemm_desc* d, const libxsmm_gemm_shape* shape, u
     }
     if (d->br_type != 0) d->br_unroll = (br->br_unroll_hint > 0 && br->br_unroll_hint < 255) ? br->br_unroll_hint : 0;
   }
-  if (xb_is_mx8(d->ta) || xb_is_mx8(d->tb) || xb_is_mx8(d->tc)) {   /* MX fp8: its own layout rules, exact-order kernel only */
-    if (!xb_mx8_desc_ok(d, ext) || !xb_gemm_simt_supported(d)) return 0;
-    d->backend = LIBXSMM_B200_BACKEND_SIMT;
-    return 1;
-  }
-  if (xb_is_dq_family(d)) {   /* dequantising A: its own layout rules, exact-order kernel only */
-    if (!xb_dq_desc_ok(d, ext) || !xb_gemm_simt_supported(d)) return 0;
-    d->backend = LIBXSMM_B200_BACKEND_SIMT;
-    return 1;
-  }
-  if (xb_is_lowbit_family(d)) {   /* low-bit A x 8-bit B: its own layout rules, dp4a kernel on CUDA cores */
-    if (!xb_lowbit_desc_ok(d, ext) || !xb_gemm_simt_supported(d)) return 0;
-    d->backend = LIBXSMM_B200_BACKEND_SIMT;
-    return 1;
-  }
-  /* leading-dimension sanity for the layout in use (the reference JIT rejects these too) */
-  {
-    const int trans_a = (d->flags & LIBXSMM_GEMM_FLAG_TRANS_A) != 0, trans_b = (d->flags & LIBXSMM_GEMM_FLAG_TRANS_B) != 0;
-    const int is8 = (d->ta == LIBXSMM_DATATYPE_I8 || d->ta == LIBXSMM_DATATYPE_U8);
-    const int is16 = (d->ta == LIBXSMM_DATATYPE_BF16 || d->ta == LIBXSMM_DATATYPE_F16 || d->ta == LIBXSMM_DATATYPE_I16);
-    const int vnni_a = (d->flags & LIBXSMM_GEMM_FLAG_VNNI_A) != 0;
-    const int is_f8 = (d->ta == LIBXSMM_DATATYPE_BF8 || d->ta == LIBXSMM_DATATYPE_HF8);      /* 8-bit float A: VNNI factor 4, or 2 next to a bf16 B */
-    const int honours_trans = (d->ta == LIBXSMM_DATATYPE_F64 || d->ta == LIBXSMM_DATATYPE_F32 || d->ta == LIBXSMM_DATATYPE_BF32
-                            || d->ta == LIBXSMM_DATATYPE_BF16 || is_f8);
-    if (is_f8 && vnni_a && (trans_a || (d->k % (d->tb == LIBXSMM_DATATYPE_BF16 ? 2 : 4)) != 0)) return 0;
-    if (honours_trans && trans_a) { if (d->lda < d->k) return 0; } else if (d->lda < d->m) return 0;
-    if ((honours_trans || d->ta == LIBXSMM_DATATYPE_F16) && trans_b) { if (d->ldb < d->n) return 0; } else if (d->ldb < d->k) return 0;
-    if (vnni_a && is8 && (d->k % 4) != 0) return 0;
-    if (vnni_a && is16 && (d->k % 2) != 0) return 0;
-    if (is8 && d->tc == LIBXSMM_DATATYPE_F32 && (d->k % 4) != 0) return 0;
-  }
-  if ((d->flags & LIBXSMM_GEMM_FLAG_VNNI_C) != 0 && ((d->n % 2) != 0 || libxsmm_typesize((libxsmm_datatype)d->tc) != 2)) return 0;   /* 16-bit C in column pairs */
-  if (!xb_gemm_simt_supported(d)) return 0;
+  d->path = xb_gemm_path(d);
+  if (d->path == XB_PATH_NONE) return 0;
   d->backend = (!g_force_simt && (xb_gemm_tc_supported(d) || xb_gemm_ts_supported(d))) ? LIBXSMM_B200_BACKEND_TCGEN05 : LIBXSMM_B200_BACKEND_SIMT;
   return 1;
 }
@@ -435,7 +442,8 @@ LIBXSMM_API libxsmm_gemmfunction_ext libxsmm_dispatch_brgemm_ext(const libxsmm_g
   if (unary_argops.cp_unary_type != LIBXSMM_MELTW_TYPE_UNARY_NONE || binary_postops.d_binary_type != LIBXSMM_MELTW_TYPE_BINARY_NONE) {
     d.fuse_colbias = (binary_postops.d_binary_type == LIBXSMM_MELTW_TYPE_BINARY_ADD); d.d_type = d.tc; d.ldd = binary_postops.ldd;
     d.cp_op = (int)unary_argops.cp_unary_type; d.cp_flags = (int)(unary_argops.cp_unary_flags & LIBXSMM_MELTW_FLAG_UNARY_BITMASK_2BYTEMULT); d.ldcp = unary_argops.ldcp;
-    if (!xb_gemm_simt_supported(&d)) return NULL;       /* float C only */
+    d.path = xb_gemm_path(&d);
+    if (d.path == XB_PATH_NONE) return NULL;             /* float C only */
     d.backend = LIBXSMM_B200_BACKEND_SIMT;               /* the fused epilogue lives in the exact-order kernel */
   }
   slot = xb_registry_get(XB_KIND_GEMM_EXT, &d, sizeof(d), 2u * (unsigned int)d.m * (unsigned int)d.n * (unsigned int)d.k);
@@ -461,39 +469,31 @@ LIBXSMM_API libxsmm_tilecfgfunction libxsmm_dispatch_tilecfg_gemm(const libxsmm_
 typedef struct xb_copyback { void* host; const void* dev; size_t bytes; } xb_copyback;
 
 static size_t xb_extent_a(const xb_gemm_desc* d) {   /* elements touched in one A operand */
-  if (xb_dq_form(d) != XB_DQ_NONE) {                  /* bytes: int4 pairs [k/2][lda], bf8 VNNI2 [k/2][lda][2], else flat [k][lda] */
-    if (xb_dq_form(d) == XB_DQ_I4_F16) return (size_t)(d->k / 2 - 1) * d->lda + (size_t)d->m;
-    if ((d->flags & LIBXSMM_GEMM_FLAG_VNNI_A) != 0) return (size_t)(d->k / 2 - 1) * d->lda * 2 + (size_t)d->m * 2;
-    return (size_t)(d->k - 1) * d->lda + d->m;
-  }
-  switch (xb_lowbit_form(d)) {                        /* bytes: I2 [k/4][lda], I1 [k/4][lda/2], MXFP4 [k/8][lda][4] */
-    case XB_LB_I2: return (size_t)(d->k / 4 - 1) * d->lda + (size_t)d->m;
-    case XB_LB_I1: return (size_t)(d->k / 4 - 1) * (d->lda / 2) + (size_t)(d->m / 2);
-    case XB_LB_MXFP4: return (size_t)(d->k / 8 - 1) * d->lda * 4 + (size_t)d->m * 4;
+  int trans, v;
+  switch (d->path) {
+    case P_DQ:       /* bytes: int4 pairs [k/2][lda], bf8 VNNI2 [k/2][lda][2], else flat [k][lda] */
+      if (xb_dq_form(d) == XB_DQ_I4_F16) return (size_t)(d->k / 2 - 1) * d->lda + (size_t)d->m;
+      if ((d->flags & LIBXSMM_GEMM_FLAG_VNNI_A) != 0) return (size_t)(d->k / 2 - 1) * d->lda * 2 + (size_t)d->m * 2;
+      return (size_t)(d->k - 1) * d->lda + d->m;
+    case P_LOWBIT:   /* bytes: I2 [k/4][lda], I1 [k/4][lda/2], MXFP4 [k/8][lda][4] */
+      if (xb_lowbit_form(d) == XB_LB_I2) return (size_t)(d->k / 4 - 1) * d->lda + (size_t)d->m;
+      if (xb_lowbit_form(d) == XB_LB_I1) return (size_t)(d->k / 4 - 1) * (d->lda / 2) + (size_t)(d->m / 2);
+      return (size_t)(d->k / 8 - 1) * d->lda * 4 + (size_t)d->m * 4;
+    case P_I4_I32: return (size_t)(d->k / 8 - 1) * d->lda * 4 + (size_t)d->m * 4;   /* bytes: 8 k per 4 bytes */
+    case P_MX8: return (size_t)(d->k / 4 - 1) * d->lda * 4 + (size_t)d->m * 4;      /* VNNI4 */
     default: break;
   }
-  if (d->ta == LIBXSMM_DATATYPE_I4X2 || d->ta == LIBXSMM_DATATYPE_U4X2) return (size_t)(d->k / 8 - 1) * d->lda * 4 + (size_t)d->m * 4;   /* bytes: 8 k per 4 bytes */
-  if (xb_is_mx8(d->ta)) return (size_t)(d->k / 4 - 1) * d->lda * 4 + (size_t)d->m * 4;                                                 /* VNNI4 */
-  const int trans_a = (d->flags & LIBXSMM_GEMM_FLAG_TRANS_A) != 0, vnni_a = (d->flags & LIBXSMM_GEMM_FLAG_VNNI_A) != 0;
-  const int is8 = (d->ta == LIBXSMM_DATATYPE_I8 || d->ta == LIBXSMM_DATATYPE_U8);
-  const int is_f8 = (d->ta == LIBXSMM_DATATYPE_BF8 || d->ta == LIBXSMM_DATATYPE_HF8);
-  const int v = (is8 || (is_f8 && d->tb != LIBXSMM_DATATYPE_BF16)) ? 4 : 2;
-  const int honours_trans = (d->ta == LIBXSMM_DATATYPE_F64 || d->ta == LIBXSMM_DATATYPE_F32 || d->ta == LIBXSMM_DATATYPE_BF32
-                          || d->ta == LIBXSMM_DATATYPE_BF16 || is_f8);
-  if (honours_trans && trans_a && !vnni_a) return (size_t)(d->m - 1) * d->lda + d->k;
-  if ((vnni_a && d->ta != LIBXSMM_DATATYPE_F64 && d->ta != LIBXSMM_DATATYPE_F32) || (is8 && d->tc == LIBXSMM_DATATYPE_F32)) {
-    return (size_t)(d->k / v - 1) * d->lda * v + (size_t)d->m * v;
-  }
+  v = xb_layout_a(d, &trans);
+  if (v > 1) return (size_t)(d->k / v - 1) * d->lda * v + (size_t)d->m * v;
+  if (trans && (d->flags & LIBXSMM_GEMM_FLAG_VNNI_A) == 0) return (size_t)(d->m - 1) * d->lda + d->k;
   return (size_t)(d->k - 1) * d->lda + d->m;
 }
 
 static size_t xb_extent_b(const xb_gemm_desc* d) {
-  if (xb_is_mx8(d->tb)) return (size_t)(d->k / 4 - 1) * d->ldb * 4 + (size_t)d->n * 4;                                                 /* VNNI4-T */
-  const int trans_b = (d->flags & LIBXSMM_GEMM_FLAG_TRANS_B) != 0, vnni_b = (d->flags & LIBXSMM_GEMM_FLAG_VNNI_B) != 0;
-  const int honours = (d->tb == LIBXSMM_DATATYPE_F64 || d->tb == LIBXSMM_DATATYPE_F32 || d->tb == LIBXSMM_DATATYPE_BF32
-                    || d->tb == LIBXSMM_DATATYPE_BF16 || d->tb == LIBXSMM_DATATYPE_F16 || d->tb == LIBXSMM_DATATYPE_BF8 || d->tb == LIBXSMM_DATATYPE_HF8);
-  if (honours && trans_b && vnni_b && d->tb == LIBXSMM_DATATYPE_BF16) return (size_t)(d->k / 2 - 1) * d->ldb * 2 + (size_t)d->n * 2;
-  if (honours && trans_b) return (size_t)(d->k - 1) * d->ldb + d->n;
+  int trans;
+  const int v = xb_layout_b(d, &trans);
+  if (v > 1) return (size_t)(d->k / v - 1) * d->ldb * v + (size_t)d->n * v;   /* VNNI-T */
+  if (trans) return (size_t)(d->k - 1) * d->ldb + d->n;
   return (size_t)(d->n - 1) * d->ldb + d->k;
 }
 
@@ -537,38 +537,43 @@ static const void* xb_stage_ptr_array(const void* arr, unsigned long long br, si
 static void xb_stage_sides(const xb_gemm_desc* d, const libxsmm_gemm_param* p, unsigned long long br, xb_gemm_rec* one, int* staged) {
   const int sides = xb_gemm_sides(d);
   if (sides == 0) return;
-  if (xb_dq_form(d) != XB_DQ_NONE) {   /* a.tertiary: m row scales (f32 next to a bf16 B, else f16); int4: a.quaternary, m f16 zero points.
-                                        * One set for every r. */
-    one->a_s = xb_stage_in(p->a.tertiary, (size_t)d->m * (xb_dq_form(d) == XB_DQ_I8_BF16 ? 4 : 2), staged);
-    if (sides & XB_SIDE_A_Q) one->a_q = xb_stage_in(p->a.quaternary, (size_t)d->m * 2, staged);
-  } else if (xb_lowbit_form(d) == XB_LB_MXFP4) {   /* a.tertiary: E8M0 bytes [k/32][lda]; b.tertiary: f32 [n][ldb/32]; block r's as in xb_gemm_simt */
-    const size_t ea = (size_t)(d->k / 32 - 1) * d->lda + (size_t)d->m, eb = ((size_t)(d->n - 1) * (size_t)(d->ldb / 32) + (size_t)(d->k / 32)) * 4;
-    if (d->br_type == 1) {
-      one->a_s = xb_stage_ptr_array(p->a.tertiary, br, ea, staged);
-      one->b_s = xb_stage_ptr_array(p->b.tertiary, br, eb, staged);
-    } else {
-      size_t span_sa = ea, span_sb = eb;
-      unsigned long long r;
-      if (d->br_type == 3 && br > 0) { span_sa += (size_t)(br - 1) * (size_t)((d->br_stride_a * 2) / 32); span_sb += (size_t)(br - 1) * (size_t)(d->br_stride_b / 32) * 4; }
-      if (d->br_type == 2) for (r = 0; r < br; ++r) {
-        const long long oa = (((const long long*)p->a.secondary)[r] * 2) / 32, ob = ((const long long*)p->b.secondary)[r] / 32;
-        if (oa > 0 && ea + (size_t)oa > span_sa) span_sa = ea + (size_t)oa;
-        if (ob > 0 && eb + (size_t)ob * 4 > span_sb) span_sb = eb + (size_t)ob * 4;
+  switch (d->path) {
+    case P_DQ:       /* a.tertiary: m row scales (f32 next to a bf16 B, else f16); int4: a.quaternary, m f16 zero points. One set for every r. */
+      one->a_s = xb_stage_in(p->a.tertiary, (size_t)d->m * (xb_dq_form(d) == XB_DQ_I8_BF16 ? 4 : 2), staged);
+      if (sides & XB_SIDE_A_Q) one->a_q = xb_stage_in(p->a.quaternary, (size_t)d->m * 2, staged);
+      break;
+    case P_LOWBIT: { /* MXFP4: a.tertiary, E8M0 bytes [k/32][lda]; b.tertiary, f32 [n][ldb/32]; block r's as in xb_gemm_simt */
+      const size_t ea = (size_t)(d->k / 32 - 1) * d->lda + (size_t)d->m, eb = ((size_t)(d->n - 1) * (size_t)(d->ldb / 32) + (size_t)(d->k / 32)) * 4;
+      if (d->br_type == 1) {
+        one->a_s = xb_stage_ptr_array(p->a.tertiary, br, ea, staged);
+        one->b_s = xb_stage_ptr_array(p->b.tertiary, br, eb, staged);
+      } else {
+        size_t span_sa = ea, span_sb = eb;
+        unsigned long long r;
+        if (d->br_type == 3 && br > 0) { span_sa += (size_t)(br - 1) * (size_t)((d->br_stride_a * 2) / 32); span_sb += (size_t)(br - 1) * (size_t)(d->br_stride_b / 32) * 4; }
+        if (d->br_type == 2) for (r = 0; r < br; ++r) {
+          const long long oa = (((const long long*)p->a.secondary)[r] * 2) / 32, ob = ((const long long*)p->b.secondary)[r] / 32;
+          if (oa > 0 && ea + (size_t)oa > span_sa) span_sa = ea + (size_t)oa;
+          if (ob > 0 && eb + (size_t)ob * 4 > span_sb) span_sb = eb + (size_t)ob * 4;
+        }
+        one->a_s = xb_stage_in(p->a.tertiary, span_sa, staged);
+        one->b_s = xb_stage_in(p->b.tertiary, span_sb, staged);
       }
-      one->a_s = xb_stage_in(p->a.tertiary, span_sa, staged);
-      one->b_s = xb_stage_in(p->b.tertiary, span_sb, staged);
+      break;
     }
-  } else if (sides == XB_SIDE_A_Q) {   /* int4 A x 8-bit B: a.quaternary, one zero-point byte per row (and per reduce step) */
-    const size_t zb = (size_t)d->m + ((d->br_type == 3 && br > 0) ? (size_t)(br - 1) * (size_t)((d->br_stride_a * 2) / d->k) : 0);
-    one->a_q = xb_stage_in(p->a.quaternary, zb, staged);
-  } else {   /* MX fp8, E8M0 block scales: a.tertiary [br][k/32][lda], b.tertiary [br][k/32][ldb] and, for an MXBF8 C, c.tertiary [n][ldc/32] */
-    one->a_s = xb_stage_in(p->a.tertiary, xb_extent_mx_scales(d, br, d->lda, d->m), staged);
-    one->b_s = xb_stage_in(p->b.tertiary, xb_extent_mx_scales(d, br, d->ldb, d->n), staged);
-    if (sides & XB_SIDE_C_S) {
-      *staged = 1;                     /* the f32 image lives in the scratch arena until the caller's sync */
-      one->c_s = (p->c.tertiary != NULL && xb_rt_ptr_kind(p->c.tertiary) == 0) ? xb_rt_scratch((size_t)(d->n - 1) * (d->ldc / 32) + (size_t)(d->m / 32))
-                                                                               : p->c.tertiary;
+    case P_I4_I32: { /* int4 A x 8-bit B: a.quaternary, one zero-point byte per row (and per reduce step) */
+      const size_t zb = (size_t)d->m + ((d->br_type == 3 && br > 0) ? (size_t)(br - 1) * (size_t)((d->br_stride_a * 2) / d->k) : 0);
+      one->a_q = xb_stage_in(p->a.quaternary, zb, staged);
+      break;
     }
+    default:         /* MX fp8, E8M0 block scales: a.tertiary [br][k/32][lda], b.tertiary [br][k/32][ldb] and, for an MXBF8 C, c.tertiary [n][ldc/32] */
+      one->a_s = xb_stage_in(p->a.tertiary, xb_extent_mx_scales(d, br, d->lda, d->m), staged);
+      one->b_s = xb_stage_in(p->b.tertiary, xb_extent_mx_scales(d, br, d->ldb, d->n), staged);
+      if (sides & XB_SIDE_C_S) {
+        *staged = 1;                   /* the f32 image lives in the scratch arena until the caller's sync */
+        one->c_s = (p->c.tertiary != NULL && xb_rt_ptr_kind(p->c.tertiary) == 0) ? xb_rt_scratch((size_t)(d->n - 1) * (d->ldc / 32) + (size_t)(d->m / 32))
+                                                                                 : p->c.tertiary;
+      }
   }
 }
 
@@ -650,9 +655,7 @@ static void xb_invoke_gemm(const xb_slot* s, const libxsmm_gemm_param* p) {
     cb.host = p->c.primary; cb.dev = dc; cb.bytes = ext_c; need_cb = 1; staged = 1;
     L.one.c = dc;
   } else L.one.c = p->c.primary;
-  if (d->tc == LIBXSMM_DATATYPE_F32 && (d->ta == LIBXSMM_DATATYPE_I8 || d->ta == LIBXSMM_DATATYPE_U8) && p->c.tertiary != NULL) {
-    L.one.scf = *(const float*)p->c.tertiary;
-  }
+  if (d->path == P_I8_F32 && p->c.tertiary != NULL) L.one.scf = *(const float*)p->c.tertiary;
   if (s->kind == XB_KIND_GEMM_EXT && (d->fuse_colbias != 0 || d->cp_op != 0)) {   /* d.primary: bias column; c.secondary: ReLU bitmask */
     const libxsmm_gemm_ext_param* pe = (const libxsmm_gemm_ext_param*)p;
     if (d->fuse_colbias != 0) {
@@ -772,11 +775,10 @@ static const xb_slot* xb_gemm_slot(const void* kernel) {
  * call only, the strided forms have no argument struct for the int8 -> f32 scale (c.tertiary) or for side operands
  * (xb_gemm_sides: libxsmm_b200_gemm_batch_strided_scaled takes scales), and the per-tile records carry no MX fp8 block scales. */
 static int xb_batch_refused(const xb_gemm_desc* d, int strided) {
-  const int i8 = (d->ta == LIBXSMM_DATATYPE_I8 || d->ta == LIBXSMM_DATATYPE_U8);
   if (d->fuse_colbias != 0 || (d->flags & LIBXSMM_GEMM_FLAG_VNNI_C) != 0) return 1;
-  if (strided ? xb_gemm_sides(d) != 0 : xb_is_mx8(d->ta)) return 1;
+  if (strided ? xb_gemm_sides(d) != 0 : d->path == P_MX8) return 1;
   if (d->cp_op == LIBXSMM_MELTW_TYPE_UNARY_RELU && (d->cp_flags & LIBXSMM_MELTW_FLAG_UNARY_BITMASK_2BYTEMULT) != 0) return 1;
-  return (strided && i8 && d->tc == LIBXSMM_DATATYPE_F32) ? 1 : 0;
+  return (strided && d->path == P_I8_F32) ? 1 : 0;
 }
 
 /* host-resident strided batch: chunked H2D -> kernel -> D2H through device scratch */
@@ -1079,8 +1081,8 @@ static libxsmm_b200_gemm_plan* xb_plan_make(const xb_slot* s, const libxsmm_gemm
   long long t;
   int mx_arrays, sides;
   if (s == NULL || params == NULL || count <= 0 || xb_batch_refused(&s->u.gemm, 0)) return NULL;
-  mx_arrays = (xb_lowbit_form(&s->u.gemm) == XB_LB_MXFP4);
   sides = xb_gemm_sides(&s->u.gemm);
+  mx_arrays = (s->u.gemm.path == P_LOWBIT && (sides & XB_SIDE_B_S) != 0);   /* MXFP4 x I8 */
   for (t = 0; t < count && sides != 0; ++t) {   /* every tile brings each side operand of the handle */
     xb_gemm_rec r;
     memset(&r, 0, sizeof(r));
@@ -1128,8 +1130,7 @@ static libxsmm_b200_gemm_plan* xb_plan_make(const xb_slot* s, const libxsmm_gemm
         memcpy(arrays + off, p->b.tertiary, (size_t)r->br * 8); r->b_s = (char*)plan->d_arrays + off; off += (size_t)r->br * 8;
       }
     }
-    if (s->u.gemm.tc == LIBXSMM_DATATYPE_F32 && (s->u.gemm.ta == LIBXSMM_DATATYPE_I8 || s->u.gemm.ta == LIBXSMM_DATATYPE_U8)
-        && p->c.tertiary != NULL) r->scf = *(const float*)p->c.tertiary;
+    if (s->u.gemm.path == P_I8_F32 && p->c.tertiary != NULL) r->scf = *(const float*)p->c.tertiary;
   }
   plan->d_recs = (xb_gemm_rec*)xb_rt_device_malloc((size_t)count * sizeof(xb_gemm_rec));
   if (plan->d_recs == NULL) { free(arrays); free(recs); xb_rt_device_free(plan->d_arrays); free(plan); return NULL; }

@@ -44,8 +44,12 @@ typedef struct xb_gemm_desc {
   int fuse_colbias, d_type, ldd;      /* C += colbias (binary ADD with BCAST_COL) */
   int cp_op, cp_flags, ldcp;          /* unary on C: RELU (+bitmask) or SIGMOID */
   int backend;                        /* libxsmm_b200_backend chosen at dispatch */
-  int pad_;
+  int path;                           /* exact-order path (xb_gemm_path of the fields above), computed at dispatch */
 } xb_gemm_desc;
+
+/* the exact-order paths (gemm_simt.cu): the kernels take the path as a run-time argument and switch on it */
+enum { P_F64 = 0, P_F32, P_I16, P_I8_I32, P_I8_F32, P_F16_F16, P_F16_F32, P_BF16_F32, P_BF16_BF16, P_I4_I32, P_BITMAP, P_FP8, P_MX8, P_DQ,
+       XB_PATH_NONE, P_LOWBIT };
 
 typedef struct xb_meltw_desc {
   int op_class;                       /* libxsmm_meltw_operation */
@@ -154,17 +158,13 @@ enum { XB_SIDE_A_S = 1, XB_SIDE_B_S = 2, XB_SIDE_C_S = 4, XB_SIDE_A_Q = 8 };
 __host__ __device__
 #endif
 static inline int xb_gemm_sides(const xb_gemm_desc* d) {
-  const int dq = xb_dq_form(d);
-  if (d->ta == LIBXSMM_DATATYPE_MXBF8 || d->ta == LIBXSMM_DATATYPE_MXHF8) {
-    return XB_SIDE_A_S | XB_SIDE_B_S | (d->tc == LIBXSMM_DATATYPE_MXBF8 ? XB_SIDE_C_S : 0);
+  switch (d->path) {
+    case P_MX8: return XB_SIDE_A_S | XB_SIDE_B_S | (d->tc == LIBXSMM_DATATYPE_MXBF8 ? XB_SIDE_C_S : 0);
+    case P_DQ: return (xb_dq_form(d) == XB_DQ_BF8_F16) ? 0 : XB_SIDE_A_S | (xb_dq_form(d) == XB_DQ_I4_F16 ? XB_SIDE_A_Q : 0);
+    case P_LOWBIT: return (xb_lowbit_form(d) == XB_LB_MXFP4) ? XB_SIDE_A_S | XB_SIDE_B_S : 0;
+    case P_I4_I32: return XB_SIDE_A_Q;
+    default: return 0;
   }
-  if (dq == XB_DQ_I8_BF16 || dq == XB_DQ_I8_F16) return XB_SIDE_A_S;
-  if (dq == XB_DQ_I4_F16) return XB_SIDE_A_S | XB_SIDE_A_Q;
-  if (xb_lowbit_form(d) == XB_LB_MXFP4) return XB_SIDE_A_S | XB_SIDE_B_S;
-  if ((d->ta == LIBXSMM_DATATYPE_I4X2 || d->ta == LIBXSMM_DATATYPE_U4X2) && (d->tb == LIBXSMM_DATATYPE_I8 || d->tb == LIBXSMM_DATATYPE_U8)) {
-    return XB_SIDE_A_Q;
-  }
-  return 0;
 }
 
 /* 1 if a side operand of `sides` is NULL in r */
@@ -301,6 +301,7 @@ int xb_bcsc_tc_variant(const xb_sparse_desc* d, unsigned long long n_blocks);
 void xb_bcsc_state_free(void* work);
 
 /* ---- host runtime (host_core.c) ---------------------------------------------------------------- */
+int xb_gemm_path(const xb_gemm_desc* d);   /* the exact-order path that serves d, or XB_PATH_NONE: whether d dispatches */
 xb_slot* xb_slot_of(const void* fnptr);    /* NULL if not one of our thunks */
 const xb_sparse_desc* xb_fsspmdm_desc(const libxsmm_fsspmdm* handle);   /* host_sparse.c: the descriptor of an fsspmdm handle, or NULL */
 void xb_invoke(int slot, const void* param);

@@ -16,9 +16,8 @@ extern int oracle_gemm_lowbit(const int* dims, const int* types, unsigned int fl
 int __wrap_xb_gemm_simt_launch(const xb_gemm_launch* L) {
   const xb_gemm_desc* d = &L->d;
   const int dims[6] = { d->m, d->n, d->k, d->lda, d->ldb, d->ldc }, types[4] = { d->ta, d->tb, d->tcomp, d->tc };
-  const int form = xb_lowbit_form(d);
   long long t; int rc = 0;
-  if (form == XB_LB_NONE) return __real_xb_gemm_simt_launch(L);
+  if (d->path != P_LOWBIT) return __real_xb_gemm_simt_launch(L);
   for (t = 0; t < L->count && rc == 0; ++t) {
     const xb_gemm_rec r = xb_gemm_tile(L, t);
     xb_rt_count_launch();

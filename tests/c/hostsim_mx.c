@@ -17,7 +17,7 @@ int __wrap_xb_gemm_simt_launch(const xb_gemm_launch* L) {
   const xb_gemm_desc* d = &L->d;
   const int dims[6] = { d->m, d->n, d->k, d->lda, d->ldb, d->ldc }, types[4] = { d->ta, d->tb, d->tcomp, d->tc };
   long long t; int rc = 0;
-  if (d->ta != LIBXSMM_DATATYPE_MXBF8 && d->ta != LIBXSMM_DATATYPE_MXHF8) return __real_xb_gemm_simt_launch(L);
+  if (d->path != P_MX8) return __real_xb_gemm_simt_launch(L);
   for (t = 0; t < L->count && rc == 0; ++t) {
     const xb_gemm_rec r = xb_gemm_tile(L, t);
     xb_rt_count_launch();

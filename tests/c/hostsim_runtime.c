@@ -99,8 +99,8 @@ static int sim_gemm_tile(const xb_gemm_desc* d, const xb_gemm_rec* r) {
   const int dims[6] = { d->m, d->n, d->k, d->lda, d->ldb, d->ldc }, types[4] = { d->ta, d->tb, d->tcomp, d->tc };
   const unsigned int flags = d->flags & ~(unsigned int)LIBXSMM_GEMM_FLAG_VNNI_C;
   ++g_launches; ++g_launches_by[LIBXSMM_B200_BACKEND_SIMT];
-  if ((d->flags & LIBXSMM_GEMM_FLAG_DECOMPRESS_A_VIA_BITMASK) != 0) return oracle_gemm_bitmap(dims, types, flags, r->a, r->b, r->c, (const unsigned char*)r->a_q);
-  if (d->ta == LIBXSMM_DATATYPE_I4X2 || d->ta == LIBXSMM_DATATYPE_U4X2) {
+  if (d->path == P_BITMAP) return oracle_gemm_bitmap(dims, types, flags, r->a, r->b, r->c, (const unsigned char*)r->a_q);
+  if (d->path == P_I4_I32) {
     return oracle_gemm_i4(dims, flags, d->br_type, d->br_stride_a, d->br_stride_b, r->br, (const unsigned char*)r->a, (const unsigned char*)r->b, (int*)r->c, (const unsigned char*)r->a_q);
   }
   if (d->fuse_colbias != 0 || d->cp_op != 0) {
@@ -111,7 +111,6 @@ static int sim_gemm_tile(const xb_gemm_desc* d, const xb_gemm_rec* r) {
   return oracle_gemm(dims, types, flags, d->br_type, d->br_stride_a, d->br_stride_b, r->br, (void*)(uintptr_t)r->a, (void*)(uintptr_t)r->b, r->c,
                      (long long*)(uintptr_t)r->a_aux, (long long*)(uintptr_t)r->b_aux, r->scf, 0);
 }
-int xb_gemm_simt_supported(const xb_gemm_desc* d) { return d->m > 0 && d->n > 0 && d->k > 0; }
 int xb_gemm_simt_launch(const xb_gemm_launch* L) {
   long long t; int rc = 0;
   for (t = 0; t < L->count && rc == 0; ++t) { const xb_gemm_rec r = xb_gemm_tile(L, t); rc = sim_gemm_tile(&L->d, &r); }
