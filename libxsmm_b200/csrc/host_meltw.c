@@ -9,6 +9,7 @@
 #include <stdlib.h>
 #include <string.h>
 #include "xb_internal.h"
+#include "xb_device.cuh"
 
 extern int xb_host_registry_get(int kind, const void* key, size_t key_size, unsigned int nflops);
 
@@ -44,10 +45,136 @@ LIBXSMM_API libxsmm_meltw_ternary_shape libxsmm_create_meltw_ternary_shape(libxs
   return s;
 }
 
+/* ---- the rules: which family serves a descriptor, and which side operands its calls carry --------------------------------- */
+static int is_f(int t) {
+  return t == LIBXSMM_DATATYPE_F32 || t == LIBXSMM_DATATYPE_BF16 || t == LIBXSMM_DATATYPE_F16 || t == LIBXSMM_DATATYPE_BF8 || t == LIBXSMM_DATATYPE_HF8;
+}
+static int is_i(int t) { return t == LIBXSMM_DATATYPE_I8 || t == LIBXSMM_DATATYPE_I16 || t == LIBXSMM_DATATYPE_I32; }
+
+int xb_meltw_family(const xb_meltw_desc* d) {
+  const int f_in_out = is_f(d->t_in0) && is_f(d->t_out), ts = xb_dev_typesize(d->t_in0);
+  const int in64 = d->t_in0 == LIBXSMM_DATATYPE_F64 && d->t_out == LIBXSMM_DATATYPE_F64;
+  if (d->op_class == LIBXSMM_MELTW_OPERATION_UNARY) {
+    switch (d->op) {
+      case LIBXSMM_MELTW_TYPE_UNARY_IDENTITY: case LIBXSMM_MELTW_TYPE_UNARY_XOR: case LIBXSMM_MELTW_TYPE_UNARY_X2: case LIBXSMM_MELTW_TYPE_UNARY_DUMP:
+      case LIBXSMM_MELTW_TYPE_UNARY_SQRT: case LIBXSMM_MELTW_TYPE_UNARY_NEGATE: case LIBXSMM_MELTW_TYPE_UNARY_INC:
+      case LIBXSMM_MELTW_TYPE_UNARY_RECIPROCAL: case LIBXSMM_MELTW_TYPE_UNARY_RECIPROCAL_SQRT:
+        if (in64 && d->t_comp == LIBXSMM_DATATYPE_F64) return (d->op == LIBXSMM_MELTW_TYPE_UNARY_DUMP) ? XB_FAM_NONE : XB_FAM_MAP;
+        return f_in_out ? XB_FAM_MAP : XB_FAM_NONE;
+      case LIBXSMM_MELTW_TYPE_UNARY_TANH: case LIBXSMM_MELTW_TYPE_UNARY_TANH_INV: case LIBXSMM_MELTW_TYPE_UNARY_SIGMOID:
+      case LIBXSMM_MELTW_TYPE_UNARY_SIGMOID_INV: case LIBXSMM_MELTW_TYPE_UNARY_GELU: case LIBXSMM_MELTW_TYPE_UNARY_GELU_INV:
+      case LIBXSMM_MELTW_TYPE_UNARY_EXP: case LIBXSMM_MELTW_TYPE_UNARY_REPLICATE_COL_VAR:
+      case LIBXSMM_MELTW_TYPE_UNARY_RELU: case LIBXSMM_MELTW_TYPE_UNARY_RELU_INV: case LIBXSMM_MELTW_TYPE_UNARY_LEAKY_RELU:
+      case LIBXSMM_MELTW_TYPE_UNARY_LEAKY_RELU_INV: case LIBXSMM_MELTW_TYPE_UNARY_ELU: case LIBXSMM_MELTW_TYPE_UNARY_ELU_INV:
+        return f_in_out ? XB_FAM_MAP : XB_FAM_NONE;
+      case LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X_OP_ADD: case LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X2_OP_ADD:
+      case LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X_X2_OP_ADD: case LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X_OP_MAX:
+      case LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X_OP_MIN: case LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X_OP_ABSMAX:
+      case LIBXSMM_MELTW_TYPE_UNARY_REDUCE_COLS_IDX_OP_ADD: case LIBXSMM_MELTW_TYPE_UNARY_REDUCE_COLS_IDX_OP_MAX:
+      case LIBXSMM_MELTW_TYPE_UNARY_REDUCE_COLS_IDX_OP_MIN:
+        return (in64 || f_in_out) ? XB_FAM_REDUCE : XB_FAM_NONE;
+      case LIBXSMM_MELTW_TYPE_UNARY_REDUCE_TO_SCALAR_OP_ADD: return (in64 || f_in_out) ? XB_FAM_SCALAR : XB_FAM_NONE;
+      case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_NORMT: return XB_FAM_TRANSFORM;
+      case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_VNNI2: case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_VNNI2_PAD:
+      case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_VNNI2T: case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_VNNI2_TO_VNNI2T:
+      case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_VNNI2T_TO_NORM: case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_VNNI4T:
+      case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_VNNI4T_TO_NORM: case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_VNNI8T:
+      case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_VNNI8T_TO_NORM: case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_PADM_MOD2:
+      case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_PADN_MOD2: case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_PADNM_MOD2:
+        return (ts == 2) ? XB_FAM_TRANSFORM : XB_FAM_NONE;
+      case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_VNNI4: case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_VNNI4_PAD:
+      case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_VNNI4_TO_VNNI4T:
+        return (ts <= 2) ? XB_FAM_TRANSFORM : XB_FAM_NONE;
+      case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_VNNI4_TO_NORM: case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_PADM_MOD4:
+      case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_PADN_MOD4: case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_PADNM_MOD4:
+      case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_VNNI4_TO_VNNI2:
+        return (ts == 1) ? XB_FAM_TRANSFORM : XB_FAM_NONE;
+      case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_VNNI8: case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_VNNI8_PAD:
+      case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_VNNI8_TO_VNNI8T:
+        return (ts >= 1 && ts <= 2) ? XB_FAM_TRANSFORM : XB_FAM_NONE;
+      case LIBXSMM_MELTW_TYPE_UNARY_GATHER: case LIBXSMM_MELTW_TYPE_UNARY_SCATTER: return (ts >= 1 && ts <= 4) ? XB_FAM_GS : XB_FAM_NONE;
+      case LIBXSMM_MELTW_TYPE_UNARY_QUANT:
+        if (d->t_in0 == LIBXSMM_DATATYPE_BF16 && (d->t_out == LIBXSMM_DATATYPE_MXFP4X2 || d->t_out == LIBXSMM_DATATYPE_NVFP4X2 || d->t_out == LIBXSMM_DATATYPE_MXBF8)) return XB_FAM_MXQUANT;
+        return (d->t_in0 == LIBXSMM_DATATYPE_F32 && is_i(d->t_out)) ? XB_FAM_QUANT : XB_FAM_NONE;
+      case LIBXSMM_MELTW_TYPE_UNARY_DEQUANT: return (d->t_out == LIBXSMM_DATATYPE_F32 && is_i(d->t_in0)) ? XB_FAM_QUANT : XB_FAM_NONE;
+      case LIBXSMM_MELTW_TYPE_UNARY_DROPOUT: case LIBXSMM_MELTW_TYPE_UNARY_DROPOUT_INV: return f_in_out ? XB_FAM_DROPOUT : XB_FAM_NONE;
+      case LIBXSMM_MELTW_TYPE_UNARY_UNZIP: case LIBXSMM_MELTW_TYPE_UNARY_DECOMP_FP32_TO_BF16X2: case LIBXSMM_MELTW_TYPE_UNARY_DECOMP_FP32_TO_BF16X3:
+        return (d->t_in0 == LIBXSMM_DATATYPE_F32) ? XB_FAM_SPLIT : XB_FAM_NONE;
+      default: return XB_FAM_NONE;
+    }
+  }
+  if (d->op_class == LIBXSMM_MELTW_OPERATION_BINARY) {
+    const int all64 = in64 && d->t_in1 == LIBXSMM_DATATYPE_F64 && d->t_comp == LIBXSMM_DATATYPE_F64, f3 = f_in_out && is_f(d->t_in1);
+    switch (d->op) {
+      case LIBXSMM_MELTW_TYPE_BINARY_ADD: case LIBXSMM_MELTW_TYPE_BINARY_MUL: case LIBXSMM_MELTW_TYPE_BINARY_SUB:
+      case LIBXSMM_MELTW_TYPE_BINARY_DIV: case LIBXSMM_MELTW_TYPE_BINARY_MULADD: case LIBXSMM_MELTW_TYPE_BINARY_MAX:
+      case LIBXSMM_MELTW_TYPE_BINARY_MIN:
+        return (all64 || f3) ? XB_FAM_MAP : XB_FAM_NONE;
+      case LIBXSMM_MELTW_TYPE_BINARY_CMP_OP_GT: case LIBXSMM_MELTW_TYPE_BINARY_CMP_OP_GE: case LIBXSMM_MELTW_TYPE_BINARY_CMP_OP_LT:
+      case LIBXSMM_MELTW_TYPE_BINARY_CMP_OP_LE: case LIBXSMM_MELTW_TYPE_BINARY_CMP_OP_EQ: case LIBXSMM_MELTW_TYPE_BINARY_CMP_OP_NE:
+        return (is_f(d->t_in0) && is_f(d->t_in1)) ? XB_FAM_MAP : XB_FAM_NONE;
+      case LIBXSMM_MELTW_TYPE_BINARY_ZIP:
+        return (d->t_in0 == LIBXSMM_DATATYPE_U16 || d->t_in0 == LIBXSMM_DATATYPE_BF16 || d->t_in0 == LIBXSMM_DATATYPE_I16) ? XB_FAM_MAP : XB_FAM_NONE;
+      case LIBXSMM_MELTW_TYPE_BINARY_MUL_AND_REDUCE_TO_SCALAR_OP_ADD: return (all64 || f3) ? XB_FAM_SCALAR : XB_FAM_NONE;
+      default: return XB_FAM_NONE;
+    }
+  }
+  if (d->op_class == LIBXSMM_MELTW_OPERATION_TERNARY) {
+    const int f3 = f_in_out && is_f(d->t_in1);
+    switch (d->op) {
+      case LIBXSMM_MELTW_TYPE_TERNARY_SELECT:
+        return ((in64 && d->t_in1 == LIBXSMM_DATATYPE_F64 && d->t_in2 == LIBXSMM_DATATYPE_F64 && d->t_comp == LIBXSMM_DATATYPE_F64) || f3) ? XB_FAM_MAP : XB_FAM_NONE;
+      case LIBXSMM_MELTW_TYPE_TERNARY_MULADD: case LIBXSMM_MELTW_TYPE_TERNARY_NMULADD: return (f3 && is_f(d->t_in2)) ? XB_FAM_MAP : XB_FAM_NONE;
+      default: return XB_FAM_NONE;
+    }
+  }
+  return XB_FAM_NONE;
+}
+
+/* Which side operands a call of a served descriptor carries (reference src/generator_mateltwise_reference_impl.c: the relu family
+ * :2138-2194, dropout :2091 and :43-73, quantisers :2195-2360, reductions :1065-1443, gather / scatter :1444-1794). Stochastic rounding
+ * draws from op.secondary when it rounds to BF8 (:310-316): in the element-wise unary ops of the generic loop (:2470-2498) over a
+ * non-F64 input, and in every binary map and ternary op. */
+int xb_meltw_sides(const xb_meltw_desc* d) {
+  const int fam = xb_meltw_family(d);
+  const unsigned int f = d->flags;
+  const int to_bf8 = d->t_out == LIBXSMM_DATATYPE_BF8;
+  const int sr = ((f & LIBXSMM_MELTW_FLAG_UNARY_STOCHASTIC_ROUND) && to_bf8 && d->t_in0 != LIBXSMM_DATATYPE_F64) ? XB_MSIDE_STATE : 0;
+  if (d->op_class == LIBXSMM_MELTW_OPERATION_BINARY) {
+    return ((f & LIBXSMM_MELTW_FLAG_BINARY_STOCHASTIC_ROUND) && to_bf8 && d->op < LIBXSMM_MELTW_TYPE_BINARY_CMP_OP_GT
+            && d->op != LIBXSMM_MELTW_TYPE_BINARY_MUL_AND_REDUCE_TO_SCALAR_OP_ADD && d->op != LIBXSMM_MELTW_TYPE_BINARY_ZIP) ? XB_MSIDE_STATE : 0;
+  }
+  if (d->op_class == LIBXSMM_MELTW_OPERATION_TERNARY) return ((f & LIBXSMM_MELTW_FLAG_TERNARY_STOCHASTIC_ROUND) && to_bf8) ? XB_MSIDE_STATE : 0;
+  switch (d->op) {
+    case LIBXSMM_MELTW_TYPE_UNARY_RELU: return (f & LIBXSMM_MELTW_FLAG_UNARY_BITMASK_2BYTEMULT) ? XB_MSIDE_MASK_OUT : 0;
+    case LIBXSMM_MELTW_TYPE_UNARY_LEAKY_RELU: case LIBXSMM_MELTW_TYPE_UNARY_ELU:
+      return XB_MSIDE_ALPHA | ((f & LIBXSMM_MELTW_FLAG_UNARY_BITMASK_2BYTEMULT) ? XB_MSIDE_MASK_OUT : 0);
+    case LIBXSMM_MELTW_TYPE_UNARY_RELU_INV: return XB_MSIDE_IN_AUX;
+    case LIBXSMM_MELTW_TYPE_UNARY_LEAKY_RELU_INV: case LIBXSMM_MELTW_TYPE_UNARY_ELU_INV: case LIBXSMM_MELTW_TYPE_UNARY_DROPOUT_INV:
+      return XB_MSIDE_ALPHA | XB_MSIDE_IN_AUX;
+    case LIBXSMM_MELTW_TYPE_UNARY_DROPOUT:
+      return XB_MSIDE_ALPHA | XB_MSIDE_STATE | ((f & LIBXSMM_MELTW_FLAG_UNARY_BITMASK_2BYTEMULT) ? XB_MSIDE_MASK_OUT : 0);
+    case LIBXSMM_MELTW_TYPE_UNARY_QUANT: case LIBXSMM_MELTW_TYPE_UNARY_DEQUANT:   /* the scale: NO_SCF_QUANT or a NULL pointer stand for 1 */
+      return (fam == XB_FAM_MXQUANT) ? XB_MSIDE_OUT_AUX : XB_MSIDE_IN_AUX;
+    case LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X_OP_MAX: case LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X_OP_MIN: case LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X_OP_ABSMAX:
+      return ((f & LIBXSMM_MELTW_FLAG_UNARY_REDUCE_RECORD_ARGOP) && !(f & LIBXSMM_MELTW_FLAG_UNARY_REDUCE_ROWS)) ? XB_MSIDE_ARGOP : 0;
+    case LIBXSMM_MELTW_TYPE_UNARY_REDUCE_COLS_IDX_OP_MAX: case LIBXSMM_MELTW_TYPE_UNARY_REDUCE_COLS_IDX_OP_MIN:
+      if (f & LIBXSMM_MELTW_FLAG_UNARY_REDUCE_RECORD_ARGOP) return XB_MSIDE_IN_AUX | XB_MSIDE_COUNT | XB_MSIDE_RUNTIME | XB_MSIDE_ARGOP;
+      /* fall through */
+    case LIBXSMM_MELTW_TYPE_UNARY_REDUCE_COLS_IDX_OP_ADD: return XB_MSIDE_IN_AUX | XB_MSIDE_COUNT | XB_MSIDE_RUNTIME;
+    case LIBXSMM_MELTW_TYPE_UNARY_GATHER: return XB_MSIDE_IN_AUX | XB_MSIDE_RUNTIME;
+    case LIBXSMM_MELTW_TYPE_UNARY_SCATTER: case LIBXSMM_MELTW_TYPE_UNARY_UNZIP: case LIBXSMM_MELTW_TYPE_UNARY_DECOMP_FP32_TO_BF16X2:
+    case LIBXSMM_MELTW_TYPE_UNARY_DECOMP_FP32_TO_BF16X3: return XB_MSIDE_OUT_AUX | XB_MSIDE_RUNTIME;
+    case LIBXSMM_MELTW_TYPE_UNARY_REPLICATE_COL_VAR: return XB_MSIDE_COUNT | sr;
+    case LIBXSMM_MELTW_TYPE_UNARY_DUMP: return XB_MSIDE_COPY_OUT | sr;
+    default: return (fam == XB_FAM_MAP) ? sr : 0;       /* the other maps of the generic loop; transforms and reductions carry nothing */
+  }
+}
+
 static const void* xb_dispatch_meltw(xb_meltw_desc* d) {
   int slot;
   LIBXSMM_INIT
-  if (d->m <= 0 || d->n <= 0 || !xb_meltw_supported(d)) return NULL;
+  if (d->m <= 0 || d->n <= 0 || xb_meltw_family(d) == XB_FAM_NONE) return NULL;
   slot = xb_host_registry_get(XB_KIND_MELTW, d, sizeof(*d), 0);
   return (slot < 0) ? NULL : xb_thunk(slot);
 }
@@ -188,18 +315,6 @@ static size_t in_extent(const xb_meltw_desc* d, unsigned int row, unsigned int c
   return (size_t)((n - 1) * ld + d->m);
 }
 
-/* the element-wise ops that go through the reference's generic load -> f32 -> op -> store loop (:2470-2498): the only unary
- * ops that honour STOCHASTIC_ROUND */
-static int unary_is_generic_map(int op) {
-  switch (op) {
-    case LIBXSMM_MELTW_TYPE_UNARY_IDENTITY: case LIBXSMM_MELTW_TYPE_UNARY_XOR: case LIBXSMM_MELTW_TYPE_UNARY_X2: case LIBXSMM_MELTW_TYPE_UNARY_SQRT:
-    case LIBXSMM_MELTW_TYPE_UNARY_NEGATE: case LIBXSMM_MELTW_TYPE_UNARY_INC: case LIBXSMM_MELTW_TYPE_UNARY_RECIPROCAL: case LIBXSMM_MELTW_TYPE_UNARY_RECIPROCAL_SQRT:
-    case LIBXSMM_MELTW_TYPE_UNARY_TANH: case LIBXSMM_MELTW_TYPE_UNARY_TANH_INV: case LIBXSMM_MELTW_TYPE_UNARY_SIGMOID: case LIBXSMM_MELTW_TYPE_UNARY_SIGMOID_INV:
-    case LIBXSMM_MELTW_TYPE_UNARY_GELU: case LIBXSMM_MELTW_TYPE_UNARY_GELU_INV: case LIBXSMM_MELTW_TYPE_UNARY_EXP: case LIBXSMM_MELTW_TYPE_UNARY_DUMP:
-    case LIBXSMM_MELTW_TYPE_UNARY_REPLICATE_COL_VAR: return 1;
-    default: return 0;
-  }
-}
 /* STOCHASTIC_ROUND to BF8 (libxsmm_elementwise_store_value, :310-316): the 4 x 16-word generator state in op.secondary is read and
  * advanced; one random byte per element goes through device scratch */
 static void stage_stochastic(xb_stager* st, xb_meltw_args* a, const void* state, long long elements) {
@@ -214,33 +329,26 @@ static void stage_stochastic(xb_stager* st, xb_meltw_args* a, const void* state,
 static int meltw_args(const xb_meltw_desc* d, const void* param, xb_meltw_args* out_args, xb_stager* pst) {
   xb_meltw_args a; xb_stager st = *pst;
   const size_t ts_in = libxsmm_typesize((libxsmm_datatype)d->t_in0), ts_out = libxsmm_typesize((libxsmm_datatype)d->t_out);
-  const size_t mask_ld_o = (size_t)LIBXSMM_UP(d->ldo, 16), mask_ld_i = (size_t)LIBXSMM_UP(d->ldi, 16);
+  const size_t mask_ld_i = (size_t)LIBXSMM_UP(d->ldi, 16);
   memset(&a, 0, sizeof(a));
   if (d->op_class == LIBXSMM_MELTW_OPERATION_UNARY) {
     const libxsmm_meltw_unary_param* p = (const libxsmm_meltw_unary_param*)param;
-    const int op = d->op;
+    const int op = d->op, sides = xb_meltw_sides(d);
+    const size_t idx = (d->flags & LIBXSMM_MELTW_FLAG_UNARY_IDX_SIZE_4BYTES) ? 4 : 8;
     long long n = d->n;
     size_t ext_in, ext_out = ((size_t)(d->n - 1) * d->ldo + d->m) * ts_out, mx_scales = 0;
-    if (op == LIBXSMM_MELTW_TYPE_UNARY_REPLICATE_COL_VAR) { n = (long long)*(const unsigned long long*)p->op.primary; a.n_rt = (unsigned long long)n; ext_out = ((size_t)(n - 1) * d->ldo + d->m) * ts_out; }
+    if ((sides & (XB_MSIDE_COUNT | XB_MSIDE_RUNTIME)) == XB_MSIDE_COUNT) {       /* op.primary: the run-time column count */
+      n = (long long)*(const unsigned long long*)p->op.primary; a.n_rt = (unsigned long long)n; ext_out = ((size_t)(n - 1) * d->ldo + d->m) * ts_out;
+    }
     ext_in = in_extent(d, d->flags & LIBXSMM_MELTW_FLAG_UNARY_BCAST_ROW, (d->flags & LIBXSMM_MELTW_FLAG_UNARY_BCAST_COL) | (op == LIBXSMM_MELTW_TYPE_UNARY_REPLICATE_COL_VAR),
                        d->flags & LIBXSMM_MELTW_FLAG_UNARY_BCAST_SCALAR, d->ldi, n) * ts_in;
-    switch (op) {
-      case LIBXSMM_MELTW_TYPE_UNARY_LEAKY_RELU: case LIBXSMM_MELTW_TYPE_UNARY_ELU: case LIBXSMM_MELTW_TYPE_UNARY_LEAKY_RELU_INV:
-      case LIBXSMM_MELTW_TYPE_UNARY_ELU_INV: a.alpha = *(const float*)p->op.primary; break;
-      case LIBXSMM_MELTW_TYPE_UNARY_QUANT: case LIBXSMM_MELTW_TYPE_UNARY_DEQUANT: {
-        const int mx = (d->t_out == LIBXSMM_DATATYPE_MXFP4X2 || d->t_out == LIBXSMM_DATATYPE_NVFP4X2 || d->t_out == LIBXSMM_DATATYPE_MXBF8);
-        a.alpha = (mx || (d->flags & LIBXSMM_MELTW_FLAG_UNARY_NO_SCF_QUANT) != 0 || p->in.secondary == NULL) ? 1.0f : *(const float*)p->in.secondary;
-        if (mx) {   /* block formats: 4-bit data at ldo/2 bytes per column, one scale byte per block in out.secondary (reference :2247-2326) */
-          const int blk = (d->t_out == LIBXSMM_DATATYPE_NVFP4X2) ? 16 : 32;
-          const size_t per = (d->t_out == LIBXSMM_DATATYPE_MXBF8) ? 1 : 2;
-          ext_out = ((size_t)(d->n - 1) * (d->ldo / per) + (size_t)(d->m / blk) * blk / per);
-          mx_scales = ((size_t)(d->n - 1) * (d->ldo / blk) + (size_t)(d->m / blk));
-        }
-      } break;
-      case LIBXSMM_MELTW_TYPE_UNARY_DROPOUT: case LIBXSMM_MELTW_TYPE_UNARY_DROPOUT_INV: {   /* op.primary -> drop probability p */
-        if (xb_rt_ptr_kind(p->op.primary) == 1) xb_rt_memcpy(&a.alpha, p->op.primary, sizeof(float)); else a.alpha = *(const float*)p->op.primary;
-      } break;
-      default: a.alpha = 1.0f;
+    a.alpha = (sides & XB_MSIDE_ALPHA) ? xb_meltw_scalar(p->op.primary) : 1.0f;
+    if (xb_meltw_family(d) == XB_FAM_QUANT && (d->flags & LIBXSMM_MELTW_FLAG_UNARY_NO_SCF_QUANT) == 0 && p->in.secondary != NULL) a.alpha = *(const float*)p->in.secondary;
+    if (xb_meltw_family(d) == XB_FAM_MXQUANT) {   /* block formats: 4-bit data at ldo/2 bytes per column, one scale byte per block in out.secondary (reference :2247-2326) */
+      const int blk = (d->t_out == LIBXSMM_DATATYPE_NVFP4X2) ? 16 : 32;
+      const size_t per = (d->t_out == LIBXSMM_DATATYPE_MXBF8) ? 1 : 2;
+      ext_out = ((size_t)(d->n - 1) * (d->ldo / per) + (size_t)(d->m / blk) * blk / per);
+      mx_scales = ((size_t)(d->n - 1) * (d->ldo / blk) + (size_t)(d->m / blk));
     }
     /* shapes of the data-movement and reduction families */
     if (op == LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_NORMT) ext_out = ((size_t)(d->m - 1) * d->ldo + d->n) * ts_out;
@@ -265,70 +373,52 @@ static int meltw_args(const xb_meltw_desc* d, const void* param, xb_meltw_args* 
     } else if (op == LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X_OP_MIN || op == LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X_OP_ABSMAX) {
       ext_out = ((d->flags & LIBXSMM_MELTW_FLAG_UNARY_REDUCE_ROWS) ? (size_t)d->n : (size_t)d->m) * ts_out;
     }
-    if (op == LIBXSMM_MELTW_TYPE_UNARY_GATHER || op == LIBXSMM_MELTW_TYPE_UNARY_SCATTER || op == LIBXSMM_MELTW_TYPE_UNARY_REDUCE_COLS_IDX_OP_ADD
-     || op == LIBXSMM_MELTW_TYPE_UNARY_REDUCE_COLS_IDX_OP_MAX || op == LIBXSMM_MELTW_TYPE_UNARY_REDUCE_COLS_IDX_OP_MIN) {
+    if ((sides & XB_MSIDE_RUNTIME) && xb_meltw_family(d) != XB_FAM_SPLIT) {
       /* extents depend on run-time indices: operands must be device-accessible (device, managed or pinned) */
       if (xb_rt_ptr_kind(p->in.primary) == 0 || xb_rt_ptr_kind(p->out.primary) == 0) { xb_rt_note_error(1, "meltw: indexed op needs device-accessible memory"); return 1; }
       a.in0 = p->in.primary; a.out = p->out.primary; a.in_aux = p->in.secondary; a.out_aux = p->out.secondary;
-      if (op != LIBXSMM_MELTW_TYPE_UNARY_GATHER && op != LIBXSMM_MELTW_TYPE_UNARY_SCATTER) {
+      if (sides & XB_MSIDE_COUNT) {                  /* in.tertiary: the number of column indices in in.secondary */
         a.n_rt = *(const unsigned long long*)p->in.tertiary;
-        a.in_aux = stage_in(&st, p->in.secondary, (size_t)a.n_rt * ((d->flags & LIBXSMM_MELTW_FLAG_UNARY_IDX_SIZE_4BYTES) ? 4 : 8));
-        /* MAX / MIN with RECORD_ARGOP write one column index per row to out.secondary (reference :1243-1275): staged in and out like
-         * the REDUCE_X_OP_* branch below, so that a pageable index buffer is never handed to the kernel */
-        if (op != LIBXSMM_MELTW_TYPE_UNARY_REDUCE_COLS_IDX_OP_ADD && (d->flags & LIBXSMM_MELTW_FLAG_UNARY_REDUCE_RECORD_ARGOP) != 0) {
-          a.out_aux = stage_inout(&st, p->out.secondary, (size_t)d->m * ((d->flags & LIBXSMM_MELTW_FLAG_UNARY_IDX_SIZE_4BYTES) ? 4 : 8));
-          if (a.out_aux == NULL) st.failed = 1;
-        }
+        a.in_aux = stage_in(&st, p->in.secondary, (size_t)a.n_rt * idx);
       } else {
         const size_t isz = (d->flags & LIBXSMM_MELTW_FLAG_UNARY_IDX_SIZE_8BYTES) ? 8 : 4;
         const size_t cnt = (d->flags & LIBXSMM_MELTW_FLAG_UNARY_GS_COLS) ? (size_t)d->n : ((d->flags & LIBXSMM_MELTW_FLAG_UNARY_GS_ROWS) ? (size_t)d->m : (size_t)d->m * d->n);
-        if (op == LIBXSMM_MELTW_TYPE_UNARY_GATHER) a.in_aux = stage_in(&st, p->in.secondary, cnt * isz);
+        if (sides & XB_MSIDE_IN_AUX) a.in_aux = stage_in(&st, p->in.secondary, cnt * isz);
         else a.out_aux = (void*)(uintptr_t)stage_in(&st, p->out.secondary, cnt * isz);
       }
     } else {
       a.in0 = stage_in(&st, p->in.primary, ext_in);
-      if (op == LIBXSMM_MELTW_TYPE_UNARY_UNZIP || op == LIBXSMM_MELTW_TYPE_UNARY_DECOMP_FP32_TO_BF16X2 || op == LIBXSMM_MELTW_TYPE_UNARY_DECOMP_FP32_TO_BF16X3) {
+      if (sides & XB_MSIDE_RUNTIME) {
         /* several bf16 planes behind ONE output pointer at caller-given byte distances (out.secondary): the output must be
          * device-accessible, there is no single extent to stage */
         const unsigned long long* offs = (const unsigned long long*)p->out.secondary;
+        const int noff = (op == LIBXSMM_MELTW_TYPE_UNARY_DECOMP_FP32_TO_BF16X3) ? 2 : 1;
         if (offs == NULL || xb_rt_ptr_kind(p->out.primary) == 0) { xb_rt_note_error(1, "meltw: unzip/decomp need a device-accessible output and plane offsets"); xb_rt_scratch_reset(); return 1; }
-        if (xb_rt_ptr_kind(offs) == 1) xb_rt_memcpy(a.off, offs, (op == LIBXSMM_MELTW_TYPE_UNARY_DECOMP_FP32_TO_BF16X3 ? 2 : 1) * sizeof(unsigned long long));
-        else { a.off[0] = offs[0]; if (op == LIBXSMM_MELTW_TYPE_UNARY_DECOMP_FP32_TO_BF16X3) a.off[1] = offs[1]; }
+        if (xb_rt_ptr_kind(offs) == 1) xb_rt_memcpy(a.off, offs, noff * sizeof(unsigned long long)); else memcpy(a.off, offs, noff * sizeof(unsigned long long));
         a.out = p->out.primary;
       } else a.out = stage_inout(&st, p->out.primary, ext_out);
-      if (mx_scales != 0) { a.out_aux = stage_inout(&st, p->out.secondary, mx_scales); if (a.out_aux == NULL) st.failed = 1; }
-      if (op == LIBXSMM_MELTW_TYPE_UNARY_DUMP) { a.out_aux = stage_inout(&st, p->out.secondary, ext_out); if (a.out_aux == NULL) st.failed = 1; }
-      if ((d->flags & LIBXSMM_MELTW_FLAG_UNARY_STOCHASTIC_ROUND) != 0 && d->t_out == LIBXSMM_DATATYPE_BF8 && unary_is_generic_map(op)
-          && !(d->t_in0 == LIBXSMM_DATATYPE_F64)) stage_stochastic(&st, &a, p->op.secondary, (long long)d->m * n);
-      if (op == LIBXSMM_MELTW_TYPE_UNARY_DROPOUT) {      /* op.secondary: generator state, read AND advanced (:2091, :43-73) */
+      if ((sides & XB_MSIDE_OUT_AUX) && mx_scales != 0) { a.out_aux = stage_inout(&st, p->out.secondary, mx_scales); if (a.out_aux == NULL) st.failed = 1; }
+      if (sides & XB_MSIDE_COPY_OUT) { a.out_aux = stage_inout(&st, p->out.secondary, ext_out); if (a.out_aux == NULL) st.failed = 1; }
+      if ((sides & XB_MSIDE_STATE) && xb_meltw_family(d) != XB_FAM_DROPOUT) stage_stochastic(&st, &a, p->op.secondary, (long long)d->m * n);
+      else if (sides & XB_MSIDE_STATE) {             /* dropout: op.secondary, generator state, read AND advanced (:2091, :43-73) */
         a.rng = stage_inout(&st, p->op.secondary, 64 * sizeof(unsigned int));
         a.rnd = (float*)xb_rt_scratch((size_t)LIBXSMM_UPDIV(d->m, 16) * d->n * 16 * sizeof(float));
         if (a.rng == NULL || a.rnd == NULL) st.failed = 1;
-        if (d->flags & LIBXSMM_MELTW_FLAG_UNARY_BITMASK_2BYTEMULT) a.out_aux = stage_inout(&st, p->out.secondary, mask_ld_o / 8 * (size_t)d->n);
-      } else if (op == LIBXSMM_MELTW_TYPE_UNARY_DROPOUT_INV) {
-        const size_t mld = (d->flags & LIBXSMM_MELTW_FLAG_UNARY_BITMASK_2BYTEMULT) ? mask_ld_i : (size_t)d->ldi;
-        a.in_aux = stage_in(&st, p->in.secondary, (mld / 8) * (size_t)d->n + 1);
       }
-      if (op == LIBXSMM_MELTW_TYPE_UNARY_RELU || op == LIBXSMM_MELTW_TYPE_UNARY_LEAKY_RELU || op == LIBXSMM_MELTW_TYPE_UNARY_ELU) {
-        if (d->flags & LIBXSMM_MELTW_FLAG_UNARY_BITMASK_2BYTEMULT) a.out_aux = stage_inout(&st, p->out.secondary, mask_ld_o / 8 * (size_t)d->n);
-      } else if (op == LIBXSMM_MELTW_TYPE_UNARY_RELU_INV || op == LIBXSMM_MELTW_TYPE_UNARY_LEAKY_RELU_INV) {
+      if (sides & XB_MSIDE_MASK_OUT) a.out_aux = stage_inout(&st, p->out.secondary, xb_meltw_mask_bytes(d->ldo, d->n));
+      if ((sides & XB_MSIDE_IN_AUX) && xb_meltw_family(d) != XB_FAM_QUANT) {   /* the forward output of ELU_INV, else a bit mask */
         const size_t mld = (d->flags & LIBXSMM_MELTW_FLAG_UNARY_BITMASK_2BYTEMULT) ? mask_ld_i : (size_t)d->ldi;
-        a.in_aux = stage_in(&st, p->in.secondary, (mld / 8) * (size_t)d->n + 1);
-      } else if (op == LIBXSMM_MELTW_TYPE_UNARY_ELU_INV) a.in_aux = stage_in(&st, p->in.secondary, ((size_t)(d->n - 1) * d->ldi + d->m) * ts_in);
-      else if ((op == LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X_OP_MAX || op == LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X_OP_MIN || op == LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X_OP_ABSMAX)
-            && (d->flags & LIBXSMM_MELTW_FLAG_UNARY_REDUCE_RECORD_ARGOP) != 0) {
-        /* arg-max/min column indices land in out.secondary (reference :1243-1268); only the column reduction records them */
-        if ((d->flags & LIBXSMM_MELTW_FLAG_UNARY_REDUCE_ROWS) == 0) {
-          a.out_aux = stage_inout(&st, p->out.secondary, (size_t)d->m * ((d->flags & LIBXSMM_MELTW_FLAG_UNARY_IDX_SIZE_4BYTES) ? 4 : 8));
-          if (a.out_aux == NULL) st.failed = 1;
-        }
+        a.in_aux = stage_in(&st, p->in.secondary, (op == LIBXSMM_MELTW_TYPE_UNARY_ELU_INV) ? ((size_t)(d->n - 1) * d->ldi + d->m) * ts_in : (mld / 8) * (size_t)d->n + 1);
       }
     }
+    /* arg-max/min column indices land in out.secondary (reference :1243-1275), staged in and out so that a pageable index buffer is
+     * never handed to the kernel */
+    if (sides & XB_MSIDE_ARGOP) { a.out_aux = stage_inout(&st, p->out.secondary, (size_t)d->m * idx); if (a.out_aux == NULL) st.failed = 1; }
   } else if (d->op_class == LIBXSMM_MELTW_OPERATION_BINARY) {
     const libxsmm_meltw_binary_param* p = (const libxsmm_meltw_binary_param*)param;
     const size_t ts1 = libxsmm_typesize((libxsmm_datatype)d->t_in1);
     size_t ext_out = ((size_t)(d->n - 1) * d->ldo + d->m) * ts_out;
-    if (d->op >= LIBXSMM_MELTW_TYPE_BINARY_CMP_OP_GT) ext_out = mask_ld_o / 8 * (size_t)d->n;
+    if (d->op >= LIBXSMM_MELTW_TYPE_BINARY_CMP_OP_GT) ext_out = xb_meltw_mask_bytes(d->ldo, d->n);
     if (d->op == LIBXSMM_MELTW_TYPE_BINARY_MUL_AND_REDUCE_TO_SCALAR_OP_ADD) ext_out = ts_out;
     if (d->op == LIBXSMM_MELTW_TYPE_BINARY_ZIP) ext_out = ((size_t)(d->n - 1) * d->ldo + d->m) * 4;
     a.in0 = stage_in(&st, p->in0.primary, in_extent(d, d->flags & LIBXSMM_MELTW_FLAG_BINARY_BCAST_ROW_IN_0, d->flags & LIBXSMM_MELTW_FLAG_BINARY_BCAST_COL_IN_0,
@@ -336,8 +426,7 @@ static int meltw_args(const xb_meltw_desc* d, const void* param, xb_meltw_args* 
     a.in1 = stage_in(&st, p->in1.primary, in_extent(d, d->flags & LIBXSMM_MELTW_FLAG_BINARY_BCAST_ROW_IN_1, d->flags & LIBXSMM_MELTW_FLAG_BINARY_BCAST_COL_IN_1,
                                                      d->flags & LIBXSMM_MELTW_FLAG_BINARY_BCAST_SCALAR_IN_1, d->ldi2, d->n) * ts1);
     a.out = stage_inout(&st, p->out.primary, ext_out);
-    if ((d->flags & LIBXSMM_MELTW_FLAG_BINARY_STOCHASTIC_ROUND) != 0 && d->t_out == LIBXSMM_DATATYPE_BF8 && d->op < LIBXSMM_MELTW_TYPE_BINARY_CMP_OP_GT
-        && d->op != LIBXSMM_MELTW_TYPE_BINARY_MUL_AND_REDUCE_TO_SCALAR_OP_ADD && d->op != LIBXSMM_MELTW_TYPE_BINARY_ZIP) stage_stochastic(&st, &a, p->op.secondary, (long long)d->m * d->n);
+    if (xb_meltw_sides(d) & XB_MSIDE_STATE) stage_stochastic(&st, &a, p->op.secondary, (long long)d->m * d->n);
   } else {
     const libxsmm_meltw_ternary_param* p = (const libxsmm_meltw_ternary_param*)param;
     const size_t ts1 = libxsmm_typesize((libxsmm_datatype)d->t_in1), ts2 = libxsmm_typesize((libxsmm_datatype)d->t_in2);
@@ -345,11 +434,11 @@ static int meltw_args(const xb_meltw_desc* d, const void* param, xb_meltw_args* 
                                                      d->flags & LIBXSMM_MELTW_FLAG_TERNARY_BCAST_SCALAR_IN_0, d->ldi, d->n) * ts_in);
     a.in1 = stage_in(&st, p->in1.primary, in_extent(d, d->flags & LIBXSMM_MELTW_FLAG_TERNARY_BCAST_ROW_IN_1, d->flags & LIBXSMM_MELTW_FLAG_TERNARY_BCAST_COL_IN_1,
                                                      d->flags & LIBXSMM_MELTW_FLAG_TERNARY_BCAST_SCALAR_IN_1, d->ldi2, d->n) * ts1);
-    if (d->op == LIBXSMM_MELTW_TYPE_TERNARY_SELECT) a.in2 = stage_in(&st, p->in2.primary, (size_t)LIBXSMM_UP(d->ldi3, 16) / 8 * (size_t)d->n);
+    if (d->op == LIBXSMM_MELTW_TYPE_TERNARY_SELECT) a.in2 = stage_in(&st, p->in2.primary, xb_meltw_mask_bytes(d->ldi3, d->n));
     else a.in2 = stage_in(&st, p->in2.primary, in_extent(d, d->flags & LIBXSMM_MELTW_FLAG_TERNARY_BCAST_ROW_IN_2, d->flags & LIBXSMM_MELTW_FLAG_TERNARY_BCAST_COL_IN_2,
                                                           d->flags & LIBXSMM_MELTW_FLAG_TERNARY_BCAST_SCALAR_IN_2, d->ldi3, d->n) * ts2);
     a.out = stage_inout(&st, p->out.primary, ((size_t)(d->n - 1) * d->ldo + d->m) * ts_out);
-    if ((d->flags & LIBXSMM_MELTW_FLAG_TERNARY_STOCHASTIC_ROUND) != 0 && d->t_out == LIBXSMM_DATATYPE_BF8) stage_stochastic(&st, &a, p->op.secondary, (long long)d->m * d->n);
+    if (xb_meltw_sides(d) & XB_MSIDE_STATE) stage_stochastic(&st, &a, p->op.secondary, (long long)d->m * d->n);
   }
   *pst = st; *out_args = a;
   if (st.failed) { xb_rt_note_error(2, "meltw: staging failed"); xb_rt_scratch_reset(); return 1; }
@@ -370,21 +459,18 @@ void xb_invoke_meltw(const xb_slot* s, const void* param) {
 
 /* ---- strided batch: `count` calls of one handle in one launch ------------------------------------------------------------
  * Calls whose kernel carries per-call state or run-time extents are refused: the dropout generator chains call to call, stochastic
- * rounding draws from a state in op.secondary, REPLICATE_COL_VAR / the COLS_IDX reductions / gather and scatter read their extents
- * or indices at run time, unzip and decomp write planes at caller-given offsets. */
+ * rounding draws from a state in op.secondary, the others read their extents, indices or plane offsets at run time. */
 int xb_meltw_batchable(const xb_meltw_desc* d) {
-  if (d->op_class == LIBXSMM_MELTW_OPERATION_UNARY) {
-    if ((d->flags & LIBXSMM_MELTW_FLAG_UNARY_STOCHASTIC_ROUND) != 0) return 0;
-    switch (d->op) {
-      case LIBXSMM_MELTW_TYPE_UNARY_DROPOUT: case LIBXSMM_MELTW_TYPE_UNARY_REPLICATE_COL_VAR:
-      case LIBXSMM_MELTW_TYPE_UNARY_GATHER: case LIBXSMM_MELTW_TYPE_UNARY_SCATTER:
-      case LIBXSMM_MELTW_TYPE_UNARY_REDUCE_COLS_IDX_OP_ADD: case LIBXSMM_MELTW_TYPE_UNARY_REDUCE_COLS_IDX_OP_MAX: case LIBXSMM_MELTW_TYPE_UNARY_REDUCE_COLS_IDX_OP_MIN:
-      case LIBXSMM_MELTW_TYPE_UNARY_UNZIP: case LIBXSMM_MELTW_TYPE_UNARY_DECOMP_FP32_TO_BF16X2: case LIBXSMM_MELTW_TYPE_UNARY_DECOMP_FP32_TO_BF16X3: return 0;
-      default: return 1;
-    }
-  }
-  if (d->op_class == LIBXSMM_MELTW_OPERATION_BINARY) return (d->flags & LIBXSMM_MELTW_FLAG_BINARY_STOCHASTIC_ROUND) == 0;
-  return (d->flags & LIBXSMM_MELTW_FLAG_TERNARY_STOCHASTIC_ROUND) == 0;
+  const unsigned int sr = (d->op_class == LIBXSMM_MELTW_OPERATION_UNARY) ? LIBXSMM_MELTW_FLAG_UNARY_STOCHASTIC_ROUND
+                        : (d->op_class == LIBXSMM_MELTW_OPERATION_BINARY ? LIBXSMM_MELTW_FLAG_BINARY_STOCHASTIC_ROUND : LIBXSMM_MELTW_FLAG_TERNARY_STOCHASTIC_ROUND);
+  /* kept as it was (a follow-up): the STOCHASTIC_ROUND flag refuses the batch even where the op does not round stochastically */
+  return (xb_meltw_sides(d) & (XB_MSIDE_STATE | XB_MSIDE_COUNT | XB_MSIDE_RUNTIME)) == 0 && (d->flags & sr) == 0;
+}
+
+float xb_meltw_scalar(const void* p) {
+  float v;
+  if (xb_rt_ptr_kind(p) == 1) xb_rt_memcpy(&v, p, sizeof(v)); else v = *(const float*)p;
+  return v;
 }
 
 LIBXSMM_API int libxsmm_b200_meltw_batch_strided(const void* kernel, const void* param, const libxsmm_b200_meltw_strides* strides, long long count) {

@@ -208,28 +208,31 @@ static void assign_scores(xb_eqn* e, int at) {
   }
 }
 
+/* the side operands of a node's kernel (xb_meltw_sides); an argument has none */
+static int node_sides(const xb_eqn* e, int at) {
+  xb_meltw_desc d;
+  if (e->node[at].type == EQ_ARG) return 0;
+  node_desc(e, at, &d);
+  return xb_meltw_sides(&d);
+}
+
 static int check_nodes(const xb_eqn* e, int at) {
-  const xb_eqn_node* nd = &e->node[at]; int c; xb_meltw_desc d;
+  const xb_eqn_node* nd = &e->node[at]; int c, unwired; xb_meltw_desc d;
   if (nd->type == EQ_ARG) return 0;
   for (c = 0; c < arity(nd->type); ++c) if (check_nodes(e, nd->child[c]) != 0) return 1;
-  /* declined rather than mis-evaluated: nodes without a storage type (IMPLICIT: zip / unzip trees) and operations whose extra operands
-   * this evaluator does not wire -- index arrays, bit masks or forward outputs read through in.secondary, plane offsets, generator
-   * state, run-time counts, quantiser scales (samples/equation/equation_splitSGD.c, equation_gather_*.c, equation_bf16_x3_split_f32.c) */
-  if (libxsmm_typesize((libxsmm_datatype)nd->dtype) == 0) return 1;
-  if (nd->type == EQ_UNARY) switch (nd->op) {
-    case LIBXSMM_MELTW_TYPE_UNARY_UNZIP: case LIBXSMM_MELTW_TYPE_UNARY_DECOMP_FP32_TO_BF16X2: case LIBXSMM_MELTW_TYPE_UNARY_DECOMP_FP32_TO_BF16X3:
-    case LIBXSMM_MELTW_TYPE_UNARY_GATHER: case LIBXSMM_MELTW_TYPE_UNARY_SCATTER: case LIBXSMM_MELTW_TYPE_UNARY_REPLICATE_COL_VAR:
-    case LIBXSMM_MELTW_TYPE_UNARY_REDUCE_COLS_IDX_OP_ADD: case LIBXSMM_MELTW_TYPE_UNARY_REDUCE_COLS_IDX_OP_MAX: case LIBXSMM_MELTW_TYPE_UNARY_REDUCE_COLS_IDX_OP_MIN:
-    case LIBXSMM_MELTW_TYPE_UNARY_DROPOUT: case LIBXSMM_MELTW_TYPE_UNARY_DROPOUT_INV: case LIBXSMM_MELTW_TYPE_UNARY_QUANT: case LIBXSMM_MELTW_TYPE_UNARY_DEQUANT:
-    case LIBXSMM_MELTW_TYPE_UNARY_RELU_INV: case LIBXSMM_MELTW_TYPE_UNARY_LEAKY_RELU_INV: case LIBXSMM_MELTW_TYPE_UNARY_ELU_INV:
-      return 1;
-    default: if ((nd->flags & LIBXSMM_MELTW_FLAG_UNARY_STOCHASTIC_ROUND) != 0) return 1;
-  }
-  /* a relu's bit mask has one destination, output.secondary: only the head may produce it (reference :39-56) */
-  if (at != 0 && nd->type == EQ_UNARY && (nd->flags & LIBXSMM_MELTW_FLAG_UNARY_BITMASK_2BYTEMULT) != 0
-      && (nd->op == LIBXSMM_MELTW_TYPE_UNARY_RELU || nd->op == LIBXSMM_MELTW_TYPE_UNARY_LEAKY_RELU || nd->op == LIBXSMM_MELTW_TYPE_UNARY_ELU)) return 1;
   node_desc(e, at, &d);
-  return xb_meltw_supported(&d) ? 0 : 1;
+  /* declined rather than mis-evaluated: nodes without a storage type (IMPLICIT: zip / unzip trees) and nodes with side operands this
+   * evaluator does not wire (samples/equation/equation_splitSGD.c, equation_gather_*.c, equation_bf16_x3_split_f32.c). It wires the
+   * bit mask of a relu at the head, the copy of a DUMP and an alpha from ops_args. */
+  if (libxsmm_typesize((libxsmm_datatype)nd->dtype) == 0 || xb_meltw_family(&d) == XB_FAM_NONE) return 1;
+  unwired = xb_meltw_sides(&d) & ~(XB_MSIDE_MASK_OUT | XB_MSIDE_COPY_OUT | XB_MSIDE_ALPHA);
+  /* kept as they were (follow-ups): an argop reduction is accepted and its indices are not recorded; a unary node with STOCHASTIC_ROUND
+   * is declined whatever its op; a binary or ternary one is accepted and its generator state is not wired */
+  unwired &= ~XB_MSIDE_ARGOP;
+  if (nd->type != EQ_UNARY) unwired &= ~XB_MSIDE_STATE;
+  else if (nd->flags & LIBXSMM_MELTW_FLAG_UNARY_STOCHASTIC_ROUND) return 1;
+  /* a relu's bit mask has one destination, output.secondary: only the head may produce it (reference :39-56) */
+  return (unwired != 0 || (at != 0 && (xb_meltw_sides(&d) & XB_MSIDE_MASK_OUT))) ? 1 : 0;
 }
 
 LIBXSMM_API libxsmm_meqn_function libxsmm_dispatch_meqn(const libxsmm_blasint idx, const libxsmm_meqn_arg_shape out_shape) {
@@ -277,9 +280,12 @@ static void* eval_aux_out(xb_eval* ev, void* user, size_t bytes) {
   ev->back[ev->nback].host = user; ev->back[ev->nback].dev = d; ev->back[ev->nback].bytes = bytes; ev->nback++;
   return d;
 }
-static int has_bitmask_out(const xb_eqn_node* nd) {
-  return nd->type == EQ_UNARY && (nd->flags & LIBXSMM_MELTW_FLAG_UNARY_BITMASK_2BYTEMULT) != 0
-      && (nd->op == LIBXSMM_MELTW_TYPE_UNARY_RELU || nd->op == LIBXSMM_MELTW_TYPE_UNARY_LEAKY_RELU || nd->op == LIBXSMM_MELTW_TYPE_UNARY_ELU);
+static int has_bitmask_out(const xb_eqn* e, int at) { return (node_sides(e, at) & XB_MSIDE_MASK_OUT) != 0; }
+/* the alpha of a node that takes one (xb_meltw_sides: ALPHA), from its ops_args slot of call 0; 1 otherwise */
+static float node_alpha(const xb_eqn* e, int at, const libxsmm_meqn_param* p) {
+  const xb_eqn_node* nd = &e->node[at];
+  if ((node_sides(e, at) & XB_MSIDE_ALPHA) == 0 || p->ops_args == NULL || nd->pos < 0 || p->ops_args[nd->pos].primary == NULL) return 1.0f;
+  return xb_meltw_scalar(p->ops_args[nd->pos].primary);
 }
 
 static const void* eval_node(xb_eval* ev, int at, int is_root) {
@@ -307,18 +313,12 @@ static const void* eval_node(xb_eval* ev, int at, int is_root) {
     out = is_root ? ev->out_dev : xb_rt_scratch(span(nd) ? span(nd) : 16);
     if (out == NULL) { ev->failed = 1; return NULL; }
     node_desc(ev->e, at, &d);
-    a.out = out; a.alpha = 1.0f;
-    if (nd->type == EQ_UNARY && ev->p->ops_args != NULL && nd->pos >= 0) {
-      const void* op1 = ev->p->ops_args[nd->pos].primary;
-      if (op1 != NULL && (nd->op == LIBXSMM_MELTW_TYPE_UNARY_LEAKY_RELU || nd->op == LIBXSMM_MELTW_TYPE_UNARY_ELU)) {
-        if (xb_rt_ptr_kind(op1) == 1) xb_rt_memcpy(&a.alpha, op1, sizeof(float)); else a.alpha = *(const float*)op1;
-      }
-    }
+    a.out = out; a.alpha = node_alpha(ev->e, at, ev->p);
     /* secondary outputs as the reference wires them (generator_matequation_reference_impl.c:39-61): the bit mask of a relu at
      * the head goes to output.secondary, a DUMP node copies its value to its ops_args slot */
-    if (has_bitmask_out(nd)) {
+    if (has_bitmask_out(ev->e, at)) {
       if (!is_root) { ev->failed = 1; return NULL; }
-      a.out_aux = eval_aux_out(ev, ev->p->output.secondary, (size_t)LIBXSMM_UP(d.ldo, 16) / 8 * (size_t)d.n);
+      a.out_aux = eval_aux_out(ev, ev->p->output.secondary, xb_meltw_mask_bytes(d.ldo, d.n));
     } else if (nd->type == EQ_UNARY && nd->op == LIBXSMM_MELTW_TYPE_UNARY_DUMP) {
       a.out_aux = eval_aux_out(ev, (ev->p->ops_args != NULL && nd->pos >= 0) ? ev->p->ops_args[nd->pos].primary : NULL, span(nd));
     }
@@ -382,14 +382,8 @@ static const void* beval_node(xb_beval* ev, int at, int is_root, long long* stri
     else { out = ev->pool + ev->used; ev->used += (size_t)(ev->cnt * *stride); }
     node_desc(ev->e, at, &d);
     a.in0 = in[0]; a.in1 = in[1]; a.in2 = in[2]; a.s_in0 = s[0]; a.s_in1 = s[1]; a.s_in2 = s[2];
-    a.out = out; a.s_out = *stride; a.alpha = 1.0f; a.count = ev->cnt;
-    if (nd->type == EQ_UNARY && ev->p->ops_args != NULL && nd->pos >= 0) {       /* read once, from call 0 */
-      const void* op1 = ev->p->ops_args[nd->pos].primary;
-      if (op1 != NULL && (nd->op == LIBXSMM_MELTW_TYPE_UNARY_LEAKY_RELU || nd->op == LIBXSMM_MELTW_TYPE_UNARY_ELU)) {
-        if (xb_rt_ptr_kind(op1) == 1) xb_rt_memcpy(&a.alpha, op1, sizeof(float)); else a.alpha = *(const float*)op1;
-      }
-    }
-    if (has_bitmask_out(nd)) { a.out_aux = (char*)ev->p->output.secondary + ev->t0 * ev->aux_s; a.s_out_aux = ev->aux_s; }
+    a.out = out; a.s_out = *stride; a.alpha = node_alpha(ev->e, at, ev->p); a.count = ev->cnt;
+    if (has_bitmask_out(ev->e, at)) { a.out_aux = (char*)ev->p->output.secondary + ev->t0 * ev->aux_s; a.s_out_aux = ev->aux_s; }
     else if (is_dump(nd)) { a.out_aux = (char*)ev->p->ops_args[nd->pos].primary + ev->t0 * ev->ops_s[nd->pos]; a.s_out_aux = ev->ops_s[nd->pos]; }
     if (0 != (ev->rc = xb_meltw_launch(&d, &a))) ev->failed = 1;
     return out;
@@ -416,7 +410,7 @@ LIBXSMM_API int libxsmm_b200_meqn_batch_strided(libxsmm_meqn_function kernel, co
     const xb_eqn_node* nd = &e->node[i];
     if (nd->type == EQ_ARG && (input_strides == NULL || param->inputs == NULL || input_strides[nd->pos] < 0 || param->inputs[nd->pos].primary == NULL)) return -1;
     if (is_dump(nd) && (nd->pos < 0 || ops_strides == NULL || param->ops_args == NULL || ops_strides[nd->pos] < 0)) return -1;
-    if (has_bitmask_out(nd) && param->output.secondary == NULL) return -1;
+    if (has_bitmask_out(e, i) && param->output.secondary == NULL) return -1;
     if (is_dump(nd) && param->ops_args[nd->pos].primary == NULL) return -1;
   }
   /* an argument that a DUMP writes is read through the DUMP's buffer: both strides must describe the same tiles */
@@ -433,7 +427,7 @@ LIBXSMM_API int libxsmm_b200_meqn_batch_strided(libxsmm_meqn_function kernel, co
     if (output_stride < (long long)out_bytes) return -1;
     for (i = 0; i < e->nnodes; ++i) {
       const xb_eqn_node* nd = &e->node[i];
-      if (has_bitmask_out(nd) && output_aux_stride < (long long)(LIBXSMM_UP(nd->ld, 16) / 8 * nd->n)) return -1;
+      if (has_bitmask_out(e, i) && output_aux_stride < (long long)xb_meltw_mask_bytes(nd->ld, nd->n)) return -1;
       if (is_dump(nd) && ops_strides[nd->pos] < (long long)span(nd)) return -1;
     }
   }
@@ -443,7 +437,7 @@ LIBXSMM_API int libxsmm_b200_meqn_batch_strided(libxsmm_meqn_function kernel, co
     const xb_eqn_node* nd = &e->node[i];
     if (nd->type == EQ_ARG && xb_rt_ptr_kind(param->inputs[nd->pos].primary) == 0) return -4;
     if (is_dump(nd) && xb_rt_ptr_kind(param->ops_args[nd->pos].primary) == 0) return -4;
-    if (has_bitmask_out(nd) && xb_rt_ptr_kind(param->output.secondary) == 0) return -4;
+    if (has_bitmask_out(e, i) && xb_rt_ptr_kind(param->output.secondary) == 0) return -4;
     if (nd->type != EQ_ARG && i != 0) per_tile += tmp_stride(nd);
   }
   chunk = (per_tile > 0 && per_tile < XB_MEQN_BATCH_SCRATCH_BYTES) ? XB_MEQN_BATCH_SCRATCH_BYTES / per_tile : (per_tile > 0 ? 1 : count);

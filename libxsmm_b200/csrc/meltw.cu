@@ -21,100 +21,6 @@
 
 namespace {
 
-enum { FAM_NONE = 0, FAM_MAP, FAM_REDUCE, FAM_SCALAR, FAM_TRANSFORM, FAM_GS, FAM_QUANT, FAM_DROPOUT, FAM_SPLIT, FAM_MXQUANT };
-
-__host__ __device__ inline bool is_f(int t) {
-  return t == LIBXSMM_DATATYPE_F32 || t == LIBXSMM_DATATYPE_BF16 || t == LIBXSMM_DATATYPE_F16 || t == LIBXSMM_DATATYPE_BF8 || t == LIBXSMM_DATATYPE_HF8;
-}
-
-__host__ __device__ inline int family_of(const xb_meltw_desc& d) {
-  if (d.op_class == LIBXSMM_MELTW_OPERATION_UNARY) {
-    switch (d.op) {
-      case LIBXSMM_MELTW_TYPE_UNARY_IDENTITY: case LIBXSMM_MELTW_TYPE_UNARY_XOR: case LIBXSMM_MELTW_TYPE_UNARY_X2: case LIBXSMM_MELTW_TYPE_UNARY_DUMP:
-      case LIBXSMM_MELTW_TYPE_UNARY_SQRT: case LIBXSMM_MELTW_TYPE_UNARY_NEGATE: case LIBXSMM_MELTW_TYPE_UNARY_INC:
-      case LIBXSMM_MELTW_TYPE_UNARY_RECIPROCAL: case LIBXSMM_MELTW_TYPE_UNARY_RECIPROCAL_SQRT:
-        if (d.t_in0 == LIBXSMM_DATATYPE_F64 && d.t_out == LIBXSMM_DATATYPE_F64 && d.t_comp == LIBXSMM_DATATYPE_F64) return (d.op == LIBXSMM_MELTW_TYPE_UNARY_DUMP) ? FAM_NONE : FAM_MAP;
-        return (is_f(d.t_in0) && is_f(d.t_out)) ? FAM_MAP : FAM_NONE;
-      case LIBXSMM_MELTW_TYPE_UNARY_TANH: case LIBXSMM_MELTW_TYPE_UNARY_TANH_INV: case LIBXSMM_MELTW_TYPE_UNARY_SIGMOID:
-      case LIBXSMM_MELTW_TYPE_UNARY_SIGMOID_INV: case LIBXSMM_MELTW_TYPE_UNARY_GELU: case LIBXSMM_MELTW_TYPE_UNARY_GELU_INV:
-      case LIBXSMM_MELTW_TYPE_UNARY_EXP: case LIBXSMM_MELTW_TYPE_UNARY_REPLICATE_COL_VAR:
-      case LIBXSMM_MELTW_TYPE_UNARY_RELU: case LIBXSMM_MELTW_TYPE_UNARY_RELU_INV: case LIBXSMM_MELTW_TYPE_UNARY_LEAKY_RELU:
-      case LIBXSMM_MELTW_TYPE_UNARY_LEAKY_RELU_INV: case LIBXSMM_MELTW_TYPE_UNARY_ELU: case LIBXSMM_MELTW_TYPE_UNARY_ELU_INV:
-        return (is_f(d.t_in0) && is_f(d.t_out)) ? FAM_MAP : FAM_NONE;
-      case LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X_OP_ADD: case LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X2_OP_ADD:
-      case LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X_X2_OP_ADD: case LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X_OP_MAX:
-      case LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X_OP_MIN: case LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X_OP_ABSMAX:
-      case LIBXSMM_MELTW_TYPE_UNARY_REDUCE_COLS_IDX_OP_ADD: case LIBXSMM_MELTW_TYPE_UNARY_REDUCE_COLS_IDX_OP_MAX:
-      case LIBXSMM_MELTW_TYPE_UNARY_REDUCE_COLS_IDX_OP_MIN:
-        if (d.t_in0 == LIBXSMM_DATATYPE_F64 && d.t_out == LIBXSMM_DATATYPE_F64) return FAM_REDUCE;
-        return (is_f(d.t_in0) && is_f(d.t_out)) ? FAM_REDUCE : FAM_NONE;
-      case LIBXSMM_MELTW_TYPE_UNARY_REDUCE_TO_SCALAR_OP_ADD:
-        if (d.t_in0 == LIBXSMM_DATATYPE_F64 && d.t_out == LIBXSMM_DATATYPE_F64) return FAM_SCALAR;
-        return (is_f(d.t_in0) && is_f(d.t_out)) ? FAM_SCALAR : FAM_NONE;
-      case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_NORMT: return FAM_TRANSFORM;
-      case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_VNNI2: case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_VNNI2_PAD:
-      case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_VNNI2T: case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_VNNI2_TO_VNNI2T:
-      case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_VNNI2T_TO_NORM: case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_VNNI4T:
-      case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_VNNI4T_TO_NORM:
-        return (xb_dev_typesize(d.t_in0) == 2) ? FAM_TRANSFORM : FAM_NONE;
-      case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_VNNI4: case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_VNNI4_PAD:
-      case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_VNNI4_TO_VNNI4T:
-        return (xb_dev_typesize(d.t_in0) <= 2) ? FAM_TRANSFORM : FAM_NONE;
-      case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_VNNI4_TO_NORM:
-        return (xb_dev_typesize(d.t_in0) == 1) ? FAM_TRANSFORM : FAM_NONE;
-      case LIBXSMM_MELTW_TYPE_UNARY_GATHER: case LIBXSMM_MELTW_TYPE_UNARY_SCATTER:
-        return (xb_dev_typesize(d.t_in0) <= 4 && xb_dev_typesize(d.t_in0) >= 1) ? FAM_GS : FAM_NONE;
-      case LIBXSMM_MELTW_TYPE_UNARY_QUANT:
-        if (d.t_in0 == LIBXSMM_DATATYPE_BF16 && (d.t_out == LIBXSMM_DATATYPE_MXFP4X2 || d.t_out == LIBXSMM_DATATYPE_NVFP4X2 || d.t_out == LIBXSMM_DATATYPE_MXBF8)) return FAM_MXQUANT;
-        return (d.t_in0 == LIBXSMM_DATATYPE_F32 && (d.t_out == LIBXSMM_DATATYPE_I8 || d.t_out == LIBXSMM_DATATYPE_I16 || d.t_out == LIBXSMM_DATATYPE_I32)) ? FAM_QUANT : FAM_NONE;
-      case LIBXSMM_MELTW_TYPE_UNARY_DEQUANT:
-        return (d.t_out == LIBXSMM_DATATYPE_F32 && (d.t_in0 == LIBXSMM_DATATYPE_I8 || d.t_in0 == LIBXSMM_DATATYPE_I16 || d.t_in0 == LIBXSMM_DATATYPE_I32)) ? FAM_QUANT : FAM_NONE;
-      case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_VNNI8: case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_VNNI8_PAD:
-      case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_VNNI8_TO_VNNI8T:
-        return (xb_dev_typesize(d.t_in0) <= 2 && xb_dev_typesize(d.t_in0) >= 1) ? FAM_TRANSFORM : FAM_NONE;
-      case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_VNNI8T: case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_VNNI8T_TO_NORM:
-      case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_PADM_MOD2: case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_PADN_MOD2: case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_PADNM_MOD2:
-        return (xb_dev_typesize(d.t_in0) == 2) ? FAM_TRANSFORM : FAM_NONE;
-      case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_PADM_MOD4: case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_PADN_MOD4: case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_PADNM_MOD4:
-      case LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_VNNI4_TO_VNNI2:
-        return (xb_dev_typesize(d.t_in0) == 1) ? FAM_TRANSFORM : FAM_NONE;
-      case LIBXSMM_MELTW_TYPE_UNARY_DROPOUT: case LIBXSMM_MELTW_TYPE_UNARY_DROPOUT_INV:
-        return (is_f(d.t_in0) && is_f(d.t_out)) ? FAM_DROPOUT : FAM_NONE;
-      case LIBXSMM_MELTW_TYPE_UNARY_UNZIP: case LIBXSMM_MELTW_TYPE_UNARY_DECOMP_FP32_TO_BF16X2: case LIBXSMM_MELTW_TYPE_UNARY_DECOMP_FP32_TO_BF16X3:
-        return (d.t_in0 == LIBXSMM_DATATYPE_F32) ? FAM_SPLIT : FAM_NONE;
-      default: return FAM_NONE;
-    }
-  }
-  if (d.op_class == LIBXSMM_MELTW_OPERATION_BINARY) {
-    const bool all64 = d.t_in0 == LIBXSMM_DATATYPE_F64 && d.t_in1 == LIBXSMM_DATATYPE_F64 && d.t_out == LIBXSMM_DATATYPE_F64 && d.t_comp == LIBXSMM_DATATYPE_F64;
-    switch (d.op) {
-      case LIBXSMM_MELTW_TYPE_BINARY_ADD: case LIBXSMM_MELTW_TYPE_BINARY_MUL: case LIBXSMM_MELTW_TYPE_BINARY_SUB:
-      case LIBXSMM_MELTW_TYPE_BINARY_DIV: case LIBXSMM_MELTW_TYPE_BINARY_MULADD: case LIBXSMM_MELTW_TYPE_BINARY_MAX:
-      case LIBXSMM_MELTW_TYPE_BINARY_MIN:
-        return (all64 || (is_f(d.t_in0) && is_f(d.t_in1) && is_f(d.t_out))) ? FAM_MAP : FAM_NONE;
-      case LIBXSMM_MELTW_TYPE_BINARY_CMP_OP_GT: case LIBXSMM_MELTW_TYPE_BINARY_CMP_OP_GE: case LIBXSMM_MELTW_TYPE_BINARY_CMP_OP_LT:
-      case LIBXSMM_MELTW_TYPE_BINARY_CMP_OP_LE: case LIBXSMM_MELTW_TYPE_BINARY_CMP_OP_EQ: case LIBXSMM_MELTW_TYPE_BINARY_CMP_OP_NE:
-        return (is_f(d.t_in0) && is_f(d.t_in1)) ? FAM_MAP : FAM_NONE;
-      case LIBXSMM_MELTW_TYPE_BINARY_ZIP:
-        return (d.t_in0 == LIBXSMM_DATATYPE_U16 || d.t_in0 == LIBXSMM_DATATYPE_BF16 || d.t_in0 == LIBXSMM_DATATYPE_I16) ? FAM_MAP : FAM_NONE;
-      case LIBXSMM_MELTW_TYPE_BINARY_MUL_AND_REDUCE_TO_SCALAR_OP_ADD:
-        return (all64 || (is_f(d.t_in0) && is_f(d.t_in1) && is_f(d.t_out))) ? FAM_SCALAR : FAM_NONE;
-      default: return FAM_NONE;
-    }
-  }
-  if (d.op_class == LIBXSMM_MELTW_OPERATION_TERNARY) {
-    const bool all64 = d.t_in0 == LIBXSMM_DATATYPE_F64 && d.t_in1 == LIBXSMM_DATATYPE_F64 && d.t_in2 == LIBXSMM_DATATYPE_F64
-                    && d.t_out == LIBXSMM_DATATYPE_F64 && d.t_comp == LIBXSMM_DATATYPE_F64;
-    switch (d.op) {
-      case LIBXSMM_MELTW_TYPE_TERNARY_SELECT: return (all64 || (is_f(d.t_in0) && is_f(d.t_in1) && is_f(d.t_out))) ? FAM_MAP : FAM_NONE;
-      case LIBXSMM_MELTW_TYPE_TERNARY_MULADD: case LIBXSMM_MELTW_TYPE_TERNARY_NMULADD:
-        return (is_f(d.t_in0) && is_f(d.t_in1) && is_f(d.t_in2) && is_f(d.t_out)) ? FAM_MAP : FAM_NONE;
-      default: return FAM_NONE;
-    }
-  }
-  return FAM_NONE;
-}
-
 // what a kernel sees of a call: xb_meltw_args without the tile axis, which only the batch instantiations take (as mtiles). The
 // kernels' argument struct keeps its former size, so the single-call kernels compile as they did before the axis existed.
 struct margs {
@@ -972,8 +878,6 @@ int launch_done(const char* where) {
 
 }  // namespace
 
-extern "C" int xb_meltw_supported(const xb_meltw_desc* d) { return family_of(*d) != FAM_NONE; }
-
 // which kernel a call runs (the variant numbers of libxsmm_b200_meltw_variant, include/libxsmm_b200.h). The choice depends on the
 // shape and, for the vector kernels, on the alignment of the operands the kernel reads and writes:
 //   NORM_TO_NORMT with m*n >= 4096 ................................................. 1 tiled transpose (64 x 64 tiles)
@@ -989,9 +893,9 @@ extern "C" int xb_meltw_supported(const xb_meltw_desc* d) { return family_of(*d)
 // A batch (a->count > 1) takes the same kernel as its single call, except: the 16-byte VNNI pack also needs both byte strides to be
 // multiples of 16, and column sums take the warp reduction (4) -- the two-phase reduction's scratch is sized for one call.
 extern "C" int xb_meltw_variant(const xb_meltw_desc* d, const xb_meltw_args* a) {
-  const int fam = family_of(*d);
+  const int fam = xb_meltw_family(d);
   const bool batch = a->count > 1;
-  if (fam == FAM_TRANSFORM) {
+  if (fam == XB_FAM_TRANSFORM) {
     const int ts = xb_dev_typesize(d->t_in0);
     if (d->op == LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_NORMT && (long long)d->m * d->n >= 4096) return 1;
     if ((long long)d->ldo * d->n >= 4096 && ((ts == 2 && (d->op == LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_VNNI2 || d->op == LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_VNNI2_PAD))
@@ -1005,7 +909,7 @@ extern "C" int xb_meltw_variant(const xb_meltw_desc* d, const xb_meltw_args* a) 
     }
     return 0;
   }
-  if (fam == FAM_REDUCE) {
+  if (fam == XB_FAM_REDUCE) {
     const bool sum_op = (d->op == LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X_OP_ADD || d->op == LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X2_OP_ADD || d->op == LIBXSMM_MELTW_TYPE_UNARY_REDUCE_X_X2_OP_ADD);
     if (!batch && sum_op && (d->flags & LIBXSMM_MELTW_FLAG_UNARY_REDUCE_ROWS) == 0 && d->t_in0 != LIBXSMM_DATATYPE_F64 && (long long)d->m * d->n >= (1 << 18) && d->m >= 256) {
       return (d->t_in0 == LIBXSMM_DATATYPE_F32 && (d->m % 4) == 0 && (d->ldi % 4) == 0 && ((uintptr_t)a->in0 & 15) == 0) ? 6 : 5;
@@ -1034,21 +938,20 @@ LIBXSMM_API int libxsmm_b200_meltw_variant(const void* kernel, const void* param
 
 extern "C" int xb_meltw_launch(const xb_meltw_desc* d, const xb_meltw_args* a) {
   cudaStream_t st = (cudaStream_t)xb_rt_stream();
-  const int fam = family_of(*d);
+  const int fam = xb_meltw_family(d);
   if (d->m <= 0 || d->n <= 0) return 0;
   const int variant = xb_meltw_variant(d, a);
   const long long count = (a->count > 1) ? a->count : 1;   // calls in this launch: every grid below is the single call's in x, calls in y
   const margs ka = { a->in0, a->in1, a->in2, a->out, a->in_aux, a->out_aux, a->alpha, a->n_rt, { a->off[0], a->off[1] }, a->rng, a->rnd, a->rnd8 };
   const mtiles tl = { count, a->s_in0, a->s_in1, a->s_in2, a->s_in_aux, a->s_out, a->s_out_aux };
-  if (count > 1 && (fam == FAM_GS || fam == FAM_SPLIT || a->rnd8 != nullptr || a->n_rt != 0
-                    || (fam == FAM_DROPOUT && d->op == LIBXSMM_MELTW_TYPE_UNARY_DROPOUT))) {
+  if (count > 1 && !xb_meltw_batchable(d)) {
     xb_rt_note_error(1, "meltw: this operation has per-call state or run-time extents and runs one call per launch"); return 1;
   }
   // the kernels' tile-axis flag: a batch launches <.., true>, a single call <.., false>
   const auto run = [&](auto batched) -> int {
   constexpr bool B = decltype(batched)::value;
   switch (fam) {
-    case FAM_MAP: {
+    case XB_FAM_MAP: {
       const int n_eff = (d->op_class == LIBXSMM_MELTW_OPERATION_UNARY && d->op == LIBXSMM_MELTW_TYPE_UNARY_REPLICATE_COL_VAR) ? (int)a->n_rt : d->n;
       const long long warps = (long long)((d->m + 31) / 32) * n_eff;
       long long grid = (warps + 7) / 8; if (grid > 132 * 8) grid = 132 * 8; if (grid < 1) return 0;
@@ -1059,7 +962,7 @@ extern "C" int xb_meltw_launch(const xb_meltw_desc* d, const xb_meltw_args* a) {
       meltw_map_kernel<B><<<batch_grid(grid, count, 132 * 8), 256, 0, st>>>(*d, ka, tl, n_eff);
       return launch_done("meltw_map");
     }
-    case FAM_REDUCE: {
+    case XB_FAM_REDUCE: {
       if (variant == 5 || variant == 6) {
         // big column reduction: coalesced two-phase version (partial sums per column slice, then the slices in order)
         int slices = (int)(((long long)132 * 4 * 128 + d->m - 1) / d->m); if (slices > d->n / 16) slices = d->n / 16; if (slices < 1) slices = 1; if (slices > 256) slices = 256;
@@ -1084,13 +987,13 @@ extern "C" int xb_meltw_launch(const xb_meltw_desc* d, const xb_meltw_args* a) {
       else meltw_reduce_kernel<float, B><<<g, 256, 0, st>>>(*d, ka, tl);
       return launch_done("meltw_reduce");
     }
-    case FAM_SCALAR: {
+    case XB_FAM_SCALAR: {
       const dim3 g = batch_grid(1, count, 132 * 2);
       if (d->t_in0 == LIBXSMM_DATATYPE_F64) meltw_scalar_kernel<double, B><<<g, 1024, 0, st>>>(*d, ka, tl);
       else meltw_scalar_kernel<float, B><<<g, 1024, 0, st>>>(*d, ka, tl);
       return launch_done("meltw_scalar");
     }
-    case FAM_TRANSFORM: case FAM_GS: {
+    case XB_FAM_TRANSFORM: case XB_FAM_GS: {
       const long long work = (long long)(d->ldo > d->m ? d->ldo : d->m) * ((d->n + 3) / 4 * 4);
       long long grid = (work + 255) / 256; if (grid > 132 * 16) grid = 132 * 16; if (grid < 1) grid = 1;
       const int ts = xb_dev_typesize(d->t_in0);
@@ -1121,7 +1024,7 @@ extern "C" int xb_meltw_launch(const xb_meltw_desc* d, const xb_meltw_args* a) {
         else meltw_vnni_pack_kernel<unsigned char, 4, B><<<g, 256, 0, st>>>((const unsigned char*)a->in0, (unsigned char*)a->out, d->m, d->n, d->ldi, d->ldo, count, si, so);
         return launch_done("meltw_vnni_pack");
       }
-      if (fam == FAM_TRANSFORM) {
+      if (fam == XB_FAM_TRANSFORM) {
         const dim3 g = batch_grid(grid, count, 132 * 16);
         if (ts == 8) meltw_transform_kernel<unsigned long long, B><<<g, 256, 0, st>>>(*d, ka, tl);
         else if (ts == 4) meltw_transform_kernel<unsigned int, B><<<g, 256, 0, st>>>(*d, ka, tl);
@@ -1134,12 +1037,12 @@ extern "C" int xb_meltw_launch(const xb_meltw_desc* d, const xb_meltw_args* a) {
       }
       return launch_done("meltw_move");
     }
-    case FAM_QUANT: {
+    case XB_FAM_QUANT: {
       long long grid = ((long long)d->m * d->n + 255) / 256; if (grid > 132 * 16) grid = 132 * 16;
       meltw_quant_kernel<B><<<batch_grid(grid, count, 132 * 16), 256, 0, st>>>(*d, ka, tl);
       return launch_done("meltw_quant");
     }
-    case FAM_MXQUANT: {
+    case XB_FAM_MXQUANT: {
       const int blk = (d->t_out == LIBXSMM_DATATYPE_NVFP4X2) ? 16 : 32;
       const long long items = (long long)(d->m / blk) * d->n;
       if (items <= 0) return 0;
@@ -1150,7 +1053,7 @@ extern "C" int xb_meltw_launch(const xb_meltw_desc* d, const xb_meltw_args* a) {
       else meltw_mxquant_kernel<32, 2, B><<<g, 128, 0, st>>>(in, out, sc, d->m, d->n, d->ldi, d->ldo, count, a->s_in0, a->s_out, a->s_out_aux);
       return launch_done("meltw_mxquant");
     }
-    case FAM_DROPOUT: {
+    case XB_FAM_DROPOUT: {
       const long long warps = (long long)((d->m + 31) / 32) * d->n;
       long long grid = (warps + 7) / 8; if (grid > 132 * 8) grid = 132 * 8; if (grid < 1) return 0;
       if (d->op == LIBXSMM_MELTW_TYPE_UNARY_DROPOUT) {
@@ -1160,7 +1063,7 @@ extern "C" int xb_meltw_launch(const xb_meltw_desc* d, const xb_meltw_args* a) {
       meltw_dropout_kernel<B><<<batch_grid(grid, count, 132 * 8), 256, 0, st>>>(*d, ka, tl);
       return launch_done("meltw_dropout");
     }
-    case FAM_SPLIT: {
+    case XB_FAM_SPLIT: {
       long long grid = ((long long)d->m * d->n + 255) / 256; if (grid > 132 * 16) grid = 132 * 16;
       meltw_split_kernel<<<(unsigned int)grid, 256, 0, st>>>(*d, ka);
       return launch_done("meltw_split");

@@ -288,9 +288,29 @@ typedef struct xb_meltw_args {
 } xb_meltw_args;
 void xb_invoke_meqn(const struct xb_slot* s, const void* param);
 void xb_meqn_release(void* work);
-int xb_meltw_supported(const xb_meltw_desc* d);                          /* pure host logic */
 int xb_meltw_launch(const xb_meltw_desc* d, const xb_meltw_args* a);
-int xb_meltw_batchable(const xb_meltw_desc* d);                         /* host_meltw.c: 0 if a call carries per-call state */
+/* the matrix-eltwise rules (host_meltw.c), pure host logic. The kernel family that serves a descriptor, or XB_FAM_NONE: whether it
+ * dispatches; meltw.cu launches by it. */
+enum { XB_FAM_NONE = 0, XB_FAM_MAP, XB_FAM_REDUCE, XB_FAM_SCALAR, XB_FAM_TRANSFORM, XB_FAM_GS, XB_FAM_QUANT, XB_FAM_DROPOUT, XB_FAM_SPLIT,
+       XB_FAM_MXQUANT };
+int xb_meltw_family(const xb_meltw_desc* d);
+/* side operands: what a call of a served descriptor reads or writes next to its inputs and its output, one bit each */
+enum {
+  XB_MSIDE_IN_AUX = 1,      /* in.secondary: a bit mask, an index array, the forward output or the quantiser scale */
+  XB_MSIDE_MASK_OUT = 2,    /* out.secondary: a bit mask */
+  XB_MSIDE_ARGOP = 4,       /* out.secondary: the argop indices of a column reduction */
+  XB_MSIDE_COPY_OUT = 8,    /* out.secondary: the DUMP copy */
+  XB_MSIDE_OUT_AUX = 16,    /* out.secondary: MX block scales, scatter indices or plane offsets */
+  XB_MSIDE_ALPHA = 32,      /* op.primary: a float (alpha, the drop probability) */
+  XB_MSIDE_STATE = 64,      /* op.secondary: generator state, read and advanced */
+  XB_MSIDE_COUNT = 128,     /* a run-time count: the columns (op.primary) or the indices (in.tertiary) */
+  XB_MSIDE_RUNTIME = 256    /* run-time indices or plane offsets: no extent to stage, the operands must be device-accessible */
+};
+int xb_meltw_sides(const xb_meltw_desc* d);
+int xb_meltw_batchable(const xb_meltw_desc* d);   /* 0 if a call carries per-call state or run-time extents */
+float xb_meltw_scalar(const void* p);             /* a float in host or device memory */
+/* bytes of a bit mask of n columns whose rows are ld bits rounded up to 16 */
+static inline size_t xb_meltw_mask_bytes(long long ld, long long n) { return (size_t)LIBXSMM_UP(ld, 16) / 8 * (size_t)n; }
 int xb_sreg_launch(const xb_sparse_desc* d, const void* b, void* c, long long n_total);
 int xb_packed_sp_launch(const xb_sparse_desc* d, const void* a, const void* b, void* c, long long count,
                         long long stride_a, long long stride_b, long long stride_c);

@@ -1,7 +1,8 @@
 /* TEST INFRASTRUCTURE ONLY -- never linked into libxsmm_b200.so.
  *
  * A stand-in for the CUDA side of the library (runtime.cu and the kernel launchers) so that the HOST logic above the kernels --
- * equation trees (host_meqn.c), operand staging, dispatch rules -- can be exercised in the GPU-less build container:
+ * equation trees (host_meqn.c), operand staging, dispatch rules (the mateltwise family rule of host_meltw.c included, unstubbed) --
+ * can be exercised in the GPU-less build container:
  * "device" memory is plain host memory, every elementwise launch and every dense GEMM tile is answered by the oracle
  * (oracle/liboracle.so), fsspmdm runs the library's own direct loop on the host, the tensor-core and packed / block-sparse launchers refuse. tests/test_hostsim.py links the host_*.o objects with this file into tests/c/_hostsim/libxsmm.so and
  * runs the reference's unmodified equation drivers against it; what that validates is the order of evaluation, the shapes and
@@ -157,9 +158,9 @@ int xb_bcsc_launch(xb_sparse_desc* d, const void* a, const void* b_vals, const u
 int xb_bcsc_tc_variant(const xb_sparse_desc* d, unsigned long long n_blocks) { (void)d; (void)n_blocks; return 0; }
 void xb_bcsc_state_free(void* work) { (void)work; }
 
-/* elementwise: the oracle answers. Only the argument forms an equation node uses are mapped (operands, output, the two
- * secondaries, the scalar of LEAKY_RELU/ELU/QUANT/DROPOUT, the generator state); run-time extents are refused */
-int xb_meltw_supported(const xb_meltw_desc* d) { return d->m > 0 && d->n > 0; }
+/* elementwise: the oracle answers. The arguments are mapped back to a parameter struct by the descriptor's side operands (operands,
+ * output, the two secondaries, the scalar of LEAKY_RELU/ELU/DROPOUT or the scale of QUANT/DEQUANT, the generator state); run-time
+ * extents are refused */
 int xb_meltw_launch(const xb_meltw_desc* d, const xb_meltw_args* a) {
   int desc[14]; int rc; float alpha = a->alpha;
   desc[0] = d->op_class; desc[1] = d->op; desc[2] = (int)d->flags; desc[3] = d->m; desc[4] = d->n; desc[5] = d->ldi; desc[6] = d->ldi2; desc[7] = d->ldi3;
@@ -170,7 +171,7 @@ int xb_meltw_launch(const xb_meltw_desc* d, const xb_meltw_args* a) {
     libxsmm_meltw_unary_param p; memset(&p, 0, sizeof(p));
     p.in.primary = (void*)(uintptr_t)a->in0; p.in.secondary = (void*)(uintptr_t)a->in_aux; p.out.primary = a->out; p.out.secondary = a->out_aux; p.op.primary = &alpha;
     p.op.secondary = a->rng;                 /* dropout / stochastic rounding: the staged generator state, advanced in place */
-    if ((d->op == LIBXSMM_MELTW_TYPE_UNARY_QUANT || d->op == LIBXSMM_MELTW_TYPE_UNARY_DEQUANT) && a->in_aux == NULL) p.in.secondary = &alpha;   /* the scale */
+    if ((xb_meltw_sides(d) & XB_MSIDE_IN_AUX) && a->in_aux == NULL) p.in.secondary = &alpha;   /* the quantiser's scale, read on the host */
     rc = oracle_meltw(desc, &p, 0);
   } else if (d->op_class == LIBXSMM_MELTW_OPERATION_BINARY) {
     libxsmm_meltw_binary_param p; memset(&p, 0, sizeof(p));
