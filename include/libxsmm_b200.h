@@ -158,6 +158,31 @@ typedef struct libxsmm_b200_spgemm_strides { long long a, b, c; } libxsmm_b200_s
 LIBXSMM_API int libxsmm_b200_spgemm_batch_strided(libxsmm_gemmfunction kernel, const libxsmm_gemm_param* param,
   const libxsmm_b200_spgemm_strides* strides, long long count);
 
+/* ---- batched fused BRGEMM (libxsmm_dispatch_brgemm_ext handles) ---------------------------------
+ * The batch forms of a brgemm_ext handle, which the forms above refuse: count calls of one brgemm_ext handle, with or without a
+ * fusion (column bias, ReLU with or without its bit mask, sigmoid) and VNNI_C included, in one launch of the kernel family its single call runs on (libxsmm_b200_kernel_backend). Strided form: call t
+ * is kernel(param) with a.primary, b.primary, c.primary, d.primary (the bias column) and c.secondary (the ReLU bit mask) advanced
+ * by t times their stride (BYTES; 0 = one operand shared by every call, as one bias column for every tile). Values a single call
+ * reads by value are read once, from call 0: the int8 -> f32 scale (c.tertiary), the batch-reduce count (op.tertiary) and the
+ * offset-mode arrays (a.secondary / b.secondary). Record form: one argument struct per tile, each with its own address / offset
+ * arrays, bias, mask and scale; under VNNI_C its C pointers must be evenly spaced (c.primary of tile t = tile 0's + t times the
+ * distance of tiles 0 and 1). Both return 0; -1 for a NULL or foreign handle (a libxsmm_dispatch_gemm handle has the batch forms
+ * above), count < 0, a negative stride, a C stride below the bytes one call writes through C, a mask stride below
+ * UP(ldc,16)/8 * n bytes, or a NULL operand, offset array, bias or mask the handle needs; -2 for address batch-reduce in the
+ * strided form (per-tile arrays: the record form); -4 if an operand is pageable host memory (device, managed or pinned only);
+ * the positive CUDA error if a launch fails. Nothing is launched and C and the mask are untouched on a refusal. count == 0 does
+ * nothing. Both honour libxsmm_b200_set_blocking; the record form, offset arrays and VNNI_C return after the device has finished.
+ * VNNI_C: after the product, one batched pass re-packs C from a copy in device scratch; past 64 MiB of C span (the C stride times
+ * the tiles) the batch runs in chunks of that size, each one product launch and one pass. */
+typedef struct libxsmm_b200_gemm_ext_strides {
+  long long a, b, c;   /* a.primary, b.primary, c.primary */
+  long long bias;      /* d.primary, the bias column; 0 = one column shared by every tile */
+  long long mask;      /* c.secondary, the ReLU bit mask */
+} libxsmm_b200_gemm_ext_strides;
+LIBXSMM_API int libxsmm_b200_gemm_ext_batch_strided(libxsmm_gemmfunction_ext kernel, const libxsmm_gemm_ext_param* param,
+  const libxsmm_b200_gemm_ext_strides* strides, long long count);
+LIBXSMM_API int libxsmm_b200_gemm_ext_batch(libxsmm_gemmfunction_ext kernel, const libxsmm_gemm_ext_param* params, long long count);
+
 #if defined(__cplusplus)
 }
 #endif

@@ -325,6 +325,14 @@ class SpgemmStrides(C.Structure):
 
 libxsmm_b200_spgemm_batch_strided = _sig("libxsmm_b200_spgemm_batch_strided", _I, [_P, C.POINTER(GemmParam), C.POINTER(SpgemmStrides), _LL])
 
+
+class GemmExtStrides(C.Structure):
+    _fields_ = [(n, C.c_longlong) for n in ("a", "b", "c", "bias", "mask")]
+
+
+libxsmm_b200_gemm_ext_batch_strided = _sig("libxsmm_b200_gemm_ext_batch_strided", _I, [_P, C.POINTER(GemmExtParam), C.POINTER(GemmExtStrides), _LL])
+libxsmm_b200_gemm_ext_batch = _sig("libxsmm_b200_gemm_ext_batch", _I, [_P, C.POINTER(GemmExtParam), _LL])
+
 EXPORTED = [n for n in dir() if n.startswith("libxsmm_") and callable(globals()[n])]
 
 

@@ -75,10 +75,20 @@ __device__ __forceinline__ DotGeom dot_geom(const xb_gemm_desc& d) {
   return g;
 }
 
-// ---- the reference's accumulation loops, shared by gemm_simt_kernel and gemm_simt_fused_kernel ---------------------------
+// ---- the reference's accumulation loops, shared by gemm_simt_kernel and gemm_fused_kernel --------------------------------
 // Each returns `acc` after the batch-reduce and k loops of element (i, j), in the reference's order and rounding points; the
-// seed, the scale, the epilogue and the store stay with the caller.
-__device__ __forceinline__ float dot_f32(const xb_gemm_desc& d, const DotGeom& g, const TileCtx& x, int i, int j, float acc) {   // reference :1359-1426
+// seed, the scale, the epilogue and the store stay with the caller. `x` is the operand source: a TileCtx is the tile in global
+// memory (every batch-reduce block, the k of `g`); a Staged source is one k-chunk of one block that gemm_fused_kernel copied into
+// shared memory in the operand's own layout, described by the leading dimensions and the k of `g`.
+struct Staged {
+  const char* a; const char* b;
+  static constexpr unsigned long long br = 1;
+};
+__device__ __forceinline__ void br_ptrs(const xb_gemm_desc&, const Staged& x, unsigned long long, int, int, const char*& pa, const char*& pb) {
+  pa = x.a; pb = x.b;
+}
+
+template <class S> __device__ __forceinline__ float dot_f32(const xb_gemm_desc& d, const DotGeom& g, const S& x, int i, int j, float acc) {   // reference :1359-1426
   const int k = g.k;
   const long long lda = g.lda, ldb = g.ldb;
   const bool trans_a = g.trans_a, trans_b = g.trans_b;
@@ -96,7 +106,7 @@ __device__ __forceinline__ float dot_f32(const xb_gemm_desc& d, const DotGeom& g
 }
 
 // reference :1452-1683 (four sign combinations); an f32 C always reads A as VNNI4
-__device__ __forceinline__ unsigned int dot_i8(const xb_gemm_desc& d, const DotGeom& g, const TileCtx& x, int i, int j, unsigned int acc) {
+template <class S> __device__ __forceinline__ unsigned int dot_i8(const xb_gemm_desc& d, const DotGeom& g, const S& x, int i, int j, unsigned int acc) {
   const int k = g.k;
   const long long lda = g.lda, ldb = g.ldb;
   const bool ua = g.ua, ub = g.ub;
@@ -114,7 +124,7 @@ __device__ __forceinline__ unsigned int dot_i8(const xb_gemm_desc& d, const DotG
   return acc;
 }
 
-__device__ __forceinline__ float dot_f16(const xb_gemm_desc& d, const DotGeom& g, const TileCtx& x, int i, int j, float acc) {   // reference :2025-2126
+template <class S> __device__ __forceinline__ float dot_f16(const xb_gemm_desc& d, const DotGeom& g, const S& x, int i, int j, float acc) {   // reference :2025-2126
   const int k = g.k;
   const long long lda = g.lda, ldb = g.ldb;
   const bool trans_b = g.trans_b;
@@ -134,7 +144,7 @@ __device__ __forceinline__ float dot_f16(const xb_gemm_desc& d, const DotGeom& g
   return acc;
 }
 
-__device__ __forceinline__ float dot_bf16(const xb_gemm_desc& d, const DotGeom& g, const TileCtx& x, int i, int j, float acc) {   // reference :2127-2170 and :2367-2419
+template <class S> __device__ __forceinline__ float dot_bf16(const xb_gemm_desc& d, const DotGeom& g, const S& x, int i, int j, float acc) {   // reference :2127-2170 and :2367-2419
   const int k = g.k;
   const long long lda = g.lda, ldb = g.ldb;
   const bool trans_a = g.trans_a, trans_b = g.trans_b;
@@ -171,50 +181,150 @@ __device__ __forceinline__ void fuse_st(void* p, long long i, int t, float v) {
   else if (t == LIBXSMM_DATATYPE_BF16) ((unsigned short*)p)[i] = xb_f32_to_bf16_rne(v);
   else ((unsigned short*)p)[i] = xb_f32_to_f16(v);
 }
+// the f32 image of element (i, j) before the product: the bias, plus the old C when beta = 1
+__device__ __forceinline__ float fuse_seed(const xb_gemm_desc& d, const TileCtx& x, bool bias, bool beta0, int i, long long ci) {
+  if (bias) { const float bv = fuse_ld(x.colbias, i, d.tc); return beta0 ? bv : __fadd_rn(bv, fuse_ld(x.c, ci, d.tc)); }
+  if (!beta0) return (d.tc == LIBXSMM_DATATYPE_F32) ? ((const float*)x.c)[ci] : fuse_ld(x.c, ci, d.tc);
+  return 0.0f;
+}
 
-__global__ void __launch_bounds__(256) gemm_simt_fused_kernel(const xb_gemm_launch L, const int path) {
+// gemm_fused_kernel: a CTA computes one block of C of 32*wm rows x FB_COLS/wm columns (wm = 1 for m <= 32, else 2), the blocks of
+// every tile taken in a grid-stride loop. For each batch-reduce block and each k-chunk of FB_K, the CTA copies the block's rows of A
+// and columns of B into shared memory once, in the operand's own layout (FuseLay); every thread then runs the path's dot_* loop over
+// the staged chunk for FB_NC columns of its row, carrying their accumulators in registers from chunk to chunk, so that each
+// element sees the operations of one uninterrupted loop. A warp owns 32 consecutive rows: the ReLU bitmask is one ballot per warp
+// and column. Chunks start at multiples of FB_K, a multiple of every VNNI factor, and the last one is k % FB_K long.
+constexpr int FB_THREADS = 256, FB_K = 32, FB_NC = 4, FB_COLS = (FB_THREADS / 32) * FB_NC, FB_MAX_CTAS = 4096;
+
+__host__ __device__ inline void fuse_blocks(int m, int n, int& bm, int& bn, int& per_tile) {
+  const int wm = (m > 32) ? 2 : 1;
+  bm = 32 * wm; bn = FB_COLS / wm;
+  per_tile = ((m + bm - 1) / bm) * ((n + bn - 1) / bn);
+}
+
+// how a path reads an operand at row (A) / column (B) p and k index kk: in packed groups of v k (v = 1: kk*ld + p), p-major
+// (p*ld + kk), or not at all (the reference's zero operand); es: bytes per element
+enum { FUSE_PK = 0, FUSE_PM, FUSE_ZERO };
+struct FuseLay { int form, v, es; };
+__device__ __forceinline__ void fuse_layouts(const DotGeom& g, int path, FuseLay& la, FuseLay& lb) {
+  switch (path) {
+    case P_F32: la = { g.trans_a ? FUSE_PM : FUSE_PK, 1, 4 }; lb = { g.trans_b ? FUSE_PK : FUSE_PM, 1, 4 }; break;
+    case P_I8_F32: la = { FUSE_PK, 4, 1 }; lb = { FUSE_PM, 1, 1 }; break;
+    case P_F16_F16: case P_F16_F32: la = { FUSE_PK, g.vnni_a ? 2 : 1, 2 }; lb = { g.trans_b ? FUSE_PK : FUSE_PM, 1, 2 }; break;
+    default: {   // P_BF16_F32 / P_BF16_BF16, as dot_bf16 reads them
+      const int kb = g.vnni_a ? 2 : 1;
+      la = { !g.trans_a ? FUSE_PK : (!g.vnni_a ? FUSE_PM : FUSE_ZERO), kb, 2 };
+      if (g.trans_b) lb = { FUSE_PK, g.vnni_b ? kb : 1, 2 };
+      else lb = { !g.vnni_b ? FUSE_PM : FUSE_ZERO, 1, 2 };
+    }
+  }
+}
+// local leading dimension of a staged operand with a p-extent of np
+__device__ __forceinline__ int fuse_ld_local(const FuseLay& l, int np) { return (l.form == FUSE_PK) ? np : FB_K + 1; }
+
+// copies rows / columns [p0, p0 + np) x k [k0, k0 + kc) of an operand (global leading dimension ld) into dst, laid out as in global
+// memory with the local leading dimension; p past np_ok lies outside the matrix and is staged as zero
+template <typename T>
+__device__ __forceinline__ void fuse_stage(char* dst, const char* src, const FuseLay& l, long long ld, int p0, int np, int np_ok, int k0, int kc) {
+  if (l.form == FUSE_ZERO) return;
+  const T* s = reinterpret_cast<const T*>(src);
+  T* o = reinterpret_cast<T*>(dst);
+  const int v = l.v, lv = (v == 4) ? 2 : (v == 2 ? 1 : 0), ldl = fuse_ld_local(l, np);   // v is 1, 2 or 4: shifts, no divisions
+  for (int e = threadIdx.x; e < np * kc; e += FB_THREADS) {
+    int p, kl;
+    if (l.form == FUSE_PK) { const int q = e / (np * v), w = e - q * (np * v); p = w >> lv; kl = q * v + (w & (v - 1)); }   // consecutive threads: consecutive bytes
+    else { p = e / kc; kl = e - p * kc; }
+    const int kk = k0 + kl;
+    T val = T(0);
+    if (p < np_ok) val = (l.form == FUSE_PK) ? s[(long long)(kk >> lv) * ld * v + (long long)(p0 + p) * v + (kk & (v - 1))] : s[(long long)(p0 + p) * ld + kk];
+    o[(l.form == FUSE_PK) ? (kl >> lv) * ldl * v + p * v + (kl & (v - 1)) : p * ldl + kl] = val;
+  }
+}
+__device__ __forceinline__ void fuse_stage_any(char* dst, const char* src, const FuseLay& l, long long ld, int p0, int np, int np_ok, int k0, int kc) {
+  if (l.es == 4) fuse_stage<unsigned int>(dst, src, l, ld, p0, np, np_ok, k0, kc);
+  else if (l.es == 2) fuse_stage<unsigned short>(dst, src, l, ld, p0, np, np_ok, k0, kc);
+  else fuse_stage<unsigned char>(dst, src, l, ld, p0, np, np_ok, k0, kc);
+}
+
+// the path's loop over one staged chunk for the thread's columns jl0 .. jl0 + nc - 1; an int8 sum travels in acc as its bits
+template <int PATH>
+__device__ __forceinline__ void fuse_dots(const xb_gemm_desc& d, const DotGeom& gs, const Staged& st, int il, int jl0, int nc, float (&acc)[FB_NC]) {
+#pragma unroll
+  for (int c = 0; c < FB_NC; ++c) {
+    if (c >= nc) break;
+    if (PATH == P_F32) acc[c] = dot_f32(d, gs, st, il, jl0 + c, acc[c]);
+    else if (PATH == P_I8_F32) acc[c] = __uint_as_float(dot_i8(d, gs, st, il, jl0 + c, __float_as_uint(acc[c])));
+    else if (PATH == P_F16_F16) acc[c] = dot_f16(d, gs, st, il, jl0 + c, acc[c]);
+    else acc[c] = dot_bf16(d, gs, st, il, jl0 + c, acc[c]);
+  }
+}
+
+__global__ void __launch_bounds__(FB_THREADS) gemm_fused_kernel(const xb_gemm_launch L, const int path) {
+  __shared__ __align__(16) char smem_a[64 * (FB_K + 1) * 4];
+  __shared__ __align__(16) char smem_b[FB_COLS * (FB_K + 1) * 4];
   const xb_gemm_desc& d = L.d;
   const DotGeom g = dot_geom(d);
   const int m = d.m, n = d.n;
   const long long ldc = d.ldc;
   const bool bias = d.fuse_colbias != 0, relu = d.cp_op == LIBXSMM_MELTW_TYPE_UNARY_RELU, sigm = d.cp_op == LIBXSMM_MELTW_TYPE_UNARY_SIGMOID;
-  const bool bitm = relu && (d.cp_flags & LIBXSMM_MELTW_FLAG_UNARY_BITMASK_2BYTEMULT) != 0;
+  const bool bitm_desc = relu && (d.cp_flags & LIBXSMM_MELTW_FLAG_UNARY_BITMASK_2BYTEMULT) != 0;
   const bool beta0 = (d.flags & LIBXSMM_GEMM_FLAG_BETA_0) != 0, beta0_eff = beta0 && !bias;
-  const int lane = threadIdx.x & 31, chunks = (m + 31) / 32;
+  const bool seeded = (path == P_F32 || path == P_BF16_F32 || path == P_BF16_BF16);   // the seed is the loop's starting value
   const long long mask_ld = ((ldc + 15) / 16) * 16;
-  for (long long t = blockIdx.x; t < L.count; t += gridDim.x) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  int bm, bn, per_tile; fuse_blocks(m, n, bm, bn, per_tile);
+  const int wm = bm / 32, blocks_m = (m + bm - 1) / bm;
+  const int il = (warp % wm) * 32 + lane, jl0 = (warp / wm) * FB_NC;   // the thread's row and first column in the block
+  FuseLay la, lb; fuse_layouts(g, path, la, lb);
+  DotGeom gs = g; gs.lda = fuse_ld_local(la, bm); gs.ldb = fuse_ld_local(lb, bn);
+  const Staged st = { smem_a, smem_b };
+  for (long long item = blockIdx.x; item < L.count * per_tile; item += gridDim.x) {
+    const long long t = item / per_tile;
+    const int blk = (int)(item - t * per_tile), i0 = (blk % blocks_m) * bm, j0 = (blk / blocks_m) * bn;
+    const int i = i0 + il, nc = min(FB_NC, max(0, n - j0 - jl0));   // nc is warp-uniform
+    const bool act = i < m;
     TileCtx x; resolve_tile(L, t, x);
-    // a warp owns 32 consecutive rows of one column, so that the ReLU bitmask is one ballot per warp
-    for (int w = threadIdx.x >> 5; w < chunks * n; w += blockDim.x >> 5) {
-      const int j = w / chunks, i0 = (w % chunks) * 32, i = i0 + lane;
-      const bool act = i < m;
-      const long long ci = (long long)j * ldc + i;
-      float y = 0.0f, seed = 0.0f;
-      if (act) {
-        if (bias) { const float bv = fuse_ld(x.colbias, i, d.tc); seed = beta0 ? bv : __fadd_rn(bv, fuse_ld(x.c, ci, d.tc)); }
-        else if (!beta0) seed = (d.tc == LIBXSMM_DATATYPE_F32) ? ((const float*)x.c)[ci] : fuse_ld(x.c, ci, d.tc);
-        float acc;
+    float acc[FB_NC];
+#pragma unroll
+    for (int c = 0; c < FB_NC; ++c) acc[c] = (seeded && act && c < nc) ? fuse_seed(d, x, bias, beta0, i, (long long)(j0 + jl0 + c) * ldc + i) : 0.0f;
+    for (unsigned long long r = 0; r < x.br; ++r) {
+      const char *pa, *pb; br_ptrs(d, x, r, la.es, lb.es, pa, pb);
+      for (int k0 = 0; k0 < g.k; k0 += FB_K) {
+        const int kc = min(FB_K, g.k - k0);
+        __syncthreads();                                       // the previous chunk is consumed
+        fuse_stage_any(smem_a, pa, la, g.lda, i0, bm, min(bm, m - i0), k0, kc);
+        fuse_stage_any(smem_b, pb, lb, g.ldb, j0, bn, min(bn, n - j0), k0, kc);
+        __syncthreads();
+        gs.k = kc;
         switch (path) {
-          case P_F32: acc = dot_f32(d, g, x, i, j, beta0_eff ? 0.0f : seed); break;
-          case P_I8_F32:
-            __builtin_assume(d.tc == LIBXSMM_DATATYPE_F32);   // xb_gemm_path: P_I8_F32 has an f32 C, so dot_i8 reads VNNI4
-            acc = __fmul_rn((float)(int)dot_i8(d, g, x, i, j, 0u), x.scf);
-            if (!beta0_eff) acc = __fadd_rn(acc, seed);
-            break;
-          case P_F16_F16: case P_F16_F32:
-            acc = dot_f16(d, g, x, i, j, 0.0f);
-            if (!beta0_eff) acc = __fadd_rn(acc, xb_f16_to_f32(xb_f32_to_f16(seed)));   // the F32-C variant rounds the old C through f16 (:2118-2124)
-            break;
-          default: acc = dot_bf16(d, g, x, i, j, beta0_eff ? 0.0f : seed); break;   // P_BF16_F32 / P_BF16_BF16
+          case P_F32: fuse_dots<P_F32>(d, gs, st, il, jl0, nc, acc); break;
+          case P_I8_F32: fuse_dots<P_I8_F32>(d, gs, st, il, jl0, nc, acc); break;
+          case P_F16_F16: case P_F16_F32: fuse_dots<P_F16_F16>(d, gs, st, il, jl0, nc, acc); break;
+          default: fuse_dots<P_BF16_F32>(d, gs, st, il, jl0, nc, acc); break;
         }
-        y = relu ? ((acc <= 0.0f) ? 0.0f : acc) : (sigm ? (tanhf(acc / 2.0f) + 1.0f) / 2.0f : acc);
-        fuse_st(x.c, ci, d.tc, y);
-        seed = acc;
+      }
+    }
+    const bool bitm = bitm_desc && x.relu_mask != nullptr;
+#pragma unroll
+    for (int c = 0; c < FB_NC; ++c) {
+      if (c >= nc) break;
+      const int j = j0 + jl0 + c;
+      const long long ci = (long long)j * ldc + i;
+      float a = acc[c];
+      if (act) {
+        if (path == P_I8_F32) {
+          a = __fmul_rn((float)(int)__float_as_uint(acc[c]), x.scf);
+          if (!beta0_eff) a = __fadd_rn(a, fuse_seed(d, x, bias, beta0, i, ci));
+        } else if (path == P_F16_F16 || path == P_F16_F32) {   // the F32-C variant rounds the old C through f16 (:2118-2124)
+          if (!beta0_eff) a = __fadd_rn(a, xb_f16_to_f32(xb_f32_to_f16(fuse_seed(d, x, bias, beta0, i, ci))));
+        }
+        fuse_st(x.c, ci, d.tc, relu ? ((a <= 0.0f) ? 0.0f : a) : (sigm ? (tanhf(a / 2.0f) + 1.0f) / 2.0f : a));
       }
       if (bitm) {
-        const unsigned int word = __ballot_sync(0xffffffffu, act && !(seed <= 0.0f));
+        const unsigned int word = __ballot_sync(0xffffffffu, act && !(a <= 0.0f));
+        const int iw = i0 + (il & ~31);
         if (lane < 4) {
-          const int ib = i0 + lane * 8;
+          const int ib = iw + lane * 8;
           if (ib < m) {
             unsigned char* dst = x.relu_mask + ib / 8 + (long long)j * (mask_ld / 8);
             const unsigned int valid = (m - ib >= 8) ? 0xffu : ((1u << (m - ib)) - 1u);
@@ -916,8 +1026,10 @@ extern "C" int xb_gemm_simt_launch(const xb_gemm_launch* L) {
     return launched("gemm_lowbit");
   }
   if (L->d.fuse_colbias != 0 || L->d.cp_op != 0) {
-    gemm_simt_fused_kernel<<<grid, 256, 0, st>>>(*L, path);
-    return launched("gemm_simt_fused");
+    int bm, bn, per_tile; fuse_blocks(L->d.m, L->d.n, bm, bn, per_tile);
+    const long long blocks = L->count * per_tile;
+    gemm_fused_kernel<<<(unsigned int)(blocks < FB_MAX_CTAS ? blocks : FB_MAX_CTAS), FB_THREADS, 0, st>>>(*L, path);
+    return launched("gemm_fused");
   }
   if (i8_fast_ok(*L, path) && getenv("LIBXSMM_B200_I8_EXACT_ORDER") == nullptr) {
     const int small = (L->d.m < L->d.n) ? L->d.m : L->d.n;

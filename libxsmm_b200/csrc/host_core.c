@@ -582,12 +582,29 @@ static int xb_run_gemm_launch(const xb_gemm_launch* L) {
   return xb_gemm_ts_supported(&L->d) ? xb_gemm_ts_launch(L) : xb_gemm_tc_launch(L);
 }
 
+/* bytes of C one call writes: a VNNI-packed C is re-packed as the whole ldc x n image, padding rows included */
+static int xb_vnni_c(const xb_gemm_desc* d) { return (d->flags & LIBXSMM_GEMM_FLAG_VNNI_C) != 0 && libxsmm_typesize((libxsmm_datatype)d->tc) == 2; }
+static size_t xb_extent_c(const xb_gemm_desc* d) {
+  return (xb_vnni_c(d) ? (size_t)d->n * d->ldc : ((size_t)(d->n - 1) * d->ldc + d->m)) * libxsmm_typesize((libxsmm_datatype)d->tc);
+}
+
+/* the pass that re-packs a C written in normal layout into VNNI2 (reference :2803-2815): from a copy `in` into C */
+static int xb_vnni_c_pass(const xb_gemm_desc* d, const void* in, void* c, long long count, long long stride) {
+  xb_meltw_desc md; xb_meltw_args ma;
+  memset(&md, 0, sizeof(md)); memset(&ma, 0, sizeof(ma));
+  md.op_class = LIBXSMM_MELTW_OPERATION_UNARY; md.op = LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_VNNI2; md.m = d->m; md.n = d->n;
+  md.ldi = d->ldc; md.ldo = d->ldc; md.t_in0 = md.t_out = md.t_comp = d->tc; md.t_in1 = md.t_in2 = LIBXSMM_DATATYPE_UNSUPPORTED;
+  ma.in0 = in; ma.out = c; ma.alpha = 1.0f;
+  ma.count = count; ma.s_in0 = stride; ma.s_out = stride;
+  return xb_meltw_launch(&md, &ma);
+}
+
 static void xb_invoke_gemm(const xb_slot* s, const libxsmm_gemm_param* p) {
   const xb_gemm_desc* d = &s->u.gemm;
   const size_t tsa = libxsmm_typesize((libxsmm_datatype)d->ta), tsb = libxsmm_typesize((libxsmm_datatype)d->tb);
   const size_t tsc = libxsmm_typesize((libxsmm_datatype)d->tc);
-  const int vnni_c = (d->flags & LIBXSMM_GEMM_FLAG_VNNI_C) != 0 && tsc == 2;   /* packs the whole ldc x n image, padding rows included */
-  const size_t ext_a = xb_extent_a(d) * tsa, ext_b = xb_extent_b(d) * tsb, ext_c = (vnni_c ? (size_t)d->n * d->ldc : ((size_t)(d->n - 1) * d->ldc + d->m)) * tsc;
+  const int vnni_c = xb_vnni_c(d);
+  const size_t ext_a = xb_extent_a(d) * tsa, ext_b = xb_extent_b(d) * tsb, ext_c = xb_extent_c(d);
   const unsigned long long br = (d->br_type != 0 && p->op.tertiary != NULL) ? *(const unsigned long long*)p->op.tertiary : 1ull;
   xb_gemm_launch L;
   const int sides = xb_gemm_sides(d);
@@ -674,16 +691,11 @@ static void xb_invoke_gemm(const xb_slot* s, const libxsmm_gemm_param* p) {
     }
   }
   if (0 != xb_run_gemm_launch(&L)) { xb_rt_scratch_reset(); return; }
-  if (vnni_c) {   /* C re-packed norm -> VNNI2 through a copy (reference :2803-2815) */
+  if (vnni_c) {   /* C re-packed norm -> VNNI2 through a copy */
     void* copy = xb_rt_scratch(ext_c);
-    xb_meltw_desc md; xb_meltw_args ma;
     if (copy == NULL) { xb_rt_scratch_reset(); return; }
     xb_rt_memcpy_async(copy, L.one.c, ext_c);
-    memset(&md, 0, sizeof(md)); memset(&ma, 0, sizeof(ma));
-    md.op_class = LIBXSMM_MELTW_OPERATION_UNARY; md.op = LIBXSMM_MELTW_TYPE_UNARY_TRANSFORM_NORM_TO_VNNI2; md.m = d->m; md.n = d->n;
-    md.ldi = d->ldc; md.ldo = d->ldc; md.t_in0 = md.t_out = md.t_comp = d->tc; md.t_in1 = md.t_in2 = LIBXSMM_DATATYPE_UNSUPPORTED;
-    ma.in0 = copy; ma.out = L.one.c; ma.alpha = 1.0f;
-    if (0 != xb_meltw_launch(&md, &ma)) { xb_rt_scratch_reset(); return; }
+    if (0 != xb_vnni_c_pass(d, copy, L.one.c, 1, 0)) { xb_rt_scratch_reset(); return; }
     staged = 1;
   }
   if (need_cb) {
@@ -1185,6 +1197,169 @@ LIBXSMM_API int libxsmm_b200_gemm_batch(libxsmm_gemmfunction kernel, const libxs
   rc = libxsmm_b200_gemm_plan_run(plan);
   if (rc == 0 && !xb_rt_blocking()) rc = xb_rt_sync();   /* the plan's arrays must outlive the launch */
   libxsmm_b200_gemm_plan_destroy(plan);
+  return rc;
+}
+
+/* ---- fused BRGEMM batches (libxsmm_dispatch_brgemm_ext handles) ------------------------------------------------------------ */
+#define XB_VNNI_C_SCRATCH_BYTES (64ll << 20)   /* VNNI_C batch: the copy of C the re-pack reads, scratch per chunk */
+
+static int xb_ext_mask(const xb_gemm_desc* d) {
+  return d->cp_op == LIBXSMM_MELTW_TYPE_UNARY_RELU && (d->cp_flags & LIBXSMM_MELTW_FLAG_UNARY_BITMASK_2BYTEMULT) != 0;
+}
+
+/* the rules both fused batch forms share, before any operand is read: a brgemm_ext handle and count >= 0; for the strided form
+ * (st != NULL) non-negative strides under which no two tiles' C or bit masks overlap, and no address batch-reduce (its arrays are
+ * per tile). 0, or the code the call returns. */
+static int xb_ext_batch_refused(const xb_slot* s, const libxsmm_b200_gemm_ext_strides* st, long long count) {
+  const xb_gemm_desc* d;
+  if (s == NULL || s->kind != XB_KIND_GEMM_EXT || count < 0) return -1;
+  d = &s->u.gemm;
+  if (st == NULL) return 0;
+  if (st->a < 0 || st->b < 0 || st->c < 0 || st->bias < 0 || st->mask < 0) return -1;
+  if (count > 1 && st->c < (long long)xb_extent_c(d)) return -1;
+  if (count > 1 && xb_ext_mask(d) && st->mask < (long long)xb_meltw_mask_bytes(d->ldc, d->n)) return -1;
+  return (d->br_type == 1) ? -2 : 0;
+}
+
+/* one call's operands: -1 if A, B, C, an offset array, or the bias / mask the handle needs is NULL; -4 if one of them (in address
+ * mode: a block the arrays point to) is pageable host memory */
+static int xb_ext_call_refused(const xb_gemm_desc* d, const libxsmm_gemm_ext_param* p) {
+  const void* need[5];
+  const unsigned long long br = (d->br_type != 0 && p->op.tertiary != NULL) ? *(const unsigned long long*)p->op.tertiary : 1ull;
+  int n = 0, i;
+  unsigned long long r;
+  need[n++] = p->c.primary;
+  if (d->fuse_colbias != 0) need[n++] = p->d.primary;
+  if (xb_ext_mask(d)) need[n++] = p->c.secondary;
+  if (p->a.primary == NULL || p->b.primary == NULL || (d->br_type == 2 && br > 0 && (p->a.secondary == NULL || p->b.secondary == NULL))) return -1;
+  for (i = 0; i < n; ++i) if (need[i] == NULL) return -1;
+  if (d->br_type != 1) { need[n++] = p->a.primary; need[n++] = p->b.primary; }
+  else for (r = 0; r < br; ++r) {
+    const void* const* pa = (const void* const*)p->a.primary; const void* const* pb = (const void* const*)p->b.primary;
+    if (xb_rt_ptr_kind(pa) == 1 || xb_rt_ptr_kind(pb) == 1) break;   /* device arrays: the blocks are not readable here */
+    if (pa[r] == NULL || pb[r] == NULL) return -1;
+    if (xb_rt_ptr_kind(pa[r]) == 0 || xb_rt_ptr_kind(pb[r]) == 0) return -4;
+  }
+  for (i = 0; i < n; ++i) if (xb_rt_ptr_kind(need[i]) == 0) return -4;
+  return 0;
+}
+
+/* runs the fused batch L over `count` tiles (strided: L's bases and tile strides; records: L->recs), C of tile t at c0 + t*sc. One
+ * launch; with VNNI_C, chunks of at most XB_VNNI_C_SCRATCH_BYTES of C span, each one launch, a copy of its C span into scratch and
+ * one batched re-pack from that copy, then a sync and a scratch reset. */
+static int xb_ext_batch_run(const xb_gemm_launch* L, long long count, char* c0, long long sc) {
+  const long long ext_c = (long long)xb_extent_c(&L->d), per = (sc > ext_c) ? sc : ext_c;
+  const long long chunk = xb_vnni_c(&L->d) ? ((per < XB_VNNI_C_SCRATCH_BYTES) ? XB_VNNI_C_SCRATCH_BYTES / per : 1) : count;
+  long long t0;
+  int rc = 0;
+  for (t0 = 0; t0 < count && rc == 0; t0 += chunk) {
+    xb_gemm_launch C = *L;
+    C.count = (count - t0 < chunk) ? (count - t0) : chunk;
+    if (L->recs != NULL) C.recs = L->recs + t0;
+    else {
+      C.a = (const char*)L->a + t0 * L->tile_stride_a; C.b = (const char*)L->b + t0 * L->tile_stride_b; C.c = (char*)L->c + t0 * L->tile_stride_c;
+      if (C.one.d != NULL) C.one.d = (const char*)L->one.d + t0 * L->tile_stride_d;
+      if (C.one.c_aux != NULL) C.one.c_aux = (char*)L->one.c_aux + t0 * L->tile_stride_c_aux;
+    }
+    rc = xb_run_gemm_launch(&C);
+    if (!xb_vnni_c(&L->d)) break;
+    if (rc == 0) {
+      const size_t span = (size_t)((C.count - 1) * sc + ext_c);
+      void* copy = xb_rt_scratch(span);
+      if (copy == NULL) rc = 2;
+      else if (0 == (rc = xb_rt_memcpy_async(copy, c0 + t0 * sc, span))) rc = xb_vnni_c_pass(&L->d, copy, c0 + t0 * sc, C.count, sc);
+    }
+    { const int rs = xb_rt_sync(); if (rc == 0) rc = rs; }
+    xb_rt_scratch_reset();
+  }
+  return rc;
+}
+
+LIBXSMM_API int libxsmm_b200_gemm_ext_batch_strided(libxsmm_gemmfunction_ext kernel, const libxsmm_gemm_ext_param* param,
+  const libxsmm_b200_gemm_ext_strides* strides, long long count)
+{
+  const xb_slot* s = xb_slot_of((const void*)kernel);
+  const xb_gemm_desc* d;
+  xb_gemm_launch L;
+  void* offs = NULL;
+  int rc;
+  if (param == NULL || strides == NULL) return -1;
+  if (0 != (rc = xb_ext_batch_refused(s, strides, count))) return rc;
+  if (count == 0) return 0;
+  d = &s->u.gemm;
+  if (0 != (rc = xb_ext_call_refused(d, param))) return rc;
+  memset(&L, 0, sizeof(L));
+  L.d = *d;
+  L.a = param->a.primary; L.b = param->b.primary; L.c = param->c.primary;
+  L.tile_stride_a = strides->a; L.tile_stride_b = strides->b; L.tile_stride_c = strides->c;
+  L.br = (d->br_type != 0 && param->op.tertiary != NULL) ? *(const unsigned long long*)param->op.tertiary : 1ull;
+  if (d->path == P_I8_F32 && param->c.tertiary != NULL) L.one.scf = *(const float*)param->c.tertiary;   /* call 0's, for every tile */
+  if (d->fuse_colbias != 0) { L.one.d = param->d.primary; L.tile_stride_d = strides->bias; }
+  if (xb_ext_mask(d)) { L.one.c_aux = param->c.secondary; L.tile_stride_c_aux = strides->mask; }
+  if (d->br_type == 2 && L.br > 0) {   /* call 0's offset arrays, shared by every tile */
+    const size_t bytes = (size_t)L.br * sizeof(long long);
+    offs = xb_rt_device_malloc(2 * bytes);
+    if (offs == NULL) return 2;
+    if (0 != xb_rt_memcpy(offs, param->a.secondary, bytes) || 0 != xb_rt_memcpy((char*)offs + bytes, param->b.secondary, bytes)) { xb_rt_device_free(offs); return 2; }
+    L.one.a_aux = offs; L.one.b_aux = (const char*)offs + bytes;
+  }
+  rc = xb_ext_batch_run(&L, count, (char*)param->c.primary, strides->c);
+  if (offs != NULL) { const int rs = xb_rt_sync(); if (rc == 0) rc = rs; xb_rt_device_free(offs); }
+  else if (rc == 0 && xb_rt_blocking()) rc = xb_rt_sync();
+  return rc;
+}
+
+LIBXSMM_API int libxsmm_b200_gemm_ext_batch(libxsmm_gemmfunction_ext kernel, const libxsmm_gemm_ext_param* params, long long count) {
+  const xb_slot* s = xb_slot_of((const void*)kernel);
+  const xb_gemm_desc* d;
+  xb_gemm_launch L;
+  xb_gemm_rec* recs;
+  xb_gemm_rec* d_recs;
+  char* arrays = NULL; char* d_arrays = NULL;
+  size_t arrays_bytes = 0, off = 0;
+  long long t, sc = 0;
+  int rc;
+  if (0 != (rc = xb_ext_batch_refused(s, NULL, count))) return rc;
+  if (count == 0) return 0;
+  if (params == NULL) return -1;
+  d = &s->u.gemm;
+  for (t = 0; t < count; ++t) if (0 != (rc = xb_ext_call_refused(d, &params[t]))) return rc;
+  if (xb_vnni_c(d) && count > 1) {   /* the re-pack is one strided pass: C tiles evenly spaced, none reaching into the next */
+    sc = (long long)((const char*)params[1].c.primary - (const char*)params[0].c.primary);
+    if (sc < (long long)xb_extent_c(d)) return -1;
+    for (t = 2; t < count; ++t) if ((const char*)params[t].c.primary != (const char*)params[0].c.primary + t * sc) return -1;
+  }
+  for (t = 0; t < count; ++t) {   /* address mode: 2*br pointers (host-readable arrays), offset mode: 2*br offsets */
+    const unsigned long long br = (d->br_type != 0 && params[t].op.tertiary != NULL) ? *(const unsigned long long*)params[t].op.tertiary : 1ull;
+    if ((d->br_type == 1 && xb_rt_ptr_kind(params[t].a.primary) != 1) || d->br_type == 2) arrays_bytes += 2 * (size_t)br * 8;
+  }
+  recs = (xb_gemm_rec*)calloc((size_t)count, sizeof(xb_gemm_rec));
+  d_recs = (xb_gemm_rec*)xb_rt_device_malloc((size_t)count * sizeof(xb_gemm_rec));
+  if (arrays_bytes) { arrays = (char*)malloc(arrays_bytes); d_arrays = (char*)xb_rt_device_malloc(arrays_bytes); }
+  if (recs == NULL || d_recs == NULL || (arrays_bytes && (arrays == NULL || d_arrays == NULL))) { rc = 2; goto done; }
+  for (t = 0; t < count; ++t) {
+    const libxsmm_gemm_ext_param* p = &params[t];
+    xb_gemm_rec* r = &recs[t];
+    r->br = (d->br_type != 0 && p->op.tertiary != NULL) ? *(const unsigned long long*)p->op.tertiary : 1ull;
+    r->a = p->a.primary; r->b = p->b.primary; r->c = p->c.primary;
+    if (d->br_type == 1 && xb_rt_ptr_kind(p->a.primary) != 1) {
+      memcpy(arrays + off, p->a.primary, (size_t)r->br * 8); r->a = d_arrays + off; off += (size_t)r->br * 8;
+      memcpy(arrays + off, p->b.primary, (size_t)r->br * 8); r->b = d_arrays + off; off += (size_t)r->br * 8;
+    } else if (d->br_type == 2) {
+      if (r->br > 0) { memcpy(arrays + off, p->a.secondary, (size_t)r->br * 8); memcpy(arrays + off + (size_t)r->br * 8, p->b.secondary, (size_t)r->br * 8); }
+      r->a_aux = d_arrays + off; r->b_aux = d_arrays + off + (size_t)r->br * 8; off += 2 * (size_t)r->br * 8;
+    }
+    if (d->fuse_colbias != 0) r->d = p->d.primary;
+    if (xb_ext_mask(d)) r->c_aux = p->c.secondary;
+    if (d->path == P_I8_F32 && p->c.tertiary != NULL) r->scf = *(const float*)p->c.tertiary;
+  }
+  if ((arrays_bytes && 0 != xb_rt_memcpy(d_arrays, arrays, arrays_bytes)) || 0 != xb_rt_memcpy(d_recs, recs, (size_t)count * sizeof(xb_gemm_rec))) { rc = 2; goto done; }
+  memset(&L, 0, sizeof(L));
+  L.d = *d; L.recs = d_recs;
+  rc = xb_ext_batch_run(&L, count, (char*)params[0].c.primary, sc);
+  { const int rs = xb_rt_sync(); if (rc == 0) rc = rs; }   /* the records must outlive the launch */
+done:
+  free(recs); free(arrays); xb_rt_device_free(d_recs); xb_rt_device_free(d_arrays);
   return rc;
 }
 

@@ -188,11 +188,12 @@ typedef struct xb_gemm_launch {
   /* mode 1: per-tile records (device array of xb_gemm_rec[count]) */
   const xb_gemm_rec* recs;
   xb_gemm_rec one;      /* count==1 && !recs: passed by value */
+  long long tile_stride_d, tile_stride_c_aux;   /* mode 0, fused: bias column and ReLU bit mask (bases in one.d / c_aux), bytes */
 } xb_gemm_launch;
 
 /* the complete record of tile t: the per-tile record, the single call, or a strided batch's bases advanced by t tile strides (a side
- * operand the launch lacks is NULL with a tile stride of 0). A strided batch shares `one`'s scale factor, bias column and zero
- * points, has offset arrays in offset mode only and no masks. */
+ * operand, bias column or mask the launch lacks is NULL with a tile stride of 0). A strided batch shares `one`'s scale factor and zero
+ * points, and has offset arrays in offset mode only. */
 #if defined(__CUDACC__)
 __host__ __device__
 #endif
@@ -202,7 +203,9 @@ static inline xb_gemm_rec xb_gemm_tile(const xb_gemm_launch* L, long long t) {
   else if (L->a == NULL && L->c == NULL) r = L->one;
   else {
     r.a = (const char*)L->a + t * L->tile_stride_a; r.b = (const char*)L->b + t * L->tile_stride_b; r.c = (char*)L->c + t * L->tile_stride_c;
-    r.a_aux = NULL; r.b_aux = NULL; r.br = L->br; r.scf = L->one.scf; r.d = L->one.d; r.c_aux = NULL; r.a_q = L->one.a_q;
+    r.a_aux = NULL; r.b_aux = NULL; r.br = L->br; r.scf = L->one.scf; r.a_q = L->one.a_q;
+    r.d = (L->one.d != NULL) ? (const char*)L->one.d + t * L->tile_stride_d : NULL;
+    r.c_aux = (L->one.c_aux != NULL) ? (char*)L->one.c_aux + t * L->tile_stride_c_aux : NULL;
     if (L->d.br_type == 2) { r.a_aux = L->one.a_aux; r.b_aux = L->one.b_aux; }
     r.a_s = (const char*)L->one.a_s + t * L->tile_stride_as; r.b_s = (const char*)L->one.b_s + t * L->tile_stride_bs;
     r.c_s = (L->one.c_s != NULL) ? (char*)L->one.c_s + t * L->tile_stride_cs : NULL;
