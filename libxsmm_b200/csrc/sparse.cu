@@ -158,7 +158,8 @@ __global__ void __launch_bounds__(256) sreg_direct_kernel(const SregParams P) {
 // ------------------------------------------------------------------------------------------------------
 // packed sparse: one CTA per batch item, threads over (n, p). The call axis (count, strides) of every packed kernel runs through
 // blockIdx.y: a single call launches its own grid in x with one row of CTAs, a batch stacks up to 65,535 rows of calls and loops
-// over the rest.
+// over the rest. Each product-accumulate is one explicit fma, like the VFMADD231PS/PD of the reference's packed generators on an
+// FMA host; the build's --fmad=false would otherwise round the product and the sum separately.
 struct PackedParams {
   int kind, M, N, K, P, lda, ldb, ldc, beta0, is_f64;
   const unsigned int* ptr; const unsigned int* idx;
@@ -178,17 +179,17 @@ __global__ void __launch_bounds__(256) packed_sp_kernel(const PackedParams Q) {
       if (Q.kind == XB_KIND_SP_A_CSR) {           // C[i][j][p] (+)= sum_z a[z] * B[col[z]][j][p]
         if (Q.ptr[i] == Q.ptr[i + 1]) continue;    // the reference emits nothing for an empty row, not even the BETA_0 zeroing
         T acc = Q.beta0 ? (T)0 : C[((size_t)i * Q.ldc + j) * P + p];
-        for (unsigned int z = Q.ptr[i]; z < Q.ptr[i + 1]; ++z) acc += A[z] * B[((size_t)Q.idx[z] * Q.ldb + j) * P + p];
+        for (unsigned int z = Q.ptr[i]; z < Q.ptr[i + 1]; ++z) acc = fma(A[z], B[((size_t)Q.idx[z] * Q.ldb + j) * P + p], acc);
         C[((size_t)i * Q.ldc + j) * P + p] = acc;
       } else if (Q.kind == XB_KIND_SP_B_CSC) {    // C[i][j][p] (+)= sum_{z in col j} A[i][row[z]][p] * b[z]
         T acc = Q.beta0 ? (T)0 : C[((size_t)i * Q.ldc + j) * P + p];
-        for (unsigned int z = Q.ptr[j]; z < Q.ptr[j + 1]; ++z) acc += A[((size_t)i * Q.lda + Q.idx[z]) * P + p] * B[z];
+        for (unsigned int z = Q.ptr[j]; z < Q.ptr[j + 1]; ++z) acc = fma(A[((size_t)i * Q.lda + Q.idx[z]) * P + p], B[z], acc);
         C[((size_t)i * Q.ldc + j) * P + p] = acc;
       } else if (Q.kind == XB_KIND_SP_B_CSR) {    // rows of B are k; scan each row for column j
         T acc = Q.beta0 ? (T)0 : C[((size_t)i * Q.ldc + j) * P + p];
         for (int k = 0; k < Q.K; ++k) {
           for (unsigned int z = Q.ptr[k]; z < Q.ptr[k + 1]; ++z) {
-            if ((int)Q.idx[z] == j) acc += A[((size_t)i * Q.lda + k) * P + p] * B[z];
+            if ((int)Q.idx[z] == j) acc = fma(A[((size_t)i * Q.lda + k) * P + p], B[z], acc);
           }
         }
         C[((size_t)i * Q.ldc + j) * P + p] = acc;
@@ -200,26 +201,29 @@ __global__ void __launch_bounds__(256) packed_sp_kernel(const PackedParams Q) {
 // C sparse (CSC pattern): c[z][p] (+)= sum_k A[row[z]][k][p] * B[k][col][p]
 // C sparse (CSC pattern, ldc == 0): ONE scalar per non-zero, the packed dimension is summed away:
 //   C[z] (+)= sum_k sum_p A[k][row(z)][p] * B[k][col(z)][p],   A = [K][lda][P], B = [K][ldb][P]
-// (src/generator_packed_spgemm_csc_csparse_avx_avx2_avx512.c:63-191). One warp per non-zero: lanes stride the packed
-// dimension (coalesced 128-byte rows of A and B), shuffle reduction at the end.
-template <typename T>
+// (src/generator_packed_spgemm_csc_csparse_avx_avx2_avx512.c:63-191). The reference's AVX-512 schedule, bit for bit: 16
+// accumulator lanes, lane l takes p = l, l + 16, ... with one VFMADD231PS each (:84-91), k outer; then lanes l and l + 8 are added,
+// then l and l + 4, then (0 + 2) + (1 + 3). One half-warp per non-zero: lane l of the half owns accumulator l, and the xor butterfly
+// over offsets 8, 4, 2, 1 forms exactly those sums in lane 0 (float addition is commutative, so either lane of a pair holds the same
+// value). f32 only: create() refuses other types for C-sparse, as the reference does.
 __global__ void __launch_bounds__(256) packed_csparse_kernel(const PackedParams Q) {
-  const int P = Q.P, lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
+  const int P = Q.P, l = threadIdx.x & 15, half = threadIdx.x >> 4, nhalves = blockDim.x >> 4;
+  const unsigned int mask = 0xffffu << (threadIdx.x & 16);
   const unsigned int nnz = Q.ptr[Q.N];
   for (long long item = blockIdx.y; item < Q.count; item += gridDim.y) {
-    const T* A = (const T*)(Q.a + item * Q.stride_a); const T* B = (const T*)(Q.b + item * Q.stride_b);
-    T* C = (T*)(Q.c + item * Q.stride_c);
-    for (unsigned int z = blockIdx.x * nwarps + warp; z < nnz; z += gridDim.x * nwarps) {
+    const float* A = (const float*)(Q.a + item * Q.stride_a); const float* B = (const float*)(Q.b + item * Q.stride_b);
+    float* C = (float*)(Q.c + item * Q.stride_c);
+    for (unsigned int z = blockIdx.x * nhalves + half; z < nnz; z += gridDim.x * nhalves) {
       int lo = 0, hi = Q.N;                               // column of z: last j with ptr[j] <= z
       while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (Q.ptr[mid] <= z) lo = mid; else hi = mid; }
       const int j = lo, i = (int)Q.idx[z];
-      T acc = 0;
+      float acc = 0.f;
       for (int k = 0; k < Q.K; ++k) {
-        const T* ar = A + ((size_t)k * Q.lda + i) * P; const T* br = B + ((size_t)k * Q.ldb + j) * P;
-        for (int p = lane; p < P; p += 32) acc += ar[p] * br[p];
+        const float* ar = A + ((size_t)k * Q.lda + i) * P; const float* br = B + ((size_t)k * Q.ldb + j) * P;
+        for (int p = l; p < P; p += 16) acc = fmaf(ar[p], br[p], acc);
       }
-      for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-      if (lane == 0) C[z] = Q.beta0 ? acc : acc + C[z];
+      for (int o = 8; o > 0; o >>= 1) acc += __shfl_xor_sync(mask, acc, o, 16);
+      if (l == 0) C[z] = Q.beta0 ? acc : acc + C[z];
     }
   }
 }
@@ -314,7 +318,9 @@ __global__ void __launch_bounds__(256) bcsc_simt_kernel(const BcscParams Q, cons
             const int bv = (Q.tb == LIBXSMM_DATATYPE_U8) ? (int)br : (int)(signed char)br;
             iacc += av * bv;
           } else {
-            facc = __fadd_rn(facc, __fmul_rn(bcsc_load_f(A, ai, Q.ta), bcsc_load_f(bvals, bi, Q.tb)));
+            // one fused multiply-add like the reference's VFMADD231PS; for bf16 operands the widened product is exact in f32, so
+            // fusing changes nothing there
+            facc = __fmaf_rn(bcsc_load_f(A, ai, Q.ta), bcsc_load_f(bvals, bi, Q.tb), facc);
           }
         }
       }
@@ -435,9 +441,9 @@ extern "C" int xb_packed_sp_launch(const xb_sparse_desc* d, const void* a, const
     return check_launch("packed_dense");
   }
   if (d->kind == XB_KIND_SP_C_CSC) {
-    const unsigned int gx = (d->nnz + 7) / 8 > 0 ? (d->nnz + 7) / 8 : 1;
+    const unsigned int gx = (d->nnz + 15) / 16 > 0 ? (d->nnz + 15) / 16 : 1;     // 16 half-warps per CTA, one non-zero each
     const dim3 g2(gx < 1024 ? gx : 1024, grid);
-    if (Q.is_f64) packed_csparse_kernel<double><<<g2, 256, 0, stream>>>(Q); else packed_csparse_kernel<float><<<g2, 256, 0, stream>>>(Q);
+    packed_csparse_kernel<<<g2, 256, 0, stream>>>(Q);
   } else {
     const dim3 g2(1, grid);
     if (Q.is_f64) packed_sp_kernel<double><<<g2, 256, 0, stream>>>(Q); else packed_sp_kernel<float><<<g2, 256, 0, stream>>>(Q);

@@ -8,7 +8,8 @@
  *
  * Interface mirrors oracle/ref_shim.c (ref_* -> oracle_*), so a test can run either side.
  * Build: gcc -O2 -ffp-contract=off (separate multiply and add, like the reference built for baseline
- * x86-64: no FMA contraction).
+ * x86-64: no FMA contraction). Where the reference's JIT emits a fused multiply-add (the EDGE/SeisSol
+ * packed kernels and the f32 BCSC kernel, see there), the restatement says so with an explicit fma()/fmaf().
  */
 #include <math.h>
 #include <stdint.h>
@@ -245,24 +246,27 @@ ORACLE_API int oracle_gemm(const int* dims, const int* types, unsigned int flags
 }
 
 /* ---- packed DENSE GEMM: golds of samples/xgemm_packed/gemm_packed_kernel.c:36-66 (kind 0), samples/xgemm_norm_packed/
- * dense_packedacrm.c:37-49 (kind 1) and dense_packedbcrm.c (kind 2); k outermost, plain multiply-add --------------------------- */
-#define PKD_BODY(T) do { \
+ * dense_packedacrm.c:37-49 (kind 1) and dense_packedbcrm.c (kind 2); k outermost. Every product-accumulate is ONE fused multiply-add:
+ * on an FMA-capable x86 host the packed generators set vmul_instruction to VFMADD231PS/PD (generator_gemm_common.c), and the JIT's
+ * loops keep k ascending per C element. This states that AVX2/AVX-512 path; a pre-FMA host would round twice. ----------------------- */
+#define PKD_BODY(T, FMA) do { \
   const T* A = (const T*)a; const T* B = (const T*)b; T* C = (T*)c; long long mm, nn, kk, p; \
   if (kind == 0) { \
     if (beta0) for (nn = 0; nn < N; ++nn) for (mm = 0; mm < M; ++mm) for (p = 0; p < P; ++p) C[(nn * ldc + mm) * P + p] = 0; \
-    for (kk = 0; kk < K; ++kk) for (mm = 0; mm < M; ++mm) for (nn = 0; nn < N; ++nn) for (p = 0; p < P; ++p) \
-      C[(nn * ldc + mm) * P + p] += A[(kk * lda + mm) * P + p] * B[(nn * ldb + kk) * P + p]; \
+    for (kk = 0; kk < K; ++kk) for (mm = 0; mm < M; ++mm) for (nn = 0; nn < N; ++nn) for (p = 0; p < P; ++p) { \
+      T* cp = &C[(nn * ldc + mm) * P + p]; *cp = FMA(A[(kk * lda + mm) * P + p], B[(nn * ldb + kk) * P + p], *cp); } \
   } else { \
     if (beta0) for (mm = 0; mm < M; ++mm) for (nn = 0; nn < N; ++nn) for (p = 0; p < P; ++p) C[(mm * ldc + nn) * P + p] = 0; \
-    for (kk = 0; kk < K; ++kk) for (mm = 0; mm < M; ++mm) for (nn = 0; nn < N; ++nn) for (p = 0; p < P; ++p) \
-      C[(mm * ldc + nn) * P + p] += (kind == 1) ? A[(mm * lda + kk) * P + p] * B[kk * ldb + nn] : A[mm * lda + kk] * B[(kk * ldb + nn) * P + p]; \
+    for (kk = 0; kk < K; ++kk) for (mm = 0; mm < M; ++mm) for (nn = 0; nn < N; ++nn) for (p = 0; p < P; ++p) { \
+      T* cp = &C[(mm * ldc + nn) * P + p]; \
+      *cp = (kind == 1) ? FMA(A[(mm * lda + kk) * P + p], B[kk * ldb + nn], *cp) : FMA(A[mm * lda + kk], B[(kk * ldb + nn) * P + p], *cp); } \
   } } while (0)
 ORACLE_API int oracle_packed_dense(int kind, int dtype, const int* dims, unsigned int flags, int P, const void* a, const void* b, void* c)
 {
   const long long M = dims[0], N = dims[1], K = dims[2], lda = dims[3], ldb = dims[4], ldc = dims[5];
   const int beta0 = (flags & F_BETA_0) != 0;
   if (kind < 0 || kind > 2) return 1;
-  if (dtype == T_F64) PKD_BODY(double); else if (dtype == T_F32) PKD_BODY(float); else return 1;
+  if (dtype == T_F64) PKD_BODY(double, fma); else if (dtype == T_F32) PKD_BODY(float, fmaf); else return 1;
   return 0;
 }
 
@@ -443,7 +447,13 @@ ORACLE_API int oracle_fsspmdm(int dtype, int M, int N, int K, int lda, int ldb, 
 
 /* ---- BCSC: dense gold of samples/xgemm_sparse/spmm_kernel.c:74-217 evaluated on the kernel's own inputs
  * (A as handed to the kernel: VNNI [K/v][M][v] unless TRANS_A; B in BCSC, blocks [bn][bk], optionally
- * VNNI-T re-packed, :349-372). k runs 0..K-1 like the gold; absent blocks contribute exact zeros. */
+ * VNNI-T re-packed, :349-372). k runs 0..K-1 like the gold; absent blocks contribute exact zeros.
+ * f32: one fmaf per product, like the x86 JIT (generator_packed_spgemm_bcsc_bsparse_avx_avx2_avx512_amx.c, VFMADD231PS per
+ * k of each stored block, blocks in pattern order). bf16: the widened product is exact in f32 (8 x 8 significand bits), so a
+ * fused and a separate multiply-add round the same way; that line keeps the plain form.
+ * TRANS_A (the AT_CT kernel) reads A as [M][K] and writes C as [M][N] like the gold (spmm_kernel.c:92-101), but the JIT sums k
+ * across vector lanes and reduces horizontally at the end; this restatement keeps k ascending, so there the two agree only to
+ * rounding. */
 ORACLE_API int oracle_bcsc(const int* types, const int* geo, unsigned int flags, void* A, void* Bvals, unsigned int* colptr,
                            unsigned int* rowidx, void* C)
 {
@@ -470,7 +480,7 @@ ORACLE_API int oracle_bcsc(const int* types, const int* geo, unsigned int flags,
         if (tc == T_I32) {
           const unsigned char ar = ((const unsigned char*)Ab)[ai], bw = ((const unsigned char*)Bvals)[bi];
           iacc += ((ta == T_U8) ? (int)ar : (int)(signed char)ar) * ((tb == T_U8) ? (int)bw : (int)(signed char)bw);
-        } else if (ta == T_F32) facc += ((const float*)Ab)[ai] * ((const float*)Bvals)[bi];
+        } else if (ta == T_F32) facc = fmaf(((const float*)Ab)[ai], ((const float*)Bvals)[bi], facc);
         else facc += oracle_bf16_widen(((const uint16_t*)Ab)[ai]) * oracle_bf16_widen(((const uint16_t*)Bvals)[bi]);
       }
       if (tc == T_I32) ((int*)Cb)[ci] = iacc; else if (tc == T_F32) ((float*)Cb)[ci] = facc; else ((uint16_t*)Cb)[ci] = oracle_f32_to_bf16(facc);
@@ -480,33 +490,38 @@ ORACLE_API int oracle_bcsc(const int* types, const int* geo, unsigned int flags,
 }
 
 /* ---- packed sparse: golds of samples/xgemm_norm_packed/asparse_packed_csr.c:116-128,
- * bsparse_packed_csc.c:137-150, bsparse_packed_csr.c; BETA_0 per src/generator_packed_spgemm_cs*.c --------- */
-#define PACKED_BODY(T) do { \
+ * bsparse_packed_csc.c:137-150, bsparse_packed_csr.c; BETA_0 per src/generator_packed_spgemm_cs*.c.
+ * Every product-accumulate is ONE fused multiply-add (FMA = fma / fmaf), in the order below: on an FMA-capable x86 host the packed
+ * generators' vmul_instruction is VFMADD231PS/PD (generator_gemm_common.c; generator_packed_spgemm_csr_asparse_avx_avx2_avx512.c:
+ * 420-470), and the C-sparse generator hard-codes VFMADD231PS (generator_packed_spgemm_csc_csparse_avx_avx2_avx512.c:84-91). The
+ * C-sparse schedule is the AVX-512 one: 16 accumulator lanes (lane p % 16), k outer, then the 8 / 4 / (0+2)+(1+3) fold. A host
+ * without FMA, or an AVX2 host for C-sparse (8 lanes), would give other bits. --------------------------------------------------- */
+#define PACKED_BODY(T, FMA) do { \
   const T* A = (const T*)a; const T* B = (const T*)b; T* C = (T*)c; int i, j, k, p; unsigned int z; \
   if (lda == 0) {                          /* A sparse, CSR over M rows */ \
     for (i = 0; i < M; ++i) { if (ptr[i + 1] == ptr[i]) continue;  /* empty rows are not even zeroed (..._csr_asparse_avx_avx2_avx512.c:347-348) */ \
      for (j = 0; j < N; ++j) for (p = 0; p < P; ++p) { \
       T acc = beta0 ? (T)0 : C[((size_t)i * ldc + j) * P + p]; \
-      for (z = ptr[i]; z < ptr[i + 1]; ++z) acc += A[z] * B[((size_t)idx[z] * ldb + j) * P + p]; \
+      for (z = ptr[i]; z < ptr[i + 1]; ++z) acc = FMA(A[z], B[((size_t)idx[z] * ldb + j) * P + p], acc); \
       C[((size_t)i * ldc + j) * P + p] = acc; } } \
   } else if (ldb == 0 && is_csc) {        /* B sparse, CSC over N columns */ \
     for (i = 0; i < M; ++i) for (j = 0; j < N; ++j) for (p = 0; p < P; ++p) { \
       T acc = beta0 ? (T)0 : C[((size_t)i * ldc + j) * P + p]; \
-      for (z = ptr[j]; z < ptr[j + 1]; ++z) acc += A[((size_t)i * lda + idx[z]) * P + p] * B[z]; \
+      for (z = ptr[j]; z < ptr[j + 1]; ++z) acc = FMA(A[((size_t)i * lda + idx[z]) * P + p], B[z], acc); \
       C[((size_t)i * ldc + j) * P + p] = acc; } \
   } else if (ldb == 0) {                  /* B sparse, CSR over K rows; columns past the last populated one are left alone \
       (generator_packed_spgemm_csr_bsparse_avx_avx2_avx512.c:64-70) */ \
     int ncol = 0; for (z = 0; z < ptr[K]; ++z) ncol = ((int)idx[z] + 1 > ncol) ? (int)idx[z] + 1 : ncol; \
     for (i = 0; i < M; ++i) for (j = 0; j < ncol && j < N; ++j) for (p = 0; p < P; ++p) { \
       T acc = beta0 ? (T)0 : C[((size_t)i * ldc + j) * P + p]; \
-      for (k = 0; k < K; ++k) for (z = ptr[k]; z < ptr[k + 1]; ++z) if ((int)idx[z] == j) acc += A[((size_t)i * lda + k) * P + p] * B[z]; \
+      for (k = 0; k < K; ++k) for (z = ptr[k]; z < ptr[k + 1]; ++z) if ((int)idx[z] == j) acc = FMA(A[((size_t)i * lda + k) * P + p], B[z], acc); \
       C[((size_t)i * ldc + j) * P + p] = acc; } \
   } else if (ldc == 0 && is_csc) {        /* C sparse, CSC pattern: ONE scalar per non-zero, the packed dimension is summed \
       away; A is [K][lda][P], B is [K][ldb][P] (..._csc_csparse_avx_avx2_avx512.c:63-79, 123-191) */ \
     for (j = 0; j < N; ++j) for (z = ptr[j]; z < ptr[j + 1]; ++z) { \
       T lane[16], acc; int l; for (l = 0; l < 16; ++l) lane[l] = (T)0; \
       for (k = 0; k < K; ++k) for (p = 0; p < P; ++p) \
-        lane[p % 16] += A[((size_t)k * lda + idx[z]) * P + p] * B[((size_t)k * ldb + j) * P + p]; \
+        lane[p % 16] = FMA(A[((size_t)k * lda + idx[z]) * P + p], B[((size_t)k * ldb + j) * P + p], lane[p % 16]); \
       for (l = 0; l < 8; ++l) lane[l] += lane[l + 8]; for (l = 0; l < 4; ++l) lane[l] += lane[l + 4]; \
       acc = (lane[0] + lane[2]) + (lane[1] + lane[3]); \
       C[z] = beta0 ? acc : acc + C[z]; } \
@@ -519,6 +534,6 @@ ORACLE_API int oracle_packed_sp(int is_csc, int dtype, const int* dims, unsigned
   const int beta0 = (flags & F_BETA_0) != 0;
   (void)values;
   if (ldc == 0 && (dtype != T_F32 || P % 16 != 0 || P <= 0)) return 1;  /* C-sparse exists for f32, full 16-lane vectors only */
-  if (dtype == T_F64) PACKED_BODY(double); else if (dtype == T_F32) PACKED_BODY(float); else return 1;
+  if (dtype == T_F64) PACKED_BODY(double, fma); else if (dtype == T_F32) PACKED_BODY(float, fmaf); else return 1;
   return 0;
 }

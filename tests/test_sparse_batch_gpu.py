@@ -16,7 +16,7 @@ from sparse_batch_cases import PACKED_KINDS, POISON, BcscCase, PackedCase, param
 
 pytestmark = pytest.mark.gpu
 NOT_BATCHABLE = -6
-EXACT = ("a_csr", "b_csr", "b_csc")            # same summation order as the oracle
+EXACT = ("a_csr", "b_csr", "b_csc", "c_csc", "pk_gemm", "pk_ac_rm", "pk_bc_rm")   # same order as the oracle, one FMA per product
 PACKED = [(k, t) for k in PACKED_KINDS for t in (gen.F32, gen.F64) if not (k == "c_csc" and t == gen.F64)]
 BCSC_TYPES = {"bf16": (gen.BF16, gen.BF16, gen.F32, gen.BF16), "f32": (gen.F32, gen.F32, gen.F32, gen.F32),
               "u8i8": (gen.U8, gen.I8, gen.I32, gen.I32)}

@@ -9,6 +9,8 @@ Workloads, all device-resident:
     N = 9 quantities), packed width P = 8 and 16, f32 and f64, `elements` (default 2^20) elements = elements / P calls.
   * BCSC bf16, the geometry of bench.py (M = 32, N = K = 512, 32 x 32 blocks, 50 %, 8,192 m_blocks) split into 64 calls of 128
     m_blocks (A and C per call, the block values shared); the same work as one single call over all m_blocks is timed beside it.
+  * C-sparse CSC f32: a 56 x 56 pattern at 30 %, K = 9, P = 16 and 64, elements / P calls (A, B and C per call).
+  * BCSC f32 on the exact-order kernel: M = 32, N = K = 512, 16 x 16 blocks at 50 %, 1,024 m_blocks, one call.
 For each: the median time of one batch call (CUDA events, after warm-up), the compulsory bytes (every operand element a call
 reads, once, and C also written; shared operands once), GB/s and the fraction of the data sheet's 3.35 TB/s, which kernel family
 ran, and the same handle through a loop of single calls in non-blocking mode over the first `loop_calls` calls (default 4,096),
@@ -195,6 +197,56 @@ def bcsc(args):
     return res
 
 
+def csparse(args):
+    """C-sparse f32 (one scalar per non-zero, the packed dimension summed away): a 56 x 56 pattern at 30 %, K = 9, P = 16 and 64"""
+    rng = np.random.default_rng(556)
+    Mc = Nc = 56; Kc = 9
+    keep = rng.random((Nc, Mc)) < 0.3                       # [column][row]
+    colptr = np.concatenate([[0], np.cumsum(keep.sum(1))]).astype(np.uint32); rowidx = np.nonzero(keep)[1].astype(np.uint32)
+    nnz = len(rowidx)
+    out = []
+    for P in (16, 64):
+        calls = args.elements // P
+        sh = X.libxsmm_create_gemm_shape(Mc, Nc, Kc, Mc, Nc, 0, F32, F32, F32, F32)
+        vals = np.zeros(nnz, dtype=np.float32)
+        k = X.libxsmm_create_packed_spgemm_csc(sh, 0, 0, P, colptr.ctypes.data, rowidx.ctypes.data, vals.ctypes.data)
+        assert k and X.libxsmm_b200_kernel_backend(k) == X.BACKEND_STREAM
+        sa, sb, sc = Kc * Mc * P * 4, Kc * Nc * P * 4, nnz * 4
+        a = tenths(calls * sa // 4, torch.float32, 5); b = tenths(calls * sb // 4, torch.float32, 6); c = tenths(calls * nnz, torch.float32, 7)
+        run = Run(k, (a.data_ptr(), b.data_ptr(), c.data_ptr()), (sa, sb, sc), calls)
+        check(run, c, sc)
+        r = measure(run, args.steps, args.warmup, calls * (sa + sb + 2 * sc), args.loop_calls)
+        r.update({"workload": "packed C-sparse CSC f32 56 x 56 (nnz %d) K=%d P=%d" % (nnz, Kc, P)})
+        out.append(r)
+        X.libxsmm_release_kernel(k)
+        del a, b, c
+        torch.cuda.empty_cache()
+    return out
+
+
+def bcsc_f32(args):
+    """BCSC f32 on the exact-order kernel: M = 32, N = K = 512, 16 x 16 blocks at 50 %, 1,024 m_blocks in one call"""
+    Mb, Kb, Nb, bk, bn, mblocks = 32, 512, 512, 16, 16, 1024
+    rng = np.random.default_rng(557)
+    nbr, nbc = Kb // bk, Nb // bn
+    keep = np.zeros(nbr * nbc, dtype=bool); keep[rng.permutation(nbr * nbc)[:nbr * nbc // 2]] = True
+    keep = keep.reshape(nbc, nbr)
+    colptr = np.concatenate([[0], np.cumsum(keep.sum(1))]).astype(np.uint32); rowidx = np.nonzero(keep)[1].astype(np.uint32)
+    nnzb = int(colptr[-1])
+    a = tenths(mblocks * Kb * Mb, torch.float32, 8); bv = tenths(nnzb * bk * bn, torch.float32, 9)
+    c = tenths(mblocks * Nb * Mb, torch.float32, 10)
+    d_cp = torch.from_numpy(colptr.view(np.int32).copy()).cuda(); d_ri = torch.from_numpy(rowidx.view(np.int32).copy()).cuda()
+    extra = {"colptr": d_cp.data_ptr(), "rowidx": d_ri.data_ptr(), "nbc": C.c_ulonglong(nbc)}
+    sh = X.libxsmm_create_gemm_shape(mblocks, 0, Kb, Kb, 0, Nb, F32, F32, F32, F32)
+    k = X.libxsmm_create_packed_spgemm_bcsc(sh, 0, 0, X.SpgemmConfig(Mb, bk, bn))
+    assert k and X.libxsmm_b200_bcsc_variant(k, nbc) == 0
+    run = Run(k, (a.data_ptr(), bv.data_ptr(), c.data_ptr()), (mblocks * Kb * Mb * 4, 0, mblocks * Nb * Mb * 4), 1, extra)
+    r = measure(run, args.steps, args.warmup, mblocks * (Kb + 2 * Nb) * Mb * 4 + nnzb * bk * bn * 4, args.loop_calls)
+    r.update({"workload": "BCSC f32 M=32 N=K=512 16x16 50%% m_blocks=%d, one call (beta = 1)" % mblocks})
+    X.libxsmm_release_kernel(k)
+    return [r]
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--elements", type=int, default=1 << 20)
@@ -205,7 +257,8 @@ def main():
     torch.cuda.set_device(0)
     X.libxsmm_b200_set_device(0)
     name, q = card()
-    out = {"gpu": name, "power_limit_sm_clock_max_clock": q, "peak_gbs": PEAK, "edge_packed_csr": edge(args), "bcsc_bf16": bcsc(args)}
+    out = {"gpu": name, "power_limit_sm_clock_max_clock": q, "peak_gbs": PEAK, "edge_packed_csr": edge(args), "bcsc_bf16": bcsc(args),
+           "csparse_f32": csparse(args), "bcsc_f32": bcsc_f32(args)}
     print(json.dumps(out))
 
 
