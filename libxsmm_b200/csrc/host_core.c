@@ -497,6 +497,13 @@ static size_t xb_extent_b(const xb_gemm_desc* d) {
   return (size_t)(d->n - 1) * d->ldb + d->k;
 }
 
+/* bytes of A and of B that one call of br blocks reads: one operand's extent and, in stride mode, br - 1 block strides more */
+static void xb_gemm_spans(const xb_gemm_desc* d, unsigned long long br, size_t* span_a, size_t* span_b) {
+  *span_a = xb_extent_a(d) * libxsmm_typesize((libxsmm_datatype)d->ta);
+  *span_b = xb_extent_b(d) * libxsmm_typesize((libxsmm_datatype)d->tb);
+  if (d->br_type == 3 && br > 0) { *span_a += (size_t)(br - 1) * (size_t)d->br_stride_a; *span_b += (size_t)(br - 1) * (size_t)d->br_stride_b; }
+}
+
 /* MX block scales touched by one call of br blocks: [br][k/32][ld] bytes, up to the last row in use */
 static size_t xb_extent_mx_scales(const xb_gemm_desc* d, unsigned long long br, int ld, int rows) {
   return (size_t)((br ? br : 1) * (unsigned long long)(d->k / 32) - 1) * (size_t)ld + (size_t)rows;
@@ -633,8 +640,8 @@ static void xb_invoke_gemm(const xb_slot* s, const libxsmm_gemm_param* p) {
       staged = 1;
     }
   } else {
-    size_t span_a = ext_a, span_b = ext_b;
-    if (d->br_type == 3 && br > 0) { span_a += (size_t)(br - 1) * (size_t)d->br_stride_a; span_b += (size_t)(br - 1) * (size_t)d->br_stride_b; }
+    size_t span_a, span_b;
+    xb_gemm_spans(d, br, &span_a, &span_b);
     if (d->br_type == 2 && br > 0) {
       const long long* oa = (const long long*)p->a.secondary; const long long* ob = (const long long*)p->b.secondary;
       long long ma = 0, mb = 0; unsigned long long r;
@@ -777,20 +784,78 @@ LIBXSMM_API void libxsmm_sgemm_(const char* transa, const char* transb,
 }
 
 /* ---- batch entry points -------------------------------------------------------------------------- */
-static const xb_slot* xb_gemm_slot(const void* kernel) {
-  const xb_slot* s = xb_slot_of(kernel);
-  return (s != NULL && (s->kind == XB_KIND_GEMM || s->kind == XB_KIND_GEMM_EXT)) ? s : NULL;
+/* the batch forms, one per entry point: libxsmm_b200_gemm_batch_strided, _strided_multi, _strided_scaled, libxsmm_b200_gemm_batch,
+ * libxsmm_b200_gemm_plan_create, libxsmm_b200_gemm_ext_batch_strided and libxsmm_b200_gemm_ext_batch */
+enum { XB_FORM_STRIDED, XB_FORM_MULTI, XB_FORM_SCALED, XB_FORM_RECORDS, XB_FORM_PLAN, XB_FORM_EXT_STRIDED, XB_FORM_EXT_RECORDS };
+
+static int xb_ext_mask(const xb_gemm_desc* d) {
+  return d->cp_op == LIBXSMM_MELTW_TYPE_UNARY_RELU && (d->cp_flags & LIBXSMM_MELTW_FLAG_UNARY_BITMASK_2BYTEMULT) != 0;
 }
 
-/* 1 if a batch entry point cannot run this handle as a single call would: a fused handle's bias column and ReLU bit mask are
- * per-call operands (libxsmm_gemm_ext_param) that no batch form carries, VNNI-packed C is re-packed by a pass after a single
- * call only, the strided forms have no argument struct for the int8 -> f32 scale (c.tertiary) or for side operands
- * (xb_gemm_sides: libxsmm_b200_gemm_batch_strided_scaled takes scales), and the per-tile records carry no MX fp8 block scales. */
-static int xb_batch_refused(const xb_gemm_desc* d, int strided) {
-  if (d->fuse_colbias != 0 || (d->flags & LIBXSMM_GEMM_FLAG_VNNI_C) != 0) return 1;
-  if (strided ? xb_gemm_sides(d) != 0 : d->path == P_MX8) return 1;
-  if (d->cp_op == LIBXSMM_MELTW_TYPE_UNARY_RELU && (d->cp_flags & LIBXSMM_MELTW_FLAG_UNARY_BITMASK_2BYTEMULT) != 0) return 1;
-  return (strided && d->path == P_I8_F32) ? 1 : 0;
+/* The one rule for which GEMM handles a batch form runs: 0, or the code the form returns for the handle (a plan: NULL for any code).
+ * -1: not a GEMM handle, or not one of the form's: the scaled form takes plain handles with scales and no zero points, the fused forms
+ * brgemm_ext handles only.
+ * LIBXSMM_B200_ERROR_NOT_BATCHABLE: the plain forms carry no per-call bias column or ReLU bit mask of a fused handle, and re-pack a
+ * VNNI-packed C after a single call only; their records carry no MX fp8 block scales; the strided forms have no argument struct for
+ * side operands (xb_gemm_sides) or for the int8 -> f32 scale (c.tertiary). A plan is replayed, so it takes no side operands either.
+ * -2: address and offset batch-reduce need per-tile arrays, which the strided forms do not take (the fused one shares call 0's
+ * offset arrays). The multi-device form reports -2 through the strided call each device makes. */
+static int xb_gemm_batch_refused(const xb_slot* s, int form) {
+  const xb_gemm_desc* d;
+  int sides, per_tile_arrays;
+  if (s == NULL || (s->kind != XB_KIND_GEMM && s->kind != XB_KIND_GEMM_EXT)) return -1;
+  d = &s->u.gemm;
+  sides = xb_gemm_sides(d);
+  per_tile_arrays = (d->br_type == 1 || d->br_type == 2);
+  switch (form) {
+    case XB_FORM_EXT_STRIDED: case XB_FORM_EXT_RECORDS:
+      if (s->kind != XB_KIND_GEMM_EXT) return -1;
+      return (form == XB_FORM_EXT_STRIDED && d->br_type == 1) ? -2 : 0;
+    case XB_FORM_SCALED:
+      if (s->kind != XB_KIND_GEMM || sides == 0 || (sides & XB_SIDE_A_Q) != 0) return -1;
+      return per_tile_arrays ? -2 : 0;
+    default: break;
+  }
+  if (d->fuse_colbias != 0 || (d->flags & LIBXSMM_GEMM_FLAG_VNNI_C) != 0 || xb_ext_mask(d)) return LIBXSMM_B200_ERROR_NOT_BATCHABLE;
+  if (form == XB_FORM_RECORDS || form == XB_FORM_PLAN) {
+    if (d->path == P_MX8) return LIBXSMM_B200_ERROR_NOT_BATCHABLE;
+    return (form == XB_FORM_PLAN && sides != 0) ? -1 : 0;
+  }
+  if (sides != 0 || d->path == P_I8_F32) return LIBXSMM_B200_ERROR_NOT_BATCHABLE;
+  return (form == XB_FORM_STRIDED && per_tile_arrays) ? -2 : 0;
+}
+
+#define XB_CHUNK_SCRATCH_BYTES (64ll << 20)   /* device scratch one chunk of a batch may hold */
+
+/* Runs the launch L over its L->count tiles, tile t's C at c + t*sc. A batch whose tiles need device scratch -- the f32 image of an
+ * MXBF8 C (m*n*4 bytes per tile, in the thread's arena, which keeps its size once grown), or the copy of C that the VNNI_C re-pack
+ * reads (C's span, max(sc, extent) per tile) -- runs in chunks of at most XB_CHUNK_SCRATCH_BYTES of it: per chunk one launch, the
+ * batched re-pack where the descriptor has one, then a sync and a scratch reset. Any other batch is one launch, which only enqueues;
+ * the host pipeline's callback (xb_hostbatch_launch) relies on that, and the strided forms it serves refuse VNNI_C and side operands. */
+static int xb_gemm_batch_launch(const xb_gemm_launch* L, char* c, long long sc) {
+  const int vnni_c = xb_vnni_c(&L->d);
+  const long long ext_c = (long long)xb_extent_c(&L->d);
+  const long long per_tile = vnni_c ? ((sc > ext_c) ? sc : ext_c) : ((xb_gemm_sides(&L->d) & XB_SIDE_C_S) ? (long long)L->d.m * L->d.n * 4 : 0);
+  const long long chunk = (per_tile < XB_CHUNK_SCRATCH_BYTES) ? XB_CHUNK_SCRATCH_BYTES / (per_tile ? per_tile : 1) : 1;
+  long long t0;
+  int rc = 0;
+  if (per_tile == 0) return xb_run_gemm_launch(L);
+  for (t0 = 0; t0 < L->count && rc == 0; t0 += chunk) {
+    const long long n = (L->count - t0 < chunk) ? (L->count - t0) : chunk;
+    const xb_gemm_launch S = xb_gemm_launch_slice(L, t0, n);
+    int rs;
+    rc = xb_run_gemm_launch(&S);
+    if (rc == 0 && vnni_c) {
+      const size_t span = (size_t)((n - 1) * sc + ext_c);
+      void* copy = xb_rt_scratch(span);
+      if (copy == NULL) rc = 2;
+      else if (0 == (rc = xb_rt_memcpy_async(copy, c + t0 * sc, span))) rc = xb_vnni_c_pass(&L->d, copy, c + t0 * sc, n, sc);
+    }
+    rs = xb_rt_sync();
+    if (rc == 0) rc = rs;
+    xb_rt_scratch_reset();
+  }
+  return rc;
 }
 
 /* host-resident strided batch: chunked H2D -> kernel -> D2H through device scratch */
@@ -800,12 +865,11 @@ static int xb_gemm_batch_strided_host(const xb_slot* s, const void* a, const voi
 LIBXSMM_API int libxsmm_b200_gemm_batch_strided(libxsmm_gemmfunction kernel, const void* a, const void* b, void* c,
   long long stride_a, long long stride_b, long long stride_c, unsigned long long br_count, long long count)
 {
-  const xb_slot* s = xb_gemm_slot((const void*)kernel);
+  const xb_slot* s = xb_slot_of((const void*)kernel);
   xb_gemm_launch L;
   int rc;
-  if (s == NULL || count < 0) return -1;
-  if (xb_batch_refused(&s->u.gemm, 1)) return LIBXSMM_B200_ERROR_NOT_BATCHABLE;
-  if (s->u.gemm.br_type == 1 || s->u.gemm.br_type == 2) return -2;   /* address / offset mode need per-tile arrays: use libxsmm_b200_gemm_batch */
+  if (count < 0) return -1;
+  if (0 != (rc = xb_gemm_batch_refused(s, XB_FORM_STRIDED))) return rc;
   if (count == 0) return 0;
   {
     const int ka = xb_rt_ptr_kind(a), kb = xb_rt_ptr_kind(b), kc = xb_rt_ptr_kind(c);
@@ -823,26 +887,23 @@ LIBXSMM_API int libxsmm_b200_gemm_batch_strided(libxsmm_gemmfunction kernel, con
   L.d = s->u.gemm; L.count = count;
   L.a = a; L.b = b; L.c = c; L.tile_stride_a = stride_a; L.tile_stride_b = stride_b; L.tile_stride_c = stride_c;
   L.br = (s->u.gemm.br_type == 0) ? 1ull : br_count;
-  rc = xb_run_gemm_launch(&L);
+  rc = xb_gemm_batch_launch(&L, (char*)c, stride_c);
   if (rc == 0 && xb_rt_blocking()) rc = xb_rt_sync();
   return rc;
 }
-
-#define XB_MX_IMAGE_BYTES (64ll << 20)   /* f32 image of an MXBF8-C batch: scratch per chunk */
 
 LIBXSMM_API int libxsmm_b200_gemm_batch_strided_scaled(libxsmm_gemmfunction kernel,
   const void* a, const void* b, void* c, long long stride_a, long long stride_b, long long stride_c,
   const void* scf_a, const void* scf_b, void* scf_c, long long stride_scf_a, long long stride_scf_b, long long stride_scf_c,
   unsigned long long br_count, long long count)
 {
-  const xb_slot* s = xb_gemm_slot((const void*)kernel);
+  const xb_slot* s = xb_slot_of((const void*)kernel);
+  const int refused = xb_gemm_batch_refused(s, XB_FORM_SCALED);
   xb_gemm_launch L;
   int rc, sides;
-  if (s == NULL || count < 0 || s->kind != XB_KIND_GEMM) return -1;
-  /* handles with scales and no zero points (those need libxsmm_b200_gemm_batch); tile t's are scf_x + t*stride_scf_x */
-  sides = xb_gemm_sides(&s->u.gemm);
-  if (sides == 0 || (sides & XB_SIDE_A_Q) != 0) return -1;
+  if (count < 0 || refused == -1) return -1;
   if (count == 0) return 0;
+  sides = xb_gemm_sides(&s->u.gemm);   /* tile t's scales are scf_x + t*stride_scf_x */
   memset(&L, 0, sizeof(L));
   L.d = s->u.gemm;
   L.tile_stride_a = stride_a; L.tile_stride_b = stride_b; L.tile_stride_c = stride_c;
@@ -851,35 +912,13 @@ LIBXSMM_API int libxsmm_b200_gemm_batch_strided_scaled(libxsmm_gemmfunction kern
   if (sides & XB_SIDE_B_S) { L.one.b_s = scf_b; L.tile_stride_bs = stride_scf_b; }
   if (sides & XB_SIDE_C_S) { L.one.c_s = scf_c; L.tile_stride_cs = stride_scf_c; }
   if (a == NULL || b == NULL || c == NULL || xb_gemm_rec_lacks(&L.one, sides)) return -1;
-  if (L.d.br_type == 1 || L.d.br_type == 2) return -2;   /* per-tile arrays: libxsmm_b200_gemm_batch */
+  if (refused != 0) return refused;   /* -2, after the checks on the operands */
   if (xb_rt_ptr_kind(a) == 0 || xb_rt_ptr_kind(b) == 0 || xb_rt_ptr_kind(c) == 0 || (L.one.a_s != NULL && xb_rt_ptr_kind(L.one.a_s) == 0)
    || (L.one.b_s != NULL && xb_rt_ptr_kind(L.one.b_s) == 0) || (L.one.c_s != NULL && xb_rt_ptr_kind(L.one.c_s) == 0)) return -4;   /* device-accessible operands only */
-  if ((sides & XB_SIDE_C_S) == 0) {
-    L.count = count; L.a = a; L.b = b; L.c = c;
-    rc = xb_run_gemm_launch(&L);
-    if (rc == 0 && xb_rt_blocking()) rc = xb_rt_sync();
-    return rc;
-  }
-  {
-    /* MXBF8 C: the product goes through an f32 image of m*n*4 bytes per tile in the thread's scratch arena, which keeps its size
-     * once grown. The batch runs in chunks of at most XB_MX_IMAGE_BYTES of image, each synchronised before the arena is reused. */
-    const long long per_tile = (long long)L.d.m * L.d.n * 4;
-    const long long chunk = (per_tile < XB_MX_IMAGE_BYTES) ? XB_MX_IMAGE_BYTES / per_tile : 1;
-    long long t0;
-    rc = 0;
-    for (t0 = 0; t0 < count && rc == 0; t0 += chunk) {
-      int rs;
-      L.count = (count - t0 < chunk) ? (count - t0) : chunk;
-      L.a = (const char*)a + t0 * stride_a; L.b = (const char*)b + t0 * stride_b; L.c = (char*)c + t0 * stride_c;
-      L.one.a_s = (const char*)scf_a + t0 * stride_scf_a; L.one.b_s = (const char*)scf_b + t0 * stride_scf_b;
-      L.one.c_s = (char*)scf_c + t0 * stride_scf_c;
-      rc = xb_run_gemm_launch(&L);
-      rs = xb_rt_sync();
-      if (rc == 0) rc = rs;
-      xb_rt_scratch_reset();
-    }
-    return rc;
-  }
+  L.count = count; L.a = a; L.b = b; L.c = c;
+  rc = xb_gemm_batch_launch(&L, (char*)c, stride_c);
+  if (rc == 0 && xb_rt_blocking()) rc = xb_rt_sync();
+  return rc;
 }
 
 /* ---- one process, several GPUs: the batch is the only shard axis (SURVEY.md 8e). Host-resident operands are cut into
@@ -907,8 +946,8 @@ LIBXSMM_API int libxsmm_b200_gemm_batch_strided_multi(libxsmm_gemmfunction kerne
   xb_multi_job jobs[64]; pthread_t th[64];
   int d, rc = 0, started = 0, prev_dev;
   const int avail = xb_rt_device_count();
-  if (xb_gemm_slot((const void*)kernel) == NULL || count < 0 || ndevices <= 0) return -1;
-  if (xb_batch_refused(&xb_gemm_slot((const void*)kernel)->u.gemm, 1)) return LIBXSMM_B200_ERROR_NOT_BATCHABLE;
+  if (count < 0 || ndevices <= 0) return -1;
+  if (0 != (rc = xb_gemm_batch_refused(xb_slot_of((const void*)kernel), XB_FORM_MULTI))) return rc;
   if (ndevices > avail) ndevices = avail;
   if (ndevices > 64) ndevices = 64;
   if (ndevices <= 0) return -1;
@@ -949,7 +988,7 @@ static int xb_hostbatch_launch(void* ctx, const xb_pipe_chunk* ch, void* da, voi
   memset(&L, 0, sizeof(L));
   L.d = *h->d; L.count = ch->count; L.a = da; L.b = db; L.c = dc;
   L.tile_stride_a = h->sa; L.tile_stride_b = h->sb; L.tile_stride_c = h->sc; L.br = (h->d->br_type == 0) ? 1ull : h->br;
-  return xb_run_gemm_launch(&L);
+  return xb_gemm_batch_launch(&L, dc, h->sc);
 }
 
 static int xb_gemm_batch_strided_host(const xb_slot* s, const void* a, const void* b, void* c,
@@ -959,15 +998,12 @@ static int xb_gemm_batch_strided_host(const xb_slot* s, const void* a, const voi
    * overlap the kernel of chunk i. Every chunk is a dense range of tiles, which requires the tile strides to cover the
    * tile footprint (checked: positive strides). Returns when C is valid in host memory. */
   const xb_gemm_desc* d = &s->u.gemm;
-  const size_t tsa = libxsmm_typesize((libxsmm_datatype)d->ta), tsb = libxsmm_typesize((libxsmm_datatype)d->tb);
-  const size_t tsc = libxsmm_typesize((libxsmm_datatype)d->tc);
   xb_hostbatch h;
   long long nchunks;
   if (sa <= 0 || sb <= 0 || sc <= 0 || d->br_type == 2) return -3;
   memset(&h, 0, sizeof(h));
   h.d = d; h.a = (const char*)a; h.b = (const char*)b; h.c = (char*)c; h.sa = sa; h.sb = sb; h.sc = sc; h.br = br; h.count = count;
-  h.fa = xb_extent_a(d) * tsa; h.fb = xb_extent_b(d) * tsb; h.fc = ((size_t)(d->n - 1) * d->ldc + d->m) * tsc;
-  if (d->br_type == 3 && br > 0) { h.fa += (size_t)(br - 1) * (size_t)d->br_stride_a; h.fb += (size_t)(br - 1) * (size_t)d->br_stride_b; }
+  xb_gemm_spans(d, br, &h.fa, &h.fb); h.fc = xb_extent_c(d);
   h.copy_c_in = ((d->flags & LIBXSMM_GEMM_FLAG_BETA_0) == 0 || (size_t)sc != h.fc) ? 1 : 0;
   {
     const size_t per_tile = (size_t)sa + (size_t)sb + (size_t)sc;
@@ -1085,16 +1121,69 @@ static void xb_param_sides(xb_gemm_rec* r, const libxsmm_gemm_param* p, int side
   if (sides & XB_SIDE_A_Q) r->a_q = p->a.quaternary;
 }
 
-/* the per-tile records of a batch: libxsmm_b200_gemm_batch and libxsmm_b200_gemm_plan_create */
+/* The record of one call p of a record-form batch into *r, and the arrays of br entries the kernel has to find in device memory: the
+ * address arrays unless they are device memory already, the offset arrays, and MXFP4 x I8's arrays of scale pointers in address mode.
+ * They are copied to img + *off and the record points at dev + *off; with r == NULL only *off advances (the sizing pass). A fused
+ * handle's p is a libxsmm_gemm_ext_param, which begins with the layout of libxsmm_gemm_param: its bias column and bit mask are read
+ * where the descriptor has them. */
+static void xb_gemm_rec_of(const xb_gemm_desc* d, const libxsmm_gemm_param* p, xb_gemm_rec* r, char* img, char* dev, size_t* off) {
+  const int sides = xb_gemm_sides(d);
+  const unsigned long long br = (d->br_type != 0 && p->op.tertiary != NULL) ? *(const unsigned long long*)p->op.tertiary : 1ull;
+  const void* src[4]; const void** dst[4];
+  xb_gemm_rec scratch;
+  int n = 0, i;
+  if (r == NULL) r = &scratch;
+  memset(r, 0, sizeof(*r));
+  r->br = br; r->a = p->a.primary; r->b = p->b.primary; r->c = p->c.primary;
+  xb_param_sides(r, p, sides);
+  if (d->path == P_I8_F32 && p->c.tertiary != NULL) r->scf = *(const float*)p->c.tertiary;
+  if (d->fuse_colbias != 0) r->d = ((const libxsmm_gemm_ext_param*)p)->d.primary;
+  if (xb_ext_mask(d)) r->c_aux = ((const libxsmm_gemm_ext_param*)p)->c.secondary;
+  if (d->br_type == 1 && xb_rt_ptr_kind(p->a.primary) != 1) { src[n] = p->a.primary; dst[n++] = &r->a; src[n] = p->b.primary; dst[n++] = &r->b; }
+  if (d->br_type == 2) { src[n] = p->a.secondary; dst[n++] = &r->a_aux; src[n] = p->b.secondary; dst[n++] = &r->b_aux; }
+  if (d->br_type == 1 && d->path == P_LOWBIT && (sides & XB_SIDE_B_S) != 0) {
+    if (xb_rt_ptr_kind(p->a.tertiary) != 1) { src[n] = p->a.tertiary; dst[n++] = &r->a_s; }
+    if (xb_rt_ptr_kind(p->b.tertiary) != 1) { src[n] = p->b.tertiary; dst[n++] = &r->b_s; }
+  }
+  for (i = 0; i < n; ++i) {
+    if (r != &scratch) {
+      if (br > 0) memcpy(img + *off, src[i], (size_t)br * 8);
+      *dst[i] = dev + *off;
+    }
+    *off += (size_t)br * 8;
+  }
+}
+
+/* the per-tile records of a record-form batch in device memory: xb_gemm_rec[count] in *d_recs, and the arrays they point to in one
+ * block in *d_arrays (NULL if none). params[t] lies t * param_size bytes past params. 0, or 2 if memory or the upload fails. */
+static int xb_gemm_recs_upload(const xb_gemm_desc* d, const void* params, size_t param_size, long long count, xb_gemm_rec** d_recs, void** d_arrays) {
+#define XB_PARAM(T) ((const libxsmm_gemm_param*)((const char*)params + (size_t)(T) * param_size))
+  xb_gemm_rec* recs = (xb_gemm_rec*)calloc((size_t)count, sizeof(xb_gemm_rec));
+  char* img = NULL;
+  size_t bytes = 0, off = 0;
+  long long t;
+  int rc = 0;
+  for (t = 0; t < count; ++t) xb_gemm_rec_of(d, XB_PARAM(t), NULL, NULL, NULL, &bytes);
+  *d_recs = (xb_gemm_rec*)xb_rt_device_malloc((size_t)count * sizeof(xb_gemm_rec));
+  *d_arrays = NULL;
+  if (bytes) { img = (char*)malloc(bytes); *d_arrays = xb_rt_device_malloc(bytes); }
+  if (recs == NULL || *d_recs == NULL || (bytes && (img == NULL || *d_arrays == NULL))) rc = 2;
+  else {
+    for (t = 0; t < count; ++t) xb_gemm_rec_of(d, XB_PARAM(t), &recs[t], img, (char*)*d_arrays, &off);
+    if ((bytes && 0 != xb_rt_memcpy(*d_arrays, img, bytes)) || 0 != xb_rt_memcpy(*d_recs, recs, (size_t)count * sizeof(xb_gemm_rec))) rc = 2;
+  }
+  free(recs); free(img);
+  if (rc != 0) { xb_rt_device_free(*d_recs); xb_rt_device_free(*d_arrays); *d_recs = NULL; *d_arrays = NULL; }
+  return rc;
+#undef XB_PARAM
+}
+
+/* the plan of a batch of a handle xb_gemm_batch_refused lets through: libxsmm_b200_gemm_batch and libxsmm_b200_gemm_plan_create */
 static libxsmm_b200_gemm_plan* xb_plan_make(const xb_slot* s, const libxsmm_gemm_param* params, long long count) {
   libxsmm_b200_gemm_plan* plan;
-  xb_gemm_rec* recs;
-  char* arrays = NULL; size_t arrays_bytes = 0, off = 0;
+  const int sides = xb_gemm_sides(&s->u.gemm);
   long long t;
-  int mx_arrays, sides;
-  if (s == NULL || params == NULL || count <= 0 || xb_batch_refused(&s->u.gemm, 0)) return NULL;
-  sides = xb_gemm_sides(&s->u.gemm);
-  mx_arrays = (s->u.gemm.path == P_LOWBIT && (sides & XB_SIDE_B_S) != 0);   /* MXFP4 x I8 */
+  if (params == NULL || count <= 0) return NULL;
   for (t = 0; t < count && sides != 0; ++t) {   /* every tile brings each side operand of the handle */
     xb_gemm_rec r;
     memset(&r, 0, sizeof(r));
@@ -1102,53 +1191,9 @@ static libxsmm_b200_gemm_plan* xb_plan_make(const xb_slot* s, const libxsmm_gemm
     if (xb_gemm_rec_lacks(&r, sides)) return NULL;
   }
   plan = (libxsmm_b200_gemm_plan*)calloc(1, sizeof(*plan));
-  if (plan != NULL && xb_plan_try_pool(plan, s, params, count)) return plan;
-  recs = (xb_gemm_rec*)calloc((size_t)count, sizeof(xb_gemm_rec));
-  if (plan == NULL || recs == NULL) { free(plan); free(recs); return NULL; }
-  /* pass 1: size of the per-tile index arrays (address: 2*br pointers, offset: 2*br offsets) */
-  if (s->u.gemm.br_type == 1 || s->u.gemm.br_type == 2) {
-    for (t = 0; t < count; ++t) {
-      const unsigned long long br = *(const unsigned long long*)params[t].op.tertiary;
-      if (xb_rt_ptr_kind(params[t].a.primary) != 1 || s->u.gemm.br_type == 2) arrays_bytes += 2 * (size_t)br * 8;
-      if (s->u.gemm.br_type == 1 && mx_arrays) {   /* MXFP4: the scale pointer arrays, copied alike */
-        if (xb_rt_ptr_kind(params[t].a.tertiary) != 1) arrays_bytes += (size_t)br * 8;
-        if (xb_rt_ptr_kind(params[t].b.tertiary) != 1) arrays_bytes += (size_t)br * 8;
-      }
-    }
-    if (arrays_bytes) {
-      arrays = (char*)malloc(arrays_bytes);
-      plan->d_arrays = xb_rt_device_malloc(arrays_bytes);
-      if (arrays == NULL || plan->d_arrays == NULL) { free(arrays); free(recs); xb_rt_device_free(plan->d_arrays); free(plan); return NULL; }
-    }
-  }
-  for (t = 0; t < count; ++t) {
-    const libxsmm_gemm_param* p = &params[t];
-    xb_gemm_rec* r = &recs[t];
-    r->br = (s->u.gemm.br_type != 0 && p->op.tertiary != NULL) ? *(const unsigned long long*)p->op.tertiary : 1ull;
-    r->a = p->a.primary; r->b = p->b.primary; r->c = p->c.primary;
-    if (s->u.gemm.br_type == 1 && xb_rt_ptr_kind(p->a.primary) != 1) {
-      memcpy(arrays + off, p->a.primary, (size_t)r->br * 8); r->a = (char*)plan->d_arrays + off; off += (size_t)r->br * 8;
-      memcpy(arrays + off, p->b.primary, (size_t)r->br * 8); r->b = (char*)plan->d_arrays + off; off += (size_t)r->br * 8;
-    } else if (s->u.gemm.br_type == 2) {
-      memcpy(arrays + off, p->a.secondary, (size_t)r->br * 8); r->a_aux = (char*)plan->d_arrays + off; off += (size_t)r->br * 8;
-      memcpy(arrays + off, p->b.secondary, (size_t)r->br * 8); r->b_aux = (char*)plan->d_arrays + off; off += (size_t)r->br * 8;
-    }
-    xb_param_sides(r, p, sides);
-    if (mx_arrays) {   /* MXFP4 x I8 block scales, address mode: arrays of br pointers */
-      if (s->u.gemm.br_type == 1 && xb_rt_ptr_kind(p->a.tertiary) != 1) {
-        memcpy(arrays + off, p->a.tertiary, (size_t)r->br * 8); r->a_s = (char*)plan->d_arrays + off; off += (size_t)r->br * 8;
-      }
-      if (s->u.gemm.br_type == 1 && xb_rt_ptr_kind(p->b.tertiary) != 1) {
-        memcpy(arrays + off, p->b.tertiary, (size_t)r->br * 8); r->b_s = (char*)plan->d_arrays + off; off += (size_t)r->br * 8;
-      }
-    }
-    if (s->u.gemm.path == P_I8_F32 && p->c.tertiary != NULL) r->scf = *(const float*)p->c.tertiary;
-  }
-  plan->d_recs = (xb_gemm_rec*)xb_rt_device_malloc((size_t)count * sizeof(xb_gemm_rec));
-  if (plan->d_recs == NULL) { free(arrays); free(recs); xb_rt_device_free(plan->d_arrays); free(plan); return NULL; }
-  if (arrays_bytes) xb_rt_memcpy(plan->d_arrays, arrays, arrays_bytes);
-  xb_rt_memcpy(plan->d_recs, recs, (size_t)count * sizeof(xb_gemm_rec));
-  free(arrays); free(recs);
+  if (plan == NULL) return NULL;
+  if (xb_plan_try_pool(plan, s, params, count)) return plan;
+  if (0 != xb_gemm_recs_upload(&s->u.gemm, params, sizeof(*params), count, &plan->d_recs, &plan->d_arrays)) { free(plan); return NULL; }
   plan->slot = s; plan->count = count;
   return plan;
 }
@@ -1157,9 +1202,8 @@ static libxsmm_b200_gemm_plan* xb_plan_make(const xb_slot* s, const libxsmm_gemm
 LIBXSMM_API libxsmm_b200_gemm_plan* libxsmm_b200_gemm_plan_create(libxsmm_gemmfunction kernel,
   const libxsmm_gemm_param* params, long long count)
 {
-  const xb_slot* s = xb_gemm_slot((const void*)kernel);
-  if (s == NULL || xb_gemm_sides(&s->u.gemm) != 0) return NULL;
-  return xb_plan_make(s, params, count);
+  const xb_slot* s = xb_slot_of((const void*)kernel);
+  return (xb_gemm_batch_refused(s, XB_FORM_PLAN) == 0) ? xb_plan_make(s, params, count) : NULL;
 }
 
 LIBXSMM_API int libxsmm_b200_gemm_plan_run(const libxsmm_b200_gemm_plan* plan) {
@@ -1173,7 +1217,7 @@ LIBXSMM_API int libxsmm_b200_gemm_plan_run(const libxsmm_b200_gemm_plan* plan) {
   }
   memset(&L, 0, sizeof(L));
   L.d = plan->slot->u.gemm; L.count = plan->count; L.recs = plan->d_recs;
-  rc = xb_run_gemm_launch(&L);
+  rc = xb_gemm_batch_launch(&L, NULL, 0);
   if (rc == 0 && xb_rt_blocking()) rc = xb_rt_sync();
   return rc;
 }
@@ -1187,12 +1231,13 @@ LIBXSMM_API void libxsmm_b200_gemm_plan_destroy(libxsmm_b200_gemm_plan* plan) {
 }
 
 LIBXSMM_API int libxsmm_b200_gemm_batch(libxsmm_gemmfunction kernel, const libxsmm_gemm_param* params, long long count) {
-  const xb_slot* s = xb_gemm_slot((const void*)kernel);
+  const xb_slot* s = xb_slot_of((const void*)kernel);
+  const int refused = xb_gemm_batch_refused(s, XB_FORM_RECORDS);
   libxsmm_b200_gemm_plan* plan;
   int rc;
-  if (s != NULL && xb_batch_refused(&s->u.gemm, 0)) return LIBXSMM_B200_ERROR_NOT_BATCHABLE;
+  if (refused == LIBXSMM_B200_ERROR_NOT_BATCHABLE) return refused;
   if (count == 0) return 0;
-  plan = xb_plan_make(s, params, count);   /* unlike a plan, one batch call also carries each tile's side operands */
+  plan = (refused == 0) ? xb_plan_make(s, params, count) : NULL;   /* unlike a plan, one batch call also carries each tile's side operands */
   if (plan == NULL) return -1;
   rc = libxsmm_b200_gemm_plan_run(plan);
   if (rc == 0 && !xb_rt_blocking()) rc = xb_rt_sync();   /* the plan's arrays must outlive the launch */
@@ -1201,26 +1246,6 @@ LIBXSMM_API int libxsmm_b200_gemm_batch(libxsmm_gemmfunction kernel, const libxs
 }
 
 /* ---- fused BRGEMM batches (libxsmm_dispatch_brgemm_ext handles) ------------------------------------------------------------ */
-#define XB_VNNI_C_SCRATCH_BYTES (64ll << 20)   /* VNNI_C batch: the copy of C the re-pack reads, scratch per chunk */
-
-static int xb_ext_mask(const xb_gemm_desc* d) {
-  return d->cp_op == LIBXSMM_MELTW_TYPE_UNARY_RELU && (d->cp_flags & LIBXSMM_MELTW_FLAG_UNARY_BITMASK_2BYTEMULT) != 0;
-}
-
-/* the rules both fused batch forms share, before any operand is read: a brgemm_ext handle and count >= 0; for the strided form
- * (st != NULL) non-negative strides under which no two tiles' C or bit masks overlap, and no address batch-reduce (its arrays are
- * per tile). 0, or the code the call returns. */
-static int xb_ext_batch_refused(const xb_slot* s, const libxsmm_b200_gemm_ext_strides* st, long long count) {
-  const xb_gemm_desc* d;
-  if (s == NULL || s->kind != XB_KIND_GEMM_EXT || count < 0) return -1;
-  d = &s->u.gemm;
-  if (st == NULL) return 0;
-  if (st->a < 0 || st->b < 0 || st->c < 0 || st->bias < 0 || st->mask < 0) return -1;
-  if (count > 1 && st->c < (long long)xb_extent_c(d)) return -1;
-  if (count > 1 && xb_ext_mask(d) && st->mask < (long long)xb_meltw_mask_bytes(d->ldc, d->n)) return -1;
-  return (d->br_type == 1) ? -2 : 0;
-}
-
 /* one call's operands: -1 if A, B, C, an offset array, or the bias / mask the handle needs is NULL; -4 if one of them (in address
  * mode: a block the arrays point to) is pageable host memory */
 static int xb_ext_call_refused(const xb_gemm_desc* d, const libxsmm_gemm_ext_param* p) {
@@ -1244,52 +1269,26 @@ static int xb_ext_call_refused(const xb_gemm_desc* d, const libxsmm_gemm_ext_par
   return 0;
 }
 
-/* runs the fused batch L over `count` tiles (strided: L's bases and tile strides; records: L->recs), C of tile t at c0 + t*sc. One
- * launch; with VNNI_C, chunks of at most XB_VNNI_C_SCRATCH_BYTES of C span, each one launch, a copy of its C span into scratch and
- * one batched re-pack from that copy, then a sync and a scratch reset. */
-static int xb_ext_batch_run(const xb_gemm_launch* L, long long count, char* c0, long long sc) {
-  const long long ext_c = (long long)xb_extent_c(&L->d), per = (sc > ext_c) ? sc : ext_c;
-  const long long chunk = xb_vnni_c(&L->d) ? ((per < XB_VNNI_C_SCRATCH_BYTES) ? XB_VNNI_C_SCRATCH_BYTES / per : 1) : count;
-  long long t0;
-  int rc = 0;
-  for (t0 = 0; t0 < count && rc == 0; t0 += chunk) {
-    xb_gemm_launch C = *L;
-    C.count = (count - t0 < chunk) ? (count - t0) : chunk;
-    if (L->recs != NULL) C.recs = L->recs + t0;
-    else {
-      C.a = (const char*)L->a + t0 * L->tile_stride_a; C.b = (const char*)L->b + t0 * L->tile_stride_b; C.c = (char*)L->c + t0 * L->tile_stride_c;
-      if (C.one.d != NULL) C.one.d = (const char*)L->one.d + t0 * L->tile_stride_d;
-      if (C.one.c_aux != NULL) C.one.c_aux = (char*)L->one.c_aux + t0 * L->tile_stride_c_aux;
-    }
-    rc = xb_run_gemm_launch(&C);
-    if (!xb_vnni_c(&L->d)) break;
-    if (rc == 0) {
-      const size_t span = (size_t)((C.count - 1) * sc + ext_c);
-      void* copy = xb_rt_scratch(span);
-      if (copy == NULL) rc = 2;
-      else if (0 == (rc = xb_rt_memcpy_async(copy, c0 + t0 * sc, span))) rc = xb_vnni_c_pass(&L->d, copy, c0 + t0 * sc, C.count, sc);
-    }
-    { const int rs = xb_rt_sync(); if (rc == 0) rc = rs; }
-    xb_rt_scratch_reset();
-  }
-  return rc;
-}
-
 LIBXSMM_API int libxsmm_b200_gemm_ext_batch_strided(libxsmm_gemmfunction_ext kernel, const libxsmm_gemm_ext_param* param,
   const libxsmm_b200_gemm_ext_strides* strides, long long count)
 {
   const xb_slot* s = xb_slot_of((const void*)kernel);
+  const int refused = xb_gemm_batch_refused(s, XB_FORM_EXT_STRIDED);
   const xb_gemm_desc* d;
   xb_gemm_launch L;
   void* offs = NULL;
   int rc;
-  if (param == NULL || strides == NULL) return -1;
-  if (0 != (rc = xb_ext_batch_refused(s, strides, count))) return rc;
-  if (count == 0) return 0;
+  if (param == NULL || strides == NULL || count < 0 || refused == -1) return -1;
   d = &s->u.gemm;
+  /* non-negative strides under which no two tiles' C or bit masks overlap */
+  if (strides->a < 0 || strides->b < 0 || strides->c < 0 || strides->bias < 0 || strides->mask < 0) return -1;
+  if (count > 1 && strides->c < (long long)xb_extent_c(d)) return -1;
+  if (count > 1 && xb_ext_mask(d) && strides->mask < (long long)xb_meltw_mask_bytes(d->ldc, d->n)) return -1;
+  if (refused != 0) return refused;   /* -2, after the checks on the strides */
+  if (count == 0) return 0;
   if (0 != (rc = xb_ext_call_refused(d, param))) return rc;
   memset(&L, 0, sizeof(L));
-  L.d = *d;
+  L.d = *d; L.count = count;
   L.a = param->a.primary; L.b = param->b.primary; L.c = param->c.primary;
   L.tile_stride_a = strides->a; L.tile_stride_b = strides->b; L.tile_stride_c = strides->c;
   L.br = (d->br_type != 0 && param->op.tertiary != NULL) ? *(const unsigned long long*)param->op.tertiary : 1ull;
@@ -1303,7 +1302,7 @@ LIBXSMM_API int libxsmm_b200_gemm_ext_batch_strided(libxsmm_gemmfunction_ext ker
     if (0 != xb_rt_memcpy(offs, param->a.secondary, bytes) || 0 != xb_rt_memcpy((char*)offs + bytes, param->b.secondary, bytes)) { xb_rt_device_free(offs); return 2; }
     L.one.a_aux = offs; L.one.b_aux = (const char*)offs + bytes;
   }
-  rc = xb_ext_batch_run(&L, count, (char*)param->c.primary, strides->c);
+  rc = xb_gemm_batch_launch(&L, (char*)param->c.primary, strides->c);
   if (offs != NULL) { const int rs = xb_rt_sync(); if (rc == 0) rc = rs; xb_rt_device_free(offs); }
   else if (rc == 0 && xb_rt_blocking()) rc = xb_rt_sync();
   return rc;
@@ -1313,13 +1312,12 @@ LIBXSMM_API int libxsmm_b200_gemm_ext_batch(libxsmm_gemmfunction_ext kernel, con
   const xb_slot* s = xb_slot_of((const void*)kernel);
   const xb_gemm_desc* d;
   xb_gemm_launch L;
-  xb_gemm_rec* recs;
   xb_gemm_rec* d_recs;
-  char* arrays = NULL; char* d_arrays = NULL;
-  size_t arrays_bytes = 0, off = 0;
+  void* d_arrays;
   long long t, sc = 0;
   int rc;
-  if (0 != (rc = xb_ext_batch_refused(s, NULL, count))) return rc;
+  if (count < 0) return -1;
+  if (0 != (rc = xb_gemm_batch_refused(s, XB_FORM_EXT_RECORDS))) return rc;
   if (count == 0) return 0;
   if (params == NULL) return -1;
   d = &s->u.gemm;
@@ -1329,37 +1327,12 @@ LIBXSMM_API int libxsmm_b200_gemm_ext_batch(libxsmm_gemmfunction_ext kernel, con
     if (sc < (long long)xb_extent_c(d)) return -1;
     for (t = 2; t < count; ++t) if ((const char*)params[t].c.primary != (const char*)params[0].c.primary + t * sc) return -1;
   }
-  for (t = 0; t < count; ++t) {   /* address mode: 2*br pointers (host-readable arrays), offset mode: 2*br offsets */
-    const unsigned long long br = (d->br_type != 0 && params[t].op.tertiary != NULL) ? *(const unsigned long long*)params[t].op.tertiary : 1ull;
-    if ((d->br_type == 1 && xb_rt_ptr_kind(params[t].a.primary) != 1) || d->br_type == 2) arrays_bytes += 2 * (size_t)br * 8;
-  }
-  recs = (xb_gemm_rec*)calloc((size_t)count, sizeof(xb_gemm_rec));
-  d_recs = (xb_gemm_rec*)xb_rt_device_malloc((size_t)count * sizeof(xb_gemm_rec));
-  if (arrays_bytes) { arrays = (char*)malloc(arrays_bytes); d_arrays = (char*)xb_rt_device_malloc(arrays_bytes); }
-  if (recs == NULL || d_recs == NULL || (arrays_bytes && (arrays == NULL || d_arrays == NULL))) { rc = 2; goto done; }
-  for (t = 0; t < count; ++t) {
-    const libxsmm_gemm_ext_param* p = &params[t];
-    xb_gemm_rec* r = &recs[t];
-    r->br = (d->br_type != 0 && p->op.tertiary != NULL) ? *(const unsigned long long*)p->op.tertiary : 1ull;
-    r->a = p->a.primary; r->b = p->b.primary; r->c = p->c.primary;
-    if (d->br_type == 1 && xb_rt_ptr_kind(p->a.primary) != 1) {
-      memcpy(arrays + off, p->a.primary, (size_t)r->br * 8); r->a = d_arrays + off; off += (size_t)r->br * 8;
-      memcpy(arrays + off, p->b.primary, (size_t)r->br * 8); r->b = d_arrays + off; off += (size_t)r->br * 8;
-    } else if (d->br_type == 2) {
-      if (r->br > 0) { memcpy(arrays + off, p->a.secondary, (size_t)r->br * 8); memcpy(arrays + off + (size_t)r->br * 8, p->b.secondary, (size_t)r->br * 8); }
-      r->a_aux = d_arrays + off; r->b_aux = d_arrays + off + (size_t)r->br * 8; off += 2 * (size_t)r->br * 8;
-    }
-    if (d->fuse_colbias != 0) r->d = p->d.primary;
-    if (xb_ext_mask(d)) r->c_aux = p->c.secondary;
-    if (d->path == P_I8_F32 && p->c.tertiary != NULL) r->scf = *(const float*)p->c.tertiary;
-  }
-  if ((arrays_bytes && 0 != xb_rt_memcpy(d_arrays, arrays, arrays_bytes)) || 0 != xb_rt_memcpy(d_recs, recs, (size_t)count * sizeof(xb_gemm_rec))) { rc = 2; goto done; }
+  if (0 != (rc = xb_gemm_recs_upload(d, params, sizeof(*params), count, &d_recs, &d_arrays))) return rc;
   memset(&L, 0, sizeof(L));
-  L.d = *d; L.recs = d_recs;
-  rc = xb_ext_batch_run(&L, count, (char*)params[0].c.primary, sc);
+  L.d = *d; L.count = count; L.recs = d_recs;
+  rc = xb_gemm_batch_launch(&L, (char*)params[0].c.primary, sc);
   { const int rs = xb_rt_sync(); if (rc == 0) rc = rs; }   /* the records must outlive the launch */
-done:
-  free(recs); free(arrays); xb_rt_device_free(d_recs); xb_rt_device_free(d_arrays);
+  xb_rt_device_free(d_recs); xb_rt_device_free(d_arrays);
   return rc;
 }
 

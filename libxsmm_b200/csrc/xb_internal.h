@@ -213,6 +213,19 @@ static inline xb_gemm_rec xb_gemm_tile(const xb_gemm_launch* L, long long t) {
   return r;
 }
 
+/* the launch of tiles [t0, t0 + n) of L: tile t of it is tile t0 + t of L, since its records, or its strided bases, start at tile t0
+ * -- the bases are the fields xb_gemm_tile advances */
+static inline xb_gemm_launch xb_gemm_launch_slice(const xb_gemm_launch* L, long long t0, long long n) {
+  xb_gemm_launch S = *L;
+  S.count = n;
+  if (L->recs != NULL) S.recs = L->recs + t0;
+  else if (L->a != NULL || L->c != NULL) {
+    const xb_gemm_rec r = xb_gemm_tile(L, t0);
+    S.a = r.a; S.b = r.b; S.c = r.c; S.one.d = r.d; S.one.c_aux = r.c_aux; S.one.a_s = r.a_s; S.one.b_s = r.b_s; S.one.c_s = r.c_s;
+  }
+  return S;
+}
+
 /* ---- CUDA runtime layer (runtime.cu) ----------------------------------------------------------- */
 int xb_rt_device_count(void);
 int xb_rt_set_device(int ordinal);
