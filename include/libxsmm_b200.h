@@ -103,6 +103,31 @@ LIBXSMM_API int libxsmm_b200_gemm_batch_strided_scaled(libxsmm_gemmfunction kern
   const void* a, const void* b, void* c, long long stride_a, long long stride_b, long long stride_c,
   const void* scf_a, const void* scf_b, void* scf_c, long long stride_scf_a, long long stride_scf_b, long long stride_scf_c,
   unsigned long long br_count, long long count);
+/* the blocked GEMM of a BRGEMM handle over a grid_m x grid_n grid of C tiles, in one launch: tile (i, j), i < grid_m, j < grid_n, is
+ * the single call with
+ *   A + i*stride_a_m, B + j*stride_b_n, C + i*stride_c_m + j*stride_c_n      (strides in BYTES)
+ * and the handle's own batch-reduce addressing, br_count shared by every tile. Row block i of A and column block j of B are shared by
+ * the tiles of their row and column, so this is the loop nest `for mb < grid_m, for nb < grid_n: brgemm(A + mb*sa, B + nb*sb,
+ * C + mb*sc_m + nb*sc_n, br)` without copies of A or B per tile. Each tile's C is bit-identical to the same tile run through
+ * libxsmm_b200_gemm_batch_strided on the same kernel family. C tiles must not overlap, in one of two layouts (esz: C's element size,
+ * span = ((n - 1)*ldc + m)*esz, the bytes one call writes through C):
+ *   - plain matrix: the tiles abut in one column-major C: stride_c_m >= m*esz, (grid_m - 1)*stride_c_m + m*esz <= ldc*esz and
+ *     stride_c_n >= n*ldc*esz;
+ *   - blocked: stride_c_m >= span and stride_c_n >= grid_m*stride_c_m, or the same with the two roles exchanged.
+ * A 1 x N or N x 1 grid is a strided batch and takes that rule: its one stride that matters is at least span (none for 1 x 1), so
+ * an N x 1 grid in the plain-matrix layout (stride_c_m = m*esz, one column block of C) is refused with -1.
+ * Returns, checked in this order: -1 for a NULL or foreign handle or a libxsmm_dispatch_brgemm_ext handle, or a negative grid size or
+ * stride; LIBXSMM_B200_ERROR_NOT_BATCHABLE and -2 for exactly the handles libxsmm_b200_gemm_batch_strided refuses with them (side
+ * operands, int8 -> f32, VNNI_C; address / offset batch-reduce); 0 and nothing launched for an empty grid; -1 for a NULL operand, more
+ * than 2^31 - 1 tiles or C tiles that could overlap; -4 if A, B or C is pageable host memory (device, managed or pinned only); the
+ * positive CUDA error if a launch fails. On a refusal nothing is launched and C is untouched. Honours libxsmm_b200_set_blocking. A
+ * grid runs on wgmma wherever a strided batch of the handle would, unless A or B, stride_a_m or stride_b_n is not a multiple of 16
+ * bytes (the strides are tested whatever the grid's extent, as in the strided form), or a stride along an axis of more than one block
+ * is 0; then on the exact-order kernel (libxsmm_b200_launch_count_backend tells which ran). */
+LIBXSMM_API int libxsmm_b200_gemm_batch_grid(libxsmm_gemmfunction kernel,
+  const void* a, const void* b, void* c,
+  long long stride_a_m, long long stride_b_n, long long stride_c_m, long long stride_c_n,
+  unsigned long long br_count, long long grid_m, long long grid_n);
 /* general form: one reference argument struct per tile (address/offset batch-reduce modes, scale
  * factors, side operands; MXFP4 x I8 in address mode: arrays of br scale pointers). All matrix pointers must be device-accessible.
  * -1 if a tile lacks a side operand of the handle. */

@@ -303,6 +303,7 @@ libxsmm_b200_gemm_batch_strided = _sig("libxsmm_b200_gemm_batch_strided", _I, [_
 libxsmm_b200_gemm_batch_strided_scaled = _sig("libxsmm_b200_gemm_batch_strided_scaled", _I,
                                               [_P, _P, _P, _P, _LL, _LL, _LL, _P, _P, _P, _LL, _LL, _LL, _ULL, _LL])
 libxsmm_b200_gemm_batch_strided_multi = _sig("libxsmm_b200_gemm_batch_strided_multi", _I, [_P, _P, _P, _P, _LL, _LL, _LL, _ULL, _LL, _I])
+libxsmm_b200_gemm_batch_grid = _sig("libxsmm_b200_gemm_batch_grid", _I, [_P, _P, _P, _P, _LL, _LL, _LL, _LL, _ULL, _LL, _LL])
 libxsmm_b200_gemm_batch = _sig("libxsmm_b200_gemm_batch", _I, [_P, C.POINTER(GemmParam), _LL])
 libxsmm_b200_gemm_plan_create = _sig("libxsmm_b200_gemm_plan_create", _P, [_P, C.POINTER(GemmParam), _LL])
 libxsmm_b200_gemm_plan_run = _sig("libxsmm_b200_gemm_plan_run", _I, [_P])

@@ -33,8 +33,9 @@ struct TileCtx {
   const unsigned char* a_s; const unsigned char* b_s; unsigned char* c_s;   // scales of A, B and C (xb_gemm_sides)
 };
 
-__device__ inline void resolve_tile(const xb_gemm_launch& L, long long t, TileCtx& x) {
-  const xb_gemm_rec r = xb_gemm_tile(&L, t);
+// GRID: the instantiation that runs grids (libxsmm_b200_gemm_batch_grid); the others carry no grid arithmetic
+template <bool GRID> __device__ inline void resolve_tile(const xb_gemm_launch& L, long long t, TileCtx& x) {
+  const xb_gemm_rec r = xb_gemm_tile_at(&L, t, GRID ? L.grid_m : 0);
   x.a0 = (const char*)r.a; x.b0 = (const char*)r.b; x.c = (char*)r.c;
   x.a_addr = (const void* const*)r.a; x.b_addr = (const void* const*)r.b;
   x.a_offs = (const long long*)r.a_aux; x.b_offs = (const long long*)r.b_aux;
@@ -283,7 +284,7 @@ __global__ void __launch_bounds__(FB_THREADS) gemm_fused_kernel(const xb_gemm_la
     const int blk = (int)(item - t * per_tile), i0 = (blk % blocks_m) * bm, j0 = (blk / blocks_m) * bn;
     const int i = i0 + il, nc = min(FB_NC, max(0, n - j0 - jl0));   // nc is warp-uniform
     const bool act = i < m;
-    TileCtx x; resolve_tile(L, t, x);
+    TileCtx x; resolve_tile<false>(L, t, x);
     float acc[FB_NC];
 #pragma unroll
     for (int c = 0; c < FB_NC; ++c) acc[c] = (seeded && act && c < nc) ? fuse_seed(d, x, bias, beta0, i, (long long)(j0 + jl0 + c) * ldc + i) : 0.0f;
@@ -337,6 +338,7 @@ __global__ void __launch_bounds__(FB_THREADS) gemm_fused_kernel(const xb_gemm_la
   }
 }
 
+template <bool GRID>
 __global__ void __launch_bounds__(256) gemm_simt_kernel(const xb_gemm_launch L, const int path) {
   const xb_gemm_desc& d = L.d;
   const DotGeom g = dot_geom(d);
@@ -348,7 +350,7 @@ __global__ void __launch_bounds__(256) gemm_simt_kernel(const xb_gemm_launch L, 
   const bool vnni_a = (d.flags & LIBXSMM_GEMM_FLAG_VNNI_A) != 0;
 
   for (long long t = blockIdx.x; t < L.count; t += gridDim.x) {
-    TileCtx x; resolve_tile(L, t, x);
+    TileCtx x; resolve_tile<GRID>(L, t, x);
     for (int e = threadIdx.x; e < m * n; e += blockDim.x) {
       const int i = e % m, j = e / m;
       const long long ci = (long long)j * ldc + i;
@@ -549,7 +551,7 @@ __global__ void __launch_bounds__(256) gemm_mx8_kernel(const xb_gemm_launch L, f
   const long long ldc = d.ldc;
   const bool beta0 = (d.flags & LIBXSMM_GEMM_FLAG_BETA_0) != 0;
   for (long long t = blockIdx.x; t < L.count; t += gridDim.x) {
-    TileCtx x; resolve_tile(L, t, x);
+    TileCtx x; resolve_tile<false>(L, t, x);
     for (int e = threadIdx.x; e < m * n; e += blockDim.x) {
       const int i = e % m, j = e / m;
       const float acc = dot_mx8(d, x, i, j);
@@ -579,7 +581,7 @@ __global__ void __launch_bounds__(128) gemm_mx8_quant_kernel(const xb_gemm_launc
   if (e >= L.count * per_tile) return;
   const long long t = e / per_tile;
   const int j = (int)((e % per_tile) / bm), b = (int)(e % bm);
-  TileCtx x; resolve_tile(L, t, x);
+  TileCtx x; resolve_tile<false>(L, t, x);
   const float* src = img + (t * n + j) * (long long)m + b * 32;
   float v[32], amax = 0.0f;
 #pragma unroll
@@ -613,6 +615,7 @@ __global__ void __launch_bounds__(128) gemm_mx8_quant_kernel(const xb_gemm_launc
 // I8 / I4 A and an F16 B, where the old value is first rounded to f16 (:1871-1876, :2016-2021).
 __device__ __forceinline__ float dq_f16r(float v) { return xb_f16_to_f32(xb_f32_to_f16(v)); }
 
+template <bool GRID>
 __global__ void __launch_bounds__(256) gemm_dq_kernel(const xb_gemm_launch L) {
   const xb_gemm_desc& d = L.d;
   const int form = xb_dq_form(&d);
@@ -623,7 +626,7 @@ __global__ void __launch_bounds__(256) gemm_dq_kernel(const xb_gemm_launch L) {
   const bool u4 = (d.ta == LIBXSMM_DATATYPE_U4X2), i4 = (form == XB_DQ_I4_F16), b16 = (form == XB_DQ_I8_BF16);
   const int kb = (i4 || (form == XB_DQ_BF8_F16 && (d.flags & LIBXSMM_GEMM_FLAG_VNNI_A) != 0)) ? 2 : 1;
   for (long long t = blockIdx.x; t < L.count; t += gridDim.x) {
-    TileCtx x; resolve_tile(L, t, x);
+    TileCtx x; resolve_tile<GRID>(L, t, x);
     for (int e = threadIdx.x; e < m * n; e += blockDim.x) {
       const int i = e % m, j = e / m;
       const long long ci = (long long)j * ldc + i;
@@ -696,7 +699,7 @@ __device__ __forceinline__ void group_sync(int wpt, int group) {
 
 // WPT warps share one tile: each owns one (LM*TM) x (LN*TN) block of C and keeps it in registers over the whole k loop;
 // the group stages the operand chunk once. 16/WPT tiles are in flight per CTA.
-template <int TM, int TN, bool UA, bool UB>
+template <int TM, int TN, bool UA, bool UB, bool GRID>
 __global__ void __launch_bounds__(I8_WARPS * 32, 2) gemm_i8_kernel(const xb_gemm_launch L, const int to_f32, const int wpt, const int smem_words_per_group) {
   constexpr int LM = 8, LN = 4;                       // lanes along m and n
   extern __shared__ unsigned int smem_i8[];
@@ -718,7 +721,7 @@ __global__ void __launch_bounds__(I8_WARPS * 32, 2) gemm_i8_kernel(const xb_gemm
   const long long ntiles_rounded = ((L.count + (long long)gridDim.x * groups - 1) / ((long long)gridDim.x * groups)) * ((long long)gridDim.x * groups);
   for (long long t = (long long)blockIdx.x * groups + group; t < ntiles_rounded; t += (long long)gridDim.x * groups) {
     const bool live = t < L.count;                    // dead iterations only keep the group barriers balanced
-    TileCtx x; if (live) resolve_tile(L, t, x); else { x.br = 0; }
+    TileCtx x; if (live) resolve_tile<GRID>(L, t, x); else { x.br = 0; }
     unsigned int acc[TM][TN];
 #pragma unroll
     for (int i = 0; i < TM; ++i)
@@ -813,7 +816,7 @@ bool i8_fast_ok(const xb_gemm_launch& L, int path) {
   const bool single = (L.a == nullptr && L.c == nullptr);
   const uintptr_t a = (uintptr_t)(single ? L.one.a : L.a), b = (uintptr_t)(single ? L.one.b : L.b), c = (uintptr_t)(single ? L.one.c : L.c);
   if (((a | b | c) & 3) != 0) return false;
-  if (!single && (((L.tile_stride_a | L.tile_stride_b | L.tile_stride_c) & 3) != 0)) return false;
+  if (!single && (((L.tile_stride_a | L.tile_stride_b | L.tile_stride_c | L.tile_stride_c_n) & 3) != 0)) return false;
   if (d.br_type == 3 && (((d.br_stride_a | d.br_stride_b) & 3) != 0)) return false;
   return true;
 }
@@ -822,11 +825,15 @@ template <int TM, int TN>
 void launch_i8(const xb_gemm_launch& L, int path, int wpt, int words_per_group, size_t smem, unsigned int grid, cudaStream_t st) {
   const bool ua = (L.d.ta == LIBXSMM_DATATYPE_U8), ub = (L.d.tb == LIBXSMM_DATATYPE_U8);
   const int to_f32 = (path == P_I8_F32);
-#define XB_I8_CASE(A, B) do { \
+#define XB_I8_CASE(A, B, G) do { \
     static unsigned long long attr_set = 0ull; \
-    if (xb_rt_first_use_on_device(&attr_set)) cudaFuncSetAttribute(gemm_i8_kernel<TM, TN, A, B>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024); \
-    gemm_i8_kernel<TM, TN, A, B><<<grid, I8_WARPS * 32, smem, st>>>(L, to_f32, wpt, words_per_group); } while (0)
-  if (ua && ub) XB_I8_CASE(true, true); else if (ua) XB_I8_CASE(true, false); else if (ub) XB_I8_CASE(false, true); else XB_I8_CASE(false, false);
+    if (xb_rt_first_use_on_device(&attr_set)) cudaFuncSetAttribute(gemm_i8_kernel<TM, TN, A, B, G>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024); \
+    gemm_i8_kernel<TM, TN, A, B, G><<<grid, I8_WARPS * 32, smem, st>>>(L, to_f32, wpt, words_per_group); } while (0)
+  if (L.grid_m > 0) {
+    if (ua && ub) XB_I8_CASE(true, true, true); else if (ua) XB_I8_CASE(true, false, true); else if (ub) XB_I8_CASE(false, true, true); else XB_I8_CASE(false, false, true);
+  } else {
+    if (ua && ub) XB_I8_CASE(true, true, false); else if (ua) XB_I8_CASE(true, false, false); else if (ub) XB_I8_CASE(false, true, false); else XB_I8_CASE(false, false, false);
+  }
 #undef XB_I8_CASE
 }
 
@@ -869,7 +876,7 @@ __device__ __forceinline__ unsigned int lb_expand_fp4(unsigned int w) {
   return (__vneg4(mag) & neg) | (mag & ~neg);
 }
 
-template <int FORM, bool UB>
+template <int FORM, bool UB, bool GRID>
 __global__ void __launch_bounds__(LB_THREADS) gemm_lowbit_kernel(const xb_gemm_launch L) {
   __shared__ unsigned int sb[LB_NB * LB_SW];
   const xb_gemm_desc& d = L.d;
@@ -877,7 +884,7 @@ __global__ void __launch_bounds__(LB_THREADS) gemm_lowbit_kernel(const xb_gemm_l
   const long long lda = d.lda, ldb = d.ldb, ldc = d.ldc;
   const bool beta0 = (d.flags & LIBXSMM_GEMM_FLAG_BETA_0) != 0;
   for (long long t = blockIdx.x; t < L.count; t += gridDim.x) {
-    TileCtx x; resolve_tile(L, t, x);
+    TileCtx x; resolve_tile<GRID>(L, t, x);
     const unsigned char* as = x.a_s; const float* bs = (const float*)x.b_s;   // MXFP4 block scales (address mode: arrays of br pointers)
     for (int j0 = 0; j0 < n; j0 += LB_NB) {
       const int nb = (n - j0 < LB_NB) ? n - j0 : LB_NB;
@@ -972,14 +979,19 @@ __global__ void __launch_bounds__(LB_THREADS) gemm_lowbit_kernel(const xb_gemm_l
   }
 }
 
-void launch_lowbit(const xb_gemm_launch& L, unsigned int grid, cudaStream_t st) {
+template <bool GRID>
+void launch_lowbit_g(const xb_gemm_launch& L, unsigned int grid, cudaStream_t st) {
   const int form = xb_lowbit_form(&L.d);
   const bool ub = (L.d.tb == LIBXSMM_DATATYPE_U8);
-  if (form == XB_LB_I2 && ub) gemm_lowbit_kernel<XB_LB_I2, true><<<grid, LB_THREADS, 0, st>>>(L);
-  else if (form == XB_LB_I2) gemm_lowbit_kernel<XB_LB_I2, false><<<grid, LB_THREADS, 0, st>>>(L);
-  else if (form == XB_LB_I1 && ub) gemm_lowbit_kernel<XB_LB_I1, true><<<grid, LB_THREADS, 0, st>>>(L);
-  else if (form == XB_LB_I1) gemm_lowbit_kernel<XB_LB_I1, false><<<grid, LB_THREADS, 0, st>>>(L);
-  else gemm_lowbit_kernel<XB_LB_MXFP4, false><<<grid, LB_THREADS, 0, st>>>(L);
+  if (form == XB_LB_I2 && ub) gemm_lowbit_kernel<XB_LB_I2, true, GRID><<<grid, LB_THREADS, 0, st>>>(L);
+  else if (form == XB_LB_I2) gemm_lowbit_kernel<XB_LB_I2, false, GRID><<<grid, LB_THREADS, 0, st>>>(L);
+  else if (form == XB_LB_I1 && ub) gemm_lowbit_kernel<XB_LB_I1, true, GRID><<<grid, LB_THREADS, 0, st>>>(L);
+  else if (form == XB_LB_I1) gemm_lowbit_kernel<XB_LB_I1, false, GRID><<<grid, LB_THREADS, 0, st>>>(L);
+  else gemm_lowbit_kernel<XB_LB_MXFP4, false, false><<<grid, LB_THREADS, 0, st>>>(L);   // side operands: never a grid
+}
+
+void launch_lowbit(const xb_gemm_launch& L, unsigned int grid, cudaStream_t st) {
+  if (L.grid_m > 0) launch_lowbit_g<true>(L, grid, st); else launch_lowbit_g<false>(L, grid, st);
 }
 
 // after a launch: counts it and notes a launch error
@@ -1018,7 +1030,7 @@ extern "C" int xb_gemm_simt_launch(const xb_gemm_launch* L) {
     return launched("gemm_mx8_quant");
   }
   if (path == P_DQ) {
-    gemm_dq_kernel<<<grid, 256, 0, st>>>(*L);
+    if (L->grid_m > 0) gemm_dq_kernel<true><<<grid, 256, 0, st>>>(*L); else gemm_dq_kernel<false><<<grid, 256, 0, st>>>(*L);
     return launched("gemm_dq");
   }
   if (path == P_LOWBIT) {
@@ -1054,6 +1066,6 @@ extern "C" int xb_gemm_simt_launch(const xb_gemm_launch* L) {
       return launched("gemm_i8");
     }
   }
-  gemm_simt_kernel<<<grid, 256, 0, st>>>(*L, path);
+  if (L->grid_m > 0) gemm_simt_kernel<true><<<grid, 256, 0, st>>>(*L, path); else gemm_simt_kernel<false><<<grid, 256, 0, st>>>(*L, path);
   return launched("gemm_simt");
 }

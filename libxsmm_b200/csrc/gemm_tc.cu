@@ -8,7 +8,7 @@
 // registers instead of a sequential scalar loop (tolerance, not bit-exact); integer sums are exact in any order, so the
 // 8-bit path is bit-identical to the reference.
 //
-// One kernel, `gemm_wg_kernel<AMODE, NC, NCH, WG>`, persistent, tiles assigned round-robin over the CTAs:
+// One kernel, `gemm_wg_kernel<AMODE, NC, NCH, WG, GRID>`, persistent, tiles assigned round-robin over the CTAs:
 //   warps 0 .. 4*WG-1   WG consumer warpgroups; warpgroup g owns rows 64g .. 64g+63 of the tile (m <= 64: one warpgroup;
 //                       pooled pair mode: warpgroup g owns the item's tile g) and issues wgmma m64 x (NC*NCH) x k16/k32
 //   warp 4*WG           TMA producer: cp.async.bulk.tensor.4d of the A and B boxes of one (tile, r, k-chunk) per stage,
@@ -55,7 +55,13 @@ struct WgParams {
   // pooled address mode (libxsmm_b200_gemm_plan over ADDRESS/OFFSET batch-reduce): item p reads block-set sets[p].x of A (pair
   // mode: sets[p].y for its second tile) and sets[p].z of B (4th tensor-map coordinate) and writes cptrs[p] (pair mode:
   // cptrs[2p], cptrs[2p+1], the second may be null)
-  const int4* sets; char* const* cptrs; int pair;
+  // grid (libxsmm_b200_gemm_batch_grid, the GRID instantiations, which are never pooled): tile t is (i, j) = (t % grid_m, t / grid_m),
+  // reads row block i of A and column block j of B (4th tensor-map coordinates) and writes c + i * tile_stride_c + j * tile_stride_c_n.
+  // The two share storage, so that the flat and pooled instantiations see the struct they always had and compile to the same code.
+  union {
+    struct { const int4* sets; char* const* cptrs; int pair; };
+    struct { long long grid_m, tile_stride_c_n; };
+  };
 };
 
 template <int NC>
@@ -83,8 +89,9 @@ __device__ __forceinline__ void wg_mma8_rs(int sgn, float (&d)[NC / 2], const ui
 }
 #undef XB_WG_I8
 
-// NC: columns per instruction, NCH: instructions side by side (N = NC * NCH), WG: consumer warpgroups
-template <int AMODE, int NC, int NCH, int WG>
+// NC: columns per instruction, NCH: instructions side by side (N = NC * NCH), WG: consumer warpgroups, GRID: a grid launch (the flat
+// and pooled instantiations carry no grid arithmetic)
+template <int AMODE, int NC, int NCH, int WG, bool GRID>
 __global__ void __launch_bounds__(WG * 128 + 32, (NCH == 1 && WG == 1) ? 3 : 1)
 gemm_wg_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const WgParams P) {
   extern __shared__ uint8_t smem_raw[];
@@ -95,7 +102,7 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const long long G = gridDim.x, b = blockIdx.x;
   const long long n_local = (b < P.count) ? (P.count - b + G - 1) / G : 0;
-  const bool pooled = P.sets != nullptr;
+  const bool pooled = !GRID && P.sets != nullptr;
 
   if (threadIdx.x == 0) {
     asm volatile("prefetch.tensormap [%0];" :: "l"(&map_a) : "memory");
@@ -115,6 +122,8 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
         if (pooled) {
           const int4 st = P.sets[t];
           ta0 = st.x; ta1 = P.pair ? st.y : st.x; tb = st.z; m1 = P.pair ? 0 : 64;
+        } else if (GRID) {
+          ta0 = ta1 = (int)t % (int)P.grid_m; tb = (int)t / (int)P.grid_m;
         }
         for (unsigned long long r = 0; r < P.br; ++r) {
           for (int kc = 0; kc < P.kchunks; ++kc) {
@@ -186,7 +195,8 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     if (prev >= 0) { __syncwarp(); if (lane == 0) xb_mbar_arrive(empty0 + 8 * prev); }
     // epilogue
     char* ctile; int row0 = 64 * g;
-    if (!pooled) ctile = P.c + t * P.tile_stride_c;
+    if (GRID) ctile = P.c + ((int)t % (int)P.grid_m) * P.tile_stride_c + ((int)t / (int)P.grid_m) * P.tile_stride_c_n;
+    else if (!pooled) ctile = P.c + t * P.tile_stride_c;
     else if (P.pair) { ctile = P.cptrs[2 * t + g]; row0 = 0; }
     else ctile = P.cptrs[t];
     if (ctile == nullptr) continue;
@@ -218,23 +228,30 @@ int num_sms() {
 }
 
 // MaxDynamicSharedMemorySize is a per-device function attribute: one bit per (instantiation, device)
-template <int AMODE, int NC, int NCH, int WG>
+template <int AMODE, int NC, int NCH, int WG, bool GRID>
 cudaError_t launch_one(long long grid, size_t smem, cudaStream_t stream, const CUtensorMap& ma, const CUtensorMap& mb, const WgParams& P) {
   static unsigned long long done = 0ull;
-  if (xb_rt_first_use_on_device(&done)) cudaFuncSetAttribute(gemm_wg_kernel<AMODE, NC, NCH, WG>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-  gemm_wg_kernel<AMODE, NC, NCH, WG><<<(unsigned int)grid, WG * 128 + 32, smem, stream>>>(ma, mb, P);
+  if (xb_rt_first_use_on_device(&done)) cudaFuncSetAttribute(gemm_wg_kernel<AMODE, NC, NCH, WG, GRID>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+  gemm_wg_kernel<AMODE, NC, NCH, WG, GRID><<<(unsigned int)grid, WG * 128 + 32, smem, stream>>>(ma, mb, P);
   return cudaGetLastError();
 }
 
-template <int AMODE, int WG>
+template <int AMODE, int WG, bool GRID>
 cudaError_t launch_n(int nt, long long grid, size_t smem, cudaStream_t stream, const CUtensorMap& ma, const CUtensorMap& mb, const WgParams& P) {
   switch (nt) {
-    case 16:  return launch_one<AMODE, 16, 1, WG>(grid, smem, stream, ma, mb, P);
-    case 32:  return launch_one<AMODE, 32, 1, WG>(grid, smem, stream, ma, mb, P);
-    case 64:  return launch_one<AMODE, 64, 1, WG>(grid, smem, stream, ma, mb, P);
-    case 128: return launch_one<AMODE, 64, 2, WG>(grid, smem, stream, ma, mb, P);
-    default:  return launch_one<AMODE, 64, 4, WG>(grid, smem, stream, ma, mb, P);
+    case 16:  return launch_one<AMODE, 16, 1, WG, GRID>(grid, smem, stream, ma, mb, P);
+    case 32:  return launch_one<AMODE, 32, 1, WG, GRID>(grid, smem, stream, ma, mb, P);
+    case 64:  return launch_one<AMODE, 64, 1, WG, GRID>(grid, smem, stream, ma, mb, P);
+    case 128: return launch_one<AMODE, 64, 2, WG, GRID>(grid, smem, stream, ma, mb, P);
+    default:  return launch_one<AMODE, 64, 4, WG, GRID>(grid, smem, stream, ma, mb, P);
   }
+}
+
+template <int AMODE>
+cudaError_t launch_a(int wg, int nt, bool is_grid, long long grid, size_t smem, cudaStream_t stream, const CUtensorMap& ma, const CUtensorMap& mb,
+                     const WgParams& P) {
+  if (is_grid) return (wg == 2) ? launch_n<AMODE, 2, true>(nt, grid, smem, stream, ma, mb, P) : launch_n<AMODE, 1, true>(nt, grid, smem, stream, ma, mb, P);
+  return (wg == 2) ? launch_n<AMODE, 2, false>(nt, grid, smem, stream, ma, mb, P) : launch_n<AMODE, 1, false>(nt, grid, smem, stream, ma, mb, P);
 }
 
 // columns of the instruction: n rounded up to 16, 32, 64, 128 or 256
@@ -248,17 +265,27 @@ void plan_stages(WgParams& P, int nt, int wg, int* ctas) {
   P.stages = st; *ctas = c;
 }
 
-int wg_launch(int amode, int wg, int nt, const WgParams& P, int ctas, const CUtensorMap& ma, const CUtensorMap& mb, const char* where) {
+int wg_launch(int amode, int wg, int nt, bool is_grid, const WgParams& P, int ctas, const CUtensorMap& ma, const CUtensorMap& mb,
+              const char* where) {
   const size_t smem = (size_t)P.stages * P.stage_bytes + 1024 /*align slack*/ + 2 * 8 * P.stages;
   long long grid = P.count; if (grid > (long long)num_sms() * ctas) grid = (long long)num_sms() * ctas; if (grid < 1) grid = 1;
   cudaStream_t stream = (cudaStream_t)xb_rt_stream();
   cudaError_t e;
-  if (amode == XB_WG_SS16) e = (wg == 2) ? launch_n<XB_WG_SS16, 2>(nt, grid, smem, stream, ma, mb, P) : launch_n<XB_WG_SS16, 1>(nt, grid, smem, stream, ma, mb, P);
-  else if (amode == XB_WG_RS16) e = (wg == 2) ? launch_n<XB_WG_RS16, 2>(nt, grid, smem, stream, ma, mb, P) : launch_n<XB_WG_RS16, 1>(nt, grid, smem, stream, ma, mb, P);
-  else e = (wg == 2) ? launch_n<XB_WG_RS8, 2>(nt, grid, smem, stream, ma, mb, P) : launch_n<XB_WG_RS8, 1>(nt, grid, smem, stream, ma, mb, P);
+  if (amode == XB_WG_SS16) e = launch_a<XB_WG_SS16>(wg, nt, is_grid, grid, smem, stream, ma, mb, P);
+  else if (amode == XB_WG_RS16) e = launch_a<XB_WG_RS16>(wg, nt, is_grid, grid, smem, stream, ma, mb, P);
+  else e = launch_a<XB_WG_RS8>(wg, nt, is_grid, grid, smem, stream, ma, mb, P);
   xb_rt_count_launch_backend(LIBXSMM_B200_BACKEND_TCGEN05);
   if (e != cudaSuccess) { xb_rt_note_error((int)e, where); return (int)e; }
   return 0;
+}
+
+// the extents of the 4th tensor-map dimension of A and of B (a flat batch: count each; a grid: grid_m row blocks of A and grid_n
+// column blocks of B), and whether TMA can walk them: 16-byte aligned bases and strides, and a nonzero stride wherever the extent is
+// above 1. A launch that fails this runs on the exact-order kernel.
+bool tile_maps_ok(const xb_gemm_launch* L, const char* a, const char* b, long long sa, long long sb, long long* na, long long* nb) {
+  *na = (L->grid_m > 0) ? L->grid_m : L->count;
+  *nb = (L->grid_m > 0) ? L->count / L->grid_m : L->count;
+  return (((uintptr_t)a | (uintptr_t)b) & 15) == 0 && (sa % 16) == 0 && (sb % 16) == 0 && (*na == 1 || sa > 0) && (*nb == 1 || sb > 0);
 }
 
 }  // namespace
@@ -305,8 +332,8 @@ static int tc_launch_common(const xb_gemm_launch* L, const xb_tc_pool* pool) {
   if (a == nullptr && c == nullptr) { a = (const char*)L->one.a; b = (const char*)L->one.b; c = (char*)L->one.c; br = L->one.br; sa = sb = sc = 0; }
   if (d.br_type == 0 && pool == nullptr) br = 1;
   const int es = 2;
-  const bool aligned = (((uintptr_t)a | (uintptr_t)b) & 15) == 0 && (sa % 16) == 0 && (sb % 16) == 0
-                    && (L->count == 1 || (sa > 0 && sb > 0));
+  long long na, nb;
+  const bool aligned = tile_maps_ok(L, a, b, sa, sb, &na, &nb);
   xb_encode_tiled_fn enc = xb_tma_encoder();
   if (br == 0 || !aligned || L->count <= 0 || br > 0x7fffffffull || L->count > 0x7fffffffll || enc == nullptr) {
     return (pool != nullptr) ? 1 : xb_gemm_simt_launch(L);
@@ -320,6 +347,7 @@ static int tc_launch_common(const xb_gemm_launch* L, const xb_tc_pool* pool) {
   P.a_bytes = wg * 8192; P.stage_bytes = P.a_bytes + nt * 128; P.tx_bytes = P.stage_bytes;
   P.bf16 = (d.ta == LIBXSMM_DATATYPE_BF16) ? 1 : 0;
   P.br = br; P.count = L->count; P.c = c; P.tile_stride_c = sc; P.ldc = d.ldc;
+  if (L->grid_m > 0) { P.grid_m = L->grid_m; P.tile_stride_c_n = L->tile_stride_c_n; }
   if (pool != nullptr) { P.sets = (const int4*)pool->sets; P.cptrs = (char* const*)pool->cptrs; P.pair = pool->pair; }
   P.beta0 = (d.flags & LIBXSMM_GEMM_FLAG_BETA_0) ? 1 : 0;
   P.ep_mode = xb_ep_mode(d.ta, d.tc, &P.c_esz);
@@ -332,24 +360,24 @@ static int tc_launch_common(const xb_gemm_launch* L, const xb_tc_pool* pool) {
   const cuuint64_t pad_a = (ext_a + 15) & ~(size_t)15, pad_b = (ext_b + 15) & ~(size_t)15;
   CUtensorMap map_a, map_b;
   {
-    const cuuint64_t dims[4] = {(cuuint64_t)d.m, (cuuint64_t)d.k, (cuuint64_t)br, (cuuint64_t)(pool ? pool->nsets_a : L->count)};
+    const cuuint64_t dims[4] = {(cuuint64_t)d.m, (cuuint64_t)d.k, (cuuint64_t)br, (cuuint64_t)(pool ? pool->nsets_a : na)};
     const cuuint64_t strides[3] = {(cuuint64_t)d.lda * es, pool ? (cuuint64_t)pool->blk_a : ((d.br_type == 3) ? (cuuint64_t)d.br_stride_a : pad_a),
-                                   pool ? (cuuint64_t)pool->set_a : ((L->count > 1) ? (cuuint64_t)sa : pad_a)};
+                                   pool ? (cuuint64_t)pool->set_a : ((na > 1) ? (cuuint64_t)sa : pad_a)};
     const cuuint32_t box[4] = {64, 64, 1, 1};
     if (CUDA_SUCCESS != enc(&map_a, dt, 4, (void*)a, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                             CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE))
       return (pool != nullptr) ? 1 : xb_gemm_simt_launch(L);
   }
   {
-    const cuuint64_t dims[4] = {(cuuint64_t)d.k, (cuuint64_t)d.n, (cuuint64_t)br, (cuuint64_t)(pool ? pool->nsets_b : L->count)};
+    const cuuint64_t dims[4] = {(cuuint64_t)d.k, (cuuint64_t)d.n, (cuuint64_t)br, (cuuint64_t)(pool ? pool->nsets_b : nb)};
     const cuuint64_t strides[3] = {(cuuint64_t)d.ldb * es, pool ? (cuuint64_t)pool->blk_b : ((d.br_type == 3) ? (cuuint64_t)d.br_stride_b : pad_b),
-                                   pool ? (cuuint64_t)pool->set_b : ((L->count > 1) ? (cuuint64_t)sb : pad_b)};
+                                   pool ? (cuuint64_t)pool->set_b : ((nb > 1) ? (cuuint64_t)sb : pad_b)};
     const cuuint32_t box[4] = {64, (cuuint32_t)nt, 1, 1};
     if (CUDA_SUCCESS != enc(&map_b, dt, 4, (void*)b, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                             CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE))
       return (pool != nullptr) ? 1 : xb_gemm_simt_launch(L);
   }
-  return wg_launch(XB_WG_SS16, wg, nt, P, ctas, map_a, map_b, "gemm_tc");
+  return wg_launch(XB_WG_SS16, wg, nt, L->grid_m > 0, P, ctas, map_a, map_b, "gemm_tc");
 }
 
 // ---- VNNI-packed A (register-fragment form) ----------------------------------------------------------------------------
@@ -384,7 +412,8 @@ extern "C" int xb_gemm_ts_launch(const xb_gemm_launch* L) {
   if (L->recs != nullptr) return xb_gemm_simt_launch(L);
   if (a == nullptr && c == nullptr) { a = (const char*)L->one.a; b = (const char*)L->one.b; c = (char*)L->one.c; br = L->one.br; sa = sb = sc = 0; }
   if (d.br_type == 0) br = 1;
-  const bool aligned = (((uintptr_t)a | (uintptr_t)b) & 15) == 0 && (sa % 16) == 0 && (sb % 16) == 0 && (L->count == 1 || (sa > 0 && sb > 0));
+  long long na, nb;
+  const bool aligned = tile_maps_ok(L, a, b, sa, sb, &na, &nb);
   xb_encode_tiled_fn enc = xb_tma_encoder();
   if (br == 0 || !aligned || L->count <= 0 || br > 0x7fffffffull || L->count > 0x7fffffffll || enc == nullptr) return xb_gemm_simt_launch(L);
 
@@ -399,6 +428,7 @@ extern "C" int xb_gemm_ts_launch(const xb_gemm_launch* L) {
   P.bf16 = (d.ta == LIBXSMM_DATATYPE_BF16) ? 1 : 0;
   P.sgn = ((d.ta == LIBXSMM_DATATYPE_I8) ? 2 : 0) | ((d.tb == LIBXSMM_DATATYPE_I8) ? 1 : 0);
   P.br = br; P.count = L->count; P.c = c; P.tile_stride_c = sc; P.ldc = d.ldc;
+  if (L->grid_m > 0) { P.grid_m = L->grid_m; P.tile_stride_c_n = L->tile_stride_c_n; }
   P.beta0 = (d.flags & LIBXSMM_GEMM_FLAG_BETA_0) ? 1 : 0; P.scf = L->one.scf;
   P.ep_mode = xb_ep_mode(d.ta, d.tc, &P.c_esz);
   int ctas = 1;
@@ -409,19 +439,19 @@ extern "C" int xb_gemm_ts_launch(const xb_gemm_launch* L) {
   const cuuint64_t pad_a = (ext_a + 15) & ~(size_t)15, pad_b = (ext_b + 15) & ~(size_t)15;
   CUtensorMap map_a, map_b;
   {
-    const cuuint64_t dims[4] = {(cuuint64_t)d.m, (cuuint64_t)(d.k / v), (cuuint64_t)br, (cuuint64_t)L->count};
-    const cuuint64_t strides[3] = {(cuuint64_t)d.lda * 4, (d.br_type == 3) ? (cuuint64_t)d.br_stride_a : pad_a, (L->count > 1) ? (cuuint64_t)sa : pad_a};
+    const cuuint64_t dims[4] = {(cuuint64_t)d.m, (cuuint64_t)(d.k / v), (cuuint64_t)br, (cuuint64_t)na};
+    const cuuint64_t strides[3] = {(cuuint64_t)d.lda * 4, (d.br_type == 3) ? (cuuint64_t)d.br_stride_a : pad_a, (na > 1) ? (cuuint64_t)sa : pad_a};
     const cuuint32_t box[4] = {(cuuint32_t)d.m, 32, 1, 1};
     if (CUDA_SUCCESS != enc(&map_a, CU_TENSOR_MAP_DATA_TYPE_UINT32, 4, (void*)a, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                             CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE)) return xb_gemm_simt_launch(L);
   }
   {
     const CUtensorMapDataType dt = is_i8 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : (P.bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16);
-    const cuuint64_t dims[4] = {(cuuint64_t)d.k, (cuuint64_t)d.n, (cuuint64_t)br, (cuuint64_t)L->count};
-    const cuuint64_t strides[3] = {(cuuint64_t)d.ldb * es, (d.br_type == 3) ? (cuuint64_t)d.br_stride_b : pad_b, (L->count > 1) ? (cuuint64_t)sb : pad_b};
+    const cuuint64_t dims[4] = {(cuuint64_t)d.k, (cuuint64_t)d.n, (cuuint64_t)br, (cuuint64_t)nb};
+    const cuuint64_t strides[3] = {(cuuint64_t)d.ldb * es, (d.br_type == 3) ? (cuuint64_t)d.br_stride_b : pad_b, (nb > 1) ? (cuuint64_t)sb : pad_b};
     const cuuint32_t box[4] = {(cuuint32_t)P.kc_elems, (cuuint32_t)nt, 1, 1};
     if (CUDA_SUCCESS != enc(&map_b, dt, 4, (void*)b, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                             CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE)) return xb_gemm_simt_launch(L);
   }
-  return wg_launch(is_i8 ? XB_WG_RS8 : XB_WG_RS16, wg, nt, P, ctas, map_a, map_b, "gemm_ts");
+  return wg_launch(is_i8 ? XB_WG_RS8 : XB_WG_RS16, wg, nt, L->grid_m > 0, P, ctas, map_a, map_b, "gemm_ts");
 }

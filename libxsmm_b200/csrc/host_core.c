@@ -785,8 +785,8 @@ LIBXSMM_API void libxsmm_sgemm_(const char* transa, const char* transb,
 
 /* ---- batch entry points -------------------------------------------------------------------------- */
 /* the batch forms, one per entry point: libxsmm_b200_gemm_batch_strided, _strided_multi, _strided_scaled, libxsmm_b200_gemm_batch,
- * libxsmm_b200_gemm_plan_create, libxsmm_b200_gemm_ext_batch_strided and libxsmm_b200_gemm_ext_batch */
-enum { XB_FORM_STRIDED, XB_FORM_MULTI, XB_FORM_SCALED, XB_FORM_RECORDS, XB_FORM_PLAN, XB_FORM_EXT_STRIDED, XB_FORM_EXT_RECORDS };
+ * libxsmm_b200_gemm_plan_create, libxsmm_b200_gemm_ext_batch_strided, libxsmm_b200_gemm_ext_batch and libxsmm_b200_gemm_batch_grid */
+enum { XB_FORM_STRIDED, XB_FORM_MULTI, XB_FORM_SCALED, XB_FORM_RECORDS, XB_FORM_PLAN, XB_FORM_EXT_STRIDED, XB_FORM_EXT_RECORDS, XB_FORM_GRID };
 
 static int xb_ext_mask(const xb_gemm_desc* d) {
   return d->cp_op == LIBXSMM_MELTW_TYPE_UNARY_RELU && (d->cp_flags & LIBXSMM_MELTW_FLAG_UNARY_BITMASK_2BYTEMULT) != 0;
@@ -799,7 +799,8 @@ static int xb_ext_mask(const xb_gemm_desc* d) {
  * VNNI-packed C after a single call only; their records carry no MX fp8 block scales; the strided forms have no argument struct for
  * side operands (xb_gemm_sides) or for the int8 -> f32 scale (c.tertiary). A plan is replayed, so it takes no side operands either.
  * -2: address and offset batch-reduce need per-tile arrays, which the strided forms do not take (the fused one shares call 0's
- * offset arrays). The multi-device form reports -2 through the strided call each device makes. */
+ * offset arrays). The multi-device form reports -2 through the strided call each device makes.
+ * The grid form runs exactly the handles the strided form runs, brgemm_ext handles excepted (-1). */
 static int xb_gemm_batch_refused(const xb_slot* s, int form) {
   const xb_gemm_desc* d;
   int sides, per_tile_arrays;
@@ -814,6 +815,8 @@ static int xb_gemm_batch_refused(const xb_slot* s, int form) {
     case XB_FORM_SCALED:
       if (s->kind != XB_KIND_GEMM || sides == 0 || (sides & XB_SIDE_A_Q) != 0) return -1;
       return per_tile_arrays ? -2 : 0;
+    case XB_FORM_GRID:
+      return (s->kind != XB_KIND_GEMM) ? -1 : xb_gemm_batch_refused(s, XB_FORM_STRIDED);
     default: break;
   }
   if (d->fuse_colbias != 0 || (d->flags & LIBXSMM_GEMM_FLAG_VNNI_C) != 0 || xb_ext_mask(d)) return LIBXSMM_B200_ERROR_NOT_BATCHABLE;
@@ -917,6 +920,45 @@ LIBXSMM_API int libxsmm_b200_gemm_batch_strided_scaled(libxsmm_gemmfunction kern
    || (L.one.b_s != NULL && xb_rt_ptr_kind(L.one.b_s) == 0) || (L.one.c_s != NULL && xb_rt_ptr_kind(L.one.c_s) == 0)) return -4;   /* device-accessible operands only */
   L.count = count; L.a = a; L.b = b; L.c = c;
   rc = xb_gemm_batch_launch(&L, (char*)c, stride_c);
+  if (rc == 0 && xb_rt_blocking()) rc = xb_rt_sync();
+  return rc;
+}
+
+/* 1 unless the C tiles of a gm x gn grid (strides sm, sn in bytes, non-negative) are laid out so that no two can overlap. A row or a
+ * column of tiles is a strided batch and takes the strided forms' rule: a stride of at least the bytes one call writes through C,
+ * span = ((n - 1) * ldc + m) * esz. A larger grid is either a plain matrix, whose tiles abut inside one column-major C (row blocks
+ * sm >= m * esz apart and all within ldc, column blocks at least n whole columns apart), or blocked: whole tiles at least span apart
+ * along one axis, and whole rows or columns of tiles apart along the other. Divisions instead of products: nothing overflows. */
+static int xb_grid_c_overlaps(const xb_gemm_desc* d, long long sm, long long sn, long long gm, long long gn) {
+  const long long esz = libxsmm_typesize((libxsmm_datatype)d->tc), row = (long long)d->m * esz, col = (long long)d->ldc * esz;
+  const long long span = ((long long)(d->n - 1) * d->ldc + d->m) * esz;
+  if (gm == 1 || gn == 1) return (gm > 1 || gn > 1) && ((gn == 1) ? sm : sn) < span;
+  if (sm >= row && (col - row) / sm >= gm - 1 && sn >= (long long)d->n * col) return 0;
+  if (sm >= span && sn / gm >= sm) return 0;
+  if (sn >= span && sm / gn >= sn) return 0;
+  return 1;
+}
+
+LIBXSMM_API int libxsmm_b200_gemm_batch_grid(libxsmm_gemmfunction kernel, const void* a, const void* b, void* c,
+  long long stride_a_m, long long stride_b_n, long long stride_c_m, long long stride_c_n,
+  unsigned long long br_count, long long grid_m, long long grid_n)
+{
+  const xb_slot* s = xb_slot_of((const void*)kernel);
+  const int refused = xb_gemm_batch_refused(s, XB_FORM_GRID);
+  xb_gemm_launch L;
+  int rc;
+  if (refused == -1 || grid_m < 0 || grid_n < 0 || stride_a_m < 0 || stride_b_n < 0 || stride_c_m < 0 || stride_c_n < 0) return -1;
+  if (refused != 0) return refused;
+  if (grid_m == 0 || grid_n == 0) return 0;
+  if (a == NULL || b == NULL || c == NULL || grid_m > 0x7fffffffll / grid_n) return -1;
+  if (xb_grid_c_overlaps(&s->u.gemm, stride_c_m, stride_c_n, grid_m, grid_n)) return -1;
+  if (xb_rt_ptr_kind(a) == 0 || xb_rt_ptr_kind(b) == 0 || xb_rt_ptr_kind(c) == 0) return -4;   /* device-accessible operands only */
+  memset(&L, 0, sizeof(L));
+  L.d = s->u.gemm; L.count = grid_m * grid_n; L.grid_m = grid_m;
+  L.a = a; L.b = b; L.c = c;
+  L.tile_stride_a = stride_a_m; L.tile_stride_b = stride_b_n; L.tile_stride_c = stride_c_m; L.tile_stride_c_n = stride_c_n;
+  L.br = (L.d.br_type == 0) ? 1ull : br_count;
+  rc = xb_gemm_batch_launch(&L, (char*)c, stride_c_m);
   if (rc == 0 && xb_rt_blocking()) rc = xb_rt_sync();
   return rc;
 }

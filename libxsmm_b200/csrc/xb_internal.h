@@ -189,20 +189,32 @@ typedef struct xb_gemm_launch {
   const xb_gemm_rec* recs;
   xb_gemm_rec one;      /* count==1 && !recs: passed by value */
   long long tile_stride_d, tile_stride_c_aux;   /* mode 0, fused: bias column and ReLU bit mask (bases in one.d / c_aux), bytes */
+  /* mode 0 as a grid (libxsmm_b200_gemm_batch_grid) when grid_m > 0: tile t is (i, j) = (t % grid_m, t / grid_m), and reads A at
+   * i tile strides, B at j tile strides (tile_stride_b is the B column stride) and C at i * tile_stride_c + j * tile_stride_c_n.
+   * 0 (and tile_stride_c_n 0): the flat batch. A grid carries no side operand, bias or mask and is never sliced (xb_gemm_launch_slice). */
+  long long grid_m, tile_stride_c_n;
 } xb_gemm_launch;
 
 /* the complete record of tile t: the per-tile record, the single call, or a strided batch's bases advanced by t tile strides (a side
- * operand, bias column or mask the launch lacks is NULL with a tile stride of 0). A strided batch shares `one`'s scale factor and zero
- * points, and has offset arrays in offset mode only. */
+ * operand, bias column or mask the launch lacks is NULL with a tile stride of 0), or by tile t's row and column of a grid of grid_m
+ * rows. A strided batch shares `one`'s scale factor and zero points, and has offset arrays in offset mode only. A kernel instantiation
+ * that runs no grid passes grid_m = 0, a constant, and so carries none of the grid's arithmetic; everything else calls xb_gemm_tile,
+ * which takes the grid from the launch. */
 #if defined(__CUDACC__)
 __host__ __device__
 #endif
-static inline xb_gemm_rec xb_gemm_tile(const xb_gemm_launch* L, long long t) {
+static inline xb_gemm_rec xb_gemm_tile_at(const xb_gemm_launch* L, long long t, long long grid_m) {
   xb_gemm_rec r;
   if (L->recs != NULL) r = L->recs[t];
   else if (L->a == NULL && L->c == NULL) r = L->one;
   else {
-    r.a = (const char*)L->a + t * L->tile_stride_a; r.b = (const char*)L->b + t * L->tile_stride_b; r.c = (char*)L->c + t * L->tile_stride_c;
+    if (grid_m > 0) {   /* a grid has at most 2^31 - 1 tiles (libxsmm_b200_gemm_batch_grid): 32-bit division */
+      const long long i = (long long)((unsigned int)t % (unsigned int)grid_m), j = (long long)((unsigned int)t / (unsigned int)grid_m);
+      r.a = (const char*)L->a + i * L->tile_stride_a; r.b = (const char*)L->b + j * L->tile_stride_b;
+      r.c = (char*)L->c + i * L->tile_stride_c + j * L->tile_stride_c_n;
+    } else {
+      r.a = (const char*)L->a + t * L->tile_stride_a; r.b = (const char*)L->b + t * L->tile_stride_b; r.c = (char*)L->c + t * L->tile_stride_c;
+    }
     r.a_aux = NULL; r.b_aux = NULL; r.br = L->br; r.scf = L->one.scf; r.a_q = L->one.a_q;
     r.d = (L->one.d != NULL) ? (const char*)L->one.d + t * L->tile_stride_d : NULL;
     r.c_aux = (L->one.c_aux != NULL) ? (char*)L->one.c_aux + t * L->tile_stride_c_aux : NULL;
@@ -212,6 +224,10 @@ static inline xb_gemm_rec xb_gemm_tile(const xb_gemm_launch* L, long long t) {
   }
   return r;
 }
+#if defined(__CUDACC__)
+__host__ __device__
+#endif
+static inline xb_gemm_rec xb_gemm_tile(const xb_gemm_launch* L, long long t) { return xb_gemm_tile_at(L, t, L->grid_m); }
 
 /* the launch of tiles [t0, t0 + n) of L: tile t of it is tile t0 + t of L, since its records, or its strided bases, start at tile t0
  * -- the bases are the fields xb_gemm_tile advances */
